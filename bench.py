@@ -11,7 +11,7 @@ C3, C5) times one render per frame instead, as round 1 did; the C2 single-render
 `single_render`.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload C4] [--pattern auto|five|single] [--frames F]
-                  [--lanes S] [--impl b200|reference]
+                  [--lanes S] [--impl b200|reference] [--dump-outputs DIR]
 
 Legs (one JSON line, rank 0):
   value        device-resident: inputs in HBM, C ABI driven through the plan objects, the step captured in a CUDA graph
@@ -27,8 +27,15 @@ Legs (one JSON line, rank 0):
   cpu_baseline the CPU oracle (oracle/, kind "port") on the host cores, bounded sample of the same pattern (N = 1 only)
 `--impl reference` times that CPU oracle on the same pattern through the same GaussianRenderer call (reference arm).
 
-Timing: W >= 3 warm-up steps; L2 flushed (256 MiB memset) before every timed step, outside the per-step CUDA event pairs;
-per-rank time = sum of per-step event durations; max over ranks.  Clocks: NVML polled by a thread during the timed region.
+Timing: W >= 3 warm-up steps; every timed leg runs K timed steps; L2 flushed (256 MiB memset) before every timed step,
+outside the per-step CUDA event pairs; per-rank time = sum of per-step event durations; max over ranks.  Clocks: NVML
+polled by a thread during the timed region.
+
+--dump-outputs DIR: after the timed steps of the `value` leg, rank 0 writes what its last step computed -- what a caller
+of that path receives -- as DIR/<name>.npy (float32): the step's flat gradient bucket, the densification maximum and, of
+the step's last frame, every render's image, alpha and radii (five pattern) or image, depth, alpha and radii (single).
+Inputs are seeded, so two builds run with the same arguments can be compared output for output.  Beyond 64 MiB in all,
+each array is replaced by a fixed, seeded sample of its elements.
 """
 from __future__ import annotations
 
@@ -82,6 +89,8 @@ def parse():
                     help="single pattern e2e: Gaussian set host->device once per step or once per frame")
     ap.add_argument("--trace-e2e", default=None, help="write a chrome trace (CUPTI via torch.profiler) of one e2e step here")
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="CPU budget of the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (see the module docstring)")
     return ap.parse_args()
 
 
@@ -305,11 +314,29 @@ class ClockSampler:
                 "source": "nvidia-smi -lms 20"}
 
 
+DUMP_LIMIT = 64 << 20  # bytes written by --dump-outputs in all
+
+
+def dump_outputs(dirpath, arrays):
+    """Writes `arrays` (name -> tensor) as DIR/<name>.npy in float32.  When they exceed DUMP_LIMIT in all, every array is
+    replaced by a sample of its flattened elements, positions drawn with a fixed seed, sized to its share of the limit."""
+    import numpy as np
+    os.makedirs(dirpath, exist_ok=True)
+    total = 4 * sum(t.numel() for t in arrays.values())
+    room = DUMP_LIMIT - 4096 * len(arrays)  # .npy headers
+    for name, t in arrays.items():
+        a = t.detach().to(torch.float32).cpu().numpy()
+        if total > room:
+            a = a.reshape(-1)
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, a.size * room // total, replace=False))]
+        np.save(os.path.join(dirpath, name + ".npy"), a)
+
+
 # ---------------------------------------------------------------------------------------------------------------
-# B200 arm: shared plumbing
+# GPU arm: shared plumbing
 # ---------------------------------------------------------------------------------------------------------------
 class Env:
-    """Process-wide state of the B200 arm: ranks, device, the loaded library, timing helpers."""
+    """Process-wide state of the GPU arm: ranks, device, the loaded library, timing helpers."""
 
     def __init__(self, args):
         import torch.distributed as dist
@@ -319,7 +346,7 @@ class Env:
         self.world = int(os.environ.get("WORLD_SIZE", "1"))
         self.local = int(os.environ.get("LOCAL_RANK", "0"))
         if not torch.cuda.is_available():
-            raise SystemExit("bench.py: no CUDA device; the B200 arm has no CPU fallback (use --impl reference)")
+            raise SystemExit("bench.py: no CUDA device; the GPU arm has no CPU fallback (use --impl reference)")
         torch.cuda.set_device(self.local)
         self.dev = torch.device("cuda", self.local)
         if self.world > 1:
@@ -388,17 +415,20 @@ def peaks_and_traffic(workload_key, dom):
     return peaks, traffic
 
 
+HBM_GBS = 3350.0  # H100 SXM (80 GB HBM3) data-sheet bandwidth, used when no measured peak is given
+
+
 def roofline_dict(per_kernel, algo, workload_key, extra):
     dom = max(("composite_fwd", "composite_bwd"), key=lambda k: per_kernel[k]["ms_avg"] * (1 if per_kernel[k]["launches"] else 0))
     peaks, traffic = peaks_and_traffic(workload_key, dom)
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", HBM_GBS))
     ms = per_kernel[dom]["ms_avg"]
     ach = algo[dom] / (ms * 1e-3) / 1e9 if ms > 0 else 0.0
     other = "composite_fwd" if dom == "composite_bwd" else "composite_bwd"
     oms = per_kernel[other]["ms_avg"]
     r = {"bound": "hbm", "kernel": dom, "achieved": ach, "peak": peak, "unit": "GB/s",
          "frac": ach / peak if peak else None, "traffic": traffic,
-         "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "fallback 6650 GB/s",
+         "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "H100 SXM data sheet, 3350 GB/s",
          "algorithmic_bytes_per_launch": algo[dom], "kernel_ms_avg": ms,
          "other_composite": {"kernel": other, "kernel_ms_avg": oms, "algorithmic_bytes_per_launch": algo[other],
                              "frac": (algo[other] / (oms * 1e-3) / 1e9 / peak) if oms > 0 and peak else None},
@@ -543,6 +573,12 @@ def bench_five(env, args, wl, wl_key):
         step()
     clocks = ClockSampler(env.local) if rank == 0 else None
     ms_total, wall, launches_eager = env.timed(step, K)
+    if args.dump_outputs and rank == 0:  # the last frame of the step ran on lane (F - 1) mod S
+        last = engines[(len(weak_frames) - 1) % S]
+        out = {"grad_bucket": flat, "radius_max": stats["radius_max"]}
+        for r in FIVE:
+            out[r + "_color"], out[r + "_alpha"], out[r + "_radii"] = last.render_outputs(r)
+        dump_outputs(args.dump_outputs, out)
     if clocks is not None and len(clocks.samples) < 20:
         t_end = time.perf_counter() + 0.5
         while time.perf_counter() < t_end and len(clocks.samples) < 40:
@@ -590,7 +626,7 @@ def bench_five(env, args, wl, wl_key):
     per_view = None
     if engine_kind == "merged":
         from exavatar_release_b200 import _lib as LL
-        peak = float(peaks_and_traffic(wl_key, "composite_fwd")[0].get("hbm_gbs", 6650.0))
+        peak = float(peaks_and_traffic(wl_key, "composite_fwd")[0].get("hbm_gbs", HBM_GBS))
         lib.b2r_profile_enable(1)
         env.profile_read()
         per_view, last = {}, {"A": (0, 0), "B": (0, 0)}
@@ -644,7 +680,7 @@ def bench_five(env, args, wl, wl_key):
 
         for _ in range(3):
             sstep()
-        ks = max(3, min(K, 20))
+        ks = K
         ms_s, _, _ = env.timed(sstep, ks)
         strong = {"value": G * ks / (ms_s * 1e-3), "unit": UNIT, "global_batch": G, "frames_per_rank": len(mine),
                   "ms_per_step": ms_s / ks, "steps": ks,
@@ -679,7 +715,8 @@ def e2e_five(env, args, wl, wl_key, cams, st_w, st_r, scene_a, human_a, refined_
     sets = {"scene": scene_a, "human": human_a, "refined": refined_a}
     host = {n: {k: v.cpu().pin_memory() for k, v in a.items()} for n, a in sets.items()}
     host_grads = {n: {k: torch.empty_like(v).pin_memory() for k, v in a.items()} for n, a in host.items()}
-    host_targets = [torch.rand(3, H, Wd).pin_memory() for _ in range(F)]
+    gen = torch.Generator().manual_seed(2)  # seeded like every other input: runs with the same arguments compare
+    host_targets = [torch.rand(3, H, Wd, generator=gen).pin_memory() for _ in range(F)]
     host_loss = torch.empty(F).pin_memory()
     nbytes = lambda d: sum(v.numel() * 4 for a in d.values() for v in a.values())
     h2d = nbytes(host) + F * 3 * N * 4
@@ -818,7 +855,7 @@ def e2e_five(env, args, wl, wl_key, cams, st_w, st_r, scene_a, human_a, refined_
 
     for _ in range(3):
         step()
-    ke = max(3, min(K, 20))
+    ke = K
     ms_e, _, _ = env.timed(step, ke)
     if args.trace_e2e and env.rank == 0:
         from torch.profiler import ProfilerActivity, profile
@@ -901,8 +938,7 @@ def e2e_five(env, args, wl, wl_key, cams, st_w, st_r, scene_a, human_a, refined_
 
         for _ in range(2):
             eager_step()
-        kk = max(2, min(K, 5))
-        t0 = time.perf_counter()
+        kk = K
         ms_g, _, _ = env.timed(eager_step, kk)
         eager = {"value": world * F * kk / (ms_g * 1e-3), "unit": UNIT, "steps": kk,
                  "host_ms_per_render": ms_g / (kk * F * 5),
@@ -920,7 +956,7 @@ def bench_single(env, args, wl, wl_key, brief=False):
     from exavatar_release_b200.renderer import GaussianRenderer, render_settings
     dev, lib, world, rank = env.dev, env.lib, env.world, env.rank
     dist = env.dist
-    F, K, Wm = args.frames, (min(args.steps, 10) if brief else args.steps), max(args.warmup, 3)
+    F, K, Wm = args.frames, args.steps, max(args.warmup, 3)
     P, H, Wd = wl.n_avatar + wl.n_scene, wl.height, wl.width
     N = H * Wd
     use_sh = wl.sh_degree > 0
@@ -975,6 +1011,11 @@ def bench_single(env, args, wl, wl_key, brief=False):
         step()
     clocks = ClockSampler(env.local) if (rank == 0 and not brief) else None
     ms_total, wall, launches_eager = env.timed(step, K)
+    if args.dump_outputs and rank == 0 and not brief:  # the last frame of the step ran on lane (F - 1) mod S
+        last = lanes.plans[(F - 1) % S]
+        out = {"grad_bucket": lanes.bucket} if wl.backward else {}
+        out.update(color=last.color, depth=last.depth, alpha=last.alpha, radii=last.radii)
+        dump_outputs(args.dump_outputs, out)
     if clocks is not None and len(clocks.samples) < 20:
         t_end = time.perf_counter() + 0.5
         while time.perf_counter() < t_end and len(clocks.samples) < 40:
@@ -1027,7 +1068,8 @@ def bench_single(env, args, wl, wl_key, brief=False):
     e2e_eager = None
     if not args.no_e2e:
         host_assets = {k: v.cpu().pin_memory() for k, v in assets.items() if (k != "rgb" or not use_sh)}
-        host_targets = [torch.rand(3, H, Wd).pin_memory() for _ in range(F)]
+        gen = torch.Generator().manual_seed(2)  # seeded like every other input: runs with the same arguments compare
+        host_targets = [torch.rand(3, H, Wd, generator=gen).pin_memory() for _ in range(F)]
         host_grads = {k: torch.empty_like(v).pin_memory() for k, v in host_assets.items()}
         host_m2 = torch.empty(P, 3).pin_memory()
         host_loss = torch.empty(F).pin_memory()
@@ -1204,7 +1246,7 @@ def bench_single(env, args, wl, wl_key, brief=False):
 
         for _ in range(3):
             e2e_step()
-        ke = max(3, min(K, 20))
+        ke = K
         ms_e, _, _ = env.timed(e2e_step, ke)
         if args.trace_e2e and rank == 0:  # after the timed region: one more step under the profiler
             from torch.profiler import ProfilerActivity, profile
@@ -1239,7 +1281,7 @@ def bench_single(env, args, wl, wl_key, brief=False):
 
             for _ in range(2):
                 eager_step()
-            kk = max(2, min(K, 5))
+            kk = K
             ms_g, _, _ = env.timed(eager_step, kk)
             eager_call[0] = False
             e2e_eager = {"value": world * F * kk / (ms_g * 1e-3), "unit": UNIT, "steps": kk,

@@ -1,4 +1,4 @@
-"""exavatar_release_b200 -- B200-native differentiable Gaussian rasteriser for ExAvatar's render path.
+"""exavatar_release_b200 -- H100-native (sm_90a) differentiable Gaussian rasteriser for ExAvatar's render path.
 
 Public surface (mirrors what /root/reference/avatar/common/nets/module.py:11 imports):
     GaussianRasterizationSettings, GaussianRasterizer

@@ -1,7 +1,7 @@
 """ctypes binding of libb200raster.so (the C ABI in include/b200raster.h).
 
 There is NO CPU fallback: if the shared library is missing or cannot be loaded, `load()` raises.  The library is built
-in-tree by `exavatar_release_b200.build_ext.build()` (nvcc, sm_100a).
+in-tree by `exavatar_release_b200.build_ext.build()` (nvcc, sm_90a).
 """
 from __future__ import annotations
 
@@ -128,7 +128,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"b200raster: {LIB_PATH} not found. Build it with `python -m exavatar_release_b200.build_ext` "
-            "(nvcc, sm_100a). There is no CPU fallback.")
+            "(nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, restype, argtypes in SYMBOLS:
         fn = getattr(lib, name)  # AttributeError if the .so is stale

@@ -1,6 +1,6 @@
-"""Builds libb200raster.so (the C-ABI library of include/b200raster.h) in-tree with nvcc for sm_100a.
+"""Builds libb200raster.so (the C-ABI library of include/b200raster.h) in-tree with nvcc for the H100 (sm_90a).
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.  nvcc cross-compiles without a GPU.
+The .so is a build product (git-ignored); nvcc cross-compiles it without a GPU.
 """
 from __future__ import annotations
 
@@ -13,8 +13,9 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libb200raster.so")
 
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # Hopper (H100); the only architecture the kernels are tuned for
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *ARCH,
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--shared",
@@ -79,7 +80,7 @@ def build(force: bool = False, verbose: bool = False, ptxas_info: bool = False) 
 
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         list(ex.map(compile_one, zip(srcs, objs)))
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "--shared", "-o", LIB, *objs]
+    cmd = [nvcc, *ARCH, "--shared", "-o", LIB, *objs]
     if verbose:
         print(" ".join(cmd), flush=True)
     subprocess.check_call(cmd)

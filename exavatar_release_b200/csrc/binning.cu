@@ -48,7 +48,7 @@ __global__ void __launch_bounds__(256) scatter_kernel(const B2RScene sc, const C
 }
 
 // K2, aggregated variant (default when the per-tile counters fit in shared memory).  Atomics from different warps to
-// the same global address serialise in L2 (~15 ns each on the hot avatar tiles, which receive thousands), so a CTA
+// the same global address serialise in L2 (the hot avatar tiles receive thousands), so a CTA
 // claims its slots of a tile with ONE global atomic: (1) count the CTA's pairs per tile in shared memory, (2) one
 // atomicAdd per touched tile reserves a contiguous run of the tile's segment, (3) enumerate again and drop each pair
 // at run base + its rank inside the CTA (shared-memory atomic).  Both enumerations replay the projection's kept masks.
@@ -111,9 +111,8 @@ __global__ void __launch_bounds__(256) scatter_agg_kernel(const B2RScene sc, con
 // Lists of >= 2048 entries are sorted in chunks of SORT_CHUNK and merged (merge_chunks_kernel): no length limit.
 // ---------------------------------------------------------------------------------------------------------------
 
-// Lanes holding the same 8-bit digit (invalid lanes match nobody).  Eight ballots instead of MATCH.ANY: on sm_100a
-// MATCH.ANY measured an order of magnitude slower than this sequence (tools/cta_trace.py on the sort kernel: a
-// 2000-entry tile took 31 us with it).
+// Lanes holding the same 8-bit digit (invalid lanes match nobody), from eight ballots instead of MATCH.ANY (the sort
+// kernel's CTA timeline, tools/cta_trace.py, compares the two).
 __device__ __forceinline__ unsigned match_digit(const uint32_t d, const bool valid) {
   unsigned peers = __ballot_sync(0xffffffffu, valid);
 #pragma unroll
@@ -504,9 +503,9 @@ __global__ void __launch_bounds__(THREADS) sort_mixed_kernel(const Ctx cx) {
 // 64-bit (depth, id) key, which is unique, so the positions are a permutation.
 // One work item = one chunk (2048 entries, eight per thread).  The other chunk is staged in shared memory with one round
 // of coalesced loads and searched there (11 branch-free steps, the eight searches of a thread interleaved), and the
-// chunk -> list look-up runs on a staged copy of the chunk table.  Round 2's first version searched in global memory: per
-// entry ~40 DEPENDENT L2 accesses (7 for the look-up, 11 per other chunk), 16.7 us for 3.5 M instructions at 63 % warp
-// occupancy -- pure latency, and that much register-file-time taken from the frames in flight.  Exits at once when no list
+// chunk -> list look-up runs on a staged copy of the chunk table.  Searching in global memory instead would cost per entry
+// ~40 DEPENDENT L2 accesses (7 for the look-up, 11 per other chunk) -- pure latency, and that much register-file-time
+// taken from the frames in flight.  Exits at once when no list
 // is that long (the common case at ExAvatar's single-render sizes).
 constexpr int MERGE_TABLE = 1024;  // staged entries of chunk_start (lists of >= 2048 entries; more fall back to global loads)
 __global__ void __launch_bounds__(256) merge_chunks_kernel(const Ctx cx) {
@@ -603,8 +602,8 @@ int launch_binning(const B2RScene& sc, const Ctx& cx, bool rescan, cudaStream_t 
   if (sc.P > 0) {
     ProfScope p(K_SCATTER, st);
     const size_t smem = (size_t)cx.tiles * 8;
-    // worth it while the per-CTA zero / flush sweeps over the tile table stay small (measured: 1024 tiles 1.3-1.6x
-    // faster, 8160 tiles 2x slower than direct atomics)
+    // worth it while the per-CTA zero / flush sweeps over the tile table stay small (at 8160 tiles they cost more than
+    // the direct atomics save)
     if (cx.tiles <= 2048) {
       cudaFuncSetAttribute(scatter_agg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
       launch_k(scatter_agg_kernel, (sc.P + 255) / 256, 256, smem, st, true, sc, cx);

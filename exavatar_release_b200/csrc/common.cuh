@@ -1,4 +1,4 @@
-// common.cuh -- shared constants, buffer layouts and device helpers of the B200 rasteriser.
+// common.cuh -- shared constants, buffer layouts and device helpers of the rasteriser.
 // Algorithm constants follow SURVEY.md App. A (the published 3DGS rasteriser the reference imports at
 // avatar/common/nets/module.py:11); the kernel design is this repository's own.
 #pragma once
@@ -34,10 +34,9 @@ constexpr int SORT_CHUNK = 2048;  // per-tile sort: lists are sorted in chunks o
 // each (quarter tile, segment) as an independent work item.  SEG is a multiple of the forward's staging batch, so cuts are
 // batch boundaries.
 #ifndef SEG_SHIFT
-#define SEG_SHIFT 9  // log2 of the segment length; tuning hook (build_ext.py B2R_NVCC_EXTRA).  Measured on C4 (five-render training
-                     // frames/s in flight | scene-view backward alone | human-view backward alone): 256: 2005 | 111 us | 60 us,
-                     // 512: 2101 | 91 us | 63 us, 1024: 2136 | 86 us | 97 us -- every work item pays ~6 dependent global loads
-                     // before its first batch, so fewer, longer items win until the longest chain becomes the tail
+#define SEG_SHIFT 9  // log2 of the segment length; tuning hook (build_ext.py B2R_NVCC_EXTRA).  Every work item pays ~6
+                     // dependent global loads before its first batch, so fewer, longer items win until the longest chain
+                     // becomes the tail
 #endif
 constexpr int SEG = 1 << SEG_SHIFT;
 constexpr int CK_PLANE0 = TILE_PIX * 4;              // floats: per pixel (T, C_r, C_g, C_b)
@@ -531,8 +530,8 @@ __device__ __forceinline__ void trace_end(unsigned long long t0, int n) {
 
 // Kernel launch with an execution priority (a launch attribute; captured into CUDA-graph kernel nodes as well).
 // When several frames are in flight on different streams (plan.py FrameLanes) the block scheduler hands freed SM
-// resources to pending CTAs in launch order, so a 1-CTA scan or a few-hundred-CTA projection of frame B used to wait
-// behind the thousands of composite CTAs frame A still had queued (tools/lanes_timeline.py: 50-120 us gaps).  The
+// resources to pending CTAs in launch order, so a 1-CTA scan or a few-hundred-CTA projection of frame B would wait
+// behind the thousands of composite CTAs frame A still has queued (tools/lanes_timeline.py shows such gaps).  The
 // short, latency-bound kernels of the chain therefore run at high priority and the two composites at the default.
 int launch_priority(bool high);
 int device_sm_count();

@@ -343,7 +343,7 @@ __device__ __forceinline__ void bwd4_item(const B2RScene& sc, const Ctx& cx, con
 // The number of work items -- 4 quarter tiles x (segments of the multi-segment tiles + one per remaining tile) -- is only
 // known on the device, so the grid is a fixed number of CTAs that stride over the items (heaviest first: the item order
 // follows cx.tile_order).  A grid sized for the host-side worst case (capacity / SEG segments) would be mostly CTAs that
-// read two counters and exit -- 185 000 of 191 000 with a generously sized workspace (profiles/r02_notes.md).
+// read two counters and exit -- most of them with a generously sized workspace.
 template <bool HAS_DA>
 __global__ void __launch_bounds__(B4_THREADS, B4_MIN_BLOCKS) composite_bwd4_kernel(const B2RScene sc, const Ctx cx,
                                                                     const B2RBackwardArgs args, float* __restrict__ gacc) {

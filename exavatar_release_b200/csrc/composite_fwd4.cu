@@ -3,7 +3,7 @@
 // Replaces the reference rasteriser's forward render kernel for ExAvatar's render path
 // (avatar/common/nets/module.py:632 -> render_img, render_depthmap, render_mask).
 //
-// Design (B200).  The kernel is issue- and latency-bound, not HBM-bound (SURVEY.md section 7.2; ncu in profiles/), so
+// Design.  The kernel is issue- and latency-bound, not HBM-bound (SURVEY.md section 7.2; DESIGN.md section 5), so
 // the structure removes per-pixel work and idle SMs rather than bytes:
 //   * work unit = one 8x8 quarter of a 16x16 tile, one 64-thread CTA (2 warps, each an 8x4 pixel rect), launched
 //     longest-list-first (cx.tile_order).  A quarter retires as soon as its own 64 pixels are saturated, and only two
@@ -20,17 +20,16 @@
 //     independent work item instead of walking 2000 entries on one warp;
 //   * VIEWS (B2RView): Gaussians outside the view's index range are dropped when a batch is staged (no gather for
 //     them); tiles whose list holds nothing of the view's own (tile_maxid < skip_below) are skipped altogether.
-// Measured and rejected in round 2 (profiles/r02_notes.md): splitting the long lists of the forward over eight warps per
-// pixel rect (local blends from T = 1, a prefix walk over the segments' transmittance products, replay of the one
-// segment in which a pixel stops).  It was exact and shortened the kernel ALONE on long-list workloads (C4 merged
-// pass 109 -> 89 us) but cost throughput with other kernels in flight (speculative segments, replays, CTA barriers:
-// C4 1408 -> 1152 training frames/s; C5 forward 279 -> 468 us), which is how the training step runs.
+// Not done here: splitting the long lists of the forward over eight warps per pixel rect (local blends from T = 1, a
+// prefix walk over the segments' transmittance products, replay of the one segment in which a pixel stops).  It is exact
+// and shortens the kernel ALONE on long-list workloads, but spends more warp-time (speculative segments, replays, CTA
+// barriers), which costs throughput with other kernels in flight -- and that is how the training step runs.
 #include "common.cuh"
 
 namespace b2r {
 
 #ifndef FL_BATCH_N
-#define FL_BATCH_N 128  // entries staged per batch (tuning hook; 64 measured in profiles/r02_notes.md)
+#define FL_BATCH_N 128  // entries staged per batch (tuning hook)
 #endif
 constexpr int F4_BATCH = 2 * FL_BATCH_N;  // capacity of the two-half staging buffer
 #ifndef F4_GROUP_N
@@ -222,8 +221,7 @@ __global__ void __launch_bounds__(FL_THREADS, F4_MIN_BLOCKS) composite_fwd_kerne
   const uint32_t id_begin = cx.id_begin, id_span = cx.id_span;
   // The gather of a batch is two dependent global loads (list entry -> record).  The list entries of batch b+2 are
   // fetched into registers while batch b is composited, so that issue(b+1) starts its record gathers without waiting for
-  // them (ncu source page of the thin views, profiles/r02_notes.md: a quarter of the stall samples sat on that wait, and
-  // the partner warp's share of it at the batch barrier).
+  // them (otherwise the gathers of a batch, and the partner warp at the batch barrier, stall on that wait).
   constexpr int FL_PER_THREAD = FL_BATCH / FL_THREADS;
   uint32_t next_id[FL_PER_THREAD];
   auto prefetch = [&](int b) {

@@ -31,7 +31,7 @@ int device_sm_count() {
   if (dev < 0 || dev >= 64) dev = 0;
   int v = cache[dev].load(std::memory_order_relaxed);
   if (v == 0) {
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;  // H100 SXM
     cache[dev].store(v, std::memory_order_relaxed);
   }
   return v;

@@ -53,7 +53,7 @@ __device__ __forceinline__ void sh_to_rgb(int deg, const float* __restrict__ sh,
 __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2RScene sc, const Ctx cx, int32_t* __restrict__ radii,
                                                       const int aggregate) {
   // CTA-level histogram in shared memory: atomics of different warps to the SAME global address serialise in L2
-  // (~15 ns each measured on the hot avatar tiles), so each CTA adds to a tile's counter at most once.
+  // (the hot avatar tiles receive thousands), so each CTA adds to a tile's counter at most once.
   extern __shared__ uint32_t s_cnt[];
   if (aggregate) {
     for (int t = threadIdx.x; t < cx.tiles; t += blockDim.x) s_cnt[t] = 0u;
@@ -112,7 +112,7 @@ __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2R
       // Homogeneous position and pixel centre WITHOUT fma contraction, operation for operation as the oracle's C
       // expression (App. A.1 steps 2, 7).  One ulp of a pixel coordinate near 1000 is 6e-5 px; through a sharp splat's
       // exponent that is a 1e-4 relative change of alpha, enough to flip alpha >= 1/255 decisions the oracle's threshold
-      // margins do not expect (seen at 1024^2 / 1080p, profiles/r02_notes.md).  Bit-identical centres remove that source.
+      // margins do not expect (seen at 1024^2 / 1080p).  Bit-identical centres remove that source.
       const float ph_x = dot4_rn(cam.p[0], p.x, cam.p[4], p.y, cam.p[8], p.z, cam.p[12]);
       const float ph_y = dot4_rn(cam.p[1], p.x, cam.p[5], p.y, cam.p[9], p.z, cam.p[13]);
       const float ph_w = dot4_rn(cam.p[3], p.x, cam.p[7], p.y, cam.p[11], p.z, cam.p[15]);

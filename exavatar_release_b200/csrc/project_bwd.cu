@@ -285,7 +285,7 @@ __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& c
 // contiguous block of its 32 rows in with coalesced 128-byte accesses (odd row stride: conflict-free), the body
 // turns each row into its gradient in place, and the warp writes (or accumulates) the block back the same way.
 #ifndef PBWD_MIN_BLOCKS
-#define PBWD_MIN_BLOCKS 3  // 80 registers (64 bytes spilled): three CTAs per SM measured faster than two at 116; tuning hook
+#define PBWD_MIN_BLOCKS 3  // caps the kernel at 80 registers (three CTAs per SM) at the price of a small spill; tuning hook
 #endif
 __global__ void __launch_bounds__(256, PBWD_MIN_BLOCKS) project_bwd_kernel(const B2RScene sc, const Ctx cx, const B2RBackwardArgs out,
                                                           const float* __restrict__ gacc) {

@@ -2,7 +2,7 @@
 //
 // `GaussianRasterizer.forward` (exavatar_release_b200/rasterizer.py; reference call site avatar/common/nets/module.py:632-640)
 // spent ~0.2 ms of Python per render around ~0.1 ms of kernel launches: building ctypes structs, a dozen torch.empty calls,
-// the autograd.Function trampolines in both directions (profiles/r02_notes.md, eager profile).  This file is the same
+// the autograd.Function trampolines in both directions (tools/eager_profile.py).  This file is the same
 // host logic -- argument normalisation, the duplicate-capacity policy with its pinned-host status mirror, workspace
 // allocation, the saved context, the backward call -- as a C++ torch::autograd::Function over the SAME C ABI
 // (include/b200raster.h, libb200raster.so).  No kernels here and no second implementation of anything on the device.

@@ -114,7 +114,7 @@ class FrameLanes:
     """S concurrent `FramePlan`s ("lanes"), each on its own CUDA stream with its own workspace and gradient bucket.
 
     Frames of a training batch are independent (SURVEY.md section 8e; avatar/main/model.py:81 loops over them), and at
-    ExAvatar's sizes a single frame cannot fill a B200: the scan / sort kernels are latency-bound single-wave launches
+    ExAvatar's sizes a single frame cannot fill an H100: the scan / sort kernels are latency-bound single-wave launches
     and the composites end in a tail of long tile lists.  Running frame f on lane f mod S lets the hardware fill those
     holes with another frame's kernels.  The lanes fork from and join back into the caller's current stream, so the
     whole step is still one CUDA-graph capture.  Gradients of the frames of one lane are summed inside the backward

@@ -4,7 +4,7 @@ Drop-in for `from diff_gaussian_rasterization_depth import GaussianRasterization
 (/root/reference/avatar/common/nets/module.py:11): same 12-field settings tuple in the order of the call site
 (module.py:609-622), same keyword call (module.py:632-640), same 4-tuple `(color, radii, depth, alpha)` (module.py:632),
 same argument-validation exceptions, gradients for the same eight tensor inputs.  The compute is the hand-written
-sm_100a library behind include/b200raster.h, reached through ctypes with raw device pointers on the caller's current
+sm_90a library behind include/b200raster.h, reached through ctypes with raw device pointers on the caller's current
 CUDA stream; PyTorch only owns memory, streams and autograd.
 
 No CPU path exists here on purpose: CPU tensors or a missing libb200raster.so raise.

@@ -1,7 +1,7 @@
 """Host-side mirror of ExAvatar's render boundary.
 
 `GaussianRenderer.forward` restates /root/reference/avatar/common/nets/module.py:592-647 (the only
-caller of the rasteriser) without its hard-coded `.cuda()` calls, so the same code drives the B200
+caller of the rasteriser) without its hard-coded `.cuda()` calls, so the same code drives the GPU
 rasteriser on a GPU box and the CPU oracle in tests.  Argument meaning, the settings tuple
 (module.py:609-622), the dummy `mean_2d` leaf (module.py:626-629) and the returned dict
 (module.py:642-647) are the reference's.

@@ -2,7 +2,7 @@
 
 The reference trains one frame at a time on one GPU (`cfg.num_gpus = 1`, `cfg.batch_size = 1`,
 /root/reference/avatar/main/config.py:44-45) and has no collective anywhere.  Frames are independent units
-(avatar/main/model.py:81 loops per frame), so the B200 build shards them: rank r renders frames r, r+world, ... of the
+(avatar/main/model.py:81 loops per frame), so this build shards them: rank r renders frames r, r+world, ... of the
 step's batch against a full replica of the Gaussian parameters, every frame's gradients are summed into ONE flat
 fp32 bucket per rank, and the ranks sum their buckets with a single all-reduce (NCCL on GPUs, gloo in CPU tests).
 The loss of each frame is pre-divided by the global batch size so the reduced gradient equals the gradient of

@@ -1,5 +1,5 @@
 /*
- * b200raster.h -- C ABI of the B200-native differentiable 3D-Gaussian rasteriser.
+ * b200raster.h -- C ABI of the H100-native (sm_90a) differentiable 3D-Gaussian rasteriser.
  *
  * Drop-in boundary for the one hot path of mks0601/ExAvatar_RELEASE: the rasteriser that
  * `GaussianRenderer.forward` reaches through `GaussianRasterizer(raster_settings)(...)`

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -22,7 +22,7 @@ def pytest_collection_modifyitems(config, items):
         has_cuda = False
     if has_cuda:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (run on the B200 box with -m gpu)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (an H100; select with -m gpu)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

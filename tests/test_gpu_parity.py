@@ -1,4 +1,4 @@
-"""Parity of the sm_100a CUDA path against the CPU oracle, through the public autograd API and the C ABI (FramePlan).
+"""Parity of the sm_90a CUDA path against the CPU oracle, through the public autograd API and the C ABI (FramePlan).
 
 Tolerance (north_star: "within 1e-4 rel fp32"): for every output tensor, max|x - y| <= 1e-4 * max|y| over all
 elements whose discrete composite decisions (alpha < 1/255, T(1-a) < 1e-4, power > 0) are not on a threshold; the

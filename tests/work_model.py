@@ -13,8 +13,8 @@ CUDA composites are asked to do by their own culling rules (restated here in num
   lane evaluations    32 x warp hits
   useful evaluations  lanes that actually blend the splat (alive pixel, power <= 0, alpha >= 1/255)
 
-and turns them into the issue-bound time of the forward composite with the measured instruction costs
-(profiles/r01_notes.md: 31 warp-instructions per hit, ~45 per 32-entry cull test + queue append).
+and turns them into the issue-bound time of the composites on an H100 (132 SMs x 4 schedulers, 1.98 GHz) with the kernels'
+instruction costs (31 / 61 warp-instructions per forward / backward hit, ~45 per 32-entry cull test + queue append).
 """
 import argparse
 import math
@@ -32,6 +32,7 @@ from exavatar_release_b200.synthetic import WORKLOADS, make_assets  # noqa: E402
 from oracle import oracle as O  # noqa: E402
 
 LOG2E = 1.4426950408889634
+SMS, GHZ = 132, 1.98  # H100 SXM: SMs and the top SM clock of a 700 W card
 MARGIN = 0.02
 
 
@@ -141,15 +142,15 @@ def main():
     for tag, name, ipt in (("f", "forward", 31.0), ("b", "backward", 48.5 + 12.5)):
         wt, wh, us = f["warp_tests_" + tag], f["warp_hits_" + tag], f["useful_" + tag]
         inst = wh * ipt + wt / 32.0 * 45.0
-        cyc = inst / (148 * 4)
+        cyc = inst / (SMS * 4)
         print(f"  {name}: rect tests {wt:>9d}  rect hits {wh:>9d} ({100 * wh / max(wt, 1):.1f} %)  lane evaluations {LANES * wh:>10d}"
               f"  useful {us:>10d} ({100 * us / max(LANES * wh, 1):.1f} % of the lanes)")
         if LANES != 32:
             print(f"      (a {RW}x{RH} rect is {LANES} lanes: {LANES * wh / 32:.0f} warp-hit equivalents)")
             continue
-        print(f"      modelled warp-instructions {inst / 1e6:6.1f} M  ->  {cyc / 1.965e3:6.1f} us at one instruction per scheduler per cycle"
-              f" (148 SMs x 4, 1.965 GHz); useful lane-evaluations at the same rate would need"
-              f" {us / 32 * ipt / (148 * 4) / 1.965e3:5.1f} us")
+        print(f"      modelled warp-instructions {inst / 1e6:6.1f} M  ->  {cyc / GHZ / 1e3:6.1f} us at one instruction per scheduler per cycle"
+              f" ({SMS} SMs x 4, {GHZ} GHz); useful lane-evaluations at the same rate would need"
+              f" {us / 32 * ipt / (SMS * 4) / GHZ / 1e3:5.1f} us")
     print("  heaviest quarter-tile warps (forward hits of the busiest warp, list length, tile):", longest[:5])
 
 
