@@ -12,6 +12,7 @@ int validate_scene(const B2RScene* sc) {
   if (sc->width > 65535 * TILE || sc->height > 32767 * TILE) return B2R_E_INVALID;
   if (!(sc->tanfovx > 0.f) || !(sc->tanfovy > 0.f)) return B2R_E_INVALID;
   if (!sc->bg || !sc->viewmatrix || !sc->projmatrix || !sc->campos) return B2R_E_INVALID;
+  if (sc->sh_rows < 0 || sc->sh_rows > sc->P) return B2R_E_INVALID;
   if (sc->P > 0) {
     if (!sc->opacities) return B2R_E_INVALID;
     if (sc->skin_xyz) {  // fused skinning replaces means3D
@@ -21,7 +22,11 @@ int validate_scene(const B2RScene* sc) {
     } else if (!sc->means3D) {
       return B2R_E_INVALID;
     }
-    if ((sc->shs != nullptr) == (sc->colors_precomp != nullptr)) return B2R_E_INVALID;  // exactly one colour source
+    if (sc->sh_rows > 0) {  // mixed: SH rows first, then colour rows -- both sources required
+      if (!sc->shs || !sc->colors_precomp) return B2R_E_INVALID;
+    } else if ((sc->shs != nullptr) == (sc->colors_precomp != nullptr)) {
+      return B2R_E_INVALID;  // exactly one colour source
+    }
     const bool sr = sc->scales != nullptr && sc->rotations != nullptr;
     if (sr == (sc->cov3D_precomp != nullptr)) return B2R_E_INVALID;                      // exactly one covariance source
     if ((sc->scales != nullptr) != (sc->rotations != nullptr)) return B2R_E_INVALID;
@@ -45,6 +50,13 @@ int validate_ws(const B2RScene* sc, const B2RWorkspace* ws, bool need_scratch) {
   if (ws->dup_capacity > 0 && !ws->dup_ids) return B2R_E_INVALID;
   if (ws->checkpoints && ws->checkpoint_bytes < b2r_checkpoint_bytes(sc->width, sc->height, ws->dup_capacity)) return B2R_E_WORKSPACE;
   return B2R_OK;
+}
+
+// dL_dshs is required whenever the backward projection writes SH rows: every row of an SH scene, or, in a mixed scene,
+// the SH rows at or above first_row (a detached SH prefix -- cat(scene.detach(), human) -- has none).
+bool missing_dshs(const B2RScene* sc, const B2RBackwardArgs* a) {
+  if (!sc->shs || a->dL_dshs || sc->P == 0) return false;
+  return sc->sh_rows == 0 || (int64_t)a->first_row < (int64_t)sc->sh_rows;
 }
 
 }  // namespace
@@ -175,7 +187,7 @@ int b2r_backward(const B2RScene* scene, const B2RWorkspace* ws, const B2RBackwar
   if (rc) return rc;
   if (!args || !args->dL_dcolor || !bwd_scratch) return B2R_E_INVALID;
   if (bwd_scratch_bytes < b2r_backward_scratch_bytes(scene->P)) return B2R_E_WORKSPACE;
-  if (scene->shs && args->dL_dshs == nullptr && scene->P > 0) return B2R_E_INVALID;
+  if (missing_dshs(scene, args)) return B2R_E_INVALID;
   if ((int64_t)args->first_row > (int64_t)scene->P) return B2R_E_INVALID;
   if (args->dL_dposed && !scene->skin_xyz) return B2R_E_INVALID;
   const Ctx cx = resolve(ws, scene->P, scene->width, scene->height);
@@ -208,7 +220,7 @@ int b2r_backward_project(const B2RScene* scene, const B2RWorkspace* ws, const B2
   if (rc) return rc;
   if (!args || !bwd_scratch) return B2R_E_INVALID;
   if (bwd_scratch_bytes < b2r_backward_scratch_bytes(scene->P)) return B2R_E_WORKSPACE;
-  if (scene->shs && args->dL_dshs == nullptr && scene->P > 0) return B2R_E_INVALID;
+  if (missing_dshs(scene, args)) return B2R_E_INVALID;
   if ((int64_t)args->first_row > (int64_t)scene->P) return B2R_E_INVALID;
   if (args->dL_dposed && !scene->skin_xyz) return B2R_E_INVALID;
   const Ctx cx = resolve(ws, scene->P, scene->width, scene->height);

@@ -50,6 +50,9 @@ __device__ __forceinline__ void sh_to_rgb(int deg, const float* __restrict__ sh,
 #ifndef PROJ_MIN_BLOCKS
 #define PROJ_MIN_BLOCKS 4  // 64 registers: four CTAs per SM; tuning hook (build_ext.py B2R_NVCC_EXTRA)
 #endif
+// MIXED (B2RScene.sh_rows > 0): rows [0, sh_rows) take their colour from `shs`, the rest from `colors_precomp`.  A
+// separate instantiation, so the single-source kernel stays the code it was.
+template <bool MIXED>
 __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2RScene sc, const Ctx cx, int32_t* __restrict__ radii,
                                                       const int aggregate) {
   // CTA-level histogram in shared memory: atomics of different warps to the SAME global address serialise in L2
@@ -61,14 +64,15 @@ __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2R
   }
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   // SH rows (192 bytes apart for degree 3) are staged through shared memory: each warp copies the contiguous block of
-  // its 32 rows with coalesced 128-byte loads; a thread then reads its own row (odd row stride: conflict-free).
+  // its 32 rows with coalesced 128-byte loads; a thread then reads its own row (odd row stride: conflict-free).  In a
+  // mixed scene a warp stages only its rows below sh_rows (none at all past them).
   const float* shrow = nullptr;
   if (sc.shs) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int L = sc.sh_coeffs * 3, S = L | 1;
     float* wstage = reinterpret_cast<float*>(s_cnt + (aggregate ? cx.tiles : 0)) + (size_t)warp * 32 * S;
     const int row0 = blockIdx.x * blockDim.x + warp * 32;
-    const int nrows = min(32, sc.P - row0);
+    const int nrows = min(32, (MIXED ? sc.sh_rows : sc.P) - row0);
     if (nrows > 0) stage_rows<0>(wstage, const_cast<float*>(sc.shs) + (size_t)row0 * L, L, nrows, 0xffffffffu);
     __syncwarp();
     shrow = wstage + lane * S;
@@ -150,7 +154,7 @@ __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2R
           const float o = __ldg(sc.opacities + i);
           float rgb[3];
           uint32_t bits = 0;
-          if (sc.shs) {
+          if (sc.shs && (!MIXED || i < sc.sh_rows)) {  // clamp bits only for SH rows
             sh_to_rgb(sc.sh_degree, shrow, p, cam, rgb, bits);
           } else {
             rgb[0] = __ldg(sc.colors_precomp + 3 * (size_t)i);
@@ -404,8 +408,9 @@ int launch_project(const B2RScene& sc, const Ctx& cx, int32_t* radii, cudaStream
     const size_t smem = (aggregate ? (size_t)cx.tiles * 4 : 0) +
                         (sc.shs ? (size_t)8 * 32 * ((sc.sh_coeffs * 3) | 1) * sizeof(float) : 0) +
                         (sc.skin_xyz ? (size_t)8 * 32 * (sc.skin_J | 1) * sizeof(float) : 0);
-    cudaFuncSetAttribute(project_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);  // per device
-    launch_k(project_kernel, (sc.P + 255) / 256, 256, smem, st, true, sc, cx, radii, aggregate);
+    auto kern = sc.sh_rows > 0 ? project_kernel<true> : project_kernel<false>;
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);  // per device
+    launch_k(kern, (sc.P + 255) / 256, 256, smem, st, true, sc, cx, radii, aggregate);
   }
   { ProfScope p(K_TILE_SCAN, st); launch_k(tile_scan_kernel, 1, 1024, 0, st, true, cx, cx.dup_capacity > 0 ? 1 : 0); }
   return check_launch();

@@ -12,7 +12,9 @@
 namespace b2r {
 
 // Body of K6 for one Gaussian.  `shrow` (shared memory, may be null) holds the Gaussian's SH coefficients on entry and
-// its SH gradient on exit (row layout k*3 + c, as in global memory); see the staging in the kernel below.
+// its SH gradient on exit (row layout k*3 + c, as in global memory); see the staging in the kernel below.  MIXED: a
+// Gaussian with `shrow` is an SH row of a mixed scene, and its colour gradient output is zero (its colour is not an input).
+template <bool MIXED>
 __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& cx, const B2RBackwardArgs& out,
                                                 const float* __restrict__ gacc, const int i, const size_t oi,
                                                 const bool visible, const int4 aux, float* shrow,
@@ -257,7 +259,12 @@ __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& c
   const float dm2z[3] = {dm2[0], dm2[1], 0.f};
   put3(out.dL_dmeans3D, dm);
   put3(out.dL_dmeans2D, dm2z);
-  put3(out.dL_dcolors, dcol);
+  if (MIXED && shrow) {
+    const float zero3[3] = {0.f, 0.f, 0.f};
+    put3(out.dL_dcolors, zero3);
+  } else {
+    put3(out.dL_dcolors, dcol);
+  }
   put3(out.dL_dscales, dscale);
   if (out.dL_dopacities) {
     if (accumulate) out.dL_dopacities[oi] += dop; else out.dL_dopacities[oi] = dop;
@@ -284,9 +291,12 @@ __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& c
 // 128-byte lines per load instruction.  SH rows therefore move through shared memory: every warp copies the
 // contiguous block of its 32 rows in with coalesced 128-byte accesses (odd row stride: conflict-free), the body
 // turns each row into its gradient in place, and the warp writes (or accumulates) the block back the same way.
+// MIXED (B2RScene.sh_rows > 0): only rows [0, sh_rows) are staged and written to dL_dshs (row i - first_row); the other
+// rows take the colour path.  A separate instantiation, so the single-source kernel stays the code it was.
 #ifndef PBWD_MIN_BLOCKS
 #define PBWD_MIN_BLOCKS 3  // caps the kernel at 80 registers (three CTAs per SM) at the price of a small spill; tuning hook
 #endif
+template <bool MIXED>
 __global__ void __launch_bounds__(256, PBWD_MIN_BLOCKS) project_bwd_kernel(const B2RScene sc, const Ctx cx, const B2RBackwardArgs out,
                                                           const float* __restrict__ gacc) {
   extern __shared__ float sh_stage[];
@@ -307,11 +317,12 @@ __global__ void __launch_bounds__(256, PBWD_MIN_BLOCKS) project_bwd_kernel(const
   float* wstage = sh_stage + (size_t)warp * 32 * S;
   const int row0 = blockIdx.x * blockDim.x + warp * 32;
   const int nrows = min(32, sc.P - row0);
-  if (use_sh && nrows > 0) {
-    stage_rows<0>(wstage, const_cast<float*>(sc.shs) + (size_t)row0 * L, L, nrows, 0xffffffffu);
+  const int sh_nrows = MIXED ? min(32, sc.sh_rows - row0) : nrows;  // this warp's SH rows
+  if (use_sh && sh_nrows > 0) {
+    stage_rows<0>(wstage, const_cast<float*>(sc.shs) + (size_t)row0 * L, L, sh_nrows, 0xffffffffu);
     __syncwarp();
   }
-  float* shrow = use_sh ? wstage + lane * S : nullptr;
+  float* shrow = use_sh && (!MIXED || i < sc.sh_rows) ? wstage + lane * S : nullptr;
   const float* wrow = nullptr;
   if (sc.skin_xyz) {  // skinning weight rows, staged like the SH rows (after them in shared memory)
     const int J = sc.skin_J, SJ = J | 1;
@@ -320,17 +331,18 @@ __global__ void __launch_bounds__(256, PBWD_MIN_BLOCKS) project_bwd_kernel(const
     __syncwarp();
     wrow = kstage + lane * SJ;
   }
-  if (active) project_bwd_one(sc, cx, out, gacc, i, (size_t)(i - first_row), visible, aux, shrow, wrow);
+  if (active) project_bwd_one<MIXED>(sc, cx, out, gacc, i, (size_t)(i - first_row), visible, aux, shrow, wrow);
   if ((out.flags & B2R_BWD_SCRATCH_ZEROED) && in_range && visible) {  // leave the accumulator clean for the next render
     float4* row = reinterpret_cast<float4*>(const_cast<float*>(gacc)) + 3 * (size_t)i;
     row[0] = row[1] = row[2] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
-  if (use_sh && nrows > 0) {
-    const unsigned rows_active = __ballot_sync(0xffffffffu, active);
+  if (use_sh && sh_nrows > 0) {
+    // in a mixed scene dL_dshs has sh_rows - first_row rows: only SH rows at or above first_row are written
+    const unsigned rows_active = __ballot_sync(0xffffffffu, active && (!MIXED || i < sc.sh_rows));
     __syncwarp();  // every lane's row is complete before the block is written out cooperatively
     float* dst = out.dL_dshs + ((ptrdiff_t)row0 - first_row) * L;  // rows below first_row are masked off, never touched
-    if (accumulate) stage_rows<2>(wstage, dst, L, nrows, rows_active);
-    else stage_rows<1>(wstage, dst, L, nrows, rows_active);
+    if (accumulate) stage_rows<2>(wstage, dst, L, sh_nrows, rows_active);
+    else stage_rows<1>(wstage, dst, L, sh_nrows, rows_active);
   }
 }
 
@@ -340,8 +352,9 @@ int launch_project_bwd(const B2RScene& sc, const Ctx& cx, const B2RBackwardArgs&
     const bool use_sh = sc.shs != nullptr && a.dL_dshs != nullptr;
     const size_t smem = (use_sh ? (size_t)8 * 32 * ((sc.sh_coeffs * 3) | 1) * sizeof(float) : 0) +
                         (sc.skin_xyz ? (size_t)8 * 32 * (sc.skin_J | 1) * sizeof(float) : 0);
-    cudaFuncSetAttribute(project_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024);  // per device
-    launch_k(project_bwd_kernel, (sc.P + 255) / 256, 256, smem, st, true, sc, cx, a, gacc);
+    auto kern = sc.sh_rows > 0 ? project_bwd_kernel<true> : project_bwd_kernel<false>;
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024);  // per device
+    launch_k(kern, (sc.P + 255) / 256, 256, smem, st, true, sc, cx, a, gacc);
   }
   return check_launch();
 }

@@ -38,25 +38,28 @@ from typing import Dict, Optional
 import torch
 from torch import nn
 
-from .plan import RENDERS, MergedFivePlan, _views_of
+from .plan import RENDERS, MergedFivePlan, _views_of, merged_bucket_layout, merged_pass_a_views
 from .rasterizer import GaussianRasterizationSettings, _f32c
 from .renderer import render_settings
 
 _KEYS = ("mean_3d", "opacity", "scale", "rotation", "rgb")
+_SH_KEYS = ("mean_3d", "opacity", "scale", "rotation", "shs")  # a scene coloured from SH inside the kernels
 _GRAD_OF = {"mean_3d": "means3D", "opacity": "opacities", "scale": "scales", "rotation": "rotations", "rgb": "colors"}
 
 
 class _FrameFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, mod, settings, settings_h, scene_m2d, *tensors):
+    def forward(ctx, mod, settings, settings_h, sh_degree, scene_m2d, *tensors):
         plan: MergedFivePlan = mod.plan
-        scene, human, refined = (dict(zip(_KEYS, (_f32c(t.detach(), k) for k, t in zip(_KEYS, tensors[i * 5:i * 5 + 5]))))
-                                 for i in range(3))
+        scene, human, refined = (dict(zip(keys, (_f32c(t.detach(), k) for k, t in zip(keys, tensors[i * 5:i * 5 + 5]))))
+                                 for i, keys in enumerate((mod._scene_keys, _KEYS, _KEYS)))
+        if plan.M > 0:
+            scene["sh_degree"] = sh_degree
         mod._frame_no += 1
         if mod.use_graph:
             mod._graph_forward(settings, settings_h, scene, human, refined)
         else:
-            plan.set_scene(scene)
+            plan.set_scene(scene)  # an SH scene: both passes read the caller's coefficient tensor itself
             plan.forward_frame(None, settings, settings_h, scene, human, refined)  # no descriptor cache: cameras change
         outs = []
         for r in RENDERS:  # fresh tensors: the plan's image buffers are overwritten by the next frame
@@ -83,30 +86,40 @@ class _FrameFn(torch.autograd.Function):
         if mod.use_graph:
             flat_a, flat_b = mod._graph_backward(gc, gd, ga)  # fresh copies of the resident gradient buffers
         else:
-            flat_a = torch.empty(plan.PER * plan.P, dtype=torch.float32, device=dev)
+            flat_a = torch.empty(mod._flat_a_numel, dtype=torch.float32, device=dev)
             flat_b = torch.empty(plan.PER * plan.Ph, dtype=torch.float32, device=dev)
-        _, va = _views_of(flat_a, plan.P)
+        va = merged_pass_a_views(flat_a, plan.Ps, plan.Ph, plan.M)
         _, vb = _views_of(flat_b, plan.Ph)
         if not mod.use_graph:
             plan.backward_frame(gc, va, vb, g_depths=gd, g_alphas=ga, densify=mod.densify)
         Ps = plan.Ps
-        out = [None, None, None, va["means2D"][:Ps].reshape(ctx.m2d_shape)]
-        for part in (lambda v: v[:Ps], lambda v: v[Ps:]):
-            for k in _KEYS:
-                out.append(part(va[_GRAD_OF[k]]))
+        out = [None, None, None, None, va["means2D"][:Ps].reshape(ctx.m2d_shape)]
+        for k in mod._scene_keys:
+            out.append(va["shs"] if k == "shs" else va[_GRAD_OF[k]][:Ps])
+        for k in _KEYS:
+            out.append(va[_GRAD_OF[k]][Ps:])
         for k in _KEYS:
             out.append(vb[_GRAD_OF[k]])
         for i, shp in enumerate(ctx.shapes):
-            out[4 + i] = out[4 + i].reshape(shp)
+            out[5 + i] = out[5 + i].reshape(shp)
         return tuple(out)
 
 
 class TrainingFrameRenderer(nn.Module):
+    """sh_coeffs = M > 0: the scene asset dict carries `shs` (P_scene, M, 3) + `sh_degree` instead of `rgb` -- what
+    `renderer.scene_gaussian_assets(..., in_kernel_sh=True)` returns -- and the scene is coloured inside the projection
+    kernels of both merged passes (SURVEY.md section 8f-4); its gradient reaches `shs` and, through the view direction,
+    `mean_3d`.  The human sets keep `rgb`."""
+
     def __init__(self, P_scene: int, P_human: int, img_shape, device, dup_capacity: Optional[Dict[str, int]] = None,
-                 use_graph: bool = False, graph_depth_alpha: bool = False):
+                 use_graph: bool = False, graph_depth_alpha: bool = False, sh_coeffs: int = 0):
         super().__init__()
         self.img_shape = (int(img_shape[0]), int(img_shape[1]))
-        self.plan = MergedFivePlan(P_scene, P_human, self.img_shape[1], self.img_shape[0], dup_capacity, device)
+        self.plan = MergedFivePlan(P_scene, P_human, self.img_shape[1], self.img_shape[0], dup_capacity, device,
+                                   sh_coeffs=sh_coeffs)
+        self._scene_keys = _SH_KEYS if self.plan.M > 0 else _KEYS
+        lay = merged_bucket_layout(self.plan.Ps, self.plan.Ph, self.plan.M)
+        self._flat_a_numel = lay["A"][1] + lay["A_shs"][1]  # pass A's gradients (+ the scene's dL/dSH)
         self.densify = None  # optional {'grad_accum','count','radius_max'} (P_scene) tensors updated by the backward
         self._frame_no = 0
         self.use_graph = bool(use_graph)
@@ -119,9 +132,11 @@ class TrainingFrameRenderer(nn.Module):
             # dL/ddepth and dL/dalpha inputs only when asked for: their backward variant is the slower one
             self._gin_d = {r: torch.zeros(1, H, W, dtype=torch.float32, device=dev) for r in RENDERS} if graph_depth_alpha else None
             self._gin_a = {r: torch.zeros(1, H, W, dtype=torch.float32, device=dev) for r in RENDERS} if graph_depth_alpha else None
-            self._flat_a = torch.zeros(plan.PER * plan.P, dtype=torch.float32, device=dev)
+            self._flat_a = torch.zeros(self._flat_a_numel, dtype=torch.float32, device=dev)
             self._flat_b = torch.zeros(plan.PER * plan.Ph, dtype=torch.float32, device=dev)
-            self._graphs = {}  # (tanfovx, tanfovy) -> (settings, settings_h, forward graph, backward graph)
+            # (tanfovx, tanfovy, scale_modifier, densify buffers, sh_degree) -> (settings, settings_h, forward graph,
+            # backward graph)
+            self._graphs = {}
             self._cur = None
 
     # ---- use_graph=True ----
@@ -142,43 +157,52 @@ class TrainingFrameRenderer(nn.Module):
         c[38:41].copy_(settings_h.bg.reshape(3))
         pa, pb = plan.passes["A"], plan.passes["B"]
         for k in _KEYS:
-            pa.cat[k][: plan.Ps].copy_(scene[k].reshape(plan.Ps, -1))
+            if k in scene:  # an SH scene has no `rgb`: its coefficients go to the plan's resident buffer below
+                pa.cat[k][: plan.Ps].copy_(scene[k].reshape(plan.Ps, -1))
             pa.cat[k][plan.Ps:].copy_(human[k].reshape(plan.Ph, -1))
             pb.cat[k][plan.Ps:].copy_(refined[k].reshape(plan.Ph, -1))
+        if plan.M > 0:  # the captured kernels read the coefficients at a fixed address
+            plan.use_scene_shs(scene["shs"], scene["sh_degree"], copy=True)
 
     def _graph_forward(self, settings, settings_h, scene, human, refined):
         plan = self.plan
         self._load_inputs(settings, settings_h, scene, human, refined)
         dn = self.densify or {}
+        # the SH degree is a kernel argument frozen in the graphs: ExAvatar raises it on a schedule (module.py:152-153),
+        # so each degree is captured once and replayed afterwards
         key = (float(settings.tanfovx), float(settings.tanfovy), float(settings.scale_modifier),
-               tuple(0 if dn.get(k) is None else dn[k].data_ptr() for k in ("grad_accum", "count", "radius_max")))
+               tuple(0 if dn.get(k) is None else dn[k].data_ptr() for k in ("grad_accum", "count", "radius_max")),
+               plan.sh_degree if plan.M > 0 else None)
         if key not in self._graphs:
             st, st_h = self._resident_settings(settings, settings_h)
             pa, pb = plan.passes["A"], plan.passes["B"]
-            _, va = _views_of(self._flat_a, plan.P)
+            va = merged_pass_a_views(self._flat_a, plan.Ps, plan.Ph, plan.M)
             _, vb = _views_of(self._flat_b, plan.Ph)
+            scene_keys = [k for k in _KEYS if k != "rgb" or plan.M == 0]
 
             def fwd():
-                for k in _KEYS:  # the scene rows of pass B come from pass A's copy
+                for k in scene_keys:  # the scene rows of pass B come from pass A's copy
                     pb.cat[k][: plan.Ps].copy_(pa.cat[k][: plan.Ps])
                 plan.forward_frame(("graph", key), st, st_h, None, None, None, copy_inputs=False)
 
-            def bwd():
-                plan.backward_frame(self._gin, va, vb, g_depths=self._gin_d, g_alphas=self._gin_a, densify=self.densify)
+            def bwd(densify):
+                plan.backward_frame(self._gin, va, vb, g_depths=self._gin_d, g_alphas=self._gin_a, densify=densify)
 
             cur = torch.cuda.current_stream(plan.device)
             side = torch.cuda.Stream(plan.device)
             side.wait_stream(cur)
             with torch.cuda.stream(side):  # warm-up (also primes the ctx counters), then capture
                 fwd()
-                bwd()
+                # no densification bookkeeping in the warm-up: it would count a frame that is not one (with the
+                # previous frame's dL/dimage still in the resident inputs) every time a new key is captured
+                bwd(None)
             cur.wait_stream(side)
             torch.cuda.synchronize(plan.device)
             gf, gb = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
             with torch.cuda.graph(gf):
                 fwd()
             with torch.cuda.graph(gb, pool=gf.pool()):
-                bwd()
+                bwd(self.densify)
             self._graphs[key] = (st, st_h, gf, gb)
         self._cur = self._graphs[key]
         self._cur[2].replay()
@@ -203,9 +227,15 @@ class TrainingFrameRenderer(nn.Module):
 
     def forward(self, scene_asset, human_asset, human_asset_refined, cam_param, bg_human, bg=None, raster_settings=None,
                 raster_settings_human=None):
-        """Asset dicts as `GaussianRenderer.forward` takes them (mean_3d, opacity, scale, rotation, rgb); `bg_human` is the
+        """Asset dicts as `GaussianRenderer.forward` takes them (mean_3d, opacity, scale, rotation, rgb; the scene asset
+        carries shs + sh_degree instead of rgb when the renderer was built with sh_coeffs > 0); `bg_human` is the
         background of the two human-only renders (model.py:72), `bg` of the others (white by default, module.py:592).
         Returns {render name: {img, depthmap, mask, radius, is_vis[, mean_2d]}} for the five renders of plan.RENDERS."""
+        sh_scene = "shs" in scene_asset and "rgb" not in scene_asset
+        if sh_scene != (self.plan.M > 0):
+            raise ValueError("TrainingFrameRenderer: " + (
+                "the scene asset carries `shs`: build the renderer with sh_coeffs=M" if sh_scene else
+                f"built with sh_coeffs={self.plan.M}: the scene asset must carry `shs` + `sh_degree` instead of `rgb`"))
         dev = scene_asset["mean_3d"].device
         if bg is None:
             bg = torch.ones(3, dtype=torch.float32, device=dev)
@@ -213,8 +243,9 @@ class TrainingFrameRenderer(nn.Module):
         st_h = raster_settings_human or st._replace(bg=bg_human)
         Ps = scene_asset["mean_3d"].shape[0]
         mean_2d = torch.zeros((Ps, 3), dtype=torch.float32, device=dev, requires_grad=True)  # module.py:626-629
-        flat = [a[k] for a in (scene_asset, human_asset, human_asset_refined) for k in _KEYS]
-        res = _FrameFn.apply(self, st, st_h, mean_2d, *flat)
+        flat = [scene_asset[k] for k in self._scene_keys] + [a[k] for a in (human_asset, human_asset_refined) for k in _KEYS]
+        sh_degree = int(scene_asset["sh_degree"]) if sh_scene else 0
+        res = _FrameFn.apply(self, st, st_h, sh_degree, mean_2d, *flat)
         radii_a, radii_b = res[15], res[16]
         radius = {"scene": radii_a[:Ps], "human": radii_a[Ps:], "scene_human": radii_a, "human_refined": radii_b[Ps:],
                   "scene_human_refined": radii_b}

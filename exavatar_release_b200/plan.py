@@ -341,6 +341,35 @@ class _Pass:
                 "consumed_bwd": int(s.consumed_bwd)}
 
 
+def merged_bucket_layout(P_scene: int, P_human: int, sh_coeffs: int = 0) -> Dict[str, tuple]:
+    """(offset, numel) of every region of `MergedFivePlan`'s flat gradient buffer, in floats:
+
+        A      pass A, `_views_of` layout with P_scene + P_human rows (means3D | means2D | opacities | scales | rotations
+               | colors); with an SH scene the colour rows of the scene are written as zeros
+        A_shs  (P_scene, M, 3) dL/dSH of the scene Gaussians (sh_coeffs = M > 0 only; numel 0 otherwise)
+        B      pass B, `_views_of` layout with P_human rows (the refined human set)
+        stats  per-step densification sums of the scene Gaussians (grad_accum | count), the tail of the buffer
+        total  the whole buffer
+
+    sh_coeffs = 0 is the layout of a plan without SH: A | B | stats."""
+    PER = FiveRenderPlan.PER
+    Ps, Ph, M = int(P_scene), int(P_human), int(sh_coeffs)
+    nA, nS, nB = PER * (Ps + Ph), 3 * M * Ps, PER * Ph
+    return {"A": (0, nA), "A_shs": (nA, nS), "B": (nA + nS, nB), "stats": (nA + nS + nB, 2 * Ps),
+            "total": (0, nA + nS + nB + 2 * Ps)}
+
+
+def merged_pass_a_views(flat: torch.Tensor, P_scene: int, P_human: int, sh_coeffs: int = 0) -> Dict[str, torch.Tensor]:
+    """Named views of a pass-A gradient buffer laid out as the A | A_shs regions of `merged_bucket_layout`:
+    `_views_of` views with P_scene + P_human rows, plus "shs" (P_scene, M, 3) when sh_coeffs > 0."""
+    lay = merged_bucket_layout(P_scene, P_human, sh_coeffs)
+    (oa, na), (os_, ns) = lay["A"], lay["A_shs"]
+    _, views = _views_of(flat[oa:oa + na], int(P_scene) + int(P_human))
+    if sh_coeffs > 0:
+        views["shs"] = flat[os_:os_ + ns].view(int(P_scene), int(sh_coeffs), 3)
+    return views
+
+
 class MergedFivePlan:
     """ExAvatar's five renders per training frame (avatar/main/model.py:81-162) from TWO projection + binning passes
     instead of five (SURVEY.md section 8f-3, kernel half):
@@ -355,25 +384,37 @@ class MergedFivePlan:
     combined view skips the detached scene prefix, `first_row`), and the backward projection runs once per pass: scene
     rows carry the scene render's gradient, human rows the sum of the human-only and the combined render's -- what
     `loss.backward()` leaves in the leaves of model.py:117-125.  Same results as five separate renders (tests/), 2/5 of
-    the projection / scatter / sort work.  Interface of FiveRenderPlan."""
+    the projection / scatter / sort work.  Interface of FiveRenderPlan.
+
+    sh_coeffs = M > 0: the scene Gaussians are coloured from (P_scene, M, 3) SH coefficients inside the projection
+    kernels (SURVEY.md section 8f-4) and the human sets from RGB -- both passes are mixed-source scenes
+    (B2RScene.sh_rows = P_scene) reading ONE coefficient buffer (`use_scene_shs`).  The scene assets then carry `shs` +
+    `sh_degree` instead of `rgb`, and `grads("scene")` holds `shs` instead of `colors`."""
     PER = FiveRenderPlan.PER
     VIEWS = {"A": ("scene", "human", "scene_human"), "B": ("human_refined", "scene_human_refined")}
     SKIP = os.environ.get("B2R_SKIP_TILES", "1") != "0"  # A/B switch of the skipped human-free tiles
 
-    def __init__(self, P_scene: int, P_human: int, width: int, height: int, caps: Optional[Dict[str, int]], device):
+    def __init__(self, P_scene: int, P_human: int, width: int, height: int, caps: Optional[Dict[str, int]], device,
+                 sh_coeffs: int = 0):
         self.lib = L.load()
         self.Ps, self.Ph, self.P = int(P_scene), int(P_human), int(P_scene) + int(P_human)
         self.W, self.H = int(width), int(height)
+        self.M = int(sh_coeffs)
         self.device = torch.device(device)
         caps = caps or {"A": 8_000_000, "B": 8_000_000}
         self.passes = {k: _Pass(self.lib, self.P, self.W, self.H, caps[k], len(v), self.device) for k, v in self.VIEWS.items()}
         self.pass_streams = {k: torch.cuda.Stream(self.device) for k in self.passes}
-        # one flat gradient buffer: [pass A: scene rows | human rows][pass B: refined rows]
-        nA, nB = self.PER * self.P, self.PER * self.Ph
-        self.all_flat = torch.zeros(nA + nB + 2 * self.Ps, dtype=torch.float32, device=device)
-        self._stats = self.all_flat[nA + nB:]  # per-step densification sums ride in the all-reduced buffer (stats())
-        _, self.views_A = _views_of(self.all_flat[:nA], self.P)
-        _, self.views_B = _views_of(self.all_flat[nA:], self.Ph)
+        # one flat gradient buffer: [pass A: scene rows | human rows][scene dL/dSH][pass B: refined rows][stats]
+        lay = merged_bucket_layout(self.Ps, self.Ph, self.M)
+        self.all_flat = torch.zeros(lay["total"][1], dtype=torch.float32, device=device)
+        o, n = lay["stats"]
+        self._stats = self.all_flat[o:o + n]  # per-step densification sums ride in the all-reduced buffer (stats())
+        self.views_A = merged_pass_a_views(self.all_flat, self.Ps, self.Ph, self.M)
+        o, n = lay["B"]
+        _, self.views_B = _views_of(self.all_flat[o:o + n], self.Ph)
+        # the scene's SH coefficients: the caller's tensor (eager) or this resident copy (`use_scene_shs`)
+        self.shs = torch.zeros(self.Ps, self.M, 3, dtype=torch.float32, device=device) if self.M > 0 else None
+        self._shs_src, self.sh_degree = self.shs, 0
         Ps, P = self.Ps, self.P
         self.ranges = {"scene": (0, Ps), "human": (Ps, P), "scene_human": (0, P), "human_refined": (Ps, P),
                        "scene_human_refined": (0, P)}
@@ -388,21 +429,60 @@ class MergedFivePlan:
     def set_scene(self, scene_assets: Dict[str, torch.Tensor]) -> None:
         for ps in self.passes.values():
             for k, buf in ps.cat.items():
+                if k == "rgb" and self.M > 0:
+                    continue  # SH scene: the colour rows of the scene are never read
                 buf[: self.Ps].copy_(scene_assets[k].reshape(self.Ps, -1))
+        if self.M > 0:
+            self.use_scene_shs(scene_assets["shs"], scene_assets["sh_degree"])
+
+    def use_scene_shs(self, shs: torch.Tensor, sh_degree: int, copy: bool = False) -> None:
+        """The scene's (P_scene, M, 3) SH coefficients and active degree for the next frames.  Both passes read ONE
+        buffer: the caller's tensor itself when it is contiguous fp32 on the plan's device (it must then stay unchanged
+        until the backward), otherwise -- or with copy=True, for a captured graph that reads fixed addresses -- the plan's
+        resident copy `self.shs`."""
+        if self.M == 0:
+            raise ValueError("MergedFivePlan: built without SH (sh_coeffs=0); pass the scene colours as `rgb`")
+        t = shs.detach()
+        if tuple(t.shape) != (self.Ps, self.M, 3):
+            raise ValueError(f"MergedFivePlan: scene `shs` must be ({self.Ps}, {self.M}, 3), got {tuple(t.shape)}")
+        if copy or t.dtype != torch.float32 or not t.is_contiguous() or t.device != self.device:
+            self.shs.copy_(t)
+            t = self.shs
+        self._shs_src, self.sh_degree = t, int(sh_degree)
 
     def _scene_desc(self, key, ps, settings):
         """B2RScene of a pass for one camera; cached under `key` (the settings' tensors are then kept alive), or built
         afresh when key[0] is None (a caller with a new camera every frame)."""
-        if key[0] is None:
-            sc, keep = _make_scene(settings, ps.cat["mean_3d"], None, ps.cat["rgb"], ps.cat["opacity"], ps.cat["scale"],
+        def make():
+            shs = self._shs_src if self.M > 0 else None
+            sc, keep = _make_scene(settings, ps.cat["mean_3d"], shs, ps.cat["rgb"], ps.cat["opacity"], ps.cat["scale"],
                                    ps.cat["rotation"], None, 0)
+            if shs is not None:  # scene rows from SH, human rows from RGB
+                sc.sh_rows, sc.sh_degree = self.Ps, self.sh_degree
+            return sc, keep
+
+        if key[0] is None:
+            sc, keep = make()
             ps.last_scene = (sc, keep)  # alive until the pass is used again
             return sc
+        if self.M > 0:  # the descriptor holds the coefficient pointer and the degree
+            key = (key, self._shs_src.data_ptr(), self.sh_degree)
         if key not in self._scenes:
-            sc, keep = _make_scene(settings, ps.cat["mean_3d"], None, ps.cat["rgb"], ps.cat["opacity"], ps.cat["scale"],
-                                   ps.cat["rotation"], None, 0)
-            self._scenes[key] = (sc, keep)
+            self._scenes[key] = make()
         return self._scenes[key][0]
+
+    def _project_args(self, pk, g, accumulate, densify):
+        """B2RBackwardArgs of the backward projection of pass `pk` into the gradient views `g`."""
+        a = L.B2RBackwardArgs(None, None, None, _ptr(g["means3D"]), _ptr(g["means2D"]),
+                              _ptr(g.get("shs")) if pk == "A" else None, _ptr(g["colors"]),
+                              _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), None)
+        a.flags = (L.B2R_BWD_ACCUMULATE if accumulate else 0) | L.B2R_BWD_SCRATCH_ZEROED
+        a.first_row = 0 if pk == "A" else self.Ps  # pass B: the scene prefix (SH rows included) is detached
+        if pk == "A" and densify is not None:
+            a.densify_grad_accum, a.densify_count = _ptr(densify.get("grad_accum")), _ptr(densify.get("count"))
+            a.densify_radius_max = _ptr(densify.get("radius_max"))
+            a.densify_rows = self.Ps
+        return a
 
     def _view(self, ps, v, name, bg):
         lo, hi = self.ranges[name]
@@ -473,17 +553,10 @@ class MergedFivePlan:
                     for v in range(len(names)):
                         st.wait_stream(ps.streams[v])
                 # one backward projection per pass
-                g = self.views_A if pk == "A" else self.views_B
-                a = L.B2RBackwardArgs(None, None, None, _ptr(g["means3D"]), _ptr(g["means2D"]), None, _ptr(g["colors"]),
-                                      _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), None)
-                a.flags = (L.B2R_BWD_ACCUMULATE if accumulate else 0) | L.B2R_BWD_SCRATCH_ZEROED
-                a.first_row = 0 if pk == "A" else self.Ps
-                if pk == "A" and densify is not None:
-                    a.densify_grad_accum, a.densify_count = _ptr(densify.get("grad_accum")), _ptr(densify.get("count"))
-                    a.densify_radius_max = _ptr(densify.get("radius_max"))
-                    a.densify_rows = self.Ps
+                a = self._project_args(pk, self.views_A if pk == "A" else self.views_B, accumulate, densify)
                 L.check(lib.b2r_backward_project(C.byref(sc), C.byref(ps.ws), C.byref(a), ps.bwd_scratch.data_ptr(),
                                                  ps.bwd_bytes, sp), "b2r_backward_project")
+                probe(f"{pk}:project_bwd")
         if not serial:
             for pk in self.passes:
                 cur.wait_stream(self.pass_streams[pk])
@@ -574,15 +647,7 @@ class MergedFivePlan:
                         self._keep.append((gc, gd, ga))
                 for v in range(len(names)):
                     st.wait_stream(ps.streams[v])
-                g = grads_A if pk == "A" else grads_B
-                a = L.B2RBackwardArgs(None, None, None, _ptr(g["means3D"]), _ptr(g["means2D"]), None, _ptr(g["colors"]),
-                                      _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), None)
-                a.flags = (L.B2R_BWD_ACCUMULATE if accumulate else 0) | L.B2R_BWD_SCRATCH_ZEROED
-                a.first_row = 0 if pk == "A" else self.Ps
-                if pk == "A" and densify is not None:
-                    a.densify_grad_accum, a.densify_count = _ptr(densify.get("grad_accum")), _ptr(densify.get("count"))
-                    a.densify_radius_max = _ptr(densify.get("radius_max"))
-                    a.densify_rows = self.Ps
+                a = self._project_args(pk, grads_A if pk == "A" else grads_B, accumulate, densify)
                 L.check(lib.b2r_backward_project(C.byref(sc), C.byref(ps.ws), C.byref(a), ps.bwd_scratch.data_ptr(),
                                                  ps.bwd_bytes, st.cuda_stream), "b2r_backward_project")
         for pk in self.passes:
@@ -602,10 +667,15 @@ class MergedFivePlan:
         return self.grads("scene"), self.grads("human"), self.grads("human_refined")
 
     def grads(self, which: str) -> Dict[str, torch.Tensor]:
+        """Named gradient tensors of one parameter set; an SH scene has `shs` (P_scene, M, 3) instead of `colors`."""
         if which == "scene":
-            return {k: v[: self.Ps] for k, v in self.views_A.items()}
+            out = {k: v[: self.Ps] for k, v in self.views_A.items() if k != "shs"}
+            if self.M > 0:
+                del out["colors"]
+                out["shs"] = self.views_A["shs"]
+            return out
         if which == "human":
-            return {k: v[self.Ps:] for k, v in self.views_A.items()}
+            return {k: v[self.Ps:] for k, v in self.views_A.items() if k != "shs"}
         return dict(self.views_B)
 
     def flat_bucket(self) -> torch.Tensor:

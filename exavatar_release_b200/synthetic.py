@@ -125,3 +125,17 @@ def make_population_assets(workload, seed=0, device="cpu", focal_ratio=1.465):
     refined["rgb"] = (human["rgb"] + 0.05 * torch.randn(wl.n_avatar, 3, generator=g)).clamp(0, 1)
     to = lambda d: {k: v.to(device) for k, v in d.items()}
     return to(scene), to(human), to(refined)
+
+
+def make_scene_sh_params(scene, sh_degree=3, seed=0):
+    """Pre-activation parameters of the scene population as `SceneGaussian` stores them (module.py:103-108): mean,
+    opacity logit, log scale, rotation, `feature_dc` (P,1,3) = RGB2SH(rgb) and `feature_rest` (P,(d+1)^2-1,3) seeded
+    N(0, 0.3^2) -- the inputs of `renderer.scene_gaussian_assets` for a degree-`sh_degree` SH scene."""
+    g = torch.Generator().manual_seed(7000 + seed)
+    n = scene["mean_3d"].shape[0]
+    m = (sh_degree + 1) ** 2
+    rest = 0.3 * torch.randn(n, m - 1, 3, generator=g)
+    return {"mean": scene["mean_3d"], "opacity_logit": torch.logit(scene["opacity"].clamp(1e-4, 1 - 1e-4)),
+            "log_scale": torch.log(scene["scale"]), "rotation": scene["rotation"],
+            "feature_dc": ((scene["rgb"] - 0.5) / SH_C0).reshape(n, 1, 3).contiguous(),  # RGB2SH, transforms.py:169-170
+            "feature_rest": rest.to(scene["mean_3d"].device)}

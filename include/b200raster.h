@@ -36,7 +36,7 @@ extern "C" {
 #define B2R_ABI_VERSION 3
 
 #define B2R_OK 0
-#define B2R_E_INVALID (-1)      /* bad argument (null pointer, negative size, both / neither colour source ...) */
+#define B2R_E_INVALID (-1)      /* bad argument (null pointer, negative size, both / neither colour source, sh_rows > P ...) */
 #define B2R_E_WORKSPACE (-2)    /* ctx / scratch buffer smaller than b2r_*_bytes() reports */
 #define B2R_E_CUDA (-3)         /* a CUDA launch failed; b2r_last_cuda_error() has the cudaError_t */
 #define B2R_E_DUP_OVERFLOW (-4) /* only ever reported through B2RStatus.overflow (device side) */
@@ -53,7 +53,7 @@ extern "C" {
 typedef struct B2RScene {
   int32_t P;              /* number of Gaussians */
   int32_t width, height;  /* image_width, image_height */
-  int32_t sh_degree;      /* active SH degree (0..3); ignored when colors_precomp != NULL */
+  int32_t sh_degree;      /* active SH degree (0..3); ignored when only colors_precomp is set */
   int32_t sh_coeffs;      /* M: coefficients per Gaussian in `shs` (0 when shs == NULL) */
   uint32_t flags;         /* B2R_FLAG_* */
   float scale_modifier;
@@ -63,8 +63,8 @@ typedef struct B2RScene {
   const float* projmatrix;    /* (16) full projection (proj*view), [4c+r] */
   const float* campos;        /* (3) */
   const float* means3D;       /* (P,3) */
-  const float* shs;           /* (P,M,3) or NULL */
-  const float* colors_precomp;/* (P,3) or NULL  (exactly one of shs / colors_precomp) */
+  const float* shs;           /* (P,M,3) or NULL; (sh_rows,M,3) when sh_rows > 0 */
+  const float* colors_precomp;/* (P,3) or NULL  (exactly one of shs / colors_precomp, unless sh_rows > 0) */
   const float* opacities;     /* (P) */
   const float* scales;        /* (P,3) or NULL */
   const float* rotations;     /* (P,4) (r,x,y,z), used un-normalised, or NULL */
@@ -84,7 +84,13 @@ typedef struct B2RScene {
   const float* skin_cam_t;      /* (3) camera translation (used with skin_cam_Rinv) */
   float* skin_means_out;        /* (P,3) optional OUTPUT: the posed world positions (other ExAvatar modules read them) */
   int32_t skin_J;               /* joints (55 for SMPL-X); <= 64 */
-  int32_t skin_reserved;
+  /* Mixed colour source.  0: exactly one of shs / colors_precomp colours every Gaussian.  0 < sh_rows <= P: BOTH are
+   * required; Gaussians [0, sh_rows) are coloured from `shs`, which then holds sh_rows rows of sh_coeffs coefficients
+   * (sh_degree / sh_coeffs rules as above), and Gaussians [sh_rows, P) read colors_precomp[i] -- the global index, so
+   * colors_precomp keeps P rows and its first sh_rows are never read.  This is ExAvatar's cat(scene, human) with the
+   * scene coloured from SH and the human from RGB (avatar/main/model.py:117-125).  Backward: dL_dshs has
+   * sh_rows - first_row rows (none, and it may be NULL, when first_row >= sh_rows); dL_dcolors is zero on SH rows. */
+  int32_t sh_rows;
 } B2RScene;
 
 /* Device-side status block; lives at offset 0 of the ctx buffer (read it back with a 64-byte D2H copy). */
@@ -154,8 +160,8 @@ typedef struct B2RBackwardArgs {
   /* outputs; every element is written (zeros for culled Gaussians).  Any may be NULL. */
   float* dL_dmeans3D;   /* (P,3) */
   float* dL_dmeans2D;   /* (P,3) NDC-scaled screen gradient, z = 0 (module.py:626-629 reads its .grad) */
-  float* dL_dshs;       /* (P,M,3) */
-  float* dL_dcolors;    /* (P,3) */
+  float* dL_dshs;       /* (P,M,3); (sh_rows - first_row, M, 3) in a mixed scene (B2RScene.sh_rows) */
+  float* dL_dcolors;    /* (P,3); zero on the SH rows of a mixed scene */
   float* dL_dopacities; /* (P) */
   float* dL_dscales;    /* (P,3) */
   float* dL_drotations; /* (P,4) */
