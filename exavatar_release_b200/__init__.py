@@ -8,6 +8,7 @@ frame-sharding helper used by bench.py.
 """
 from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians  # noqa: F401
 from .renderer import GaussianRenderer, render_settings  # noqa: F401
+from .skinning import skin_gaussians  # noqa: F401
 
 
 def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loaded on first use
@@ -18,4 +19,4 @@ def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loa
 
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "GaussianRenderer",
-           "render_settings", "TrainingFrameRenderer"]
+           "render_settings", "TrainingFrameRenderer", "skin_gaussians"]

@@ -59,6 +59,15 @@ class B2RView(C.Structure):
     ]
 
 
+class B2RSkin(C.Structure):
+    """Standalone skinning of one or two Gaussian sets sharing a rig (b2r_skin_forward / b2r_skin_backward)."""
+    _fields_ = [
+        ("P", C.c_int32), ("J", C.c_int32), ("V", C.c_int32), ("reserved", C.c_int32),
+        ("weights", _fp), ("rows", _fp), ("joint_mats", _fp), ("trans", _fp), ("cam_Rinv", _fp), ("cam_t", _fp),
+        ("xyz", _fp * 2), ("posed", _fp * 2),
+    ]
+
+
 class B2RForwardOutputs(C.Structure):
     _fields_ = [("color", _fp), ("depth", _fp), ("alpha", _fp), ("radii", _fp)]
 
@@ -107,6 +116,9 @@ SYMBOLS = [
     ("b2r_backward", C.c_int, [C.POINTER(B2RScene), C.POINTER(B2RWorkspace), C.POINTER(B2RBackwardArgs), _fp,
                                C.c_size_t, _fp]),
     ("b2r_mark_visible", C.c_int, [C.c_int32, _fp, _fp, _fp, _fp]),
+    ("b2r_skin_forward", C.c_int, [C.POINTER(B2RSkin), _fp]),
+    ("b2r_skin_backward", C.c_int, [C.POINTER(B2RSkin), C.POINTER(_fp), C.POINTER(_fp), _fp, _fp, _fp, C.c_size_t, _fp]),
+    ("b2r_skin_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32]),
     ("b2r_profile_enable", None, [C.c_int]),
     ("b2r_profile_read", C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int]),
     ("b2r_launch_count", C.c_uint64, []),
@@ -137,7 +149,7 @@ def load():
         fn.argtypes = argtypes
     if lib.b2r_abi_version() != ABI_VERSION:
         raise RuntimeError("b200raster: ABI version mismatch between the Python binding and libb200raster.so")
-    for idx, cls in enumerate((B2RScene, B2RStatus, B2RWorkspace, B2RForwardOutputs, B2RBackwardArgs, B2RView)):
+    for idx, cls in enumerate((B2RScene, B2RStatus, B2RWorkspace, B2RForwardOutputs, B2RBackwardArgs, B2RView, B2RSkin)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

@@ -30,7 +30,9 @@ NVCC_FLAGS = [
 # binning.cu: its scatter repeats the projection's tile region test for rects of more than 32 tiles (smaller ones replay
 # a stored mask); the two must agree on every (splat, tile) pair or a list slot stays unfilled, so the unit is compiled
 # with the same contraction setting (its kernels are integer sorts otherwise).
-PER_FILE_FLAGS = {"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"]}
+# skin.cu: the standalone skinning op evaluates the blend of project.cu's fused skinning (gaussian_math.cuh skin_apply);
+# compiled with the same contraction setting, both paths write bit-identical posed positions.
+PER_FILE_FLAGS = {"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"]}
 
 
 def sources():

@@ -59,6 +59,20 @@ bool missing_dshs(const B2RScene* sc, const B2RBackwardArgs* a) {
   return sc->sh_rows == 0 || (int64_t)a->first_row < (int64_t)sc->sh_rows;
 }
 
+// the rules of the fused skinning in validate_scene, for the standalone op
+int validate_skin(const B2RSkin* s) {
+  if (!s) return B2R_E_INVALID;
+  if (s->P < 0 || s->V <= 0) return B2R_E_INVALID;
+  if (s->J <= 0 || s->J > 64) return B2R_E_INVALID;
+  if (s->cam_Rinv && !s->cam_t) return B2R_E_INVALID;
+  if (s->posed[1] && !s->xyz[1]) return B2R_E_INVALID;
+  if (s->P > 0) {
+    if (!s->weights || !s->joint_mats || !s->trans || !s->xyz[0]) return B2R_E_INVALID;
+    if (!s->rows && s->V < s->P) return B2R_E_INVALID;  // row i of the table for Gaussian i
+  }
+  return B2R_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -86,6 +100,7 @@ size_t b2r_sizeof(int which) {
     case 3: return sizeof(B2RForwardOutputs);
     case 4: return sizeof(B2RBackwardArgs);
     case 5: return sizeof(B2RView);
+    case 6: return sizeof(B2RSkin);
     default: return 0;
   }
 }
@@ -225,6 +240,27 @@ int b2r_backward_project(const B2RScene* scene, const B2RWorkspace* ws, const B2
   if (args->dL_dposed && !scene->skin_xyz) return B2R_E_INVALID;
   const Ctx cx = resolve(ws, scene->P, scene->width, scene->height);
   return launch_project_bwd(*scene, cx, *args, (const float*)bwd_scratch, (cudaStream_t)stream);
+}
+
+size_t b2r_skin_scratch_bytes(int32_t P, int32_t J) { return skin_scratch_bytes(P, J); }
+
+int b2r_skin_forward(const B2RSkin* skin, void* stream) {
+  const int rc = validate_skin(skin);
+  if (rc) return rc;
+  if (skin->P > 0 && !skin->posed[0]) return B2R_E_INVALID;
+  return launch_skin_forward(*skin, (cudaStream_t)stream);
+}
+
+int b2r_skin_backward(const B2RSkin* skin, const float* const dL_dposed[2], float* const dL_dxyz[2], float* dL_djoint,
+                      float* dL_dtrans, void* scratch, size_t scratch_bytes, void* stream) {
+  const int rc = validate_skin(skin);
+  if (rc) return rc;
+  if (dL_dposed && dL_dposed[1] && !skin->xyz[1]) return B2R_E_INVALID;
+  if ((dL_djoint || dL_dtrans) && skin->P > 0) {
+    if (!scratch) return B2R_E_INVALID;
+    if (scratch_bytes < skin_scratch_bytes(skin->P, skin->J)) return B2R_E_WORKSPACE;
+  }
+  return launch_skin_backward(*skin, dL_dposed, dL_dxyz, dL_djoint, dL_dtrans, scratch, (cudaStream_t)stream);
 }
 
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {

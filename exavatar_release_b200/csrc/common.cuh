@@ -491,6 +491,10 @@ int launch_composite_bwd(const B2RScene& sc, const Ctx& cx, const B2RBackwardArg
 
 int launch_project_bwd(const B2RScene& sc, const Ctx& cx, const B2RBackwardArgs& a, const float* gacc, cudaStream_t st);
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t st);
+int launch_skin_forward(const B2RSkin& s, cudaStream_t st);
+int launch_skin_backward(const B2RSkin& s, const float* const dposed[2], float* const dxyz[2], float* djoint,
+                         float* dtrans, void* scratch, cudaStream_t st);
+size_t skin_scratch_bytes(int P, int J);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

@@ -235,14 +235,7 @@ __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& c
     float gc[3] = {dm[0], dm[1], dm[2]}, dx[3] = {0.f, 0.f, 0.f}, G[12];
     float xs[4] = {0.f, 0.f, 0.f, 0.f};
     if (visible || posed_in) {
-      if (sc.skin_cam_Rinv) {  // g_cam = Rinv^T g_world
-        const float* R = sc.skin_cam_Rinv;
-        gc[0] = __ldg(R) * dm[0] + __ldg(R + 3) * dm[1] + __ldg(R + 6) * dm[2];
-        gc[1] = __ldg(R + 1) * dm[0] + __ldg(R + 4) * dm[1] + __ldg(R + 7) * dm[2];
-        gc[2] = __ldg(R + 2) * dm[0] + __ldg(R + 5) * dm[1] + __ldg(R + 8) * dm[2];
-      }
-#pragma unroll
-      for (int c = 0; c < 3; c++) dx[c] = skin.M[c] * gc[0] + skin.M[4 + c] * gc[1] + skin.M[8 + c] * gc[2];
+      skin_transpose(skin.M, sc.skin_cam_Rinv, dm, gc, dx);  // g_cam = Rinv^T g_world, dx = M3^T g_cam
       xs[0] = skin.x.x; xs[1] = skin.x.y; xs[2] = skin.x.z; xs[3] = 1.f;
     }
 #pragma unroll

@@ -194,6 +194,28 @@ typedef struct B2RBackwardArgs {
   uint32_t densify_rows;
   uint32_t reserved;
 } B2RBackwardArgs;
+/* Standalone linear-blend skinning of one or two Gaussian sets that share a rig (SURVEY section 8f-2).  ExAvatar poses
+ * `mean_3d` and `mean_3d_refined` of its human Gaussians with the same weight rows, joint transforms, translation and
+ * camera (avatar/common/nets/module.py:549-557):  M_i = sum_j W[rows[i], j] A_j,  posed_s,i = M_i [xyz_s,i, 1] + trans,
+ * then Rinv (posed - t) with a camera.  b2r_skin_forward blends M_i once per Gaussian and writes both posed sets, which
+ * the caller's normal / colour networks and the renders then read -- unlike B2RScene.skin_*, which poses inside one
+ * render's projection.  Same device code as that fused path: the posed positions agree bit for bit. */
+typedef struct B2RSkin {
+  int32_t P;                /* Gaussians per set */
+  int32_t J;                /* joints (55 for SMPL-X); 1..64 */
+  int32_t V;                /* rows of the weight table */
+  int32_t reserved;
+  const float* weights;     /* (V,J) skinning weight table */
+  const int32_t* rows;      /* (P) row of `weights` for each Gaussian (nn_vertex_idxs, module.py:414; every value in
+                               [0, V)), or NULL: row i (then V >= P) */
+  const float* joint_mats;  /* (J,16) row-major 4x4 transform per joint; rows 0..2 are read */
+  const float* trans;       /* (3) root translation added after blending */
+  const float* cam_Rinv;    /* (9) row-major inverse camera rotation, or NULL to stay in the posed frame */
+  const float* cam_t;       /* (3) camera translation (required with cam_Rinv) */
+  const float* xyz[2];      /* (P,3) canonical positions of set 0 / set 1 (set 1 may be NULL) */
+  float* posed[2];          /* (P,3) OUTPUT posed positions; posed[1] requires xyz[1] (NULL: set 1 is not posed) */
+} B2RSkin;
+
 #define B2R_BWD_ACCUMULATE 1u
 /* The caller guarantees `bwd_scratch` is all zero on entry; b2r_backward then skips its memset and leaves the scratch
  * all zero again on return (the backward projection kernel clears each row after consuming it).  For callers that
@@ -204,7 +226,7 @@ int b2r_abi_version(void);
 const char* b2r_strerror(int code);
 int b2r_last_cuda_error(void);
 /* sizeof() of the ABI structs, for bindings to verify their mirror: 0 B2RScene, 1 B2RStatus, 2 B2RWorkspace,
- * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView; 0 for anything else. */
+ * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin; 0 for anything else. */
 size_t b2r_sizeof(int which);
 
 size_t b2r_ctx_bytes(int32_t P, int32_t width, int32_t height);
@@ -243,11 +265,24 @@ int b2r_backward_composite(const B2RScene* scene, const B2RWorkspace* ws, const 
 int b2r_backward_project(const B2RScene* scene, const B2RWorkspace* ws, const B2RBackwardArgs* args, void* bwd_scratch,
                          size_t bwd_scratch_bytes, void* stream);
 
+/* Skinning (B2RSkin).  Forward: writes posed[0] and, when given, posed[1].  Backward: dL_dposed (host array of two
+ * device pointers; either may be NULL = no gradient reaches that set, dL_dposed[1] requires xyz[1]) ->
+ *   dL_dxyz[s]  (P,3) = M_i[:3,:3]^T g_cam,s,i  with  g_cam = Rinv^T dL/dposed  (zeros when dL_dposed[s] is NULL);
+ *   dL_djoint (J,3,4) = sum_i W[rows[i], j] sum_s g_cam,s,i [xyz_s,i, 1]^T   (row 3 of each 4x4 has no gradient);
+ *   dL_dtrans (3)     = sum_i sum_s g_cam,s,i.
+ * dL_dxyz (host array) and each output may be NULL.  The joint / translation sums are deterministic (block partials
+ * added in a fixed order, no float atomics): bit-identical from run to run.  `scratch` >= b2r_skin_scratch_bytes(P, J)
+ * when dL_djoint or dL_dtrans is given.  No gradient for the weights or the camera.  Neither call allocates or syncs. */
+int b2r_skin_forward(const B2RSkin* skin, void* stream);
+int b2r_skin_backward(const B2RSkin* skin, const float* const dL_dposed[2], float* const dL_dxyz[2], float* dL_djoint,
+                      float* dL_dtrans, void* scratch, size_t scratch_bytes, void* stream);
+size_t b2r_skin_scratch_bytes(int32_t P, int32_t J);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
