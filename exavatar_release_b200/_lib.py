@@ -93,6 +93,16 @@ B2R_BWD_ACCUMULATE = 1
 B2R_BWD_SCRATCH_ZEROED = 2
 
 
+def read_status(ctx_buf) -> dict:
+    """Decodes the B2RStatus block at the head of a ctx buffer (uint8 tensor).  Copies it to the host, which synchronises
+    with the device: for tests, bench accounting and debugging."""
+    s = B2RStatus.from_buffer_copy(ctx_buf[: C.sizeof(B2RStatus)].cpu().numpy().tobytes())
+    return {"num_dups": int(s.num_dups), "dup_capacity": int(s.dup_capacity), "overflow": int(s.overflow),
+            "num_visible": int(s.num_visible), "consumed_fwd": int(s.consumed_fwd), "consumed_bwd": int(s.consumed_bwd),
+            # the composites count staged list entries per CTA; these divisors turn the sums into entries per TILE
+            "consumed_fwd_div": float(CONSUMED_FWD_DIV), "consumed_bwd_div": float(CONSUMED_BWD_DIV)}
+
+
 # every symbol include/b200raster.h declares: (name, restype, argtypes)
 SYMBOLS = [
     ("b2r_abi_version", C.c_int, []),

@@ -22,16 +22,16 @@ from . import _lib as L
 from .rasterizer import _f32c, _make_scene, _ptr
 
 
-class FramePlan:
-    def __init__(self, P: int, width: int, height: int, dup_capacity: int, device, sh_coeffs: int = 0,
-                 segmented: bool = True):
+class _Workspace:
+    """The resident buffers of one projection + binning of P Gaussians with a fixed duplicate capacity, and the
+    B2RWorkspace pointing at them: ctx (status block first), duplicate ids, forward scratch, backward scratch and,
+    with `checkpoints`, the forward composite's segment table + blend-state checkpoints."""
+
+    def __init__(self, P: int, width: int, height: int, dup_capacity: int, device, checkpoints: bool = True):
         self.lib = L.load()
-        self.P, self.W, self.H, self.M = int(P), int(width), int(height), int(sh_coeffs)
-        self.device = torch.device(device)
+        self.P, self.W, self.H = int(P), int(width), int(height)
+        self.device = dev = torch.device(device)
         self.capacity = int(dup_capacity)
-        dev = self.device
-        f = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
-        self.color, self.depth, self.alpha = f(3, height, width), f(1, height, width), f(1, height, width)
         self.radii = torch.empty(P, dtype=torch.int32, device=dev)
         self.ctx_bytes = self.lib.b2r_ctx_bytes(P, width, height)
         self.ctx_buf = torch.empty(self.ctx_bytes, dtype=torch.uint8, device=dev)
@@ -41,14 +41,26 @@ class FramePlan:
         self.bwd_bytes = self.lib.b2r_backward_scratch_bytes(P)
         # zero once: every backward leaves it zero again (B2R_BWD_SCRATCH_ZEROED), so no memset node per render
         self.bwd_scratch = torch.zeros(self.bwd_bytes, dtype=torch.uint8, device=dev)
+        self.ckpt_bytes = self.lib.b2r_checkpoint_bytes(width, height, self.capacity) if checkpoints else 0
+        self.ckpt = torch.empty(max(self.ckpt_bytes, 1), dtype=torch.uint8, device=dev) if checkpoints else None
+        self.ws = L.B2RWorkspace(self.ctx_buf.data_ptr(), self.ctx_bytes, self.ids.data_ptr(), self.capacity,
+                                 self.scratch.data_ptr(), self.scratch_bytes, None, 0,
+                                 self.ckpt.data_ptr() if checkpoints else None, self.ckpt_bytes)
+
+    def status(self) -> dict:
+        return L.read_status(self.ctx_buf)
+
+
+class FramePlan(_Workspace):
+    def __init__(self, P: int, width: int, height: int, dup_capacity: int, device, sh_coeffs: int = 0,
+                 segmented: bool = True):
         # segment table + blend-state checkpoints of the forward composite (lets the backward replay 512-entry list
         # segments as independent work items); `segmented=False` reproduces the round-1 whole-list backward
         segmented = segmented and os.environ.get("B2R_SEGMENTED", "1") != "0"  # A/B switch for measurements
-        self.ckpt_bytes = self.lib.b2r_checkpoint_bytes(width, height, self.capacity) if segmented else 0
-        self.ckpt = torch.empty(max(self.ckpt_bytes, 1), dtype=torch.uint8, device=dev) if segmented else None
-        self.ws = L.B2RWorkspace(self.ctx_buf.data_ptr(), self.ctx_bytes, self.ids.data_ptr(), self.capacity,
-                                 self.scratch.data_ptr(), self.scratch_bytes, None, 0,
-                                 self.ckpt.data_ptr() if segmented else None, self.ckpt_bytes)
+        super().__init__(P, width, height, dup_capacity, device, checkpoints=segmented)
+        self.M = int(sh_coeffs)
+        f = lambda *s: torch.empty(s, dtype=torch.float32, device=self.device)
+        self.color, self.depth, self.alpha = f(3, height, width), f(1, height, width), f(1, height, width)
         self.out = L.B2RForwardOutputs(self.color.data_ptr(), self.depth.data_ptr(), self.alpha.data_ptr(),
                                        self.radii.data_ptr())
         self._scenes = {}
@@ -93,15 +105,6 @@ class FramePlan:
             st = torch.cuda.current_stream(self.device).cuda_stream
             L.check(self.lib.b2r_backward(C.byref(sc), C.byref(self.ws), C.byref(a), self.bwd_scratch.data_ptr(),
                                           self.bwd_bytes, st), "b2r_backward")
-
-    def status(self) -> dict:
-        raw = self.ctx_buf[: C.sizeof(L.B2RStatus)].cpu().numpy().tobytes()
-        s = L.B2RStatus.from_buffer_copy(raw)
-        return {"num_dups": int(s.num_dups), "dup_capacity": int(s.dup_capacity), "overflow": int(s.overflow),
-                "num_visible": int(s.num_visible), "consumed_fwd": int(s.consumed_fwd),
-                "consumed_bwd": int(s.consumed_bwd),
-                # the composites count staged list entries per CTA; these divisors turn the sums into entries per TILE
-                "consumed_fwd_div": float(L.CONSUMED_FWD_DIV), "consumed_bwd_div": float(L.CONSUMED_BWD_DIV)}
 
 
 def grad_bucket(P: int, device, sh_coeffs: int = 0):
@@ -308,24 +311,14 @@ class FiveRenderPlan:
         return any(p.status()["overflow"] for p in self.plans.values())
 
 
-class _Pass:
+class _Pass(_Workspace):
     """One projection + binning of cat(scene, X) and the views composited from it (MergedFivePlan)."""
 
-    def __init__(self, lib, P, W, H, cap, n_views, device):
-        dev = device
-        self.P, self.cap = P, int(cap)
-        self.ctx_bytes = lib.b2r_ctx_bytes(P, W, H)
-        self.ctx_buf = torch.empty(self.ctx_bytes, dtype=torch.uint8, device=dev)
-        self.ids = torch.empty(max(self.cap, 1), dtype=torch.int32, device=dev)
-        self.scratch_bytes = lib.b2r_scratch_bytes(P, W, H, self.cap)
-        self.scratch = torch.empty(self.scratch_bytes, dtype=torch.uint8, device=dev)
-        self.bwd_bytes = lib.b2r_backward_scratch_bytes(P)
-        self.bwd_scratch = torch.zeros(self.bwd_bytes, dtype=torch.uint8, device=dev)  # stays zero across renders
-        self.ck_bytes = lib.b2r_checkpoint_bytes(W, H, self.cap)
-        self.ck = [torch.empty(self.ck_bytes, dtype=torch.uint8, device=dev) for _ in range(n_views)]
-        self.radii = torch.empty(P, dtype=torch.int32, device=dev)
-        self.ws = L.B2RWorkspace(self.ctx_buf.data_ptr(), self.ctx_bytes, self.ids.data_ptr(), self.cap,
-                                 self.scratch.data_ptr(), self.scratch_bytes, None, 0, self.ck[0].data_ptr(), self.ck_bytes)
+    def __init__(self, P, W, H, cap, n_views, device):
+        super().__init__(P, W, H, cap, device)
+        dev = self.device
+        # every view keeps its own checkpoints for its backward; the workspace points at the first view's
+        self.ck = [self.ckpt] + [torch.empty_like(self.ckpt) for _ in range(n_views - 1)]
         f = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
         self.img = [(f(3, H, W), f(1, H, W), f(1, H, W)) for _ in range(n_views)]
         self.state = [(f(H * W), torch.empty(H * W, dtype=torch.int32, device=dev)) for _ in range(n_views)]
@@ -333,12 +326,6 @@ class _Pass:
         self.cat = {k: f(P, w) for k, w in widths.items()}
         self.streams = [torch.cuda.Stream(dev) for _ in range(n_views)]
         self.primed = False
-
-    def status(self) -> dict:
-        raw = self.ctx_buf[: C.sizeof(L.B2RStatus)].cpu().numpy().tobytes()
-        s = L.B2RStatus.from_buffer_copy(raw)
-        return {"num_dups": int(s.num_dups), "overflow": int(s.overflow), "consumed_fwd": int(s.consumed_fwd),
-                "consumed_bwd": int(s.consumed_bwd)}
 
 
 def merged_bucket_layout(P_scene: int, P_human: int, sh_coeffs: int = 0) -> Dict[str, tuple]:
@@ -402,7 +389,7 @@ class MergedFivePlan:
         self.M = int(sh_coeffs)
         self.device = torch.device(device)
         caps = caps or {"A": 8_000_000, "B": 8_000_000}
-        self.passes = {k: _Pass(self.lib, self.P, self.W, self.H, caps[k], len(v), self.device) for k, v in self.VIEWS.items()}
+        self.passes = {k: _Pass(self.P, self.W, self.H, caps[k], len(v), self.device) for k, v in self.VIEWS.items()}
         self.pass_streams = {k: torch.cuda.Stream(self.device) for k in self.passes}
         # one flat gradient buffer: [pass A: scene rows | human rows][scene dL/dSH][pass B: refined rows][stats]
         lay = merged_bucket_layout(self.Ps, self.Ph, self.M)
@@ -420,6 +407,7 @@ class MergedFivePlan:
                        "scene_human_refined": (0, P)}
         self.first_row = {"scene": 0, "human": Ps, "scene_human": Ps, "human_refined": Ps, "scene_human_refined": Ps}
         self._scenes = {}
+        self._current = {}  # pass -> (descriptor, views) of the frame in flight
         self._keep = []
 
     def describe(self) -> str:
@@ -471,8 +459,76 @@ class MergedFivePlan:
             self._scenes[key] = make()
         return self._scenes[key][0]
 
-    def _project_args(self, pk, g, accumulate, densify):
-        """B2RBackwardArgs of the backward projection of pass `pk` into the gradient views `g`."""
+    def _human_bg(self, settings_human_bg) -> torch.Tensor:
+        """The background of the human-only views on the device, kept alive while views that read it may be queued."""
+        bg_h = _f32c(settings_human_bg.bg.to(self.device), "bg")
+        self._keep.append(bg_h)
+        del self._keep[:-64]
+        return bg_h
+
+    def _view(self, ps, v, name, bg):
+        lo, hi = self.ranges[name]
+        fT, nc = ps.state[v]
+        # Tiles no human Gaussian reaches: a combined view equals the scene-only view there and carries no gradient; a
+        # human-only view shows the bare background there.  Both are pre-filled (`_forward_view`) and skipped by the
+        # kernels.
+        skip = self.Ps if (self.SKIP and name != "scene") else 0
+        return L.B2RView(lo, hi, _ptr(bg), fT.data_ptr(), nc.data_ptr(), ps.ck[v].data_ptr(), ps.ckpt_bytes, skip, 0)
+
+    # ---- the steps of a frame; each enqueues on the stream `s` it is given, which is also the current stream ----
+    def _start_pass(self, s, pk, key, settings, src, bg_h) -> None:
+        """Copies the rows of `src` (the human or refined set) behind the scene prefix of the pass -- src None: the
+        caller already wrote them -- then projects and bins it.  Its descriptor and views stay in `_current[pk]` until
+        the next frame."""
+        ps = self.passes[pk]
+        if src is not None:
+            for k, buf in ps.cat.items():
+                buf[self.Ps:].copy_(src[k].reshape(self.Ph, -1))
+        sc = self._scene_desc((key, pk), ps, settings)
+        sc.flags = L.B2R_FLAG_CTX_CLEAN if ps.primed else 0  # every pass leaves its ctx counters zero
+        ps.primed = True
+        L.check(self.lib.b2r_forward_project(C.byref(sc), C.byref(ps.ws), ps.radii.data_ptr(), s.cuda_stream),
+                "b2r_forward_project")
+        L.check(self.lib.b2r_forward_bin(C.byref(sc), C.byref(ps.ws), s.cuda_stream), "b2r_forward_bin")
+        views = [self._view(ps, v, n, bg_h if n in ("human", "human_refined") else None)
+                 for v, n in enumerate(self.VIEWS[pk])]
+        self._current[pk] = (sc, views)
+
+    def _forward_view(self, s, pk, v, bg_h, scene_done) -> None:
+        """Forward composite of view v of pass pk, after the pre-fill of the tiles it skips.  The scene-only view records
+        `scene_done`; the combined views of both passes copy its image."""
+        ps, name = self.passes[pk], self.VIEWS[pk][v]
+        sc, views = self._current[pk]
+        color, depth, alpha = ps.img[v]
+        if views[v].skip_below and name in ("human", "human_refined"):  # bare background, no depth / alpha
+            color.copy_(bg_h.view(3, 1, 1).expand_as(color))
+            depth.zero_()
+            alpha.zero_()
+        elif views[v].skip_below:  # pre-fill with the scene-only render; the composite overwrites human tiles
+            s.wait_event(scene_done)
+            for dst, src in zip(ps.img[v], self.passes["A"].img[0]):
+                dst.copy_(src)
+        out = L.B2RForwardOutputs(color.data_ptr(), depth.data_ptr(), alpha.data_ptr(), ps.radii.data_ptr())
+        L.check(self.lib.b2r_forward_composite(C.byref(sc), C.byref(ps.ws), C.byref(views[v]), C.byref(out),
+                                               s.cuda_stream), "b2r_forward_composite")
+        if name == "scene":
+            scene_done.record(s)
+
+    def _backward_view(self, s, pk, v, g_color, g_depth=None, g_alpha=None) -> None:
+        """Backward composite of view v of pass pk: its screen-space gradients are added into the pass's scratch."""
+        ps = self.passes[pk]
+        sc, views = self._current[pk]
+        a = L.B2RBackwardArgs(_ptr(g_color), _ptr(g_depth), _ptr(g_alpha))
+        a.flags = L.B2R_BWD_SCRATCH_ZEROED
+        a.first_row = self.first_row[self.VIEWS[pk][v]]
+        L.check(self.lib.b2r_backward_composite(C.byref(sc), C.byref(ps.ws), C.byref(views[v]), C.byref(a),
+                                                ps.bwd_scratch.data_ptr(), ps.bwd_bytes, s.cuda_stream),
+                "b2r_backward_composite")
+
+    def _backward_project(self, s, pk, g, accumulate, densify) -> None:
+        """The one backward projection of pass pk, from the scratch its views filled into the gradient views `g`."""
+        ps = self.passes[pk]
+        sc, _ = self._current[pk]
         a = L.B2RBackwardArgs(None, None, None, _ptr(g["means3D"]), _ptr(g["means2D"]),
                               _ptr(g.get("shs")) if pk == "A" else None, _ptr(g["colors"]),
                               _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), None)
@@ -482,27 +538,18 @@ class MergedFivePlan:
             a.densify_grad_accum, a.densify_count = _ptr(densify.get("grad_accum")), _ptr(densify.get("count"))
             a.densify_radius_max = _ptr(densify.get("radius_max"))
             a.densify_rows = self.Ps
-        return a
-
-    def _view(self, ps, v, name, bg):
-        lo, hi = self.ranges[name]
-        fT, nc = ps.state[v]
-        # Tiles no human Gaussian reaches: a combined view equals the scene-only view there and carries no gradient; a
-        # human-only view shows the bare background there.  Both are pre-filled by the caller and skipped by the kernels.
-        skip = self.Ps if (self.SKIP and name != "scene") else 0
-        return L.B2RView(lo, hi, _ptr(bg), fT.data_ptr(), nc.data_ptr(), ps.ck[v].data_ptr(), ps.ck_bytes, skip, 0)
+        L.check(self.lib.b2r_backward_project(C.byref(sc), C.byref(ps.ws), C.byref(a), ps.bwd_scratch.data_ptr(),
+                                              ps.bwd_bytes, s.cuda_stream), "b2r_backward_project")
 
     def frame(self, key, settings, settings_human_bg, scene, human, refined, g_colors: Dict[str, torch.Tensor],
               accumulate: bool, densify: Optional[Dict[str, torch.Tensor]] = None, serial: bool = False, probe=None) -> None:
-        """`probe(label)` (serial mode): called after every stage -- bench.py reads the in-library profiler there to get
-        per-view kernel times."""
-        lib = self.lib
+        """Forward + backward of the five renders.  Each pass runs on its own stream and forks one stream per view, on
+        which the view's backward composite follows its forward composite; the pass joins its views, then runs its
+        backward projection.  `serial`: everything on the caller's stream.  `probe(label)` (serial mode): called after
+        every stage -- bench.py reads the in-library profiler there to get per-view kernel times."""
         probe = probe if (probe is not None and serial) else (lambda label: None)
         cur = torch.cuda.current_stream(self.device)
-        bg_h = _f32c(settings_human_bg.bg.to(self.device), "bg")
-        self._keep.append(bg_h)
-        del self._keep[:-64]
-        scene_img = self.passes["A"].img[0]  # the scene-only view: what the combined views equal away from the human
+        bg_h = self._human_bg(settings_human_bg)
         scene_done = torch.cuda.Event()
         for pk, names in self.VIEWS.items():
             ps = self.passes[pk]
@@ -510,52 +557,21 @@ class MergedFivePlan:
             if not serial:
                 st.wait_stream(cur)
             with torch.cuda.stream(st):
-                src = human if pk == "A" else refined
-                for k, buf in ps.cat.items():
-                    buf[self.Ps:].copy_(src[k].reshape(self.Ph, -1))
-                sc = self._scene_desc((key, pk), ps, settings)
-                sc.flags = L.B2R_FLAG_CTX_CLEAN if ps.primed else 0  # every pass leaves its ctx counters zero
-                ps.primed = True
-                sp = st.cuda_stream
-                L.check(lib.b2r_forward_project(C.byref(sc), C.byref(ps.ws), ps.radii.data_ptr(), sp), "b2r_forward_project")
-                L.check(lib.b2r_forward_bin(C.byref(sc), C.byref(ps.ws), sp), "b2r_forward_bin")
+                self._start_pass(st, pk, key, settings, human if pk == "A" else refined, bg_h)
                 probe(f"{pk}:bin")
-                views = [self._view(ps, v, n, bg_h if n in ("human", "human_refined") else None) for v, n in enumerate(names)]
-                # forward + backward composite of every view; the views of a pass are independent of each other
                 for v, n in enumerate(names):
                     vs = st if serial else ps.streams[v]
                     if not serial:
                         vs.wait_stream(st)
                     with torch.cuda.stream(vs):
-                        color, depth, alpha = ps.img[v]
-                        if views[v].skip_below and n in ("human", "human_refined"):  # bare background, no depth / alpha
-                            color.copy_(bg_h.view(3, 1, 1).expand_as(color))
-                            depth.zero_()
-                            alpha.zero_()
-                        elif views[v].skip_below:  # pre-fill with the scene-only render; the composite overwrites human tiles
-                            vs.wait_event(scene_done)
-                            for dst, src in zip(ps.img[v], scene_img):
-                                dst.copy_(src)
-                        out = L.B2RForwardOutputs(color.data_ptr(), depth.data_ptr(), alpha.data_ptr(), ps.radii.data_ptr())
-                        L.check(lib.b2r_forward_composite(C.byref(sc), C.byref(ps.ws), C.byref(views[v]), C.byref(out),
-                                                          vs.cuda_stream), "b2r_forward_composite")
-                        if n == "scene":
-                            scene_done.record(vs)
+                        self._forward_view(vs, pk, v, bg_h, scene_done)
                         probe(f"{pk}:{n}:fwd")
-                        a = L.B2RBackwardArgs(_ptr(g_colors[n]))
-                        a.flags = L.B2R_BWD_SCRATCH_ZEROED
-                        a.first_row = self.first_row[n]
-                        L.check(lib.b2r_backward_composite(C.byref(sc), C.byref(ps.ws), C.byref(views[v]), C.byref(a),
-                                                           ps.bwd_scratch.data_ptr(), ps.bwd_bytes, vs.cuda_stream),
-                                "b2r_backward_composite")
+                        self._backward_view(vs, pk, v, g_colors[n])
                         probe(f"{pk}:{n}:bwd")
                 if not serial:
                     for v in range(len(names)):
                         st.wait_stream(ps.streams[v])
-                # one backward projection per pass
-                a = self._project_args(pk, self.views_A if pk == "A" else self.views_B, accumulate, densify)
-                L.check(lib.b2r_backward_project(C.byref(sc), C.byref(ps.ws), C.byref(a), ps.bwd_scratch.data_ptr(),
-                                                 ps.bwd_bytes, sp), "b2r_backward_project")
+                self._backward_project(st, pk, self.views_A if pk == "A" else self.views_B, accumulate, densify)
                 probe(f"{pk}:project_bwd")
         if not serial:
             for pk in self.passes:
@@ -566,49 +582,21 @@ class MergedFivePlan:
         """Forward of the five renders; images in `render_outputs()`, per-pixel state and checkpoints stay in the plan
         until `backward_frame` (so the plan must not start another frame in between).  copy_inputs=False: the caller
         already wrote the human / refined rows into `passes[*].cat` (a captured graph keeps the copies outside)."""
-        lib = self.lib
         cur = torch.cuda.current_stream(self.device)
-        bg_h = _f32c(settings_human_bg.bg.to(self.device), "bg")
-        self._keep.append(bg_h)
-        del self._keep[:-64]
-        scene_img = self.passes["A"].img[0]
+        bg_h = self._human_bg(settings_human_bg)
         scene_done = torch.cuda.Event()
-        self._pending = {}
         for pk, names in self.VIEWS.items():
             ps = self.passes[pk]
             st = self.pass_streams[pk]
             st.wait_stream(cur)
             with torch.cuda.stream(st):
-                if copy_inputs:
-                    src = human if pk == "A" else refined
-                    for k, buf in ps.cat.items():
-                        buf[self.Ps:].copy_(src[k].reshape(self.Ph, -1))
-                sc = self._scene_desc((key, pk), ps, settings)
-                sc.flags = L.B2R_FLAG_CTX_CLEAN if ps.primed else 0
-                ps.primed = True
-                sp = st.cuda_stream
-                L.check(lib.b2r_forward_project(C.byref(sc), C.byref(ps.ws), ps.radii.data_ptr(), sp), "b2r_forward_project")
-                L.check(lib.b2r_forward_bin(C.byref(sc), C.byref(ps.ws), sp), "b2r_forward_bin")
-                views = [self._view(ps, v, n, bg_h if n in ("human", "human_refined") else None) for v, n in enumerate(names)]
-                self._pending[pk] = (sc, views)
-                for v, n in enumerate(names):
+                src = (human if pk == "A" else refined) if copy_inputs else None
+                self._start_pass(st, pk, key, settings, src, bg_h)
+                for v in range(len(names)):
                     vs = ps.streams[v]
                     vs.wait_stream(st)
                     with torch.cuda.stream(vs):
-                        color, depth, alpha = ps.img[v]
-                        if views[v].skip_below and n in ("human", "human_refined"):
-                            color.copy_(bg_h.view(3, 1, 1).expand_as(color))
-                            depth.zero_()
-                            alpha.zero_()
-                        elif views[v].skip_below:
-                            vs.wait_event(scene_done)
-                            for dst, src_ in zip(ps.img[v], scene_img):
-                                dst.copy_(src_)
-                        out = L.B2RForwardOutputs(color.data_ptr(), depth.data_ptr(), alpha.data_ptr(), ps.radii.data_ptr())
-                        L.check(lib.b2r_forward_composite(C.byref(sc), C.byref(ps.ws), C.byref(views[v]), C.byref(out),
-                                                          vs.cuda_stream), "b2r_forward_composite")
-                        if n == "scene":
-                            scene_done.record(vs)
+                        self._forward_view(vs, pk, v, bg_h, scene_done)
                 for v in range(len(names)):
                     st.wait_stream(ps.streams[v])
         for pk in self.passes:
@@ -621,11 +609,9 @@ class MergedFivePlan:
         """Backward of the frame `forward_frame` rendered.  g_colors[name] = dL/dimage of a render, or None when the render
         was not used downstream.  grads_A / grads_B: `_views_of`-style dicts with P / P_human rows (pass A: scene rows then
         human rows; pass B: refined rows)."""
-        lib = self.lib
         cur = torch.cuda.current_stream(self.device)
         for pk, names in self.VIEWS.items():
             ps = self.passes[pk]
-            sc, views = self._pending[pk]
             st = self.pass_streams[pk]
             st.wait_stream(cur)
             with torch.cuda.stream(st):
@@ -638,18 +624,11 @@ class MergedFivePlan:
                     with torch.cuda.stream(vs):
                         if gc is None:
                             gc = torch.zeros(3, self.H, self.W, dtype=torch.float32, device=self.device)
-                        a = L.B2RBackwardArgs(_ptr(gc), _ptr(gd), _ptr(ga))
-                        a.flags = L.B2R_BWD_SCRATCH_ZEROED
-                        a.first_row = self.first_row[n]
-                        L.check(lib.b2r_backward_composite(C.byref(sc), C.byref(ps.ws), C.byref(views[v]), C.byref(a),
-                                                           ps.bwd_scratch.data_ptr(), ps.bwd_bytes, vs.cuda_stream),
-                                "b2r_backward_composite")
+                        self._backward_view(vs, pk, v, gc, gd, ga)
                         self._keep.append((gc, gd, ga))
                 for v in range(len(names)):
                     st.wait_stream(ps.streams[v])
-                a = self._project_args(pk, grads_A if pk == "A" else grads_B, accumulate, densify)
-                L.check(lib.b2r_backward_project(C.byref(sc), C.byref(ps.ws), C.byref(a), ps.bwd_scratch.data_ptr(),
-                                                 ps.bwd_bytes, st.cuda_stream), "b2r_backward_project")
+                self._backward_project(st, pk, grads_A if pk == "A" else grads_B, accumulate, densify)
         for pk in self.passes:
             cur.wait_stream(self.pass_streams[pk])
 

@@ -38,6 +38,15 @@ def test_struct_layouts_and_version():
     assert C.sizeof(L.B2RStatus) == 64
 
 
+def test_status_block_decodes_every_field():
+    import torch
+    s = L.B2RStatus(num_dups=7, dup_capacity=9, overflow=1, num_visible=5, consumed_fwd=80, consumed_bwd=40, token=3)
+    ctx = torch.tensor(list(bytes(s)) + [0xAB] * 64, dtype=torch.uint8)  # the rest of a ctx buffer follows the block
+    assert L.read_status(ctx) == {"num_dups": 7, "dup_capacity": 9, "overflow": 1, "num_visible": 5, "consumed_fwd": 80,
+                                  "consumed_bwd": 40, "consumed_fwd_div": float(L.CONSUMED_FWD_DIV),
+                                  "consumed_bwd_div": float(L.CONSUMED_BWD_DIV)}
+
+
 def test_size_queries():
     lib = L.load()
     a = lib.b2r_ctx_bytes(1000, 64, 64)
