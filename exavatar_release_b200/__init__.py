@@ -3,12 +3,14 @@
 Public surface (mirrors what /root/reference/avatar/common/nets/module.py:11 imports):
     GaussianRasterizationSettings, GaussianRasterizer
 plus the host-side mirror of the caller (`GaussianRenderer`, module.py:588-647), `TrainingFrameRenderer` (the five
-renders of a training frame, avatar/main/model.py:117-162, as one autograd call), synthetic workloads and the
+renders of a training frame, avatar/main/model.py:117-162, as one autograd call), `skin_gaussians` (both human sets
+posed by one rig), `l1_ssim` (the L1 + SSIM terms of the loss block, model.py:196-215), synthetic workloads and the
 frame-sharding helper used by bench.py.
 """
 from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians  # noqa: F401
 from .renderer import GaussianRenderer, render_settings  # noqa: F401
 from .skinning import skin_gaussians  # noqa: F401
+from .losses import l1_ssim  # noqa: F401
 
 
 def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loaded on first use
@@ -19,4 +21,4 @@ def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loa
 
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "GaussianRenderer",
-           "render_settings", "TrainingFrameRenderer", "skin_gaussians"]
+           "render_settings", "TrainingFrameRenderer", "skin_gaussians", "l1_ssim"]

@@ -129,6 +129,10 @@ SYMBOLS = [
     ("b2r_skin_forward", C.c_int, [C.POINTER(B2RSkin), _fp]),
     ("b2r_skin_backward", C.c_int, [C.POINTER(B2RSkin), C.POINTER(_fp), C.POINTER(_fp), _fp, _fp, _fp, C.c_size_t, _fp]),
     ("b2r_skin_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32]),
+    ("b2r_l1ssim_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32]),
+    ("b2r_l1ssim_forward", C.c_int, [C.c_int32, C.c_int32, _fp, _fp, _fp, _fp, C.c_int32, _fp, _fp, C.c_size_t, _fp]),
+    ("b2r_l1ssim_backward", C.c_int, [C.c_int32, C.c_int32, _fp, _fp, _fp, _fp, C.c_int32, _fp, _fp, _fp, C.c_size_t,
+                                      _fp]),
     ("b2r_profile_enable", None, [C.c_int]),
     ("b2r_profile_read", C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int]),
     ("b2r_launch_count", C.c_uint64, []),

@@ -73,6 +73,11 @@ int validate_skin(const B2RSkin* s) {
   return B2R_OK;
 }
 
+// l1ssim.cu: 16-pixel tiles on a 2-D grid (grid.y <= 65535); the 9 per-pixel partial planes stay addressable
+bool valid_l1ssim_size(int32_t width, int32_t height) {
+  return width > 0 && height > 0 && height <= 65535 * 16 && (int64_t)width * height <= (int64_t)1 << 31;
+}
+
 }  // namespace
 
 extern "C" {
@@ -261,6 +266,29 @@ int b2r_skin_backward(const B2RSkin* skin, const float* const dL_dposed[2], floa
     if (scratch_bytes < skin_scratch_bytes(skin->P, skin->J)) return B2R_E_WORKSPACE;
   }
   return launch_skin_backward(*skin, dL_dposed, dL_dxyz, dL_djoint, dL_dtrans, scratch, (cudaStream_t)stream);
+}
+
+size_t b2r_l1ssim_scratch_bytes(int32_t width, int32_t height) { return l1ssim_scratch_bytes(width, height); }
+
+int b2r_l1ssim_forward(int32_t width, int32_t height, const float* img, const float* target, const float* mask,
+                       const float* bbox, int32_t with_ssim, float* out, void* scratch, size_t scratch_bytes,
+                       void* stream) {
+  if (!valid_l1ssim_size(width, height) || !img || !target || !out || !scratch) return B2R_E_INVALID;
+  if (scratch_bytes < l1ssim_scratch_bytes(width, height)) return B2R_E_WORKSPACE;
+  return launch_l1ssim_forward(width, height, img, target, mask, bbox, with_ssim != 0, out, scratch,
+                               (cudaStream_t)stream);
+}
+
+int b2r_l1ssim_backward(int32_t width, int32_t height, const float* img, const float* target, const float* mask,
+                        const float* bbox, int32_t with_ssim, const float* dL_dout, float* dL_dimg, const void* scratch,
+                        size_t scratch_bytes, void* stream) {
+  if (!valid_l1ssim_size(width, height) || !img || !target || !dL_dout || !dL_dimg) return B2R_E_INVALID;
+  if (with_ssim) {  // the forward's per-pixel SSIM partials
+    if (!scratch) return B2R_E_INVALID;
+    if (scratch_bytes < l1ssim_scratch_bytes(width, height)) return B2R_E_WORKSPACE;
+  }
+  return launch_l1ssim_backward(width, height, img, target, mask, bbox, with_ssim != 0, dL_dout, dL_dimg, scratch,
+                                (cudaStream_t)stream);
 }
 
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {

@@ -495,6 +495,11 @@ int launch_skin_forward(const B2RSkin& s, cudaStream_t st);
 int launch_skin_backward(const B2RSkin& s, const float* const dposed[2], float* const dxyz[2], float* djoint,
                          float* dtrans, void* scratch, cudaStream_t st);
 size_t skin_scratch_bytes(int P, int J);
+int launch_l1ssim_forward(int W, int H, const float* img, const float* target, const float* mask, const float* bbox,
+                          bool with_ssim, float* out, void* scratch, cudaStream_t st);
+int launch_l1ssim_backward(int W, int H, const float* img, const float* target, const float* mask, const float* bbox,
+                           bool with_ssim, const float* dout, float* dimg, const void* scratch, cudaStream_t st);
+size_t l1ssim_scratch_bytes(int W, int H);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

@@ -278,11 +278,29 @@ int b2r_skin_backward(const B2RSkin* skin, const float* const dL_dposed[2], floa
                       float* dL_dtrans, void* scratch, size_t scratch_bytes, void* stream);
 size_t b2r_skin_scratch_bytes(int32_t P, int32_t J);
 
+/* Photometric L1 + SSIM of one (3,H,W) image against a target (avatar/common/nets/loss.py RGBLoss / SSIM, reduced with
+ * .mean() as avatar/main/model.py:196-215 does).  `mask` (H,W) or NULL multiplies both images first; `bbox` is a DEVICE
+ * float[4] {xmin, ymin, width, height} or NULL (the whole image), read on the device with the reference's integer rules:
+ * x0 = max(trunc(xmin), 0), x1 = min(x0 + trunc(width), W), likewise for y, crop [y0:y1, x0:x1].  The SSIM window
+ * (11 taps, sigma 1.5) runs over the crop with zero padding at the crop's border.  Forward writes out[0] = mean |x - y|
+ * and, with with_ssim != 0, out[1] = mean SSIM, both over 3 h w (NaN for an empty crop).  Backward reads dL_dout[2]
+ * (device) and writes every element of dL_dimg (3,H,W): zero outside the crop.  `scratch` >= b2r_l1ssim_scratch_bytes
+ * (W, H) holds the forward's per-pixel SSIM partials until the backward (the backward without SSIM does not read it,
+ * and it may then be NULL).  Fixed-order reductions, no float atomics: bit-identical runs.  Neither call allocates or
+ * syncs. */
+size_t b2r_l1ssim_scratch_bytes(int32_t width, int32_t height);
+int b2r_l1ssim_forward(int32_t width, int32_t height, const float* img, const float* target, const float* mask,
+                       const float* bbox, int32_t with_ssim, float* out, void* scratch, size_t scratch_bytes,
+                       void* stream);
+int b2r_l1ssim_backward(int32_t width, int32_t height, const float* img, const float* target, const float* mask,
+                        const float* bbox, int32_t with_ssim, const float* dL_dout, float* dL_dimg, const void* scratch,
+                        size_t scratch_bytes, void* stream);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_* and b2r_l1ssim_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
