@@ -133,6 +133,9 @@ SYMBOLS = [
     ("b2r_l1ssim_forward", C.c_int, [C.c_int32, C.c_int32, _fp, _fp, _fp, _fp, C.c_int32, _fp, _fp, C.c_size_t, _fp]),
     ("b2r_l1ssim_backward", C.c_int, [C.c_int32, C.c_int32, _fp, _fp, _fp, _fp, C.c_int32, _fp, _fp, _fp, C.c_size_t,
                                       _fp]),
+    ("b2r_nearest_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32]),
+    ("b2r_nearest_rows", C.c_int, [C.c_int32, _fp, C.c_int32, _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
+    ("b2r_vertex_normals", C.c_int, [C.c_int32, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     ("b2r_profile_enable", None, [C.c_int]),
     ("b2r_profile_read", C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int]),
     ("b2r_launch_count", C.c_uint64, []),

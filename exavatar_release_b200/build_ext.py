@@ -32,7 +32,10 @@ NVCC_FLAGS = [
 # with the same contraction setting (its kernels are integer sorts otherwise).
 # skin.cu: the standalone skinning op evaluates the blend of project.cu's fused skinning (gaussian_math.cuh skin_apply);
 # compiled with the same contraction setting, both paths write bit-identical posed positions.
-PER_FILE_FLAGS = {"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"]}
+# geometry.cu: the nearest-vertex search evaluates dx*dx + dy*dy + dz*dz exactly as its torch restatement does (three
+# rounded products, two rounded sums), so the argmin -- ties included -- is the restatement's, index for index.
+PER_FILE_FLAGS = {"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
+                  "geometry.cu": ["--fmad=false"]}
 
 
 def sources():

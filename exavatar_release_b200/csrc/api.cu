@@ -291,6 +291,28 @@ int b2r_l1ssim_backward(int32_t width, int32_t height, const float* img, const f
                                 (cudaStream_t)stream);
 }
 
+size_t b2r_nearest_scratch_bytes(int32_t P, int32_t V) {
+  (void)P;  // the grid is sized from the targets alone
+  return nearest_scratch_bytes(V);
+}
+
+int b2r_nearest_rows(int32_t P, const float* queries, int32_t V, const float* targets, const uint8_t* self_map,
+                     int32_t* rows, void* scratch, size_t scratch_bytes, void* stream) {
+  if (P < 0 || V < 0 || V >= (1 << 29)) return B2R_E_INVALID;  // cell counts 2V + 64 stay in int32
+  if (P == 0) return B2R_OK;
+  if (V < 1 || !queries || !targets || !rows || !scratch) return B2R_E_INVALID;
+  if (scratch_bytes < nearest_scratch_bytes(V)) return B2R_E_WORKSPACE;
+  return launch_nearest_rows(P, queries, V, targets, self_map, rows, scratch, (cudaStream_t)stream);
+}
+
+int b2r_vertex_normals(int32_t P, const float* xyz, const int32_t* faces, const int32_t* vf_offsets,
+                       const int32_t* vf_entries, const uint8_t* flip, float* normals, void* stream) {
+  if (P < 0) return B2R_E_INVALID;
+  if (P == 0) return B2R_OK;
+  if (!xyz || !faces || !vf_offsets || !vf_entries || !normals) return B2R_E_INVALID;
+  return launch_vertex_normals(P, xyz, faces, vf_offsets, vf_entries, flip, normals, (cudaStream_t)stream);
+}
+
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {
   if (P < 0 || (P > 0 && (!means3D || !present)) || !viewmatrix) return B2R_E_INVALID;
   return launch_mark_visible(P, means3D, viewmatrix, present, (cudaStream_t)stream);

@@ -500,6 +500,11 @@ int launch_l1ssim_forward(int W, int H, const float* img, const float* target, c
 int launch_l1ssim_backward(int W, int H, const float* img, const float* target, const float* mask, const float* bbox,
                            bool with_ssim, const float* dout, float* dimg, const void* scratch, cudaStream_t st);
 size_t l1ssim_scratch_bytes(int W, int H);
+int launch_nearest_rows(int P, const float* queries, int V, const float* targets, const uint8_t* self_map,
+                        int32_t* rows, void* scratch, cudaStream_t st);
+size_t nearest_scratch_bytes(int V);
+int launch_vertex_normals(int P, const float* xyz, const int32_t* faces, const int32_t* vf_offsets,
+                          const int32_t* vf_entries, const uint8_t* flip, float* normals, cudaStream_t st);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

@@ -12,6 +12,7 @@ from __future__ import annotations
 import math
 from dataclasses import dataclass
 
+import numpy as np
 import torch
 
 SH_C0 = 0.28209479177387814
@@ -125,6 +126,74 @@ def make_population_assets(workload, seed=0, device="cpu", focal_ratio=1.465):
     refined["rgb"] = (human["rgb"] + 0.05 * torch.randn(wl.n_avatar, 3, generator=g)).clamp(0, 1)
     to = lambda d: {k: v.to(device) for k, v in d.items()}
     return to(scene), to(human), to(refined)
+
+
+def _subdivide(verts, faces):
+    """One midpoint subdivision (each triangle into four, no smoothing), the input vertices kept first -- the order
+    ExAvatar's `lr_idx_to_hr_idx` relies on (module.py:511-514)."""
+    e = np.sort(np.stack([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]], 1).reshape(-1, 2), axis=1)
+    uniq, inv = np.unique(e, axis=0, return_inverse=True)
+    mid = (len(verts) + inv.reshape(-1, 3)).astype(np.int64)  # new vertex of edge (a,b), (b,c), (c,a)
+    ab, bc, ca = mid[:, 0], mid[:, 1], mid[:, 2]
+    a, b, c = faces[:, 0], faces[:, 1], faces[:, 2]
+    nf = np.stack([np.stack([a, ab, ca], 1), np.stack([b, bc, ab], 1), np.stack([c, ca, bc], 1),
+                   np.stack([ab, bc, ca], 1)], 1).reshape(-1, 3)
+    return np.concatenate([verts, 0.5 * (verts[uniq[:, 0]] + verts[uniq[:, 1]])]), nf
+
+
+def make_human_mesh(seed=0, rings=97, segments=108):
+    """A seeded stand-in for ExAvatar's SMPL-X meshes, for `geometry.nearest_rows` / `VertexNormals`.
+
+    The base mesh is a latitude-longitude triangulation of the body-sized ellipsoid shell of `_avatar` (0.25 x 0.85 x
+    0.15 m around (0, 0, 4.24), poles on the long axis): rings * segments + 2 = 10 478 vertices by default, like
+    SMPL-X's 10 475.  A small dent on the front is the "cavity": its vertices are pushed inward and flagged in `flip`.
+    Two midpoint subdivisions in numpy keep the base vertices first (like `smpl_x.face_upsampled`): 167 618 vertices,
+    335 232 faces.  Returns float32 / int64 / bool CPU tensors:
+        targets   (V,3)  the base vertices (`mesh_neutral_pose_wo_upsample`)
+        verts     (P,3)  the subdivided vertices (`mesh_neutral_pose`)
+        faces     (F,3)  the subdivided faces, outward winding
+        queries   (P,3)  verts + N(0, 1 mm) offsets (`mean_3d`)
+        self_map  (P,)   head cap and both flanks, about 30 % (is_rhand | is_lhand | is_face)
+        flip      (P,)   the cavity's vertices (is_cavity)
+    """
+    th = np.pi * np.arange(1, rings + 1) / (rings + 1)
+    ph = 2 * np.pi * np.arange(segments) / segments
+    u = np.concatenate([[[0.0, 1.0, 0.0]],
+                        np.stack([np.sin(th)[:, None] * np.cos(ph)[None], np.cos(th)[:, None] * np.ones_like(ph)[None],
+                                  np.sin(th)[:, None] * np.sin(ph)[None]], -1).reshape(-1, 3),
+                        [[0.0, -1.0, 0.0]]])
+    ring = lambda i, j: 1 + i * segments + j % segments  # noqa: E731
+    j = np.arange(segments)
+    faces = [np.stack([np.zeros_like(j), ring(0, j + 1), ring(0, j)], 1)]
+    for i in range(rings - 1):
+        faces += [np.stack([ring(i, j), ring(i, j + 1), ring(i + 1, j)], 1),
+                  np.stack([ring(i + 1, j), ring(i, j + 1), ring(i + 1, j + 1)], 1)]
+    south = len(u) - 1
+    faces.append(np.stack([np.full_like(j, south), ring(rings - 1, j), ring(rings - 1, j + 1)], 1))
+    faces = np.concatenate(faces).astype(np.int64)
+    semi = np.array([0.25, 0.85, 0.15])
+    # the cavity: a smooth dent, 15 mm deep, 6 cm across, on the front of the "head"
+    dent_dir = np.array([0.0, 0.6, -0.8])
+    ang = np.arccos(np.clip(u @ dent_dir, -1, 1))
+    r0 = 0.2
+    depth = np.where(ang < r0, 0.015 * 0.5 * (1 + np.cos(np.pi * ang / r0)), 0.0)
+    pos = u * semi * (1 - depth / 0.15)[:, None]
+    pos[:, 2] += 4.24
+    v0, v1, v2 = pos[faces[:, 0]], pos[faces[:, 1]], pos[faces[:, 2]]
+    outward = (np.cross(v1 - v0, v2 - v0) * ((v0 + v1 + v2) / 3 - [0.0, 0.0, 4.24])).sum(1) > 0
+    faces[~outward] = faces[~outward][:, [0, 2, 1]]
+    V = len(pos)
+    verts, fs = _subdivide(pos, faces)
+    verts, fs = _subdivide(verts, fs)
+    c = verts - [0.0, 0.0, 4.24]
+    d = c / semi
+    flip = np.arccos(np.clip((d / np.linalg.norm(d, axis=1, keepdims=True)) @ dent_dir, -1, 1)) < 0.8 * r0
+    self_map = (c[:, 1] > 0.6) | (np.abs(c[:, 0]) > 0.23)
+    g = np.random.default_rng(seed)
+    queries = verts + 0.001 * g.standard_normal(verts.shape)
+    f32 = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))  # noqa: E731
+    return {"targets": f32(verts[:V]), "verts": f32(verts), "faces": torch.from_numpy(fs), "queries": f32(queries),
+            "self_map": torch.from_numpy(self_map), "flip": torch.from_numpy(flip)}
 
 
 def make_scene_sh_params(scene, sh_degree=3, seed=0):

@@ -296,11 +296,32 @@ int b2r_l1ssim_backward(int32_t width, int32_t height, const float* img, const f
                         const float* bbox, int32_t with_ssim, const float* dL_dout, float* dL_dimg, const void* scratch,
                         size_t scratch_bytes, void* stream);
 
+/* Nearest mesh vertex of every human Gaussian (avatar/common/nets/module.py:541-546: knn_points(K=1) and the
+ * hand / face self-map).  rows[i] = i where self_map[i] != 0 (self_map (P) may be NULL: none); otherwise the smallest j
+ * minimising d(i,j) = dx*dx + dy*dy + dz*dz (dx = queries[i].x - targets[j].x ..., fp32, left to right, no fma), which
+ * is torch.argmin's answer, ties included; a query with a non-finite coordinate gets row 0.  queries (P,3), targets
+ * (V,3) must be finite (other targets give unspecified rows, never an out-of-bounds access); rows (P) int32 is what
+ * B2RSkin.rows reads.  Every call builds a uniform grid over the targets in `scratch` (>= b2r_nearest_scratch_bytes(P,
+ * V), which depends on V only) and searches it exactly.  P = 0 launches nothing.  No allocation, no sync. */
+size_t b2r_nearest_scratch_bytes(int32_t P, int32_t V);
+int b2r_nearest_rows(int32_t P, const float* queries, int32_t V, const float* targets, const uint8_t* self_map,
+                     int32_t* rows, void* scratch, size_t scratch_bytes, void* stream);
+
+/* Area-weighted vertex normals of a triangle mesh with P vertices (module.py:501-504: verts_normals_packed and the
+ * cavity flip).  xyz (P,3); faces (F,3) int32, every index in [0, P).  The vertex -> face CSR: vf_offsets (P+1) int32,
+ * vf_offsets[0] = 0, non-decreasing, vf_offsets[P] = 3F; vf_entries (3F) int32 face indices, the incident faces of
+ * vertex v at [vf_offsets[v], vf_offsets[v+1]) in ascending order, one entry per corner (a face that repeats v lists it
+ * twice).  normals[v] = n / max(|n|, 1e-6) with n the fp32 sum, in CSR order, of (x1 - x0) x (x2 - x0) over v's
+ * entries (0 for a vertex in no face), negated where flip (P, may be NULL) is set.  No float atomics: bit-identical
+ * runs.  P = 0 launches nothing.  No allocation, no sync. */
+int b2r_vertex_normals(int32_t P, const float* xyz, const int32_t* faces, const int32_t* vf_offsets,
+                       const int32_t* vf_entries, const uint8_t* flip, float* normals, void* stream);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_* and b2r_l1ssim_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows and b2r_vertex_normals kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
