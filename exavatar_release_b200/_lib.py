@@ -68,6 +68,17 @@ class B2RSkin(C.Structure):
     ]
 
 
+class B2RMeshRender(C.Structure):
+    """Textured mesh render (b2r_mesh_render_forward / b2r_mesh_render_backward): ExAvatar's face render."""
+    _fields_ = [
+        ("V", C.c_int32), ("F", C.c_int32), ("Vt", C.c_int32), ("C", C.c_int32),
+        ("tex_height", C.c_int32), ("tex_width", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
+        ("mesh", _fp), ("faces", _fp), ("vertex_uv", _fp), ("face_uv", _fp), ("texture", _fp),
+        ("cam_R", _fp), ("cam_t", _fp), ("focal", _fp), ("princpt", _fp), ("keys", _fp),
+        ("vf_offsets", _fp), ("vf_entries", _fp),
+    ]
+
+
 class B2RForwardOutputs(C.Structure):
     _fields_ = [("color", _fp), ("depth", _fp), ("alpha", _fp), ("radii", _fp)]
 
@@ -136,6 +147,9 @@ SYMBOLS = [
     ("b2r_nearest_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32]),
     ("b2r_nearest_rows", C.c_int, [C.c_int32, _fp, C.c_int32, _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
     ("b2r_vertex_normals", C.c_int, [C.c_int32, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
+    ("b2r_mesh_render_scratch_bytes", C.c_size_t, [C.c_int32]),
+    ("b2r_mesh_render_forward", C.c_int, [C.POINTER(B2RMeshRender), _fp, _fp, _fp, C.c_size_t, _fp]),
+    ("b2r_mesh_render_backward", C.c_int, [C.POINTER(B2RMeshRender), _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
     ("b2r_profile_enable", None, [C.c_int]),
     ("b2r_profile_read", C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int]),
     ("b2r_launch_count", C.c_uint64, []),
@@ -166,7 +180,9 @@ def load():
         fn.argtypes = argtypes
     if lib.b2r_abi_version() != ABI_VERSION:
         raise RuntimeError("b200raster: ABI version mismatch between the Python binding and libb200raster.so")
-    for idx, cls in enumerate((B2RScene, B2RStatus, B2RWorkspace, B2RForwardOutputs, B2RBackwardArgs, B2RView, B2RSkin)):
+    # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8
+    for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
+                     (5, B2RView), (6, B2RSkin), (8, B2RMeshRender)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

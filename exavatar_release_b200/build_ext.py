@@ -34,8 +34,10 @@ NVCC_FLAGS = [
 # compiled with the same contraction setting, both paths write bit-identical posed positions.
 # geometry.cu: the nearest-vertex search evaluates dx*dx + dy*dy + dz*dz exactly as its torch restatement does (three
 # rounded products, two rounded sums), so the argmin -- ties included -- is the restatement's, index for index.
+# mesh_raster.cu: the face render's coverage test and depth pz are, operation for operation, the float32 restatement's
+# (mesh_render.face_render_reference), so the per-pixel face is identical to it instead of "equal except at ulp ties".
 PER_FILE_FLAGS = {"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
-                  "geometry.cu": ["--fmad=false"]}
+                  "geometry.cu": ["--fmad=false"], "mesh_raster.cu": ["--fmad=false"]}
 
 
 def sources():

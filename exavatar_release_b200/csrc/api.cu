@@ -78,6 +78,21 @@ bool valid_l1ssim_size(int32_t width, int32_t height) {
   return width > 0 && height > 0 && height <= 65535 * 16 && (int64_t)width * height <= (int64_t)1 << 31;
 }
 
+// sizes and the pointers both directions read; the index tables' contents are the caller's (see b200raster.h)
+int validate_mesh_render(const B2RMeshRender* m) {
+  if (!m) return B2R_E_INVALID;
+  if (m->V < 0 || m->F < 0 || m->Vt < 0 || m->C < 1 || m->C > 4) return B2R_E_INVALID;
+  if (m->width <= 0 || m->height <= 0 || (int64_t)m->width * m->height >= ((int64_t)1 << 31)) return B2R_E_INVALID;
+  if (m->F >= (1 << 29) || m->V >= (1 << 29)) return B2R_E_INVALID;  // 9 F floats and 3 V indices stay in int32
+  if (!m->cam_R || !m->cam_t || !m->focal || !m->princpt) return B2R_E_INVALID;
+  if (m->F > 0) {
+    if (m->V < 1 || m->Vt < 1 || m->tex_height < 1 || m->tex_width < 1) return B2R_E_INVALID;
+    if ((int64_t)m->C * m->tex_height * m->tex_width >= ((int64_t)1 << 31)) return B2R_E_INVALID;
+    if (!m->mesh || !m->faces || !m->vertex_uv || !m->face_uv || !m->texture) return B2R_E_INVALID;
+  }
+  return B2R_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -106,6 +121,7 @@ size_t b2r_sizeof(int which) {
     case 4: return sizeof(B2RBackwardArgs);
     case 5: return sizeof(B2RView);
     case 6: return sizeof(B2RSkin);
+    case 8: return sizeof(B2RMeshRender);  // 7 stays unused
     default: return 0;
   }
 }
@@ -311,6 +327,27 @@ int b2r_vertex_normals(int32_t P, const float* xyz, const int32_t* faces, const 
   if (P == 0) return B2R_OK;
   if (!xyz || !faces || !vf_offsets || !vf_entries || !normals) return B2R_E_INVALID;
   return launch_vertex_normals(P, xyz, faces, vf_offsets, vf_entries, flip, normals, (cudaStream_t)stream);
+}
+
+size_t b2r_mesh_render_scratch_bytes(int32_t F) { return mesh_render_scratch_bytes(F); }
+
+int b2r_mesh_render_forward(const B2RMeshRender* mr, float* image, int32_t* pix_to_face, void* scratch,
+                            size_t scratch_bytes, void* stream) {
+  const int rc = validate_mesh_render(mr);
+  if (rc) return rc;
+  if (!mr->keys || !image || !pix_to_face || !scratch) return B2R_E_INVALID;
+  if (scratch_bytes < mesh_render_scratch_bytes(mr->F)) return B2R_E_WORKSPACE;
+  return launch_mesh_render_forward(*mr, image, pix_to_face, scratch, (cudaStream_t)stream);
+}
+
+int b2r_mesh_render_backward(const B2RMeshRender* mr, const int32_t* pix_to_face, const float* dL_dimage,
+                             float* dL_dmesh, void* scratch, size_t scratch_bytes, void* stream) {
+  const int rc = validate_mesh_render(mr);
+  if (rc) return rc;
+  if (!pix_to_face || !dL_dimage || !scratch) return B2R_E_INVALID;
+  if (mr->V > 0 && (!dL_dmesh || !mr->vf_offsets || !mr->vf_entries)) return B2R_E_INVALID;
+  if (scratch_bytes < mesh_render_scratch_bytes(mr->F)) return B2R_E_WORKSPACE;
+  return launch_mesh_render_backward(*mr, pix_to_face, dL_dimage, dL_dmesh, scratch, (cudaStream_t)stream);
 }
 
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {

@@ -505,6 +505,11 @@ int launch_nearest_rows(int P, const float* queries, int V, const float* targets
 size_t nearest_scratch_bytes(int V);
 int launch_vertex_normals(int P, const float* xyz, const int32_t* faces, const int32_t* vf_offsets,
                           const int32_t* vf_entries, const uint8_t* flip, float* normals, cudaStream_t st);
+size_t mesh_render_scratch_bytes(int F);
+int launch_mesh_render_forward(const B2RMeshRender& m, float* image, int32_t* pix_to_face, void* scratch,
+                               cudaStream_t st);
+int launch_mesh_render_backward(const B2RMeshRender& m, const int32_t* pix_to_face, const float* dimage, float* dmesh,
+                                void* scratch, cudaStream_t st);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

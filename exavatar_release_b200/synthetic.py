@@ -196,6 +196,46 @@ def make_human_mesh(seed=0, rings=97, segments=108):
             "self_map": torch.from_numpy(self_map), "flip": torch.from_numpy(flip)}
 
 
+def make_face_mesh(seed=0, num_vertices=5023, tex_size=512):
+    """A seeded stand-in for ExAvatar's FLAME face mesh and texture, for `mesh_render.FaceMeshRenderer`.
+
+    The mesh is a cap on the upper front of `make_human_mesh`'s "head" (facing the synthetic camera, like a face): the
+    `num_vertices` vertices (5 023 like FLAME) nearest the direction (0, 0.75, -0.66) of the shell's parameter sphere and
+    the faces among them (about 10 k, outward winding; the cavity's dent lies inside).  Returns CPU tensors / arrays:
+        vertex_idx  (V,)      int64 indices into make_human_mesh()["verts"] (stands in for smpl_x.face_vertex_idx)
+        faces       (F,3)     int64 indices into vertex_idx (flame.face)
+        vertex_uv   (Vt,2)    float32 planar layout (x, z of the cap) with a seam: the faces left of x = 0 use a
+                              second copy of the layout moved 0.02 left, so Vt = 2 V and face_uv != faces
+        face_uv     (F,3)     int64 rows of vertex_uv (flame.face_uv)
+        texture     (4,T,T)   float32 RGB in [0, 1] plus a mask channel in {0, 1} (flame.texture + texture_mask)
+    """
+    m = make_human_mesh(seed)
+    verts, faces = m["verts"].numpy().astype(np.float64), m["faces"].numpy()
+    d = (verts - [0.0, 0.0, 4.24]) / [0.25, 0.85, 0.15]
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    order = np.argsort(-(d @ np.array([0.0, 0.75, -0.66])), kind="stable")
+    idx = np.sort(order[:num_vertices])
+    local = np.full(len(verts), -1, np.int64)
+    local[idx] = np.arange(len(idx))
+    fl = local[faces]
+    fl = fl[(fl >= 0).all(1)]
+    p = verts[idx]
+    c = p - p.mean(0)
+    ext = np.abs(c).max(0)
+    uv = np.stack([0.5 + 0.45 * c[:, 0] / ext[0], 0.5 + 0.45 * c[:, 2] / ext[2]], 1)
+    left = c[fl].mean(1)[:, 0] < 0
+    vertex_uv = np.concatenate([uv, uv - [0.02, 0.0]]).astype(np.float32)
+    face_uv = np.where(left[:, None], fl + len(idx), fl)
+    g = torch.Generator().manual_seed(9000 + seed)
+    low = torch.rand(1, 3, 16, 16, generator=g)
+    rgb = torch.nn.functional.interpolate(low, size=(tex_size, tex_size), mode="bilinear", align_corners=True)[0]
+    rgb = (rgb + 0.1 * torch.rand(3, tex_size, tex_size, generator=g)).clamp(0, 1)
+    mask = torch.nn.functional.interpolate((torch.rand(1, 1, 8, 8, generator=g) > 0.3).float(),
+                                           size=(tex_size, tex_size), mode="nearest")[0]
+    return {"vertex_idx": torch.from_numpy(idx), "faces": torch.from_numpy(fl), "vertex_uv": torch.from_numpy(vertex_uv),
+            "face_uv": torch.from_numpy(face_uv), "texture": torch.cat([rgb, mask]).contiguous()}
+
+
 def make_scene_sh_params(scene, sh_degree=3, seed=0):
     """Pre-activation parameters of the scene population as `SceneGaussian` stores them (module.py:103-108): mean,
     opacity logit, log scale, rotation, `feature_dc` (P,1,3) = RGB2SH(rgb) and `feature_rest` (P,(d+1)^2-1,3) seeded

@@ -226,7 +226,8 @@ int b2r_abi_version(void);
 const char* b2r_strerror(int code);
 int b2r_last_cuda_error(void);
 /* sizeof() of the ABI structs, for bindings to verify their mirror: 0 B2RScene, 1 B2RStatus, 2 B2RWorkspace,
- * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin; 0 for anything else. */
+ * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin, 8 B2RMeshRender; 0 for anything else (7 is
+ * unused and reports 0). */
 size_t b2r_sizeof(int which);
 
 size_t b2r_ctx_bytes(int32_t P, int32_t width, int32_t height);
@@ -317,11 +318,62 @@ int b2r_nearest_rows(int32_t P, const float* queries, int32_t V, const float* ta
 int b2r_vertex_normals(int32_t P, const float* xyz, const int32_t* faces, const int32_t* vf_offsets,
                        const int32_t* vf_entries, const uint8_t* flip, float* normals, void* stream);
 
+/* Textured render of a triangle mesh: ExAvatar's face render (avatar/main/model.py:170-175 -> MeshRenderer,
+ * avatar/common/nets/layer.py:23-68: pytorch3d's MeshRasterizer with blur_radius 0, faces_per_pixel 1, perspective-
+ * correct barycentrics, no culling or clipping, then TexturesUV), restated from pytorch3d's implementation:
+ *   camera   p_c = R p + t;  u = fx x_c / z_c + cx,  v = fy y_c / z_c + cy;  x_ndc = (W/2 - u) / s, y_ndc = (H/2 - v) / s
+ *            with s = min(H, W) / 2; a corner's z is z_c.
+ *   pixel    (row r, col c) sits at NDC (PixToNonSquareNdc(W-1-c, W, H), PixToNonSquareNdc(H-1-r, H, W)), the point
+ *            u = c + 0.5, v = r + 0.5.
+ *   coverage a face is skipped if max z < 0, |E(v0,v1,v2)| <= 1e-8, or a corner is not finite.  A pixel centre p is
+ *            covered if it lies in the face's closed NDC xy box (pytorch3d's CheckPointOutsideBoundingBox), pz = b.z >= 0
+ *            and all three perspective-corrected barycentrics b are > 0, where
+ *            b0 = (E(p,v1,v2), E(p,v2,v0), E(p,v0,v1)) / (E(v2,v0,v1) + 1e-8),
+ *            b = (b0.x z1 z2, z0 b0.y z2, z0 z1 b0.z) / max(sum, 1e-8),  E(p,a,b) = (p.x-a.x)(b.y-a.y) - (p.y-a.y)(b.x-a.x).
+ *            The covering face of least pz wins, equal pz to the lowest index.
+ *   texture  uv = sum_k b_k (a_k, 1 - b_k) over the corners' vertex_uv rows (a_k, b_k) chosen by face_uv; the texture
+ *            flipped vertically is sampled at grid 2 uv - 1 (bilinear, align_corners, border padding).
+ *   output   image (C,H,W), -1 in every channel where no face covers the pixel; pix_to_face (H*W) int32, -1 there.
+ * The backward gives dL/dmesh only (texture and uv are constants), the derivative of the above with the per-pixel face
+ * held fixed.  All arithmetic is fp32; the per-pixel face is computed exactly as a float32 restatement with no fma. */
+typedef struct B2RMeshRender {
+  int32_t V;                    /* mesh vertices */
+  int32_t F;                    /* faces */
+  int32_t Vt;                   /* rows of vertex_uv */
+  int32_t C;                    /* texture channels, 1..4 */
+  int32_t tex_height, tex_width;
+  int32_t height, width;        /* output size; height * width < 2^31 */
+  const float* mesh;            /* (V,3) world positions */
+  const int32_t* faces;         /* (F,3) vertex indices in [0, V) (a face with an index outside is skipped) */
+  const float* vertex_uv;       /* (Vt,2) */
+  const int32_t* face_uv;       /* (F,3) rows of vertex_uv, every one in [0, Vt) */
+  const float* texture;         /* (C, tex_height, tex_width), row 0 at the top (the map is NOT pre-flipped) */
+  const float* cam_R;           /* (9) row-major, read on the device */
+  const float* cam_t;           /* (3) */
+  const float* focal;           /* (2) fx, fy */
+  const float* princpt;         /* (2) cx, cy */
+  uint64_t* keys;               /* forward: (height * width) per-pixel depth keys, all ~0 on entry and left all ~0 */
+  const int32_t* vf_offsets;    /* backward: the vertex -> face CSR of b2r_vertex_normals over (V, faces) */
+  const int32_t* vf_entries;
+} B2RMeshRender;
+
+/* `scratch` >= b2r_mesh_render_scratch_bytes(F): per-face records the forward writes and the backward reads (keep it
+ * until the backward), plus the backward's per-face gradients.  Forward: writes every element of image (C,H,W) and
+ * pix_to_face (H*W).  Backward: reads the forward's pix_to_face and scratch and dL_dimage (C,H,W), writes every element
+ * of dL_dmesh (V,3) -- the per-face sums walk each face's pixels in raster order and each vertex sums its corners in
+ * CSR order, no float atomics: bit-identical runs.  Neither allocates, syncs or reads device data on the host, so a
+ * captured graph replays with new mesh and camera contents. */
+size_t b2r_mesh_render_scratch_bytes(int32_t F);
+int b2r_mesh_render_forward(const B2RMeshRender* mr, float* image, int32_t* pix_to_face, void* scratch,
+                            size_t scratch_bytes, void* stream);
+int b2r_mesh_render_backward(const B2RMeshRender* mr, const int32_t* pix_to_face, const float* dL_dimage,
+                             float* dL_dmesh, void* scratch, size_t scratch_bytes, void* stream);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows and b2r_vertex_normals kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals and b2r_mesh_render_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
