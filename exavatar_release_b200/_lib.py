@@ -132,6 +132,10 @@ SYMBOLS = [
     ("b2r_backward_project", C.c_int, [C.POINTER(B2RScene), C.POINTER(B2RWorkspace), C.POINTER(B2RBackwardArgs), _fp,
                                        C.c_size_t, _fp]),
     ("b2r_forward_project", C.c_int, [C.POINTER(B2RScene), C.POINTER(B2RWorkspace), _fp, _fp]),
+    ("b2r_split_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_uint64]),
+    ("b2r_forward_project_split", C.c_int, [C.POINTER(B2RScene), C.POINTER(B2RWorkspace), C.c_uint32, _fp, _fp]),
+    ("b2r_forward_bin_split", C.c_int, [C.POINTER(B2RScene), C.POINTER(B2RWorkspace), C.POINTER(B2RWorkspace),
+                                        C.c_uint32, _fp, _fp]),
     ("b2r_forward_render", C.c_int, [C.POINTER(B2RScene), C.POINTER(B2RWorkspace), C.POINTER(B2RForwardOutputs), _fp]),
     ("b2r_forward", C.c_int, [C.POINTER(B2RScene), C.POINTER(B2RWorkspace), C.POINTER(B2RForwardOutputs), _fp]),
     ("b2r_backward", C.c_int, [C.POINTER(B2RScene), C.POINTER(B2RWorkspace), C.POINTER(B2RBackwardArgs), _fp,

@@ -191,6 +191,43 @@ int b2r_forward_bin(const B2RScene* scene, const B2RWorkspace* ws, void* stream)
   return launch_binning(*scene, cx, false, (cudaStream_t)stream);
 }
 
+size_t b2r_split_scratch_bytes(int32_t P, int32_t width, int32_t height, uint64_t dup_capacity) {
+  return split_scratch_bytes(P, width, height, dup_capacity);
+}
+
+int b2r_forward_project_split(const B2RScene* scene, const B2RWorkspace* ws, uint32_t first_row, int32_t* radii,
+                              void* stream) {
+  int rc = validate_scene(scene);
+  if (rc) return rc;
+  rc = validate_ws(scene, ws, false);
+  if (rc) return rc;
+  if ((int64_t)first_row > (int64_t)scene->P) return B2R_E_INVALID;
+  if (ws->dup_capacity == 0) return B2R_E_INVALID;  // the split pass bins with the capacity it was given
+  if (scene->P > 0 && !radii) return B2R_E_INVALID;
+  const Ctx cx = resolve(ws, scene->P, scene->width, scene->height);
+  return launch_project(*scene, cx, radii, (cudaStream_t)stream, (int)first_row);
+}
+
+int b2r_forward_bin_split(const B2RScene* scene, const B2RWorkspace* ws, const B2RWorkspace* base, uint32_t first_row,
+                          int32_t* radii, void* stream) {
+  int rc = validate_scene(scene);
+  if (rc) return rc;
+  rc = validate_ws(scene, ws, true);
+  if (rc) return rc;
+  if ((int64_t)first_row > (int64_t)scene->P) return B2R_E_INVALID;
+  if (ws->dup_capacity == 0 || (scene->P > 0 && !radii)) return B2R_E_INVALID;
+  if (ws->scratch_bytes < split_scratch_bytes(scene->P, scene->width, scene->height, ws->dup_capacity))
+    return B2R_E_WORKSPACE;
+  if (!base || base == ws || !base->ctx || !base->dup_ids) return B2R_E_INVALID;
+  if (base->ctx_bytes < b2r_ctx_bytes(scene->P, scene->width, scene->height)) return B2R_E_WORKSPACE;
+  Ctx cx = resolve(ws, scene->P, scene->width, scene->height);
+  cx.sort_len = (uint32_t*)((char*)ws->ctx + ctx_layout(scene->P, scene->width, scene->height).split_len);
+  const Ctx bx = resolve(base, scene->P, scene->width, scene->height);
+  uint32_t* own_ids = (uint32_t*)((char*)ws->scratch + scratch_layout(scene->P, scene->width, scene->height,
+                                                                      ws->dup_capacity).total);
+  return launch_binning_split(*scene, cx, bx, own_ids, (int)first_row, radii, (cudaStream_t)stream);
+}
+
 int b2r_forward_composite(const B2RScene* scene, const B2RWorkspace* ws, const B2RView* view,
                           const B2RForwardOutputs* out, void* stream) {
   int rc = validate_scene(scene);

@@ -14,8 +14,8 @@
 
 namespace b2r {
 
-__global__ void __launch_bounds__(256) scatter_kernel(const B2RScene sc, const Ctx cx) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__global__ void __launch_bounds__(256) scatter_kernel(const B2RScene sc, const Ctx cx, const int first_row) {
+  const int i = first_row + blockIdx.x * blockDim.x + threadIdx.x;
   int4 aux = make_int4(0, 0, 0, 0);
   float4 g0 = make_float4(0.f, 0.f, 0.f, 0.f), g1 = g0;
   uint32_t depth_bits = 0u;
@@ -52,13 +52,13 @@ __global__ void __launch_bounds__(256) scatter_kernel(const B2RScene sc, const C
 // claims its slots of a tile with ONE global atomic: (1) count the CTA's pairs per tile in shared memory, (2) one
 // atomicAdd per touched tile reserves a contiguous run of the tile's segment, (3) enumerate again and drop each pair
 // at run base + its rank inside the CTA (shared-memory atomic).  Both enumerations replay the projection's kept masks.
-__global__ void __launch_bounds__(256) scatter_agg_kernel(const B2RScene sc, const Ctx cx) {
+__global__ void __launch_bounds__(256) scatter_agg_kernel(const B2RScene sc, const Ctx cx, const int first_row) {
   extern __shared__ uint32_t s_mem[];
   uint32_t* s_cnt = s_mem;              // [tiles] pairs of this CTA per tile, then the running rank
   uint32_t* s_base = s_mem + cx.tiles;  // [tiles] first slot of this CTA's run
   for (int t = threadIdx.x; t < cx.tiles; t += blockDim.x) s_cnt[t] = 0u;
   __syncthreads();
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int i = first_row + blockIdx.x * blockDim.x + threadIdx.x;
   int4 aux = make_int4(0, 0, 0, 0);
   float4 g0 = make_float4(0.f, 0.f, 0.f, 0.f), g1 = g0;
   uint32_t depth_bits = 0u;
@@ -466,14 +466,14 @@ __global__ void __launch_bounds__(THREADS) sort_mixed_kernel(const Ctx cx) {
       const uint32_t tile = cx.tile_order[lo];
       const uint2 r = cx.ranges[tile];
       const int off = (b - (int)cx.chunk_start[lo]) * SORT_CHUNK;
-      const int len = min(SORT_CHUNK, (int)(r.y - r.x) - off);
+      const int len = min(SORT_CHUNK, sort_length(cx, (int)tile, r) - off);
       if (len > 1) radix_sort_tile<CAP, THREADS, true>(cx.keys + r.x + off, nullptr, len, smem_raw, cx.tile_maxid + tile);
       else if (len == 1 && threadIdx.x == 0) atomicMax(cx.tile_maxid + tile, cx.keys[r.x + off].y);
       last_n = len;
     } else if (b < n_chunks + n_cta) {
       const uint32_t tile = cx.tile_order[n_large + (b - n_chunks)];
       const uint2 r = cx.ranges[tile];
-      const int n = (int)(r.y - r.x);  // < 2048; can be below 512 when the duplicate capacity clamped the range
+      const int n = sort_length(cx, (int)tile, r);  // < 2048; can be below 512 when the duplicate capacity clamped the range
       const uint2* src = cx.keys + r.x;
       uint32_t* dst = cx.dup_ids + r.x;
       if (n > 32) {
@@ -489,9 +489,9 @@ __global__ void __launch_bounds__(THREADS) sort_mixed_kernel(const Ctx cx) {
       if (t < cx.tiles) {
         const uint32_t tile = cx.tile_order[t];
         const uint2 r = cx.ranges[tile];
-        last_n = -(int)(r.y - r.x);
-        warp_sort_tile(cx.keys + r.x, cx.dup_ids + r.x, (int)(r.y - r.x), smem_raw + (size_t)warp * WSORT_BYTES,
-                       cx.tile_maxid + tile);
+        const int n = sort_length(cx, (int)tile, r);
+        last_n = -n;
+        warp_sort_tile(cx.keys + r.x, cx.dup_ids + r.x, n, smem_raw + (size_t)warp * WSORT_BYTES, cx.tile_maxid + tile);
       }
     }
   }
@@ -526,12 +526,13 @@ __global__ void __launch_bounds__(256) merge_chunks_kernel(const Ctx cx) {
       const int cs = mid < n_tab ? (int)table[mid] : (int)cx.chunk_start[mid];
       if (cs <= b) lo = mid; else hi = mid - 1;
     }
-    const uint2 r = cx.ranges[cx.tile_order[lo]];
-    const int n = (int)(r.y - r.x);
+    const uint32_t tile = cx.tile_order[lo];
+    const uint2 r = cx.ranges[tile];
+    const int n = sort_length(cx, (int)tile, r);
     const int c = b - (int)(lo < n_tab ? table[lo] : cx.chunk_start[lo]);
     const uint2* pairs = cx.keys + r.x;
     const int chunks = (n + SORT_CHUNK - 1) / SORT_CHUNK;
-    const int len = min(SORT_CHUNK, n - c * SORT_CHUNK);  // entries of my chunk (<= 0 only if the table were inconsistent)
+    const int len = min(SORT_CHUNK, n - c * SORT_CHUNK);  // entries of my chunk (<= 0: past a split pass's own entries)
     unsigned long long key[PER];
     uint32_t id[PER];
     int rank[PER];
@@ -589,6 +590,7 @@ __global__ void __launch_bounds__(256) merge_chunks_kernel(const Ctx cx) {
 }
 
 constexpr int SORT_SMALL = SORT_CHUNK;  // capacity of the CTA-wide sort = chunk size of the long lists
+void launch_sort(const Ctx& cx, cudaStream_t st);
 
 int launch_binning(const B2RScene& sc, const Ctx& cx, bool rescan, cudaStream_t st) {
   // the two-phase entry re-derives ranges and cursors for the capacity the caller finally chose
@@ -606,11 +608,16 @@ int launch_binning(const B2RScene& sc, const Ctx& cx, bool rescan, cudaStream_t 
     // the direct atomics save)
     if (cx.tiles <= 2048) {
       cudaFuncSetAttribute(scatter_agg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-      launch_k(scatter_agg_kernel, (sc.P + 255) / 256, 256, smem, st, true, sc, cx);
+      launch_k(scatter_agg_kernel, (sc.P + 255) / 256, 256, smem, st, true, sc, cx, 0);
     } else {
-      launch_k(scatter_kernel, (sc.P + 255) / 256, 256, 0, st, true, sc, cx);
+      launch_k(scatter_kernel, (sc.P + 255) / 256, 256, 0, st, true, sc, cx, 0);
     }
   }
+  launch_sort(cx, st);
+  return check_launch();
+}
+
+void launch_sort(const Ctx& cx, cudaStream_t st) {
   const int sms = device_sm_count();
   constexpr int ST = 256;
   constexpr size_t cta_bytes = RadixSmem<SORT_SMALL, ST>::bytes, warp_bytes = (ST / 32) * WSORT_BYTES;
@@ -624,6 +631,154 @@ int launch_binning(const B2RScene& sc, const Ctx& cx, bool rescan, cudaStream_t 
   {
     ProfScope p(K_SORT_LARGE, st);
     launch_k(merge_chunks_kernel, 2 * sms, 256, 0, st, true, cx);  // strides over the chunks; surplus CTAs exit at once
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Split pass (b2r_forward_project_split / b2r_forward_bin_split).  Rows [0, split) of this pass are the rows [0, split) of
+// a BASE pass that projected and binned them with the same camera and inputs (ExAvatar: the scene Gaussians of
+// cat(scene, human) and of cat(scene, human_refined)), so their records, their tile pairs and their depth order are the
+// base pass's.  This pass projects, scatters and sorts only its own rows [split, P), and only tiles its own rows reach get
+// a list: the base list of the tile filtered to ids < split (filtering keeps the order) merged with the own sorted
+// entries on the unique 64-bit (depth_bits, id) key -- the order the joint sort gives, entry for entry.  Other tiles get
+// empty lists (tile_maxid 0).
+// ---------------------------------------------------------------------------------------------------------------
+
+// Copies the base pass's records and radii of rows [0, split) (a view gathers them) and turns every tile count of the own
+// rows into the length of the merged list: own entries + base entries with id < split.  sort_len keeps the own count.
+__global__ void __launch_bounds__(256) split_prepare_kernel(const Ctx cx, const Ctx base, const int split,
+                                                            int32_t* __restrict__ radii) {
+  const int tid = threadIdx.x;
+  const float4* gsrc = reinterpret_cast<const float4*>(base.geom);
+  float4* gdst = reinterpret_cast<float4*>(cx.geom);
+  for (size_t k = (size_t)blockIdx.x * 256 + tid; k < (size_t)split * 3; k += (size_t)gridDim.x * 256) gdst[k] = gsrc[k];
+  for (int k = blockIdx.x * 256 + tid; k < split; k += gridDim.x * 256) radii[k] = base.aux[k].z;
+  for (int t = blockIdx.x; t < cx.tiles; t += gridDim.x) {
+    const uint32_t own = cx.tile_count[t];  // CTA-uniform
+    uint32_t s = 0;
+    if (own) {
+      const uint2 rb = base.ranges[t];
+      for (uint32_t k = rb.x; k < rb.y; k += 256)
+        s += (uint32_t)__syncthreads_count(k + tid < rb.y && base.dup_ids[k + tid] < (uint32_t)split);
+    }
+    if (tid == 0) {
+      cx.sort_len[t] = own;
+      cx.tile_count[t] = own + s;
+    }
+    __syncthreads();
+  }
+}
+
+// One CTA per tile of tile_order (the tiles with a list come first).  The own sorted ids and the filtered base list are
+// written as (depth_bits, id) keys into the tile's key range -- own entries first, then base entries -- and every entry
+// goes to its position in the merged order: its index in its own sequence plus the number of entries of the other
+// sequence below it (binary searches in shared-memory chunks of the other sequence).
+constexpr int SPLIT_CHUNK = 2048;
+constexpr int SPLIT_PER = 8;  // entries per thread and round
+__global__ void __launch_bounds__(256) split_merge_kernel(const Ctx cx, const Ctx base, const uint32_t* __restrict__ own_ids,
+                                                          const int split) {
+  __shared__ uint2 other[SPLIT_CHUNK];
+  __shared__ uint32_t wtot[8];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t tile = cx.tile_order[blockIdx.x];
+  const uint2 r = cx.ranges[tile];
+  const int n = (int)(r.y - r.x);
+  if (n == 0) return;
+  const int n_own = sort_length(cx, (int)tile, r);
+  uint2* keys = cx.keys + r.x;
+  for (int i = tid; i < n_own; i += 256) {
+    const uint32_t id = own_ids[r.x + i];
+    keys[i] = make_uint2(__float_as_uint(cx.geom[id].g1.z), id);
+  }
+  // ordered compaction of the base list's entries below the split behind the own entries (guarded: with an overflowed
+  // capacity the range can be shorter than both sequences)
+  const uint2 rb = base.ranges[tile];
+  int n_base = 0;
+  for (uint32_t k0 = rb.x; k0 < rb.y; k0 += 256) {
+    const uint32_t k = k0 + tid;
+    const uint32_t id = k < rb.y ? base.dup_ids[k] : 0xffffffffu;
+    const bool take = id < (uint32_t)split;
+    const unsigned b = __ballot_sync(0xffffffffu, take);
+    if (lane == 0) wtot[warp] = __popc(b);
+    __syncthreads();
+    int off = n_base, tot = 0;
+    for (int w = 0; w < 8; w++) {
+      off += w < warp ? (int)wtot[w] : 0;
+      tot += (int)wtot[w];
+    }
+    off += __popc(b & ((1u << lane) - 1u));
+    if (take && n_own + off < n) keys[n_own + off] = make_uint2(__float_as_uint(cx.geom[id].g1.z), id);
+    n_base += tot;
+    __syncthreads();  // wtot is rewritten by the next round
+  }
+  __syncthreads();  // the keys above are visible to the whole CTA
+  if (n_own + n_base != n) {  // capacity overflow (reported in B2RStatus): keep every entry a valid id, order is moot
+    for (int i = tid; i < n; i += 256) cx.dup_ids[r.x + i] = keys[i].y;
+    return;
+  }
+  for (int side = 0; side < 2; side++) {  // 0: own entries against the base sequence, 1: the other way round
+    const uint2* mine = side ? keys + n_own : keys;
+    const uint2* oth = side ? keys : keys + n_own;
+    const int n_mine = side ? n_base : n_own, n_oth = side ? n_own : n_base;
+    for (int x0 = 0; x0 < n_mine; x0 += 256 * SPLIT_PER) {  // CTA-uniform
+      unsigned long long key[SPLIT_PER];
+      int rank[SPLIT_PER];
+#pragma unroll
+      for (int j = 0; j < SPLIT_PER; j++) {
+        const int i = x0 + j * 256 + tid;
+        const uint2 v = i < n_mine ? mine[i] : make_uint2(0u, 0u);
+        key[j] = ((unsigned long long)v.x << 32) | v.y;
+        rank[j] = i;
+      }
+      for (int c0 = 0; c0 < n_oth; c0 += SPLIT_CHUNK) {
+        const int len2 = min(SPLIT_CHUNK, n_oth - c0);
+        __syncthreads();  // the previous chunk's searches are done
+        for (int i = tid; i < len2; i += 256) other[i] = oth[c0 + i];
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < SPLIT_PER; j++) {
+          int l = 0;  // entries of the chunk below key
+          for (int step = SPLIT_CHUNK; step >= 1; step >>= 1) {
+            const int probe = l + step;
+            if (probe <= len2) {
+              const uint2 v = other[probe - 1];
+              if ((((unsigned long long)v.x << 32) | v.y) < key[j]) l = probe;
+            }
+          }
+          rank[j] += l;
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < SPLIT_PER; j++)
+        if (x0 + j * 256 + tid < n_mine) cx.dup_ids[r.x + rank[j]] = (uint32_t)(key[j] & 0xffffffffull);
+    }
+  }
+}
+
+int launch_binning_split(const B2RScene& sc, const Ctx& cx_in, const Ctx& base, uint32_t* own_ids, const int first_row,
+                         int32_t* radii, cudaStream_t st) {
+  const Ctx& cx = cx_in;
+  {
+    ProfScope p(K_MISC, st);
+    launch_k(split_prepare_kernel, cx.tiles, 256, 0, st, true, cx, base, first_row, radii);
+  }
+  launch_tile_scan(cx, st, cx.dup_capacity > 0 ? 1 : 0);
+  if (sc.P > first_row) {
+    ProfScope p(K_SCATTER, st);
+    const unsigned grid = (unsigned)((sc.P - first_row + 255) / 256);
+    if (cx.tiles <= 2048) {
+      cudaFuncSetAttribute(scatter_agg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+      launch_k(scatter_agg_kernel, grid, 256, (size_t)cx.tiles * 8, st, true, sc, cx, first_row);
+    } else {
+      launch_k(scatter_kernel, grid, 256, 0, st, true, sc, cx, first_row);
+    }
+  }
+  Ctx own = cx;  // the own entries are sorted into the scratch; the merge writes the lists
+  own.dup_ids = own_ids;
+  launch_sort(own, st);
+  {
+    ProfScope p(K_SORT_LARGE, st);
+    launch_k(split_merge_kernel, cx.tiles, 256, 0, st, true, cx, base, own_ids, first_row);
   }
   return check_launch();
 }

@@ -64,7 +64,7 @@ static_assert(sizeof(Geom) == 48, "Geom must be 48 bytes");
 
 struct CtxLayout {
   size_t status, geom, aux, ranges, tile_count, tile_cursor, tile_order, chunk_start, seg_start, classes, tile_maxid,
-      final_T, n_contrib, total;
+      split_len, final_T, n_contrib, total;
   int gx, gy, tiles;
 };
 __host__ __device__ inline CtxLayout ctx_layout(int P, int W, int H) {
@@ -85,6 +85,7 @@ __host__ __device__ inline CtxLayout ctx_layout(int P, int W, int H) {
   L.seg_start = o; o += align_up((size_t)L.tiles * 4);
   L.classes = o; o += align_up((size_t)CLS_COUNT * 4);
   L.tile_maxid = o; o += align_up((size_t)L.tiles * 4);
+  L.split_len = o; o += align_up((size_t)L.tiles * 4);
   L.final_T = o; o += align_up(N * 4);
   L.n_contrib = o; o += align_up(N * 4);
   L.total = o;
@@ -101,6 +102,10 @@ __host__ __device__ inline ScratchLayout scratch_layout(int P, int W, int H, uin
   S.keys = o; o += align_up((size_t)(cap > 0 ? cap : 1) * 8);
   S.total = o;
   return S;
+}
+// a split pass (b2r_forward_bin_split) also keeps the sorted ids of its own rows in the scratch, behind the keys
+__host__ __device__ inline size_t split_scratch_bytes(int P, int W, int H, uint64_t cap) {
+  return scratch_layout(P, W, H, cap).total + align_up((size_t)(cap > 0 ? cap : 1) * 4);
 }
 
 // Resolved device pointers of one context.
@@ -132,7 +137,15 @@ struct Ctx {
   const float* bg;
   uint32_t* tile_maxid;  // per tile: largest Gaussian index in its list (written by the per-tile sort)
   uint32_t skip_below;   // != 0: the composites skip tiles whose tile_maxid < skip_below (B2RView.skip_below)
+  // split pass only (b2r_forward_bin_split), else null: per tile, how many entries of its range the per-tile sort covers
+  // (the pass's own rows; the rest of the range is filled by the merge with the base pass's list)
+  uint32_t* sort_len;
 };
+// entries of the tile's range the per-tile sort orders
+__device__ __forceinline__ int sort_length(const Ctx& cx, int tile, uint2 r) {
+  const int n = (int)(r.y - r.x);
+  return cx.sort_len ? min(n, (int)cx.sort_len[tile]) : n;
+}
 
 // capacity of the segment table / checkpoint store for a given duplicate capacity
 __host__ __device__ inline uint32_t max_segments(int tiles, uint64_t cap) { return (uint32_t)(cap / SEG) + (uint32_t)tiles; }
@@ -175,6 +188,7 @@ inline Ctx resolve(const B2RWorkspace* ws, int P, int W, int H) {
   x.bg = nullptr;
   x.tile_maxid = (uint32_t*)(c + L.tile_maxid);
   x.skip_below = 0;
+  x.sort_len = nullptr;
   return x;
 }
 
@@ -483,9 +497,11 @@ __device__ __forceinline__ void stage_rows(float* __restrict__ wstage, float* __
 }
 
 // launch wrappers (one per translation unit)
-int launch_project(const B2RScene& sc, const Ctx& cx, int32_t* radii, cudaStream_t st);
+int launch_project(const B2RScene& sc, const Ctx& cx, int32_t* radii, cudaStream_t st, int first_row = 0);
 int launch_binning(const B2RScene& sc, const Ctx& cx, bool rescan, cudaStream_t st);
-void launch_tile_scan(const Ctx& cx, cudaStream_t st);
+int launch_binning_split(const B2RScene& sc, const Ctx& cx, const Ctx& base, uint32_t* own_ids, int first_row,
+                         int32_t* radii, cudaStream_t st);
+void launch_tile_scan(const Ctx& cx, cudaStream_t st, int final = 2);  // final: see tile_scan_kernel
 int launch_composite_fwd(const B2RScene& sc, const Ctx& cx, const B2RForwardOutputs& out, cudaStream_t st);
 int launch_composite_bwd(const B2RScene& sc, const Ctx& cx, const B2RBackwardArgs& a, float* gacc, cudaStream_t st);
 

@@ -54,7 +54,7 @@ __device__ __forceinline__ void sh_to_rgb(int deg, const float* __restrict__ sh,
 // separate instantiation, so the single-source kernel stays the code it was.
 template <bool MIXED>
 __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2RScene sc, const Ctx cx, int32_t* __restrict__ radii,
-                                                      const int aggregate) {
+                                                      const int aggregate, const int first_row) {
   // CTA-level histogram in shared memory: atomics of different warps to the SAME global address serialise in L2
   // (the hot avatar tiles receive thousands), so each CTA adds to a tile's counter at most once.
   extern __shared__ uint32_t s_cnt[];
@@ -62,7 +62,7 @@ __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2R
     for (int t = threadIdx.x; t < cx.tiles; t += blockDim.x) s_cnt[t] = 0u;
     __syncthreads();
   }
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int i = first_row + blockIdx.x * blockDim.x + threadIdx.x;  // first_row > 0: a split pass (rows [first_row, P))
   // SH rows (192 bytes apart for degree 3) are staged through shared memory: each warp copies the contiguous block of
   // its 32 rows with coalesced 128-byte loads; a thread then reads its own row (odd row stride: conflict-free).  In a
   // mixed scene a warp stages only its rows below sh_rows (none at all past them).
@@ -71,7 +71,7 @@ __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2R
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int L = sc.sh_coeffs * 3, S = L | 1;
     float* wstage = reinterpret_cast<float*>(s_cnt + (aggregate ? cx.tiles : 0)) + (size_t)warp * 32 * S;
-    const int row0 = blockIdx.x * blockDim.x + warp * 32;
+    const int row0 = first_row + blockIdx.x * blockDim.x + warp * 32;
     const int nrows = min(32, (MIXED ? sc.sh_rows : sc.P) - row0);
     if (nrows > 0) stage_rows<0>(wstage, const_cast<float*>(sc.shs) + (size_t)row0 * L, L, nrows, 0xffffffffu);
     __syncwarp();
@@ -85,7 +85,7 @@ __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2R
     float* base = reinterpret_cast<float*>(s_cnt + (aggregate ? cx.tiles : 0));
     if (sc.shs) base += (size_t)8 * 32 * ((sc.sh_coeffs * 3) | 1);
     float* wstage = base + (size_t)warp * 32 * S;
-    const int row0 = blockIdx.x * blockDim.x + warp * 32;
+    const int row0 = first_row + blockIdx.x * blockDim.x + warp * 32;
     const int nrows = min(32, sc.P - row0);
     if (nrows > 0) stage_rows<0>(wstage, const_cast<float*>(sc.skin_weights) + (size_t)row0 * J, J, nrows, 0xffffffffu);
     __syncwarp();
@@ -399,10 +399,12 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D, co
   present[i] = vz > K_NEAR ? 1 : 0;
 }
 
-int launch_project(const B2RScene& sc, const Ctx& cx, int32_t* radii, cudaStream_t st) {
+// first_row > 0 (b2r_forward_project_split): rows [first_row, P) only, and no scan -- b2r_forward_bin_split runs it once
+// the counts of the base pass's rows are added
+int launch_project(const B2RScene& sc, const Ctx& cx, int32_t* radii, cudaStream_t st, int first_row) {
   const bool clean = (sc.flags & B2R_FLAG_CTX_CLEAN) != 0;  // the previous render's final scan left the counters zero
   if (!clean) { ProfScope p(K_MISC, st); launch_k(status_reset_kernel, (cx.tiles + 1023) / 1024, 1024, 0, st, true, cx); }
-  if (sc.P > 0) {
+  if (sc.P > first_row) {
     ProfScope p(K_PROJECT, st);
     const int aggregate = cx.tiles <= 2048;  // beyond that the per-CTA sweeps over the tile table cost more than they save
     const size_t smem = (aggregate ? (size_t)cx.tiles * 4 : 0) +
@@ -410,15 +412,18 @@ int launch_project(const B2RScene& sc, const Ctx& cx, int32_t* radii, cudaStream
                         (sc.skin_xyz ? (size_t)8 * 32 * (sc.skin_J | 1) * sizeof(float) : 0);
     auto kern = sc.sh_rows > 0 ? project_kernel<true> : project_kernel<false>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);  // per device
-    launch_k(kern, (sc.P + 255) / 256, 256, smem, st, true, sc, cx, radii, aggregate);
+    launch_k(kern, (sc.P - first_row + 255) / 256, 256, smem, st, true, sc, cx, radii, aggregate, first_row);
   }
-  { ProfScope p(K_TILE_SCAN, st); launch_k(tile_scan_kernel, 1, 1024, 0, st, true, cx, cx.dup_capacity > 0 ? 1 : 0); }
+  if (first_row == 0) {
+    ProfScope p(K_TILE_SCAN, st);
+    launch_k(tile_scan_kernel, 1, 1024, 0, st, true, cx, cx.dup_capacity > 0 ? 1 : 0);
+  }
   return check_launch();
 }
 
-void launch_tile_scan(const Ctx& cx, cudaStream_t st) {
+void launch_tile_scan(const Ctx& cx, cudaStream_t st, int final) {
   ProfScope p(K_TILE_SCAN, st);
-  launch_k(tile_scan_kernel, 1, 1024, 0, st, true, cx, 2);
+  launch_k(tile_scan_kernel, 1, 1024, 0, st, true, cx, final);
 }
 
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t st) {

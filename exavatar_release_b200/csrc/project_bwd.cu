@@ -293,7 +293,8 @@ template <bool MIXED>
 __global__ void __launch_bounds__(256, PBWD_MIN_BLOCKS) project_bwd_kernel(const B2RScene sc, const Ctx cx, const B2RBackwardArgs out,
                                                           const float* __restrict__ gacc) {
   extern __shared__ float sh_stage[];
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int blk = blockIdx.x + (int)out.first_row / 256;  // no CTA for a block of rows wholly inside the detached prefix
+  const int i = blk * blockDim.x + threadIdx.x;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const bool in_range = i < sc.P;
   const bool accumulate = (out.flags & B2R_BWD_ACCUMULATE) != 0;
@@ -308,7 +309,7 @@ __global__ void __launch_bounds__(256, PBWD_MIN_BLOCKS) project_bwd_kernel(const
   const bool use_sh = sc.shs != nullptr && out.dL_dshs != nullptr;
   const int L = sc.sh_coeffs * 3, S = L | 1;
   float* wstage = sh_stage + (size_t)warp * 32 * S;
-  const int row0 = blockIdx.x * blockDim.x + warp * 32;
+  const int row0 = blk * blockDim.x + warp * 32;
   const int nrows = min(32, sc.P - row0);
   const int sh_nrows = MIXED ? min(32, sc.sh_rows - row0) : nrows;  // this warp's SH rows
   if (use_sh && sh_nrows > 0) {
@@ -340,14 +341,15 @@ __global__ void __launch_bounds__(256, PBWD_MIN_BLOCKS) project_bwd_kernel(const
 }
 
 int launch_project_bwd(const B2RScene& sc, const Ctx& cx, const B2RBackwardArgs& a, const float* gacc, cudaStream_t st) {
-  ProfScope p(K_PROJECT_BWD, st, sc.P > 0 ? 1 : 0);
-  if (sc.P > 0) {
+  const int grid = (sc.P + 255) / 256 - (int)a.first_row / 256;
+  ProfScope p(K_PROJECT_BWD, st, grid > 0 ? 1 : 0);
+  if (grid > 0) {
     const bool use_sh = sc.shs != nullptr && a.dL_dshs != nullptr;
     const size_t smem = (use_sh ? (size_t)8 * 32 * ((sc.sh_coeffs * 3) | 1) * sizeof(float) : 0) +
                         (sc.skin_xyz ? (size_t)8 * 32 * (sc.skin_J | 1) * sizeof(float) : 0);
     auto kern = sc.sh_rows > 0 ? project_bwd_kernel<true> : project_bwd_kernel<false>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024);  // per device
-    launch_k(kern, (sc.P + 255) / 256, 256, smem, st, true, sc, cx, a, gacc);
+    launch_k(kern, grid, 256, smem, st, true, sc, cx, a, gacc);
   }
   return check_launch();
 }

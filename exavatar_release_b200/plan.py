@@ -27,7 +27,8 @@ class _Workspace:
     B2RWorkspace pointing at them: ctx (status block first), duplicate ids, forward scratch, backward scratch and,
     with `checkpoints`, the forward composite's segment table + blend-state checkpoints."""
 
-    def __init__(self, P: int, width: int, height: int, dup_capacity: int, device, checkpoints: bool = True):
+    def __init__(self, P: int, width: int, height: int, dup_capacity: int, device, checkpoints: bool = True,
+                 split: bool = False):
         self.lib = L.load()
         self.P, self.W, self.H = int(P), int(width), int(height)
         self.device = dev = torch.device(device)
@@ -36,7 +37,9 @@ class _Workspace:
         self.ctx_bytes = self.lib.b2r_ctx_bytes(P, width, height)
         self.ctx_buf = torch.empty(self.ctx_bytes, dtype=torch.uint8, device=dev)
         self.ids = torch.empty(max(self.capacity, 1), dtype=torch.int32, device=dev)
-        self.scratch_bytes = self.lib.b2r_scratch_bytes(P, width, height, self.capacity)
+        # a split pass (b2r_forward_bin_split) keeps the sorted ids of its own rows behind the keys
+        nbytes = self.lib.b2r_split_scratch_bytes if split else self.lib.b2r_scratch_bytes
+        self.scratch_bytes = nbytes(P, width, height, self.capacity)
         self.scratch = torch.empty(self.scratch_bytes, dtype=torch.uint8, device=dev)
         self.bwd_bytes = self.lib.b2r_backward_scratch_bytes(P)
         # zero once: every backward leaves it zero again (B2R_BWD_SCRATCH_ZEROED), so no memset node per render
@@ -314,8 +317,8 @@ class FiveRenderPlan:
 class _Pass(_Workspace):
     """One projection + binning of cat(scene, X) and the views composited from it (MergedFivePlan)."""
 
-    def __init__(self, P, W, H, cap, n_views, device):
-        super().__init__(P, W, H, cap, device)
+    def __init__(self, P, W, H, cap, n_views, device, split=False):
+        super().__init__(P, W, H, cap, device, split=split)
         dev = self.device
         # every view keeps its own checkpoints for its backward; the workspace points at the first view's
         self.ck = [self.ckpt] + [torch.empty_like(self.ckpt) for _ in range(n_views - 1)]
@@ -380,6 +383,10 @@ class MergedFivePlan:
     PER = FiveRenderPlan.PER
     VIEWS = {"A": ("scene", "human", "scene_human"), "B": ("human_refined", "scene_human_refined")}
     SKIP = os.environ.get("B2R_SKIP_TILES", "1") != "0"  # A/B switch of the skipped human-free tiles
+    # Pass B projects, bins and sorts only the refined rows and takes the scene entries of its lists from pass A (the
+    # split pass of the C ABI); its views need the skipped tiles for that.  B2R_REFINED_PASS=full: the whole
+    # cat(scene, refined) again (A/B switch for measurements).
+    SPLIT = SKIP and os.environ.get("B2R_REFINED_PASS", "split") != "full"
 
     def __init__(self, P_scene: int, P_human: int, width: int, height: int, caps: Optional[Dict[str, int]], device,
                  sh_coeffs: int = 0):
@@ -389,7 +396,8 @@ class MergedFivePlan:
         self.M = int(sh_coeffs)
         self.device = torch.device(device)
         caps = caps or {"A": 8_000_000, "B": 8_000_000}
-        self.passes = {k: _Pass(self.P, self.W, self.H, caps[k], len(v), self.device) for k, v in self.VIEWS.items()}
+        self.passes = {k: _Pass(self.P, self.W, self.H, caps[k], len(v), self.device, split=(k == "B" and self.SPLIT))
+                       for k, v in self.VIEWS.items()}
         self.pass_streams = {k: torch.cuda.Stream(self.device) for k in self.passes}
         # one flat gradient buffer: [pass A: scene rows | human rows][scene dL/dSH][pass B: refined rows][stats]
         lay = merged_bucket_layout(self.Ps, self.Ph, self.M)
@@ -476,10 +484,11 @@ class MergedFivePlan:
         return L.B2RView(lo, hi, _ptr(bg), fT.data_ptr(), nc.data_ptr(), ps.ck[v].data_ptr(), ps.ckpt_bytes, skip, 0)
 
     # ---- the steps of a frame; each enqueues on the stream `s` it is given, which is also the current stream ----
-    def _start_pass(self, s, pk, key, settings, src, bg_h) -> None:
+    def _start_pass(self, s, pk, key, settings, src, bg_h, a_binned) -> None:
         """Copies the rows of `src` (the human or refined set) behind the scene prefix of the pass -- src None: the
-        caller already wrote them -- then projects and bins it.  Its descriptor and views stay in `_current[pk]` until
-        the next frame."""
+        caller already wrote them -- then projects and bins it.  Pass A records `a_binned` once its lists exist; a split
+        pass B projects its refined rows, waits for it and merges the scene entries of pass A's lists into its own.  Its
+        descriptor and views stay in `_current[pk]` until the next frame."""
         ps = self.passes[pk]
         if src is not None:
             for k, buf in ps.cat.items():
@@ -487,9 +496,18 @@ class MergedFivePlan:
         sc = self._scene_desc((key, pk), ps, settings)
         sc.flags = L.B2R_FLAG_CTX_CLEAN if ps.primed else 0  # every pass leaves its ctx counters zero
         ps.primed = True
-        L.check(self.lib.b2r_forward_project(C.byref(sc), C.byref(ps.ws), ps.radii.data_ptr(), s.cuda_stream),
-                "b2r_forward_project")
-        L.check(self.lib.b2r_forward_bin(C.byref(sc), C.byref(ps.ws), s.cuda_stream), "b2r_forward_bin")
+        if pk == "B" and self.SPLIT:
+            L.check(self.lib.b2r_forward_project_split(C.byref(sc), C.byref(ps.ws), self.Ps, ps.radii.data_ptr(),
+                                                       s.cuda_stream), "b2r_forward_project_split")
+            s.wait_event(a_binned)
+            L.check(self.lib.b2r_forward_bin_split(C.byref(sc), C.byref(ps.ws), C.byref(self.passes["A"].ws), self.Ps,
+                                                   ps.radii.data_ptr(), s.cuda_stream), "b2r_forward_bin_split")
+        else:
+            L.check(self.lib.b2r_forward_project(C.byref(sc), C.byref(ps.ws), ps.radii.data_ptr(), s.cuda_stream),
+                    "b2r_forward_project")
+            L.check(self.lib.b2r_forward_bin(C.byref(sc), C.byref(ps.ws), s.cuda_stream), "b2r_forward_bin")
+            if pk == "A":
+                a_binned.record(s)
         views = [self._view(ps, v, n, bg_h if n in ("human", "human_refined") else None)
                  for v, n in enumerate(self.VIEWS[pk])]
         self._current[pk] = (sc, views)
@@ -550,14 +568,14 @@ class MergedFivePlan:
         probe = probe if (probe is not None and serial) else (lambda label: None)
         cur = torch.cuda.current_stream(self.device)
         bg_h = self._human_bg(settings_human_bg)
-        scene_done = torch.cuda.Event()
+        scene_done, a_binned = torch.cuda.Event(), torch.cuda.Event()
         for pk, names in self.VIEWS.items():
             ps = self.passes[pk]
             st = cur if serial else self.pass_streams[pk]
             if not serial:
                 st.wait_stream(cur)
             with torch.cuda.stream(st):
-                self._start_pass(st, pk, key, settings, human if pk == "A" else refined, bg_h)
+                self._start_pass(st, pk, key, settings, human if pk == "A" else refined, bg_h, a_binned)
                 probe(f"{pk}:bin")
                 for v, n in enumerate(names):
                     vs = st if serial else ps.streams[v]
@@ -584,14 +602,14 @@ class MergedFivePlan:
         already wrote the human / refined rows into `passes[*].cat` (a captured graph keeps the copies outside)."""
         cur = torch.cuda.current_stream(self.device)
         bg_h = self._human_bg(settings_human_bg)
-        scene_done = torch.cuda.Event()
+        scene_done, a_binned = torch.cuda.Event(), torch.cuda.Event()
         for pk, names in self.VIEWS.items():
             ps = self.passes[pk]
             st = self.pass_streams[pk]
             st.wait_stream(cur)
             with torch.cuda.stream(st):
                 src = (human if pk == "A" else refined) if copy_inputs else None
-                self._start_pass(st, pk, key, settings, src, bg_h)
+                self._start_pass(st, pk, key, settings, src, bg_h, a_binned)
                 for v in range(len(names)):
                     vs = ps.streams[v]
                     vs.wait_stream(st)

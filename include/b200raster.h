@@ -171,7 +171,9 @@ typedef struct B2RBackwardArgs {
   uint32_t first_row;   /* Gaussians [0, first_row) are a DETACHED PREFIX: no gradient is written for them and Gaussian i
                            goes to row i - first_row of every output (outputs then have P - first_row rows).  This is
                            ExAvatar's "scene + human" render, cat(scene.detach(), human) (avatar/main/model.py:117-125):
-                           the human part of the gradient lands directly in the human bucket.  0 = off. */
+                           the human part of the gradient lands directly in the human bucket.  0 = off.  The backward
+                           projection does not visit whole 256-row blocks below first_row, so (B2R_BWD_SCRATCH_ZEROED)
+                           the views composited into its scratch must not accumulate there: their first_row >= this one. */
   /* Optional fused densification bookkeeping (SURVEY section 8f-1), each (P) or NULL, updated IN PLACE for Gaussians
    * with radii > 0 exactly as ExAvatar does after backward (avatar/common/nets/module.py:155-157,
    * avatar/main/model.py:283-285):  grad_accum += ||dL/dmeans2D.xy||,  count += 1,  radius_max = max(radius_max, radii). */
@@ -265,6 +267,26 @@ int b2r_backward_composite(const B2RScene* scene, const B2RWorkspace* ws, const 
                            void* bwd_scratch, size_t bwd_scratch_bytes, void* stream);
 int b2r_backward_project(const B2RScene* scene, const B2RWorkspace* ws, const B2RBackwardArgs* args, void* bwd_scratch,
                          size_t bwd_scratch_bytes, void* stream);
+
+/* Split pass (ABI v3 addition).  Two passes that share the rows [0, first_row) -- same inputs, same camera -- need not
+ * project, bin and sort them twice.  ExAvatar's merged frame bins cat(scene, human) (the BASE pass) and
+ * cat(scene, human_refined); the second pass then covers its own rows [first_row, P) only:
+ *   b2r_forward_project_split  projects rows [first_row, P) (radii, records, tile counts of those rows); no scan yet.
+ *   b2r_forward_bin_split      after the base pass's b2r_forward_bin (stream order is the caller's): copies the base's
+ *                              records and radii of rows [0, first_row) into this pass (a view gathers them; their aux
+ *                              rows are not copied and never read), then builds a list ONLY in the tiles the own rows
+ *                              reach -- the base list of the tile filtered to ids < first_row, merged with the own rows'
+ *                              sorted entries on the (depth, id) key: entry for entry the list the whole pass would have
+ *                              built there.  Every other tile gets an empty list, so a view of this pass must skip the
+ *                              tiles without own rows (B2RView.skip_below >= first_row).  B2RStatus.num_dups counts the
+ *                              entries of these lists; `ws` needs a capacity and scratch >= b2r_split_scratch_bytes().
+ * Ids keep the numbering of the whole scene.  `base` must be a workspace of the same P, width and height whose lists
+ * stay unchanged until this call's work has run.  The composites and the backward stages take the pass as usual. */
+size_t b2r_split_scratch_bytes(int32_t P, int32_t width, int32_t height, uint64_t dup_capacity);
+int b2r_forward_project_split(const B2RScene* scene, const B2RWorkspace* ws, uint32_t first_row, int32_t* radii,
+                              void* stream);
+int b2r_forward_bin_split(const B2RScene* scene, const B2RWorkspace* ws, const B2RWorkspace* base, uint32_t first_row,
+                          int32_t* radii, void* stream);
 
 /* Skinning (B2RSkin).  Forward: writes posed[0] and, when given, posed[1].  Backward: dL_dposed (host array of two
  * device pointers; either may be NULL = no gradient reaches that set, dL_dposed[1] requires xyz[1]) ->
