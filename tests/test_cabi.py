@@ -211,6 +211,38 @@ def test_error_codes_of_the_abi_v3_entry_points_without_touching_cuda():
     args.dL_dposed = fake                    # a posed-position gradient only makes sense with fused skinning
     assert bp(fake, 1 << 20) == -1
     assert lib.b2r_backward(C.byref(sc), C.byref(ws), C.byref(args), fake, 1 << 20, None) == -1
+    # split pass: the own sorted ids ride behind the keys, 4 bytes per duplicate slot, aligned like every other region
+    for cap in (0, 1, 64, 1000, 1 << 20):
+        extra = -(-4 * max(cap, 1) // 256) * 256
+        assert lib.b2r_split_scratch_bytes(10, 32, 32, cap) == lib.b2r_scratch_bytes(10, 32, 32, cap) + extra > 0
+    # each call below is valid but for the one field under test: every rejection happens before a launch
+    launches = lib.b2r_launch_count()
+    ps = lambda first_row, radii: lib.b2r_forward_project_split(C.byref(sc), C.byref(ws), first_row, radii, None)
+    assert ps(11, fake) == -1                # the split row lies beyond P
+    ws.dup_capacity = 0
+    assert ps(10, fake) == -1                # the split pass bins with the capacity it was given
+    ws.dup_capacity = 1000
+    assert ps(0, None) == -1                 # P > 0 rows need radii
+    base = L.B2RWorkspace()
+    base.ctx, base.ctx_bytes, base.dup_ids, base.dup_capacity = fake, lib.b2r_ctx_bytes(10, 32, 32), fake, 1000
+    bs = lambda b, first_row=10: lib.b2r_forward_bin_split(C.byref(sc), C.byref(ws), b, first_row, fake, None)
+    ws.scratch_bytes = lib.b2r_scratch_bytes(10, 32, 32, 1000)  # enough for a whole pass, not for the own ids
+    assert bs(C.byref(base)) == -2
+    ws.scratch_bytes = lib.b2r_split_scratch_bytes(10, 32, 32, 1000)
+    assert bs(None) == -1                    # no base pass
+    assert bs(C.byref(ws)) == -1             # the base pass is this pass
+    base.ctx = None
+    assert bs(C.byref(base)) == -1
+    base.ctx, base.dup_ids = fake, None
+    assert bs(C.byref(base)) == -1
+    base.dup_ids, base.ctx_bytes = fake, lib.b2r_ctx_bytes(10, 32, 32) - 1
+    assert bs(C.byref(base)) == -2           # the base ctx cannot hold P rows
+    base.ctx_bytes = lib.b2r_ctx_bytes(10, 32, 32)
+    assert bs(C.byref(base), 11) == -1       # the split row lies beyond P
+    assert lib.b2r_forward_bin_split(C.byref(sc), C.byref(ws), C.byref(base), 10, None, None) == -1  # no radii
+    ws.dup_capacity, ws.scratch_bytes = 0, lib.b2r_split_scratch_bytes(10, 32, 32, 0)
+    assert bs(C.byref(base)) == -1           # no capacity
+    assert lib.b2r_launch_count() == launches
 
 
 def test_compiled_torch_binding_builds_and_loads():
