@@ -79,6 +79,15 @@ class B2RMeshRender(C.Structure):
     ]
 
 
+class B2RGnMlp(C.Structure):
+    """One GroupNorm MLP stack (b2r_gn_mlp_forward / b2r_gn_mlp_backward): HumanGaussian's networks."""
+    _fields_ = [
+        ("P", C.c_int32), ("K", C.c_int32), ("H", C.c_int32), ("reserved", C.c_int32),
+        ("x", _fp), ("w", _fp * 3), ("b", _fp * 3), ("gamma", _fp * 3), ("beta", _fp * 3),
+        ("w_head", _fp), ("b_head", _fp),
+    ]
+
+
 class B2RForwardOutputs(C.Structure):
     _fields_ = [("color", _fp), ("depth", _fp), ("alpha", _fp), ("radii", _fp)]
 
@@ -154,6 +163,13 @@ SYMBOLS = [
     ("b2r_mesh_render_scratch_bytes", C.c_size_t, [C.c_int32]),
     ("b2r_mesh_render_forward", C.c_int, [C.POINTER(B2RMeshRender), _fp, _fp, _fp, C.c_size_t, _fp]),
     ("b2r_mesh_render_backward", C.c_int, [C.POINTER(B2RMeshRender), _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
+    ("b2r_triplane_forward", C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
+    ("b2r_triplane_backward", C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp, _fp, _fp, _fp, _fp, _fp,
+                                        _fp]),
+    ("b2r_gn_mlp_scratch_bytes", C.c_size_t, [C.c_int32]),
+    ("b2r_gn_mlp_grads_count", C.c_size_t, [C.c_int32, C.c_int32]),
+    ("b2r_gn_mlp_forward", C.c_int, [C.POINTER(B2RGnMlp), _fp, _fp, _fp]),
+    ("b2r_gn_mlp_backward", C.c_int, [C.POINTER(B2RGnMlp), _fp, _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
     ("b2r_profile_enable", None, [C.c_int]),
     ("b2r_profile_read", C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int]),
     ("b2r_launch_count", C.c_uint64, []),
@@ -184,9 +200,9 @@ def load():
         fn.argtypes = argtypes
     if lib.b2r_abi_version() != ABI_VERSION:
         raise RuntimeError("b200raster: ABI version mismatch between the Python binding and libb200raster.so")
-    # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8
+    # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8, B2RGnMlp 10 (9 unused too)
     for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
-                     (5, B2RView), (6, B2RSkin), (8, B2RMeshRender)):
+                     (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

@@ -93,6 +93,22 @@ int validate_mesh_render(const B2RMeshRender* m) {
   return B2R_OK;
 }
 
+// triplane.cu: P * 3C output elements and 6 H W CSR keys (x 32 lanes) stay addressable in int32 / the grid
+bool valid_triplane(int32_t P, int32_t C, int32_t height, int32_t width) {
+  return P >= 0 && C >= 1 && height >= 1 && width >= 1 && (int64_t)P * 3 * C < ((int64_t)1 << 31) &&
+         (int64_t)height * width * 6 * 32 < ((int64_t)1 << 31);
+}
+
+// gn_mlp.cu: ExAvatar's shapes only (hidden width 128 is fixed by the kernels); P * 128 stays in int32
+int validate_gn_mlp(const B2RGnMlp* m) {
+  if (!m) return B2R_E_INVALID;
+  if (m->P < 1 || m->P >= (1 << 24) || m->K < 1 || m->K > 128 || m->H < 1 || m->H > 4) return B2R_E_INVALID;
+  if (!m->x || !m->w_head || !m->b_head) return B2R_E_INVALID;
+  for (int l = 0; l < 3; l++)
+    if (!m->w[l] || !m->b[l] || !m->gamma[l] || !m->beta[l]) return B2R_E_INVALID;
+  return B2R_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -122,6 +138,7 @@ size_t b2r_sizeof(int which) {
     case 5: return sizeof(B2RView);
     case 6: return sizeof(B2RSkin);
     case 8: return sizeof(B2RMeshRender);  // 7 stays unused
+    case 10: return sizeof(B2RGnMlp);  // 9 stays unused
     default: return 0;
   }
 }
@@ -385,6 +402,44 @@ int b2r_mesh_render_backward(const B2RMeshRender* mr, const int32_t* pix_to_face
   if (mr->V > 0 && (!dL_dmesh || !mr->vf_offsets || !mr->vf_entries)) return B2R_E_INVALID;
   if (scratch_bytes < mesh_render_scratch_bytes(mr->F)) return B2R_E_WORKSPACE;
   return launch_mesh_render_backward(*mr, pix_to_face, dL_dimage, dL_dmesh, scratch, (cudaStream_t)stream);
+}
+
+int b2r_triplane_forward(int32_t P, int32_t C, int32_t height, int32_t width, const float* planes,
+                         const float* planes_face, const uint8_t* is_face, const int32_t* corners, const float* weights,
+                         float* feat, void* stream) {
+  if (!valid_triplane(P, C, height, width)) return B2R_E_INVALID;
+  if (P == 0) return B2R_OK;
+  if (!planes || !planes_face || !corners || !weights || !feat) return B2R_E_INVALID;
+  return launch_triplane_forward(P, C, height, width, planes, planes_face, is_face, corners, weights, feat,
+                                 (cudaStream_t)stream);
+}
+
+int b2r_triplane_backward(int32_t P, int32_t C, int32_t height, int32_t width, const float* dfeat,
+                          const int32_t* offsets, const int32_t* rows, const float* w, float* dplanes,
+                          float* dplanes_face, void* stream) {
+  if (!valid_triplane(P, C, height, width)) return B2R_E_INVALID;
+  if (!offsets || !dplanes || !dplanes_face || (P > 0 && (!dfeat || !rows || !w))) return B2R_E_INVALID;
+  return launch_triplane_backward(C, height, width, dfeat, offsets, rows, w, dplanes, dplanes_face,
+                                  (cudaStream_t)stream);
+}
+
+size_t b2r_gn_mlp_scratch_bytes(int32_t P) { return gn_mlp_scratch_bytes(P); }
+size_t b2r_gn_mlp_grads_count(int32_t K, int32_t H) { return gn_mlp_grads_count(K, H); }
+
+int b2r_gn_mlp_forward(const B2RGnMlp* m, float* out, float* saved, void* stream) {
+  const int rc = validate_gn_mlp(m);
+  if (rc) return rc;
+  if (!out) return B2R_E_INVALID;
+  return launch_gn_mlp_forward(*m, out, saved, (cudaStream_t)stream);
+}
+
+int b2r_gn_mlp_backward(const B2RGnMlp* m, const float* saved, const float* dL_dout, float* dL_dx, float* grads,
+                        void* scratch, size_t scratch_bytes, void* stream) {
+  const int rc = validate_gn_mlp(m);
+  if (rc) return rc;
+  if (!saved || !dL_dout || !grads || !scratch) return B2R_E_INVALID;
+  if (scratch_bytes < gn_mlp_scratch_bytes(m->P)) return B2R_E_WORKSPACE;
+  return launch_gn_mlp_backward(*m, saved, dL_dout, dL_dx, grads, scratch, (cudaStream_t)stream);
 }
 
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {

@@ -526,6 +526,16 @@ int launch_mesh_render_forward(const B2RMeshRender& m, float* image, int32_t* pi
                                cudaStream_t st);
 int launch_mesh_render_backward(const B2RMeshRender& m, const int32_t* pix_to_face, const float* dimage, float* dmesh,
                                 void* scratch, cudaStream_t st);
+int launch_triplane_forward(int P, int C, int H, int W, const float* planes, const float* planes_face,
+                            const uint8_t* is_face, const int32_t* corners, const float* weights, float* feat,
+                            cudaStream_t st);
+int launch_triplane_backward(int C, int H, int W, const float* dfeat, const int32_t* offsets, const int32_t* rows,
+                             const float* w, float* dplanes, float* dplanes_face, cudaStream_t st);
+size_t gn_mlp_scratch_bytes(int P);
+size_t gn_mlp_grads_count(int K, int H);
+int launch_gn_mlp_forward(const B2RGnMlp& m, float* out, float* saved, cudaStream_t st);
+int launch_gn_mlp_backward(const B2RGnMlp& m, const float* saved, const float* dout, float* dx, float* grads,
+                           void* scratch, cudaStream_t st);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

@@ -228,8 +228,8 @@ int b2r_abi_version(void);
 const char* b2r_strerror(int code);
 int b2r_last_cuda_error(void);
 /* sizeof() of the ABI structs, for bindings to verify their mirror: 0 B2RScene, 1 B2RStatus, 2 B2RWorkspace,
- * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin, 8 B2RMeshRender; 0 for anything else (7 is
- * unused and reports 0). */
+ * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin, 8 B2RMeshRender, 10 B2RGnMlp; 0 for anything else
+ * (7 and 9 are unused and report 0). */
 size_t b2r_sizeof(int which);
 
 size_t b2r_ctx_bytes(int32_t P, int32_t width, int32_t height);
@@ -391,11 +391,58 @@ int b2r_mesh_render_forward(const B2RMeshRender* mr, float* image, int32_t* pix_
 int b2r_mesh_render_backward(const B2RMeshRender* mr, const int32_t* pix_to_face, const float* dL_dimage,
                              float* dL_dmesh, void* scratch, size_t scratch_bytes, void* stream);
 
+/* Triplane features of the human Gaussians (avatar/common/nets/module.py:424-457 extract_tri_feature).  planes and
+ * planes_face are (3,C,height,width); corners (P,3,4) int32 holds, per row and plane (xy, xz, yz), the texels
+ * y * width + x of F.grid_sample's four bilinear corners in its order (nw, ne, sw, se), -1 for a corner outside the
+ * plane (zero padding), and weights (P,3,4) their weights.  Forward: feat (P,3C)[r][p*C + c] = sum over the corners of
+ * w T[p][c][texel], T = planes_face where is_face[r] != 0 (is_face (P) may be NULL: none), else planes.  Backward:
+ * writes every element of dplanes and dplanes_face (both (3,C,height,width)) from dfeat (P,3C) and the texel -> row
+ * CSR of the same corners: key (s * 3 + p) * height * width + texel with s = 1 for face rows, offsets (6 * height *
+ * width + 1), rows / w the entries' rows (ascending within a key) and weights.  Sums in CSR order, no float atomics:
+ * bit-identical runs.  No allocation, no sync. */
+int b2r_triplane_forward(int32_t P, int32_t C, int32_t height, int32_t width, const float* planes,
+                         const float* planes_face, const uint8_t* is_face, const int32_t* corners, const float* weights,
+                         float* feat, void* stream);
+int b2r_triplane_backward(int32_t P, int32_t C, int32_t height, int32_t width, const float* dfeat,
+                          const int32_t* offsets, const int32_t* rows, const float* w, float* dplanes,
+                          float* dplanes_face, void* stream);
+
+/* One of HumanGaussian's GroupNorm MLP stacks (avatar/common/nets/layer.py make_linear_layers(use_gn=True)):
+ *   z_l = a_{l-1} W_l^T + b_l,  a_l = relu(GroupNorm(4, 128, eps 1e-5)(z_l) * gamma_l + beta_l),  l = 0, 1, 2,
+ *   out = a_2 Wh^T + bh,  with a_{-1} = x.
+ * A first-layer input block that is the same for every row is the caller's to fold into b[0].  Products are taken as
+ * 3xTF32 on the tensor cores (fp32-accurate), sums in fp32. */
+typedef struct B2RGnMlp {
+  int32_t P;              /* rows, >= 1 */
+  int32_t K;              /* per-row first-layer inputs, 1..128 */
+  int32_t H;              /* head outputs, 1..4 */
+  int32_t reserved;
+  const float* x;         /* (P,K) */
+  const float* w[3];      /* w[0] (128,K), w[1], w[2] (128,128), row-major [out][in] */
+  const float* b[3];      /* (128) each */
+  const float* gamma[3];  /* (128) each: the GroupNorm affine */
+  const float* beta[3];
+  const float* w_head;    /* (H,128) */
+  const float* b_head;    /* (H) */
+} B2RGnMlp;
+
+/* Forward: writes out (P,H) and, when saved is not NULL, the pre-GroupNorm z_0, z_1, z_2 into saved (3,P,128), which
+ * the backward reads.  Backward: from saved and dL_dout (P,H) writes dL_dx (P,K) when not NULL, and every element of
+ * grads (b2r_gn_mlp_grads_count(K, H) floats) = [dW_0 (128,K) | dW_1 (128,128) | dW_2 (128,128) | dgamma (3,128) |
+ * dbeta (3,128) | db (3,128) | dWh (H,128) | dbh (H)].  The parameter gradients are summed into fixed per-CTA and
+ * per-1024-row partials, then over those in a fixed order: no float atomics, bit-identical runs.  `scratch` >=
+ * b2r_gn_mlp_scratch_bytes(P).  Neither call allocates or syncs. */
+size_t b2r_gn_mlp_scratch_bytes(int32_t P);
+size_t b2r_gn_mlp_grads_count(int32_t K, int32_t H);
+int b2r_gn_mlp_forward(const B2RGnMlp* m, float* out, float* saved, void* stream);
+int b2r_gn_mlp_backward(const B2RGnMlp* m, const float* saved, const float* dL_dout, float* dL_dx, float* grads,
+                        void* scratch, size_t scratch_bytes, void* stream);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals and b2r_mesh_render_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_* and b2r_gn_mlp_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
