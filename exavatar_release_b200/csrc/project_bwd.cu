@@ -7,6 +7,8 @@
 // Conventions kept from the published backward (App. A.6): 1/(det^2 + 1e-7), frustum-clamped t.x / t.y pass no direct
 // gradient, gradient is w.r.t. the un-normalised quaternion, dL/dmeans2D is NDC-scaled (x 0.5 W, 0.5 H) with z = 0
 // -- the quantity ExAvatar thresholds for densification (module.py:155-157,176; config.py:21).
+#include <atomic>
+
 #include "gaussian_math.cuh"
 
 namespace b2r {
@@ -220,10 +222,6 @@ __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& c
     dm[1] += __ldg(out.dL_dposed + 3 * (size_t)i + 1);
     dm[2] += __ldg(out.dL_dposed + 3 * (size_t)i + 2);
   }
-  const bool track = visible && (out.densify_rows == 0u || (uint32_t)i < out.densify_rows);
-  if (track && out.densify_grad_accum) out.densify_grad_accum[oi] += sqrtf(dm2[0] * dm2[0] + dm2[1] * dm2[1]);
-  if (track && out.densify_count) out.densify_count[oi] += 1.f;
-  if (track && out.densify_radius_max) out.densify_radius_max[oi] = fmaxf(out.densify_radius_max[oi], (float)aux.z);
   auto put3 = [&](float* base, const float* v) {
     if (!base) return;
     float* d = base + 3 * oi;
@@ -249,26 +247,6 @@ __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& c
       for (int k = 0; k < 12; k++) { if (accumulate) d[k] += G[k]; else d[k] = G[k]; }
     }
   }
-  const float dm2z[3] = {dm2[0], dm2[1], 0.f};
-  put3(out.dL_dmeans3D, dm);
-  put3(out.dL_dmeans2D, dm2z);
-  if (MIXED && shrow) {
-    const float zero3[3] = {0.f, 0.f, 0.f};
-    put3(out.dL_dcolors, zero3);
-  } else {
-    put3(out.dL_dcolors, dcol);
-  }
-  put3(out.dL_dscales, dscale);
-  if (out.dL_dopacities) {
-    if (accumulate) out.dL_dopacities[oi] += dop; else out.dL_dopacities[oi] = dop;
-  }
-  if (out.dL_drotations) {
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-      float* d = out.dL_drotations + 4 * oi + k;
-      if (accumulate) *d += dq[k]; else *d = dq[k];
-    }
-  }
   if (out.dL_dcov3D) {
 #pragma unroll
     for (int k = 0; k < 6; k++) {
@@ -277,6 +255,38 @@ __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& c
       if (accumulate) *d += v; else *d = v;
     }
   }
+  // The main outputs and the densification statistics: every value a read-modify-write needs is loaded before the
+  // first of them is stored.  The compiler may not move a load of one array above a store to another (they could
+  // alias), so "load, add, store" array by array costs one dependent global round trip per array; loaded together
+  // they cost one.  The sums are the same expressions as `d += v`.
+  const float dm2z[3] = {dm2[0], dm2[1], 0.f};
+  const float zero3[3] = {0.f, 0.f, 0.f};
+  float* const dst[6] = {out.dL_dmeans3D ? out.dL_dmeans3D + 3 * oi : nullptr,
+                         out.dL_dmeans2D ? out.dL_dmeans2D + 3 * oi : nullptr,
+                         out.dL_dcolors ? out.dL_dcolors + 3 * oi : nullptr,
+                         out.dL_dscales ? out.dL_dscales + 3 * oi : nullptr,
+                         out.dL_dopacities ? out.dL_dopacities + oi : nullptr,
+                         out.dL_drotations ? out.dL_drotations + 4 * oi : nullptr};
+  const float* const src[6] = {dm, dm2z, MIXED && shrow ? zero3 : dcol, dscale, &dop, dq};
+  constexpr int width[6] = {3, 3, 3, 3, 1, 4};
+  const bool track = visible && (out.densify_rows == 0u || (uint32_t)i < out.densify_rows);
+  float* const dens[3] = {track ? out.densify_grad_accum : nullptr, track ? out.densify_count : nullptr,
+                          track ? out.densify_radius_max : nullptr};
+  float prior[17], dprior[3];
+#pragma unroll
+  for (int a = 0, k = 0; a < 6; a++)
+#pragma unroll
+    for (int c = 0; c < width[a]; c++, k++) prior[k] = accumulate && dst[a] ? dst[a][c] : 0.f;
+#pragma unroll
+  for (int a = 0; a < 3; a++) dprior[a] = dens[a] ? dens[a][oi] : 0.f;
+#pragma unroll
+  for (int a = 0, k = 0; a < 6; a++)
+#pragma unroll
+    for (int c = 0; c < width[a]; c++, k++)
+      if (dst[a]) dst[a][c] = accumulate ? prior[k] + src[a][c] : src[a][c];
+  if (dens[0]) dens[0][oi] = dprior[0] + sqrtf(dm2[0] * dm2[0] + dm2[1] * dm2[1]);
+  if (dens[1]) dens[1][oi] = dprior[1] + 1.f;
+  if (dens[2]) dens[2][oi] = fmaxf(dprior[2], (float)aux.z);
 }
 
 // K6.  The per-Gaussian body above reads / writes everything with one thread per Gaussian, which is fine for the
@@ -287,7 +297,10 @@ __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& c
 // MIXED (B2RScene.sh_rows > 0): only rows [0, sh_rows) are staged and written to dL_dshs (row i - first_row); the other
 // rows take the colour path.  A separate instantiation, so the single-source kernel stays the code it was.
 #ifndef PBWD_MIN_BLOCKS
-#define PBWD_MIN_BLOCKS 3  // caps the kernel at 80 registers (three CTAs per SM) at the price of a small spill; tuning hook
+// Two CTAs per SM: the kernel fits in 128 registers without spilling.  The 80-register cap of three CTAs per SM spills,
+// and the spill reloads in the epilogue serialise its batched loads again (C4 on an H100 at 400 W: 47 / 23 µs per pass at two
+// CTAs per SM, 69 / 42 µs at three).  Tuning hook.
+#define PBWD_MIN_BLOCKS 2
 #endif
 template <bool MIXED>
 __global__ void __launch_bounds__(256, PBWD_MIN_BLOCKS) project_bwd_kernel(const B2RScene sc, const Ctx cx, const B2RBackwardArgs out,
@@ -347,8 +360,17 @@ int launch_project_bwd(const B2RScene& sc, const Ctx& cx, const B2RBackwardArgs&
     const bool use_sh = sc.shs != nullptr && a.dL_dshs != nullptr;
     const size_t smem = (use_sh ? (size_t)8 * 32 * ((sc.sh_coeffs * 3) | 1) * sizeof(float) : 0) +
                         (sc.skin_xyz ? (size_t)8 * 32 * (sc.skin_J | 1) * sizeof(float) : 0);
+    // the shared-memory ceiling is an attribute of the kernel on the current device: set once per device, not per launch
+    static std::atomic<uint64_t> attr_set{0};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const uint64_t bit = dev < 64 ? 1ull << dev : 0ull;
+    if (!(attr_set.load(std::memory_order_relaxed) & bit)) {
+      cudaFuncSetAttribute(project_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024);
+      cudaFuncSetAttribute(project_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024);
+      attr_set.fetch_or(bit, std::memory_order_relaxed);
+    }
     auto kern = sc.sh_rows > 0 ? project_bwd_kernel<true> : project_bwd_kernel<false>;
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024);  // per device
     launch_k(kern, grid, 256, smem, st, true, sc, cx, a, gacc);
   }
   return check_launch();
