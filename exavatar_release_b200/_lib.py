@@ -12,7 +12,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "libb200raster.so")
 LIB_PATH = os.environ.get("B2R_LIB", LIB_PATH)  # tuning experiments: an alternative build of the same library
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 B2R_OK = 0
 B2R_FLAG_NO_TILE_CULL = 1
 B2R_FLAG_DEBUG = 2
@@ -29,9 +29,6 @@ class B2RScene(C.Structure):
         ("bg", _fp), ("viewmatrix", _fp), ("projmatrix", _fp), ("campos", _fp),
         ("means3D", _fp), ("shs", _fp), ("colors_precomp", _fp), ("opacities", _fp),
         ("scales", _fp), ("rotations", _fp), ("cov3D_precomp", _fp),
-        # fused linear-blend skinning (SURVEY section 8f-2); all NULL / 0 = off
-        ("skin_xyz", _fp), ("skin_weights", _fp), ("skin_joint_mats", _fp), ("skin_trans", _fp),
-        ("skin_cam_Rinv", _fp), ("skin_cam_t", _fp), ("skin_means_out", _fp), ("skin_J", C.c_int32),
         # mixed colour source: rows [0, sh_rows) from `shs`, the rest from `colors_precomp`; 0 = one source
         ("sh_rows", C.c_int32),
     ]
@@ -99,8 +96,6 @@ class B2RBackwardArgs(C.Structure):
         ("dL_dscales", _fp), ("dL_drotations", _fp), ("dL_dcov3D", _fp),
         ("flags", C.c_uint32), ("first_row", C.c_uint32),
         ("densify_grad_accum", _fp), ("densify_count", _fp), ("densify_radius_max", _fp),
-        ("dL_dskin_xyz", _fp), ("dL_dskin_G", _fp),
-        ("dL_dposed", _fp),  # ABI v3 INPUT: gradient arriving at the posed positions (fused skinning)
         ("densify_rows", C.c_uint32), ("reserved", C.c_uint32),
     ]
 

@@ -30,8 +30,8 @@ NVCC_FLAGS = [
 # binning.cu: its scatter repeats the projection's tile region test for rects of more than 32 tiles (smaller ones replay
 # a stored mask); the two must agree on every (splat, tile) pair or a list slot stays unfilled, so the unit is compiled
 # with the same contraction setting (its kernels are integer sorts otherwise).
-# skin.cu: the standalone skinning op evaluates the blend of project.cu's fused skinning (gaussian_math.cuh skin_apply);
-# compiled with the same contraction setting, both paths write bit-identical posed positions.
+# skin.cu: the posed positions feed every human render and their recorded outputs; fma contraction would move them in the
+# last bits, so the unit keeps every product and sum rounded on its own.
 # geometry.cu: the nearest-vertex search evaluates dx*dx + dy*dy + dz*dz exactly as its torch restatement does (three
 # rounded products, two rounded sums), so the argmin -- ties included -- is the restatement's, index for index.
 # mesh_raster.cu: the face render's coverage test and depth pz are, operation for operation, the float32 restatement's

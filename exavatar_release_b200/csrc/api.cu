@@ -14,14 +14,7 @@ int validate_scene(const B2RScene* sc) {
   if (!sc->bg || !sc->viewmatrix || !sc->projmatrix || !sc->campos) return B2R_E_INVALID;
   if (sc->sh_rows < 0 || sc->sh_rows > sc->P) return B2R_E_INVALID;
   if (sc->P > 0) {
-    if (!sc->opacities) return B2R_E_INVALID;
-    if (sc->skin_xyz) {  // fused skinning replaces means3D
-      if (!sc->skin_weights || !sc->skin_joint_mats || !sc->skin_trans) return B2R_E_INVALID;
-      if (sc->skin_J <= 0 || sc->skin_J > 64) return B2R_E_INVALID;
-      if (sc->skin_cam_Rinv && !sc->skin_cam_t) return B2R_E_INVALID;
-    } else if (!sc->means3D) {
-      return B2R_E_INVALID;
-    }
+    if (!sc->opacities || !sc->means3D) return B2R_E_INVALID;
     if (sc->sh_rows > 0) {  // mixed: SH rows first, then colour rows -- both sources required
       if (!sc->shs || !sc->colors_precomp) return B2R_E_INVALID;
     } else if ((sc->shs != nullptr) == (sc->colors_precomp != nullptr)) {
@@ -59,7 +52,7 @@ bool missing_dshs(const B2RScene* sc, const B2RBackwardArgs* a) {
   return sc->sh_rows == 0 || (int64_t)a->first_row < (int64_t)sc->sh_rows;
 }
 
-// the rules of the fused skinning in validate_scene, for the standalone op
+// skin.cu stages a weight row as at most two floats per lane: J <= 64
 int validate_skin(const B2RSkin* s) {
   if (!s) return B2R_E_INVALID;
   if (s->P < 0 || s->V <= 0) return B2R_E_INVALID;
@@ -279,7 +272,6 @@ int b2r_backward(const B2RScene* scene, const B2RWorkspace* ws, const B2RBackwar
   if (bwd_scratch_bytes < b2r_backward_scratch_bytes(scene->P)) return B2R_E_WORKSPACE;
   if (missing_dshs(scene, args)) return B2R_E_INVALID;
   if ((int64_t)args->first_row > (int64_t)scene->P) return B2R_E_INVALID;
-  if (args->dL_dposed && !scene->skin_xyz) return B2R_E_INVALID;
   const Ctx cx = resolve(ws, scene->P, scene->width, scene->height);
   float* gacc = (float*)bwd_scratch;
   rc = launch_composite_bwd(*scene, cx, *args, gacc, (cudaStream_t)stream);
@@ -312,7 +304,6 @@ int b2r_backward_project(const B2RScene* scene, const B2RWorkspace* ws, const B2
   if (bwd_scratch_bytes < b2r_backward_scratch_bytes(scene->P)) return B2R_E_WORKSPACE;
   if (missing_dshs(scene, args)) return B2R_E_INVALID;
   if ((int64_t)args->first_row > (int64_t)scene->P) return B2R_E_INVALID;
-  if (args->dL_dposed && !scene->skin_xyz) return B2R_E_INVALID;
   const Ctx cx = resolve(ws, scene->P, scene->width, scene->height);
   return launch_project_bwd(*scene, cx, *args, (const float*)bwd_scratch, (cudaStream_t)stream);
 }
@@ -326,16 +317,16 @@ int b2r_skin_forward(const B2RSkin* skin, void* stream) {
   return launch_skin_forward(*skin, (cudaStream_t)stream);
 }
 
-int b2r_skin_backward(const B2RSkin* skin, const float* const dL_dposed[2], float* const dL_dxyz[2], float* dL_djoint,
+int b2r_skin_backward(const B2RSkin* skin, const float* const dL_dpos[2], float* const dL_dxyz[2], float* dL_djoint,
                       float* dL_dtrans, void* scratch, size_t scratch_bytes, void* stream) {
   const int rc = validate_skin(skin);
   if (rc) return rc;
-  if (dL_dposed && dL_dposed[1] && !skin->xyz[1]) return B2R_E_INVALID;
+  if (dL_dpos && dL_dpos[1] && !skin->xyz[1]) return B2R_E_INVALID;
   if ((dL_djoint || dL_dtrans) && skin->P > 0) {
     if (!scratch) return B2R_E_INVALID;
     if (scratch_bytes < skin_scratch_bytes(skin->P, skin->J)) return B2R_E_WORKSPACE;
   }
-  return launch_skin_backward(*skin, dL_dposed, dL_dxyz, dL_djoint, dL_dtrans, scratch, (cudaStream_t)stream);
+  return launch_skin_backward(*skin, dL_dpos, dL_dxyz, dL_djoint, dL_dtrans, scratch, (cudaStream_t)stream);
 }
 
 size_t b2r_l1ssim_scratch_bytes(int32_t width, int32_t height) { return l1ssim_scratch_bytes(width, height); }

@@ -46,75 +46,6 @@ __device__ __forceinline__ float4 xform4x4(const float3 p, const float* m) {
                      m[2] * p.x + m[6] * p.y + m[10] * p.z + m[14], m[3] * p.x + m[7] * p.y + m[11] * p.z + m[15]);
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// Linear-blend skinning (SURVEY section 8f-2; avatar/common/nets/module.py:413-422, 555-557).
-//   M = sum_j w_j A_j (rows 0..2 of the 4x4),  posed = M [x,1] + trans,  world = Rinv (posed - t)
-// On plain pointers, so the projection kernels (fused skinning, B2RScene.skin_*) and the standalone skinning op
-// (skin.cu, B2RSkin) evaluate the same blend.  `wrow` is the Gaussian's weight row in the warp's shared-memory stage,
-// `A` the (J,16) row-major joint transforms in global memory (warp-uniform addresses: one broadcast line per load).
-// The arithmetic of skin_apply is contracted or not as its translation unit is compiled (project.cu and skin.cu both
-// without fma contraction: their posed positions agree bit for bit).
-// ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void skin_blend(const float* __restrict__ A, const int J, const float* __restrict__ wrow,
-                                           float* M) {
-#pragma unroll
-  for (int k = 0; k < 12; k++) M[k] = 0.f;
-  for (int j = 0; j < J; j++) {
-    const float w = wrow[j];
-    if (w != 0.f) {  // SMPL-X skinning weights are sparse (a handful of joints per vertex)
-#pragma unroll
-      for (int k = 0; k < 12; k++) M[k] = fmaf(w, __ldg(A + 16 * j + k), M[k]);
-    }
-  }
-}
-
-// posed = M [x,1] + trans; then Rinv (posed - t) when Rinv is given
-__device__ __forceinline__ float3 skin_apply(const float* M, const float3 x, const float* __restrict__ trans,
-                                             const float* __restrict__ Rinv, const float* __restrict__ t) {
-  float px = M[0] * x.x + M[1] * x.y + M[2] * x.z + M[3] + __ldg(trans);
-  float py = M[4] * x.x + M[5] * x.y + M[6] * x.z + M[7] + __ldg(trans + 1);
-  float pz = M[8] * x.x + M[9] * x.y + M[10] * x.z + M[11] + __ldg(trans + 2);
-  if (Rinv) {
-    const float dx = px - __ldg(t), dy = py - __ldg(t + 1), dz = pz - __ldg(t + 2);
-    px = __ldg(Rinv) * dx + __ldg(Rinv + 1) * dy + __ldg(Rinv + 2) * dz;
-    py = __ldg(Rinv + 3) * dx + __ldg(Rinv + 4) * dy + __ldg(Rinv + 5) * dz;
-    pz = __ldg(Rinv + 6) * dx + __ldg(Rinv + 7) * dy + __ldg(Rinv + 8) * dz;
-  }
-  return make_float3(px, py, pz);
-}
-
-// Transpose of skin_apply for one Gaussian, `g` the gradient at the output position:
-//   g_cam = Rinv^T g  (g itself without Rinv),  dL/dx = M3^T g_cam;
-// the Gaussian's share of dL/dA_j[:3, :] is w_j g_cam [x, 1]^T and of dL/dtrans g_cam.  `gc` may alias `g`.
-__device__ __forceinline__ void skin_transpose(const float* M, const float* __restrict__ Rinv, const float* g, float* gc,
-                                               float* dx) {
-  const float g0 = g[0], g1 = g[1], g2 = g[2];
-  if (Rinv) {
-    gc[0] = __ldg(Rinv) * g0 + __ldg(Rinv + 3) * g1 + __ldg(Rinv + 6) * g2;
-    gc[1] = __ldg(Rinv + 1) * g0 + __ldg(Rinv + 4) * g1 + __ldg(Rinv + 7) * g2;
-    gc[2] = __ldg(Rinv + 2) * g0 + __ldg(Rinv + 5) * g1 + __ldg(Rinv + 8) * g2;
-  } else {
-    gc[0] = g0; gc[1] = g1; gc[2] = g2;
-  }
-#pragma unroll
-  for (int c = 0; c < 3; c++) dx[c] = M[c] * gc[0] + M[4 + c] * gc[1] + M[8 + c] * gc[2];
-}
-
-struct Skin {
-  float M[12];   // blended transform, rows 0..2, row-major 3x4
-  float3 x;      // canonical position
-  float3 world;  // posed position in the frame the rasteriser works in
-};
-
-__device__ __forceinline__ Skin skin_position(const B2RScene& sc, const int i, const float* __restrict__ wrow) {
-  Skin s;
-  skin_blend(sc.skin_joint_mats, sc.skin_J, wrow, s.M);
-  s.x = make_float3(__ldg(sc.skin_xyz + 3 * (size_t)i), __ldg(sc.skin_xyz + 3 * (size_t)i + 1),
-                    __ldg(sc.skin_xyz + 3 * (size_t)i + 2));
-  s.world = skin_apply(s.M, s.x, sc.skin_trans, sc.skin_cam_Rinv, sc.skin_cam_t);
-  return s;
-}
-
 // R_std of an un-normalised quaternion (r,x,y,z), row-major R[row*3+col]
 __device__ __forceinline__ void quat_to_R(const float4 q, float* R) {
   const float r = q.x, x = q.y, y = q.z, z = q.w;

@@ -17,9 +17,11 @@ namespace b2r {
 
 int g_last_cuda_error = 0;
 
-__device__ __forceinline__ void sh_to_rgb(int deg, const float* __restrict__ sh, const float3 mean, const Cam& cam,
-                                          float* rgb, uint32_t& clamp_bits) {
-  float dx = mean.x - cam.campos[0], dy = mean.y - cam.campos[1], dz = mean.z - cam.campos[2];
+// `campos` is read here rather than taken from load_cam: held in registers across the whole projection, its three
+// floats do not fit the kernel's 64-register budget (PROJ_MIN_BLOCKS) and spill.
+__device__ __forceinline__ void sh_to_rgb(int deg, const float* __restrict__ sh, const float3 mean,
+                                          const float* __restrict__ campos, float* rgb, uint32_t& clamp_bits) {
+  float dx = mean.x - __ldg(campos), dy = mean.y - __ldg(campos + 1), dz = mean.z - __ldg(campos + 2);
   const float n = sqrtf(dx * dx + dy * dy + dz * dz);
   const float x = dx / n, y = dy / n, z = dz / n;
   clamp_bits = 0;
@@ -77,20 +79,6 @@ __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2R
     __syncwarp();
     shrow = wstage + lane * S;
   }
-  // fused skinning: the warp's 32 weight rows (J floats each) take the same staged route as the SH rows
-  const float* wrow = nullptr;
-  if (sc.skin_xyz) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int J = sc.skin_J, S = J | 1;
-    float* base = reinterpret_cast<float*>(s_cnt + (aggregate ? cx.tiles : 0));
-    if (sc.shs) base += (size_t)8 * 32 * ((sc.sh_coeffs * 3) | 1);
-    float* wstage = base + (size_t)warp * 32 * S;
-    const int row0 = first_row + blockIdx.x * blockDim.x + warp * 32;
-    const int nrows = min(32, sc.P - row0);
-    if (nrows > 0) stage_rows<0>(wstage, const_cast<float*>(sc.skin_weights) + (size_t)row0 * J, J, nrows, 0xffffffffu);
-    __syncwarp();
-    wrow = wstage + lane * S;
-  }
   const Cam cam = load_cam(sc);
   bool visible = false;
   Geom g;
@@ -99,18 +87,8 @@ __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2R
   g.g2 = make_float4(0.f, 0.f, 0.f, 0.f);
   int4 aux = make_int4(0, 0, 0, 0);
   if (i < sc.P) {
-    float3 p;
-    if (wrow) {
-      p = skin_position(sc, i, wrow).world;
-      if (sc.skin_means_out) {
-        sc.skin_means_out[3 * (size_t)i] = p.x;
-        sc.skin_means_out[3 * (size_t)i + 1] = p.y;
-        sc.skin_means_out[3 * (size_t)i + 2] = p.z;
-      }
-    } else {
-      p = make_float3(__ldg(sc.means3D + 3 * (size_t)i), __ldg(sc.means3D + 3 * (size_t)i + 1),
-                      __ldg(sc.means3D + 3 * (size_t)i + 2));
-    }
+    const float3 p = make_float3(__ldg(sc.means3D + 3 * (size_t)i), __ldg(sc.means3D + 3 * (size_t)i + 1),
+                                 __ldg(sc.means3D + 3 * (size_t)i + 2));
     const float3 pv = xform4x3(p, cam.v);
     if (pv.z > K_NEAR) {  // App. A.1 step 1
       // Homogeneous position and pixel centre WITHOUT fma contraction, operation for operation as the oracle's C
@@ -155,7 +133,7 @@ __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2R
           float rgb[3];
           uint32_t bits = 0;
           if (sc.shs && (!MIXED || i < sc.sh_rows)) {  // clamp bits only for SH rows
-            sh_to_rgb(sc.sh_degree, shrow, p, cam, rgb, bits);
+            sh_to_rgb(sc.sh_degree, shrow, p, sc.campos, rgb, bits);
           } else {
             rgb[0] = __ldg(sc.colors_precomp + 3 * (size_t)i);
             rgb[1] = __ldg(sc.colors_precomp + 3 * (size_t)i + 1);
@@ -408,8 +386,7 @@ int launch_project(const B2RScene& sc, const Ctx& cx, int32_t* radii, cudaStream
     ProfScope p(K_PROJECT, st);
     const int aggregate = cx.tiles <= 2048;  // beyond that the per-CTA sweeps over the tile table cost more than they save
     const size_t smem = (aggregate ? (size_t)cx.tiles * 4 : 0) +
-                        (sc.shs ? (size_t)8 * 32 * ((sc.sh_coeffs * 3) | 1) * sizeof(float) : 0) +
-                        (sc.skin_xyz ? (size_t)8 * 32 * (sc.skin_J | 1) * sizeof(float) : 0);
+                        (sc.shs ? (size_t)8 * 32 * ((sc.sh_coeffs * 3) | 1) * sizeof(float) : 0);
     auto kern = sc.sh_rows > 0 ? project_kernel<true> : project_kernel<false>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);  // per device
     launch_k(kern, (sc.P - first_row + 255) / 256, 256, smem, st, true, sc, cx, radii, aggregate, first_row);

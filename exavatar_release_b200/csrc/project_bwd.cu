@@ -19,8 +19,7 @@ namespace b2r {
 template <bool MIXED>
 __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& cx, const B2RBackwardArgs& out,
                                                 const float* __restrict__ gacc, const int i, const size_t oi,
-                                                const bool visible, const int4 aux, float* shrow,
-                                                const float* wrow) {
+                                                const bool visible, const int4 aux, float* shrow) {
   const int M = sc.sh_coeffs;
   const bool accumulate = (out.flags & B2R_BWD_ACCUMULATE) != 0;
 
@@ -30,11 +29,6 @@ __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& c
   uint32_t clamp_bits = 0;
   float3 p = make_float3(0.f, 0.f, 0.f);
   Cam cam;
-  Skin skin;
-  // gradient arriving at the posed position itself (other ExAvatar modules read it, model.py:172-173): also for
-  // Gaussians this render culled
-  const bool posed_in = wrow != nullptr && out.dL_dposed != nullptr;
-  if (posed_in && !visible) skin = skin_position(sc, i, wrow);
 
   if (visible) {
     cam = load_cam(sc);
@@ -49,13 +43,8 @@ __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& c
     dcol[0] = q2.x; dcol[1] = q2.y; dcol[2] = q2.z;
     clamp_bits = __float_as_uint(reinterpret_cast<const float4*>(cx.geom + i)[2].w) >> 29;
 
-    if (wrow) {
-      skin = skin_position(sc, i, wrow);
-      p = skin.world;
-    } else {
-      p = make_float3(__ldg(sc.means3D + 3 * (size_t)i), __ldg(sc.means3D + 3 * (size_t)i + 1),
-                      __ldg(sc.means3D + 3 * (size_t)i + 2));
-    }
+    p = make_float3(__ldg(sc.means3D + 3 * (size_t)i), __ldg(sc.means3D + 3 * (size_t)i + 1),
+                    __ldg(sc.means3D + 3 * (size_t)i + 2));
     float c6[6];
     float3 scl = make_float3(0.f, 0.f, 0.f);
     float4 q = make_float4(1.f, 0.f, 0.f, 0.f);
@@ -210,43 +199,15 @@ __device__ __forceinline__ void project_bwd_one(const B2RScene& sc, const Ctx& c
         ddir[1] += dry * gc;
         ddir[2] += drz * gc;
       }
-      const float dot = x * ddir[0] + y * ddir[1] + z * ddir[2];
+      // rounding order spelled out: left to the compiler, which product gets fused into the FMA chain moves with
+      // unrelated edits of this kernel, and dL/dmeans3D with it
+      const float dot = fmaf(z, ddir[2], fmaf(y, ddir[1], __fmul_rn(x, ddir[0])));
       dm[0] += (ddir[0] - x * dot) / n;
       dm[1] += (ddir[1] - y * dot) / n;
       dm[2] += (ddir[2] - z * dot) / n;
     }
   }
 
-  if (posed_in) {
-    dm[0] += __ldg(out.dL_dposed + 3 * (size_t)i);
-    dm[1] += __ldg(out.dL_dposed + 3 * (size_t)i + 1);
-    dm[2] += __ldg(out.dL_dposed + 3 * (size_t)i + 2);
-  }
-  auto put3 = [&](float* base, const float* v) {
-    if (!base) return;
-    float* d = base + 3 * oi;
-    if (accumulate) { d[0] += v[0]; d[1] += v[1]; d[2] += v[2]; }
-    else { d[0] = v[0]; d[1] = v[1]; d[2] = v[2]; }
-  };
-  // fused skinning: world-space gradient -> canonical position and the outer product the joint-transform GEMM needs
-  if (wrow && (out.dL_dskin_xyz || out.dL_dskin_G)) {
-    float gc[3] = {dm[0], dm[1], dm[2]}, dx[3] = {0.f, 0.f, 0.f}, G[12];
-    float xs[4] = {0.f, 0.f, 0.f, 0.f};
-    if (visible || posed_in) {
-      skin_transpose(skin.M, sc.skin_cam_Rinv, dm, gc, dx);  // g_cam = Rinv^T g_world, dx = M3^T g_cam
-      xs[0] = skin.x.x; xs[1] = skin.x.y; xs[2] = skin.x.z; xs[3] = 1.f;
-    }
-#pragma unroll
-    for (int r = 0; r < 3; r++)
-#pragma unroll
-      for (int c = 0; c < 4; c++) G[4 * r + c] = gc[r] * xs[c];
-    put3(out.dL_dskin_xyz, dx);
-    if (out.dL_dskin_G) {
-      float* d = out.dL_dskin_G + 12 * oi;
-#pragma unroll
-      for (int k = 0; k < 12; k++) { if (accumulate) d[k] += G[k]; else d[k] = G[k]; }
-    }
-  }
   if (out.dL_dcov3D) {
 #pragma unroll
     for (int k = 0; k < 6; k++) {
@@ -317,8 +278,8 @@ __global__ void __launch_bounds__(256, PBWD_MIN_BLOCKS) project_bwd_kernel(const
   // out.first_row: Gaussians below it are a detached prefix (ExAvatar renders cat(scene.detach(), human),
   // model.py:117-125): nothing is written for them and Gaussian i lands in output row i - first_row
   const int first_row = (int)out.first_row;
-  // an invisible Gaussian has nothing to add -- unless a gradient arrives at its posed position
-  const bool active = in_range && i >= first_row && !(accumulate && !visible && out.dL_dposed == nullptr);
+  // an invisible Gaussian has nothing to add
+  const bool active = in_range && i >= first_row && !(accumulate && !visible);
   const bool use_sh = sc.shs != nullptr && out.dL_dshs != nullptr;
   const int L = sc.sh_coeffs * 3, S = L | 1;
   float* wstage = sh_stage + (size_t)warp * 32 * S;
@@ -330,15 +291,7 @@ __global__ void __launch_bounds__(256, PBWD_MIN_BLOCKS) project_bwd_kernel(const
     __syncwarp();
   }
   float* shrow = use_sh && (!MIXED || i < sc.sh_rows) ? wstage + lane * S : nullptr;
-  const float* wrow = nullptr;
-  if (sc.skin_xyz) {  // skinning weight rows, staged like the SH rows (after them in shared memory)
-    const int J = sc.skin_J, SJ = J | 1;
-    float* kstage = sh_stage + (use_sh ? (size_t)8 * 32 * S : 0) + (size_t)warp * 32 * SJ;
-    if (nrows > 0) stage_rows<0>(kstage, const_cast<float*>(sc.skin_weights) + (size_t)row0 * J, J, nrows, 0xffffffffu);
-    __syncwarp();
-    wrow = kstage + lane * SJ;
-  }
-  if (active) project_bwd_one<MIXED>(sc, cx, out, gacc, i, (size_t)(i - first_row), visible, aux, shrow, wrow);
+  if (active) project_bwd_one<MIXED>(sc, cx, out, gacc, i, (size_t)(i - first_row), visible, aux, shrow);
   if ((out.flags & B2R_BWD_SCRATCH_ZEROED) && in_range && visible) {  // leave the accumulator clean for the next render
     float4* row = reinterpret_cast<float4*>(const_cast<float*>(gacc)) + 3 * (size_t)i;
     row[0] = row[1] = row[2] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -358,8 +311,7 @@ int launch_project_bwd(const B2RScene& sc, const Ctx& cx, const B2RBackwardArgs&
   ProfScope p(K_PROJECT_BWD, st, grid > 0 ? 1 : 0);
   if (grid > 0) {
     const bool use_sh = sc.shs != nullptr && a.dL_dshs != nullptr;
-    const size_t smem = (use_sh ? (size_t)8 * 32 * ((sc.sh_coeffs * 3) | 1) * sizeof(float) : 0) +
-                        (sc.skin_xyz ? (size_t)8 * 32 * (sc.skin_J | 1) * sizeof(float) : 0);
+    const size_t smem = use_sh ? (size_t)8 * 32 * ((sc.sh_coeffs * 3) | 1) * sizeof(float) : 0;
     // the shared-memory ceiling is an attribute of the kernel on the current device: set once per device, not per launch
     static std::atomic<uint64_t> attr_set{0};
     int dev = 0;

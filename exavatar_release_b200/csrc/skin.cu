@@ -3,20 +3,69 @@
 // ExAvatar poses `mean_3d` and `mean_3d_refined` of its human Gaussians with the same weight rows, joint transforms,
 // root translation and camera (avatar/common/nets/module.py:549-557), each through a (P,55) gather, a (P,55)x(55,16)
 // matmul into (P,4,4), a bmm and a torch.inverse.  Here one thread per Gaussian blends M = sum_j w_j A_j once
-// (gaussian_math.cuh skin_blend, the blend the projection kernels evaluate for B2RScene.skin_*) and applies it to both
-// canonical sets; the weight rows are read through the (P) row index straight from the (V,J) table, never gathered.
+// (skin_blend) and applies it to both canonical sets; the weight rows are read through the (P) row index straight from
+// the (V,J) table, never gathered.
 //
-// Backward: per Gaussian, g_cam = Rinv^T dL/dposed and dL/dx = M3^T g_cam (skin_transpose, shared with K6); M is
-// recomputed, not stored.  The joint gradient dL/dA_j[:3,:] = sum_i w_ij sum_s g_cam,s,i [x_s,i, 1]^T is reduced
-// DETERMINISTICALLY: each warp accumulates its 32 Gaussians in lane order into a shared-memory (J,12) table (only the
-// non-zero weights of a row are visited), the block adds its eight warp tables in warp order and writes one partial
-// row to the scratch, and skin_reduce_kernel sums the partials in a fixed order -- no float atomics, bit-identical runs.
+// Backward: per Gaussian, g_cam = Rinv^T dL/dposed and dL/dx = M3^T g_cam (skin_transpose); M is recomputed, not
+// stored.  The joint gradient dL/dA_j[:3,:] = sum_i w_ij sum_s g_cam,s,i [x_s,i, 1]^T is reduced DETERMINISTICALLY:
+// each warp accumulates its 32 Gaussians in lane order into a shared-memory (J,12) table (only the non-zero weights of a
+// row are visited), the block adds its eight warp tables in warp order and writes one partial row to the scratch, and
+// skin_reduce_kernel sums the partials in a fixed order -- no float atomics, bit-identical runs.
 //
-// Compiled WITHOUT fma contraction (build_ext.py PER_FILE_FLAGS), like project.cu: skin_apply then rounds exactly as
-// the projection kernel's fused skinning does, and the posed positions of the two paths agree bit for bit.
-#include "gaussian_math.cuh"
+// Compiled WITHOUT fma contraction (build_ext.py PER_FILE_FLAGS): skin_apply rounds every product and sum on its own,
+// so the posed positions the renders read do not move in the last bits.
+#include "common.cuh"
 
 namespace b2r {
+
+// Linear-blend skinning (avatar/common/nets/module.py:413-422, 555-557):
+//   M = sum_j w_j A_j (rows 0..2 of the 4x4),  posed = M [x,1] + trans,  world = Rinv (posed - t)
+// `wrow` is the Gaussian's weight row in the warp's shared-memory stage, `A` the (J,16) row-major joint transforms in
+// global memory (warp-uniform addresses: one broadcast line per load).
+__device__ __forceinline__ void skin_blend(const float* __restrict__ A, const int J, const float* __restrict__ wrow,
+                                           float* M) {
+#pragma unroll
+  for (int k = 0; k < 12; k++) M[k] = 0.f;
+  for (int j = 0; j < J; j++) {
+    const float w = wrow[j];
+    if (w != 0.f) {  // SMPL-X skinning weights are sparse (a handful of joints per vertex)
+#pragma unroll
+      for (int k = 0; k < 12; k++) M[k] = fmaf(w, __ldg(A + 16 * j + k), M[k]);
+    }
+  }
+}
+
+// posed = M [x,1] + trans; then Rinv (posed - t) when Rinv is given
+__device__ __forceinline__ float3 skin_apply(const float* M, const float3 x, const float* __restrict__ trans,
+                                             const float* __restrict__ Rinv, const float* __restrict__ t) {
+  float px = M[0] * x.x + M[1] * x.y + M[2] * x.z + M[3] + __ldg(trans);
+  float py = M[4] * x.x + M[5] * x.y + M[6] * x.z + M[7] + __ldg(trans + 1);
+  float pz = M[8] * x.x + M[9] * x.y + M[10] * x.z + M[11] + __ldg(trans + 2);
+  if (Rinv) {
+    const float dx = px - __ldg(t), dy = py - __ldg(t + 1), dz = pz - __ldg(t + 2);
+    px = __ldg(Rinv) * dx + __ldg(Rinv + 1) * dy + __ldg(Rinv + 2) * dz;
+    py = __ldg(Rinv + 3) * dx + __ldg(Rinv + 4) * dy + __ldg(Rinv + 5) * dz;
+    pz = __ldg(Rinv + 6) * dx + __ldg(Rinv + 7) * dy + __ldg(Rinv + 8) * dz;
+  }
+  return make_float3(px, py, pz);
+}
+
+// Transpose of skin_apply for one Gaussian, `g` the gradient at the output position:
+//   g_cam = Rinv^T g  (g itself without Rinv),  dL/dx = M3^T g_cam;
+// the Gaussian's share of dL/dA_j[:3, :] is w_j g_cam [x, 1]^T and of dL/dtrans g_cam.  `gc` may alias `g`.
+__device__ __forceinline__ void skin_transpose(const float* M, const float* __restrict__ Rinv, const float* g, float* gc,
+                                               float* dx) {
+  const float g0 = g[0], g1 = g[1], g2 = g[2];
+  if (Rinv) {
+    gc[0] = __ldg(Rinv) * g0 + __ldg(Rinv + 3) * g1 + __ldg(Rinv + 6) * g2;
+    gc[1] = __ldg(Rinv + 1) * g0 + __ldg(Rinv + 4) * g1 + __ldg(Rinv + 7) * g2;
+    gc[2] = __ldg(Rinv + 2) * g0 + __ldg(Rinv + 5) * g1 + __ldg(Rinv + 8) * g2;
+  } else {
+    gc[0] = g0; gc[1] = g1; gc[2] = g2;
+  }
+#pragma unroll
+  for (int c = 0; c < 3; c++) dx[c] = M[c] * gc[0] + M[4 + c] * gc[1] + M[8 + c] * gc[2];
+}
 
 constexpr int SKIN_THREADS = 256;
 constexpr int SKIN_WARPS = SKIN_THREADS / 32;

@@ -7,8 +7,8 @@
 // allocation, the saved context, the backward call -- as a C++ torch::autograd::Function over the SAME C ABI
 // (include/b200raster.h, libb200raster.so).  No kernels here and no second implementation of anything on the device.
 //
-// Scope: the plain (un-skinned) rasteriser call with adaptive capacity.  rasterizer.py keeps the Python route for
-// debug=True (snapshot dump on failure), fixed-capacity / CUDA-graph capture, statistics requests and fused skinning.
+// Scope: the rasteriser call with adaptive capacity.  rasterizer.py keeps the Python route for debug=True (snapshot
+// dump on failure), fixed-capacity / CUDA-graph capture and statistics requests.
 #include <torch/extension.h>
 
 #include <c10/cuda/CUDAGuard.h>

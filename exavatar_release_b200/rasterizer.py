@@ -117,9 +117,7 @@ class _Context:
     __slots__ = ("scene", "ws", "keep", "ctx_buf", "dup_ids", "num_dups", "P", "W", "H", "M", "flags", "ckpt")
 
 
-def _make_scene(settings: GaussianRasterizationSettings, means3D, shs, colors, opac, scales, rots, cov, flags, skin=None):
-    """`skin` (fused skinning, SURVEY section 8f-2): dict(xyz, weights, joint_mats, trans, Rinv, t); `means3D` is then the
-    (P,3) tensor that RECEIVES the posed positions."""
+def _make_scene(settings: GaussianRasterizationSettings, means3D, shs, colors, opac, scales, rots, cov, flags):
     dev = means3D.device
     keep = {
         "bg": _f32c(settings.bg.to(dev), "bg"),
@@ -142,14 +140,7 @@ def _make_scene(settings: GaussianRasterizationSettings, means3D, shs, colors, o
     sc.viewmatrix = _ptr(keep["view"])
     sc.projmatrix = _ptr(keep["proj"])
     sc.campos = _ptr(keep["campos"])
-    sc.means3D = None if skin is not None else _ptr(means3D)
-    if skin is not None:
-        keep["skin"] = skin
-        sc.skin_xyz, sc.skin_weights = _ptr(skin["xyz"]), _ptr(skin["weights"])
-        sc.skin_joint_mats, sc.skin_trans = _ptr(skin["joint_mats"]), _ptr(skin["trans"])
-        sc.skin_cam_Rinv, sc.skin_cam_t = _ptr(skin.get("Rinv")), _ptr(skin.get("t"))
-        sc.skin_means_out = _ptr(means3D)
-        sc.skin_J = int(skin["weights"].shape[1])
+    sc.means3D = _ptr(means3D)
     sc.shs = _ptr(shs)
     sc.colors_precomp = _ptr(colors)
     sc.opacities = _ptr(opac)
@@ -159,7 +150,7 @@ def _make_scene(settings: GaussianRasterizationSettings, means3D, shs, colors, o
     return sc, keep
 
 
-def _forward_impl(settings, means3D, shs, colors, opac, scales, rots, cov, want_stats=False, skin=None, need_grad=True):
+def _forward_impl(settings, means3D, shs, colors, opac, scales, rots, cov, want_stats=False, need_grad=True):
     """need_grad: a backward may follow, so the forward composite also stores its blend-state checkpoints (the segmented
     backward replays 512-entry list segments independently from them); inference calls skip that buffer."""
     lib = L.load()
@@ -178,7 +169,7 @@ def _forward_impl(settings, means3D, shs, colors, opac, scales, rots, cov, want_
     with torch.cuda.device(dev):
         stream = torch.cuda.current_stream(dev)
         sptr = stream.cuda_stream
-        sc, keep = _make_scene(settings, means3D, shs, colors, opac, scales, rots, cov, flags, skin)
+        sc, keep = _make_scene(settings, means3D, shs, colors, opac, scales, rots, cov, flags)
         st = None if FIXED_CAPACITY is not None else _state(dev)  # no pinned allocation inside a graph capture
         ctx_bytes = lib.b2r_ctx_bytes(P, W, H)
         ctx_buf = torch.empty(ctx_bytes, dtype=torch.uint8, device=dev)
@@ -269,17 +260,14 @@ def read_status(cx: _Context) -> dict:
     return L.read_status(cx.ctx_buf)
 
 
-def _backward_impl(cx: _Context, g_color, g_depth, g_alpha, g_posed=None):
+def _backward_impl(cx: _Context, g_color, g_depth, g_alpha):
     lib = L.load()
-    keep = cx.keep
-    dev = keep["means3D"].device
+    dev = cx.keep["means3D"].device
     P, M = cx.P, cx.M
     f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
     d_means3D, d_means2D, d_colors, d_opac = f(P, 3), f(P, 3), f(P, 3), f(P, 1)
     d_scales, d_rots, d_cov = f(P, 3), f(P, 4), f(P, 6)
     d_shs = f(P, M, 3) if M > 0 else None
-    skin = keep.get("skin")
-    d_xyz, d_G = (f(P, 3), f(P, 12)) if skin is not None else (None, None)
     with torch.cuda.device(dev):
         stream = torch.cuda.current_stream(dev)
         g_color = _f32c(g_color, "grad_color")
@@ -288,15 +276,11 @@ def _backward_impl(cx: _Context, g_color, g_depth, g_alpha, g_posed=None):
         sbytes = lib.b2r_backward_scratch_bytes(P)
         scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
         args = L.B2RBackwardArgs(_ptr(g_color), _ptr(g_depth), _ptr(g_alpha), _ptr(d_means3D), _ptr(d_means2D),
-                                 _ptr(d_shs), _ptr(d_colors), _ptr(d_opac), _ptr(d_scales), _ptr(d_rots), _ptr(d_cov),
-                                 0, 0, None, None, None, _ptr(d_xyz), _ptr(d_G),
-                                 None if g_posed is None else _ptr(_f32c(g_posed, "grad_posed")))
+                                 _ptr(d_shs), _ptr(d_colors), _ptr(d_opac), _ptr(d_scales), _ptr(d_rots), _ptr(d_cov))
         L.check(lib.b2r_backward(C.byref(cx.scene), C.byref(cx.ws), C.byref(args), scratch.data_ptr(), sbytes,
                                  stream.cuda_stream), "b2r_backward")
         if cx.flags & L.B2R_FLAG_DEBUG:
             stream.synchronize()
-    if skin is not None:
-        return d_means3D, d_means2D, d_shs, d_colors, d_opac, d_scales, d_rots, d_cov, d_xyz, d_G
     return d_means3D, d_means2D, d_shs, d_colors, d_opac, d_scales, d_rots, d_cov
 
 
@@ -430,64 +414,19 @@ class GaussianRasterizer(nn.Module):
                                    raster_settings)
 
 
-# ---------------------------------------------------------------------------------------------------------------
-# SURVEY.md section 8f-2: linear-blend skinning fused into the projection kernels
-# ---------------------------------------------------------------------------------------------------------------
-class _RasterizeSkinned(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, xyz, skin_weights, joint_mats, trans, cam_R, cam_t, means2D, colors_precomp, opacities, scales,
-                rotations, raster_settings):
-        dev = xyz.device
-        P = xyz.shape[0]
-        skin = {"xyz": _f32c(xyz, "xyz"), "weights": _f32c(skin_weights, "skin_weights"),
-                "joint_mats": _f32c(joint_mats, "joint_mats").reshape(-1, 16), "trans": _f32c(trans.reshape(3), "trans")}
-        if cam_R is not None:
-            skin["Rinv"] = _f32c(_inv3(cam_R), "cam_R")
-            skin["t"] = _f32c(cam_t.reshape(3), "cam_t")
-        posed = torch.empty((P, 3), dtype=torch.float32, device=dev)
-        color, radii, depth, alpha, cx = _forward_impl(raster_settings, posed, None, _f32c(colors_precomp, "colors_precomp"),
-                                                       _f32c(opacities, "opacities"), _f32c(scales, "scales"),
-                                                       _f32c(rotations, "rotations"), None, skin=skin,
-                                                       need_grad=any(ctx.needs_input_grad))
-        ctx.set_materialize_grads(False)
-        ctx.cx = cx
-        ctx.shapes = (means2D.shape, opacities.shape, joint_mats.shape, trans.shape)
-        ctx.mark_non_differentiable(radii)
-        return color, radii, depth, alpha, posed
-
-    @staticmethod
-    def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha, grad_posed):
-        cx = ctx.cx
-        if grad_color is None and grad_depth is None and grad_alpha is None and grad_posed is None:
-            return (None,) * 12
-        if grad_color is None:  # only depth / alpha / the posed positions were used downstream
-            grad_color = torch.zeros((3, cx.H, cx.W), dtype=torch.float32, device=cx.keep["means3D"].device)
-        m2s, ops, js, ts = ctx.shapes
-        # `posed` is differentiable: ExAvatar reads the posed mean_3d elsewhere (face_mesh_renderer, model.py:172-173, and
-        # the cat(scene.detach(), human) renders, model.py:117-125); its gradient joins dL/dworld inside the backward
-        # projection kernel, i.e. d_xyz += M^T Rinv^T g, d_G += (Rinv^T g) [x, 1]^T
-        _, d_m2, _, d_col, d_op, d_sc, d_rot, _, d_xyz, d_G = _backward_impl(cx, grad_color, grad_depth, grad_alpha, grad_posed)
-        W = cx.keep["skin"]["weights"]
-        J = W.shape[1]
-        d_joint = torch.zeros((J, 4, 4), dtype=torch.float32, device=W.device)
-        d_joint[:, :3, :] = _tall_skinny_tn(W, d_G).view(J, 3, 4)  # the one dense contraction of this path: library GEMMs
-        d_trans = d_G.view(-1, 3, 4)[:, :, 3].sum(0)
-        return (d_xyz, None, d_joint.reshape(js), d_trans.reshape(ts), None, None, d_m2.reshape(m2s), d_col,
-                d_op.reshape(ops), d_sc, d_rot, None)
-
-
 class SkinnedGaussianRasterizer(nn.Module):
-    """`GaussianRasterizer` with ExAvatar's linear-blend skinning in front of it, evaluated inside the projection
-    kernels: replaces `get_transform_mat_vertex` + `lbs` + the camera->world transform
-    (avatar/common/nets/module.py:413-422, 549-557) AND the rasteriser call (module.py:632-640) for the human Gaussians.
+    """`GaussianRasterizer` with ExAvatar's linear-blend skinning in front of it: replaces `get_transform_mat_vertex` +
+    `lbs` + the camera->world transform (avatar/common/nets/module.py:413-422, 549-557) AND the rasteriser call
+    (module.py:632-640) for the human Gaussians.
 
         color, radii, depth, alpha, posed = SkinnedGaussianRasterizer(settings)(
             xyz, skin_weights, joint_mats, trans, cam_R, cam_t, means2D, opacities, colors_precomp, scales, rotations)
 
     xyz (P,3) canonical positions; skin_weights (P,J) rows gathered per Gaussian (module.py:414); joint_mats (J,4,4);
     trans (3); cam_R (3,3) / cam_t (3) or None to stay in the posed frame (`is_world_coord=True`).  `posed` (P,3) is the
-    world position ExAvatar's other modules read; it is a differentiable output: a gradient arriving at it is added to
-    dL/dworld inside the backward projection kernel and reaches xyz, joint_mats and trans like the render's own."""
+    world position ExAvatar's other modules read, a differentiable output.  The call is `skinning.skin_gaussians`
+    followed by `GaussianRasterizer` on the posed positions: autograd adds a gradient arriving at `posed` to the
+    render's own, and the skinning op's backward carries the sum to xyz, joint_mats and trans."""
 
     def __init__(self, raster_settings):
         super().__init__()
@@ -495,23 +434,12 @@ class SkinnedGaussianRasterizer(nn.Module):
 
     def forward(self, xyz, skin_weights, joint_mats, trans, cam_R, cam_t, means2D, opacities, colors_precomp, scales,
                 rotations):
-        return _RasterizeSkinned.apply(xyz, skin_weights, joint_mats, trans, cam_R, cam_t, means2D, colors_precomp,
-                                       opacities, scales, rotations, self.raster_settings)
-
-
-def _tall_skinny_tn(W: torch.Tensor, G: torch.Tensor, chunks: int = 64) -> torch.Tensor:
-    """W^T G for W (P,J), G (P,n) with P ~ 10^5 and J, n ~ 10: a batched GEMM over `chunks` row blocks plus a tiny sum.
-    A single (J x P)(P x n) GEMM leaves the library with one long-K tile and, depending on its heuristic, almost no
-    parallelism; the batched form always fills the machine."""
-    P, J = W.shape
-    n = G.shape[1]
-    pad = (-P) % chunks
-    if pad:
-        W = torch.cat((W, W.new_zeros(pad, J)))
-        G = torch.cat((G, G.new_zeros(pad, n)))
-    Wc = W.view(chunks, -1, J)
-    Gc = G.view(chunks, -1, n)
-    return torch.bmm(Wc.transpose(1, 2), Gc).sum(0)
+        from .skinning import skin_gaussians  # skinning.py imports this module's tensor helpers
+        posed = skin_gaussians(xyz, None, skin_weights, None, joint_mats, trans, cam_R, cam_t)[0]
+        color, radii, depth, alpha = GaussianRasterizer(self.raster_settings)(
+            means3D=posed, means2D=means2D, opacities=opacities, colors_precomp=colors_precomp, scales=scales,
+            rotations=rotations)
+        return color, radii, depth, alpha, posed
 
 
 def _inv3(R: torch.Tensor) -> torch.Tensor:

@@ -151,8 +151,9 @@ def scene_gaussian_assets(mean, opacity_logit, log_scale, rotation, feature_dc, 
 
 def lbs_reference(xyz, skin_weights, joint_mats, trans, cam_R=None, cam_t=None, cam_R_inv=None):
     """Caller-side mirror of how `HumanGaussian.forward` poses its Gaussians -- `get_transform_mat_vertex`, `lbs` and the
-    camera->world transform, op for op (module.py:413-422, 555-557); device-agnostic, differentiable.  This is the unfused
-    path `SkinnedGaussianRasterizer` (SURVEY section 8f-2) is compared against; the product path never calls it.
+    camera->world transform, op for op (module.py:413-422, 555-557); device-agnostic, differentiable.  This is the
+    reference the skinning op `skinning.skin_gaussians` and `SkinnedGaussianRasterizer` (SURVEY section 8f-2) are
+    compared against; the product path never calls it.
     `cam_R_inv` (optional) skips the `torch.inverse` call, e.g. inside a CUDA-graph capture."""
     P, J = skin_weights.shape
     tmv = torch.matmul(skin_weights, joint_mats.reshape(J, 16)).view(P, 4, 4)

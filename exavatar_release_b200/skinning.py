@@ -13,9 +13,7 @@ those colours.  `skin_gaussians` replaces those lines: one kernel blends M_i = s
 (reading the (V,J) weight table through the row index, without the (P,55) gather) and applies it to both sets; the
 backward recomputes M and reduces the joint-transform gradient deterministically (include/b200raster.h B2RSkin).
 
-It evaluates the same device code as `SkinnedGaussianRasterizer`, which stays the route for a single render that poses
-inside its projection kernel (the posed positions are then an optional by-product); the two write bit-identical posed
-positions.  CUDA tensors only: there is no CPU path.
+`rasterizer.SkinnedGaussianRasterizer` is this op followed by one render.  CUDA tensors only: there is no CPU path.
 """
 from __future__ import annotations
 

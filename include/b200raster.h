@@ -33,7 +33,7 @@
 extern "C" {
 #endif
 
-#define B2R_ABI_VERSION 3
+#define B2R_ABI_VERSION 4
 
 #define B2R_OK 0
 #define B2R_E_INVALID (-1)      /* bad argument (null pointer, negative size, both / neither colour source, sh_rows > P ...) */
@@ -69,21 +69,6 @@ typedef struct B2RScene {
   const float* scales;        /* (P,3) or NULL */
   const float* rotations;     /* (P,4) (r,x,y,z), used un-normalised, or NULL */
   const float* cov3D_precomp; /* (P,6) or NULL  (exactly one of scales+rotations / cov3D_precomp) */
-  /* Optional fused linear-blend skinning in front of the projection (SURVEY section 8f-2).  ExAvatar poses its human
-   * Gaussians with  M_i = sum_j w_ij A_j,  posed_i = M_i [xyz_i, 1] + trans,  world_i = Rinv (posed_i - t)
-   * (avatar/common/nets/module.py:413-422 `get_transform_mat_vertex` / `lbs`, module.py:555-557) as five PyTorch
-   * kernels that write a (P,4,4) matrix per Gaussian.  With skin_xyz != NULL the projection kernels evaluate this per
-   * Gaussian in registers instead of reading `means3D` (which may then be NULL); the backward emits the gradient with
-   * respect to the canonical positions and the per-Gaussian outer products the joint-transform gradient is a GEMM of
-   * (B2RBackwardArgs.dL_dskin_xyz / dL_dskin_G). */
-  const float* skin_xyz;        /* (P,3) canonical ("big pose") positions, or NULL = no skinning */
-  const float* skin_weights;    /* (P,J) skinning weights of each Gaussian (rows already gathered, module.py:414) */
-  const float* skin_joint_mats; /* (J,16) row-major 4x4 transform per joint (module.py:385-411) */
-  const float* skin_trans;      /* (3) root translation added after blending (module.py:421) */
-  const float* skin_cam_Rinv;   /* (9) row-major inverse camera rotation, or NULL to stay in the posed frame */
-  const float* skin_cam_t;      /* (3) camera translation (used with skin_cam_Rinv) */
-  float* skin_means_out;        /* (P,3) optional OUTPUT: the posed world positions (other ExAvatar modules read them) */
-  int32_t skin_J;               /* joints (55 for SMPL-X); <= 64 */
   /* Mixed colour source.  0: exactly one of shs / colors_precomp colours every Gaussian.  0 < sh_rows <= P: BOTH are
    * required; Gaussians [0, sh_rows) are coloured from `shs`, which then holds sh_rows rows of sh_coeffs coefficients
    * (sh_degree / sh_coeffs rules as above), and Gaussians [sh_rows, P) read colors_precomp[i] -- the global index, so
@@ -180,17 +165,6 @@ typedef struct B2RBackwardArgs {
   float* densify_grad_accum;
   float* densify_count;
   float* densify_radius_max;
-  /* Fused skinning (B2RScene.skin_*), each may be NULL:
-   *   dL_dskin_xyz (P,3):  gradient w.r.t. the canonical positions,  (M_i[:3,:3])^T Rinv^T dL/dworld_i
-   *   dL_dskin_G   (P,12): row-major 3x4 outer product  (Rinv^T dL/dworld_i) [xyz_i, 1]^T ; the joint-transform gradient
-   *                        is the plain GEMM  dL/dA[:, :3, :] = W^T G  and  dL/dtrans = sum_i G_i[:, 3].
-   * Both follow `flags` (write / accumulate) and `first_row` like every other output. */
-  float* dL_dskin_xyz;
-  float* dL_dskin_G;
-  /* INPUT (ABI v3), (P,3) or NULL: gradient arriving at the posed world positions the forward wrote to
-   * B2RScene.skin_means_out (other ExAvatar modules read them: face_mesh_renderer, avatar/main/model.py:172-173); it is
-   * added to dL/dworld_i before the skinning transpose, so it reaches dL_dskin_xyz / dL_dskin_G (and dL_dmeans3D). */
-  const float* dL_dposed;
   /* (ABI v3) the densification statistics above are updated for Gaussians [0, densify_rows) only; 0 = all.  A merged
    * cat(scene, human) pass keeps ExAvatar's bookkeeping to the scene Gaussians this way (model.py:193). */
   uint32_t densify_rows;
@@ -200,8 +174,8 @@ typedef struct B2RBackwardArgs {
  * `mean_3d` and `mean_3d_refined` of its human Gaussians with the same weight rows, joint transforms, translation and
  * camera (avatar/common/nets/module.py:549-557):  M_i = sum_j W[rows[i], j] A_j,  posed_s,i = M_i [xyz_s,i, 1] + trans,
  * then Rinv (posed - t) with a camera.  b2r_skin_forward blends M_i once per Gaussian and writes both posed sets, which
- * the caller's normal / colour networks and the renders then read -- unlike B2RScene.skin_*, which poses inside one
- * render's projection.  Same device code as that fused path: the posed positions agree bit for bit. */
+ * the caller's normal / colour networks and the renders then read as B2RScene.means3D.  It poses ahead of the render
+ * rather than inside its projection because those networks need the posed positions before anything is rendered. */
 typedef struct B2RSkin {
   int32_t P;                /* Gaussians per set */
   int32_t J;                /* joints (55 for SMPL-X); 1..64 */
@@ -288,16 +262,17 @@ int b2r_forward_project_split(const B2RScene* scene, const B2RWorkspace* ws, uin
 int b2r_forward_bin_split(const B2RScene* scene, const B2RWorkspace* ws, const B2RWorkspace* base, uint32_t first_row,
                           int32_t* radii, void* stream);
 
-/* Skinning (B2RSkin).  Forward: writes posed[0] and, when given, posed[1].  Backward: dL_dposed (host array of two
- * device pointers; either may be NULL = no gradient reaches that set, dL_dposed[1] requires xyz[1]) ->
- *   dL_dxyz[s]  (P,3) = M_i[:3,:3]^T g_cam,s,i  with  g_cam = Rinv^T dL/dposed  (zeros when dL_dposed[s] is NULL);
+/* Skinning (B2RSkin).  Forward: writes posed[0] and, when given, posed[1].  Backward: dL_dpos (host array of two
+ * device pointers, the gradients at posed[0] / posed[1]; either may be NULL = no gradient reaches that set, dL_dpos[1]
+ * requires xyz[1]) ->
+ *   dL_dxyz[s]  (P,3) = M_i[:3,:3]^T g_cam,s,i  with  g_cam = Rinv^T dL/dposed  (zeros when dL_dpos[s] is NULL);
  *   dL_djoint (J,3,4) = sum_i W[rows[i], j] sum_s g_cam,s,i [xyz_s,i, 1]^T   (row 3 of each 4x4 has no gradient);
  *   dL_dtrans (3)     = sum_i sum_s g_cam,s,i.
  * dL_dxyz (host array) and each output may be NULL.  The joint / translation sums are deterministic (block partials
  * added in a fixed order, no float atomics): bit-identical from run to run.  `scratch` >= b2r_skin_scratch_bytes(P, J)
  * when dL_djoint or dL_dtrans is given.  No gradient for the weights or the camera.  Neither call allocates or syncs. */
 int b2r_skin_forward(const B2RSkin* skin, void* stream);
-int b2r_skin_backward(const B2RSkin* skin, const float* const dL_dposed[2], float* const dL_dxyz[2], float* dL_djoint,
+int b2r_skin_backward(const B2RSkin* skin, const float* const dL_dpos[2], float* const dL_dxyz[2], float* dL_djoint,
                       float* dL_dtrans, void* scratch, size_t scratch_bytes, void* stream);
 size_t b2r_skin_scratch_bytes(int32_t P, int32_t J);
 

@@ -31,7 +31,7 @@ def test_library_exports_every_declared_symbol():
 
 def test_struct_layouts_and_version():
     lib = L.load()
-    assert lib.b2r_abi_version() == 3 == L.ABI_VERSION
+    assert lib.b2r_abi_version() == 4 == L.ABI_VERSION
     for idx, cls in enumerate((L.B2RScene, L.B2RStatus, L.B2RWorkspace, L.B2RForwardOutputs, L.B2RBackwardArgs, L.B2RView)):
         assert lib.b2r_sizeof(idx) == C.sizeof(cls)
     assert lib.b2r_sizeof(99) == 0
@@ -103,8 +103,8 @@ def test_kernel_names():
 
 
 def test_error_codes_of_the_round1_additions_without_touching_cuda():
-    """Validation of the fields added in ABI v2 (fused skinning, detached prefix, SH row limit, id width) happens on the
-    host before any launch, so it is testable without a GPU."""
+    """Validation of means3D, the detached prefix, the SH row limit and the id width happens on the host before any
+    launch, so it is testable without a GPU."""
     lib = L.load()
     fake = 0x1000
     sc = L.B2RScene()
@@ -115,23 +115,8 @@ def test_error_codes_of_the_round1_additions_without_touching_cuda():
     ws.ctx, ws.ctx_bytes = fake, 16  # too small on purpose: a scene that validates reaches the workspace check (-2)
     out = L.B2RForwardOutputs()
     fwd = lambda: lib.b2r_forward(C.byref(sc), C.byref(ws), C.byref(out), None)
-    assert fwd() == -1                      # neither means3D nor skinning
+    assert fwd() == -1                      # no means3D
     sc.means3D = fake
-    assert fwd() == -2
-    # fused skinning replaces means3D, but needs all of its inputs and a sane joint count
-    sc.means3D = None
-    sc.skin_xyz = fake
-    assert fwd() == -1
-    sc.skin_weights = sc.skin_joint_mats = sc.skin_trans = fake
-    sc.skin_J = 0
-    assert fwd() == -1
-    sc.skin_J = 65
-    assert fwd() == -1
-    sc.skin_J = 55
-    assert fwd() == -2
-    sc.skin_cam_Rinv = fake                 # camera rotation without its translation
-    assert fwd() == -1
-    sc.skin_cam_t = fake
     assert fwd() == -2
     # SH rows are staged through shared memory: at most 16 coefficients, degree <= 3, enough coefficients for the degree
     sc.colors_precomp = None
@@ -162,7 +147,7 @@ def test_error_codes_of_the_round1_additions_without_touching_cuda():
 
 
 def test_error_codes_of_the_abi_v3_entry_points_without_touching_cuda():
-    """Views, the split pipeline stages, the checkpoint store and the posed-position gradient are validated on the host."""
+    """Views, the split pipeline stages and the checkpoint store are validated on the host."""
     lib = L.load()
     fake = 0x1000
     sc = L.B2RScene()
@@ -207,10 +192,6 @@ def test_error_codes_of_the_abi_v3_entry_points_without_touching_cuda():
     assert bp(None, 1 << 20) == -1
     args.first_row = 11
     assert bc(fake, 1 << 20) == -1 and bp(fake, 1 << 20) == -1
-    args.first_row = 0
-    args.dL_dposed = fake                    # a posed-position gradient only makes sense with fused skinning
-    assert bp(fake, 1 << 20) == -1
-    assert lib.b2r_backward(C.byref(sc), C.byref(ws), C.byref(args), fake, 1 << 20, None) == -1
     # split pass: the own sorted ids ride behind the keys, 4 bytes per duplicate slot, aligned like every other region
     for cap in (0, 1, 64, 1000, 1 << 20):
         extra = -(-4 * max(cap, 1) // 256) * 256

@@ -38,9 +38,10 @@ def test_sh_rows_takes_the_place_of_the_reserved_field():
     assert C.sizeof(L.B2RScene) == lib.b2r_sizeof(0)
     names = [f[0] for f in L.B2RScene._fields_]
     assert "skin_reserved" not in names and names[-1] == "sh_rows"
-    # the old reserved int32 sat right after skin_J, at the end of the struct
-    assert L.B2RScene.sh_rows.offset == L.B2RScene.skin_J.offset + 4
-    assert L.B2RScene.sh_rows.offset + 4 == C.sizeof(L.B2RScene)
+    # the int32 sits right after the last per-Gaussian pointer, at the end of the struct (then 4 bytes of tail padding
+    # to the pointers' 8-byte alignment)
+    assert L.B2RScene.sh_rows.offset == L.B2RScene.cov3D_precomp.offset + 8
+    assert L.B2RScene.sh_rows.offset + 8 == C.sizeof(L.B2RScene)
     assert L.B2RScene.sh_rows.size == 4
 
 

@@ -1,8 +1,8 @@
-"""SURVEY.md section 8f-2: linear-blend skinning fused into the projection kernels.
+"""SURVEY.md section 8f-2: `SkinnedGaussianRasterizer`, linear-blend skinning in front of the rasteriser.
 
 The unfused path is ExAvatar's own sequence of PyTorch ops (`get_transform_mat_vertex`, `lbs`, camera->world:
 avatar/common/nets/module.py:413-422, 555-557; restated op for op in `renderer.lbs_reference`) followed by the
-rasteriser.  The fused path evaluates the same blend per Gaussian inside the projection kernels and returns gradients
+rasteriser.  `SkinnedGaussianRasterizer` poses with the skinning op (`skinning.skin_gaussians`) and returns gradients
 with respect to the canonical positions, the joint transforms and the root translation.  The two paths round the
 posed positions differently (a (P,55)x(55,16) GEMM vs. a sparse in-register blend), so discrete per-(pixel, splat)
 decisions that sit on a threshold may flip; the comparison therefore allows a small fraction of outliers, like the
@@ -114,8 +114,8 @@ def test_fused_skinning_matches_the_unfused_path(world):
 def test_posed_positions_of_the_fused_path_are_differentiable(only_posed):
     """ExAvatar reads the posed mean_3d outside the rasteriser too (face_mesh_renderer, avatar/main/model.py:172-173; the
     cat(scene.detach(), human) renders, model.py:117-125).  A loss that touches `posed` must reach xyz, the joint
-    transforms and the translation through the fused path exactly as through the unfused ops -- for Gaussians the render
-    culled as well, and also when the image is not used at all."""
+    transforms and the translation through SkinnedGaussianRasterizer exactly as through the unfused ops -- for Gaussians
+    the render culled as well, and also when the image is not used at all."""
     from exavatar_release_b200 import rasterizer as RZ
     dev = torch.device("cuda:0")
     H, W = 96, 128
@@ -156,13 +156,9 @@ def test_posed_positions_of_the_fused_path_are_differentiable(only_posed):
 
 
 def test_host_helpers_of_the_skinning_backward():
-    """`_inv3` (graph-capturable 3x3 inverse) and `_tall_skinny_tn` (W^T G as a batched GEMM) against the plain ops."""
-    from exavatar_release_b200.rasterizer import _inv3, _tall_skinny_tn
+    """`_inv3` (graph-capturable 3x3 inverse) against torch.inverse."""
+    from exavatar_release_b200.rasterizer import _inv3
     g = torch.Generator().manual_seed(11)
     for _ in range(5):
         R = torch.randn(3, 3, generator=g, dtype=torch.float64) + 2 * torch.eye(3, dtype=torch.float64)
         assert torch.allclose(_inv3(R), torch.inverse(R), rtol=1e-10, atol=1e-12)
-    for P, J, n, chunks in ((1000, 55, 12, 64), (1001, 7, 3, 8), (5, 4, 2, 64)):
-        W = torch.rand(P, J, generator=g, dtype=torch.float64)
-        G = torch.randn(P, n, generator=g, dtype=torch.float64)
-        assert torch.allclose(_tall_skinny_tn(W, G, chunks), W.t() @ G, rtol=1e-10, atol=1e-10)

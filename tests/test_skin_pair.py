@@ -4,7 +4,7 @@ ExAvatar poses `mean_3d` and `mean_3d_refined` with one rig (avatar/common/nets/
 rendered.  These tests pin
   * the C ABI (struct layout, exported symbols, host-side validation) and a float64 restatement of the backward
     formulas against autograd through `renderer.lbs_reference`, without a device;
-  * on the GPU at C4 human size: posed positions against lbs_reference, bit-identity with the fused skinning of
+  * on the GPU at C4 human size: posed positions against lbs_reference, bit-identity with the fifth output of
     `SkinnedGaussianRasterizer`, gradients against float64 autograd, bit-reproducible backward, CUDA-graph capture,
     and one C4 training frame through `TrainingFrameRenderer` posed by the op vs. by the unfused ops.
 """
@@ -31,7 +31,7 @@ J = 55
 
 def test_skin_struct_layout_and_symbols():
     lib = L.load()
-    assert lib.b2r_abi_version() == 3
+    assert lib.b2r_abi_version() == 4
     assert C.sizeof(L.B2RSkin) == lib.b2r_sizeof(6)
     assert lib.b2r_sizeof(7) == 0
     raw = C.CDLL(L.LIB_PATH)
@@ -84,7 +84,7 @@ def test_skin_validation_without_touching_cuda():
     s.xyz[1] = None
     assert fwd(s) == -1 and bwd(s) == -1                   # posed[1] without xyz[1]
     s.posed[1] = None
-    assert bwd(s) == -1                                    # dL_dposed[1] without xyz[1]
+    assert bwd(s) == -1                                    # dL_dpos[1] without xyz[1]
     s = _valid_skin()
     s.rows, s.V = None, 63
     assert fwd(s) == -1                                    # row i of the table without `rows`: V >= P
@@ -202,7 +202,7 @@ def test_posed_positions_match_lbs_reference(dev, world):
 
 @pytest.mark.gpu
 def test_posed_positions_equal_the_fused_rasteriser_bit_for_bit(dev):
-    """Same device code: the op and SkinnedGaussianRasterizer's fifth output write the same bits, for both sets."""
+    """The op and SkinnedGaussianRasterizer's fifth output write the same bits, for both sets."""
     from exavatar_release_b200 import rasterizer as RZ
     from exavatar_release_b200.skinning import skin_gaussians
     rig = _c4_rig(dev)

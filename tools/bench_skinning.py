@@ -1,8 +1,8 @@
-"""SURVEY.md section 8f-2 measurement: ExAvatar's human path (skinning ops + rasteriser, forward + backward) unfused vs fused.
+"""SURVEY.md section 8f-2 measurement: ExAvatar's human path (skinning + rasteriser, forward + backward), its ops vs ours.
 
   python tools/bench_skinning.py [--workload C4]
 Unfused = `lbs_reference` (the reference's five PyTorch ops, module.py:413-422, 555-557) + GaussianRasterizer;
-fused = SkinnedGaussianRasterizer.  Public autograd API, fixed-capacity mode, CUDA events, L2 flushed between iterations.
+fused = SkinnedGaussianRasterizer (the skinning op `skin_gaussians`, then GaussianRasterizer).  Public autograd API, fixed-capacity mode, CUDA events, L2 flushed between iterations.
 """
 import argparse
 import os
@@ -88,7 +88,10 @@ def main():
             fn(lv)
 
         out[name] = timed(eager)
-        # the same work captured in a CUDA graph: removes the host cost of the extra PyTorch launches from the picture
+        # the same work captured in a CUDA graph: removes the host cost of the extra PyTorch launches from the picture.
+        # Fresh leaves: the gradient-accumulation nodes of the eager ones belong to the default stream, which a capture
+        # may not wait on.
+        lv = leaves()
         side = torch.cuda.Stream(dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
