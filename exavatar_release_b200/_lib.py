@@ -85,6 +85,24 @@ class B2RGnMlp(C.Structure):
     ]
 
 
+class B2RRegs(C.Structure):
+    """ExAvatar's human regularisers (b2r_regs_forward / b2r_regs_backward): the inputs and the model's tables."""
+    _fields_ = [
+        ("P", C.c_int32), ("J", C.c_int32), ("n_arm", C.c_int32), ("n_pairs", C.c_int32), ("n_hand", C.c_int32),
+        ("n_rhand", C.c_int32), ("reserved", C.c_int32 * 2),
+        ("mesh", _fp), ("mean_offset", _fp), ("mean_offset_offset", _fp), ("scale_offset", _fp), ("scale", _fp),
+        ("scale_refined", _fp), ("rgb", _fp), ("rgb_refined", _fp), ("scale_reg", _fp), ("joint_offset", _fp),
+        ("faces", _fp), ("vf_offsets", _fp), ("vf_entries", _fp), ("nbr_idx", _fp), ("nbr_w", _fp),
+        ("lapT_offsets", _fp), ("lapT_src", _fp), ("lapT_w", _fp), ("weights", _fp), ("hand", _fp), ("arm_idx", _fp),
+        ("arm_slot", _fp), ("joint_target", _fp), ("joint_weight", _fp), ("sym_pairs", _fp),
+    ]
+
+
+class B2RRegsGrads(C.Structure):
+    _fields_ = [(n, _fp) for n in ("mean_offset", "mean_offset_offset", "scale_offset", "scale", "scale_refined", "rgb",
+                                   "rgb_refined", "scale_reg", "joint_offset")]
+
+
 class B2RForwardOutputs(C.Structure):
     _fields_ = [("color", _fp), ("depth", _fp), ("alpha", _fp), ("radii", _fp)]
 
@@ -165,6 +183,9 @@ SYMBOLS = [
     ("b2r_gn_mlp_grads_count", C.c_size_t, [C.c_int32, C.c_int32]),
     ("b2r_gn_mlp_forward", C.c_int, [C.POINTER(B2RGnMlp), _fp, _fp, _fp]),
     ("b2r_gn_mlp_backward", C.c_int, [C.POINTER(B2RGnMlp), _fp, _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
+    ("b2r_regs_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32]),
+    ("b2r_regs_forward", C.c_int, [C.POINTER(B2RRegs), _fp, _fp, C.c_size_t, _fp]),
+    ("b2r_regs_backward", C.c_int, [C.POINTER(B2RRegs), _fp, C.POINTER(B2RRegsGrads), _fp, C.c_size_t, _fp]),
     ("b2r_profile_enable", None, [C.c_int]),
     ("b2r_profile_read", C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int]),
     ("b2r_launch_count", C.c_uint64, []),
@@ -195,9 +216,11 @@ def load():
         fn.argtypes = argtypes
     if lib.b2r_abi_version() != ABI_VERSION:
         raise RuntimeError("b200raster: ABI version mismatch between the Python binding and libb200raster.so")
-    # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8, B2RGnMlp 10 (9 unused too)
+    # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8, B2RGnMlp 10 (9 unused too), B2RRegs 11,
+    # B2RRegsGrads 12
     for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
-                     (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp)):
+                     (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp), (11, B2RRegs),
+                     (12, B2RRegsGrads)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

@@ -36,8 +36,11 @@ NVCC_FLAGS = [
 # rounded products, two rounded sums), so the argmin -- ties included -- is the restatement's, index for index.
 # mesh_raster.cu: the face render's coverage test and depth pz are, operation for operation, the float32 restatement's
 # (mesh_render.face_render_reference), so the per-pixel face is identical to it instead of "equal except at ulp ties".
+# regularizers.cu: the arm window |fl(l_x - u_x)| < 0.01f and the fp32 distances that pick the 50 nearest upper-arm rows
+# are the reference's expressions rounded operation by operation, so the selection (ties included) is the reference's.
 PER_FILE_FLAGS = {"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
-                  "geometry.cu": ["--fmad=false"], "mesh_raster.cu": ["--fmad=false"]}
+                  "geometry.cu": ["--fmad=false"], "mesh_raster.cu": ["--fmad=false"],
+                  "regularizers.cu": ["--fmad=false"]}
 
 
 def sources():

@@ -102,6 +102,22 @@ int validate_gn_mlp(const B2RGnMlp* m) {
   return B2R_OK;
 }
 
+// regularizers.cu: the joint gradients are written by the threads of one CTA (J <= 256); every table is required,
+// and the means need at least one vertex, one joint and one symmetric pair
+int validate_regs(const B2RRegs* r) {
+  if (!r) return B2R_E_INVALID;
+  if (r->P < 1 || r->P >= (1 << 28) || r->J < 1 || r->J > 256 || r->n_arm < 0 || r->n_arm > r->P) return B2R_E_INVALID;
+  if (r->n_pairs < 1 || r->n_hand < 0 || r->n_rhand < 0 || r->n_hand > r->P) return B2R_E_INVALID;
+  if (!r->mesh || !r->mean_offset || !r->mean_offset_offset || !r->scale_offset || !r->scale || !r->scale_refined ||
+      !r->rgb || !r->rgb_refined || !r->joint_offset)
+    return B2R_E_INVALID;
+  if (!r->faces || !r->vf_offsets || !r->vf_entries || !r->nbr_idx || !r->nbr_w || !r->lapT_offsets || !r->lapT_src ||
+      !r->lapT_w || !r->weights || !r->hand || !r->arm_slot || (r->n_arm > 0 && !r->arm_idx) || !r->joint_target ||
+      !r->joint_weight || !r->sym_pairs)
+    return B2R_E_INVALID;
+  return B2R_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -132,6 +148,8 @@ size_t b2r_sizeof(int which) {
     case 6: return sizeof(B2RSkin);
     case 8: return sizeof(B2RMeshRender);  // 7 stays unused
     case 10: return sizeof(B2RGnMlp);  // 9 stays unused
+    case 11: return sizeof(B2RRegs);
+    case 12: return sizeof(B2RRegsGrads);
     default: return 0;
   }
 }
@@ -431,6 +449,29 @@ int b2r_gn_mlp_backward(const B2RGnMlp* m, const float* saved, const float* dL_d
   if (!saved || !dL_dout || !grads || !scratch) return B2R_E_INVALID;
   if (scratch_bytes < gn_mlp_scratch_bytes(m->P)) return B2R_E_WORKSPACE;
   return launch_gn_mlp_backward(*m, saved, dL_dout, dL_dx, grads, scratch, (cudaStream_t)stream);
+}
+
+size_t b2r_regs_scratch_bytes(int32_t P, int32_t n_arm) { return regs_scratch_bytes(P, n_arm); }
+
+int b2r_regs_forward(const B2RRegs* r, float* out, void* scratch, size_t scratch_bytes, void* stream) {
+  const int rc = validate_regs(r);
+  if (rc) return rc;
+  if (!out || !scratch) return B2R_E_INVALID;
+  if (scratch_bytes < regs_scratch_bytes(r->P, r->n_arm)) return B2R_E_WORKSPACE;
+  return launch_regs_forward(*r, out, scratch, (cudaStream_t)stream);
+}
+
+int b2r_regs_backward(const B2RRegs* r, const float* dL_dout, const B2RRegsGrads* grads, const void* scratch,
+                      size_t scratch_bytes, void* stream) {
+  const int rc = validate_regs(r);
+  if (rc) return rc;
+  if (!dL_dout || !grads || !scratch) return B2R_E_INVALID;
+  if (!grads->mean_offset || !grads->mean_offset_offset || !grads->scale_offset || !grads->scale ||
+      !grads->scale_refined || !grads->rgb || !grads->rgb_refined || !grads->joint_offset ||
+      (r->scale_reg && !grads->scale_reg))
+    return B2R_E_INVALID;
+  if (scratch_bytes < regs_scratch_bytes(r->P, r->n_arm)) return B2R_E_WORKSPACE;
+  return launch_regs_backward(*r, dL_dout, *grads, scratch, (cudaStream_t)stream);
 }
 
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {

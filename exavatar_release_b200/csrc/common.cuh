@@ -536,6 +536,10 @@ size_t gn_mlp_grads_count(int K, int H);
 int launch_gn_mlp_forward(const B2RGnMlp& m, float* out, float* saved, cudaStream_t st);
 int launch_gn_mlp_backward(const B2RGnMlp& m, const float* saved, const float* dout, float* dx, float* grads,
                            void* scratch, cudaStream_t st);
+size_t regs_scratch_bytes(int P, int n_arm);
+int launch_regs_forward(const B2RRegs& r, float* out, void* scratch, cudaStream_t st);
+int launch_regs_backward(const B2RRegs& r, const float* dout, const B2RRegsGrads& g, const void* scratch,
+                         cudaStream_t st);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

@@ -196,6 +196,38 @@ def make_human_mesh(seed=0, rings=97, segments=108):
             "self_map": torch.from_numpy(self_map), "flip": torch.from_numpy(flip)}
 
 
+def make_regs_labels(mesh, hand_fraction=0.03, arm_half_width=0.05, arm_ny=(0.3, 0.7)):
+    """Vertex labels of `make_human_mesh` for `regularizers.HumanRegularizers`, from the vertex positions alone:
+        is_rhand / is_lhand  the round(hand_fraction * P) vertices of largest / smallest x (equal counts, as HandRGBReg
+                             needs), ties to the lower index
+        is_face              the head cap (y > 0.6 above the centre) and the front half of the right hand, so the
+                             weight columns' later assignments overwrite earlier ones
+        is_face_expr         the front of the head cap
+        is_cavity            the mesh's `flip` rows
+        is_arm               the band arm_ny[0] < n_y < arm_ny[1] of the shell's analytic normal with |x| <
+                             arm_half_width: around n_y = 0.5 the per-frame normals straddle it, so both upper and lower
+                             rows occur and, the band being narrow in x, lower rows find upper rows within 1 cm in x;
+                             narrower bands give fewer of them (k < 50, or none: k = 0)
+    Returns (P,) bool CPU tensors."""
+    verts = mesh["verts"].double()
+    P = verts.shape[0]
+    c = verts - torch.tensor([0.0, 0.0, 4.24], dtype=torch.float64)
+    n_hand = int(round(hand_fraction * P))
+    order = torch.sort(c[:, 0], stable=True).indices
+    is_lhand = torch.zeros(P, dtype=torch.bool)
+    is_rhand = torch.zeros(P, dtype=torch.bool)
+    is_lhand[order[:n_hand]] = True
+    is_rhand[torch.sort(-c[:, 0], stable=True).indices[:n_hand]] = True
+    is_face = (c[:, 1] > 0.6) | (is_rhand & (c[:, 2] < 0))
+    is_face_expr = (c[:, 1] > 0.6) & (c[:, 2] < 0)
+    semi = torch.tensor([0.25, 0.85, 0.15], dtype=torch.float64)
+    n = c / semi ** 2
+    n = n / n.norm(dim=1, keepdim=True)
+    is_arm = (n[:, 1] > arm_ny[0]) & (n[:, 1] < arm_ny[1]) & (c[:, 0].abs() < arm_half_width)
+    return {"is_rhand": is_rhand, "is_lhand": is_lhand, "is_face": is_face, "is_face_expr": is_face_expr,
+            "is_cavity": mesh["flip"].clone(), "is_arm": is_arm}
+
+
 def make_face_mesh(seed=0, num_vertices=5023, tex_size=512):
     """A seeded stand-in for ExAvatar's FLAME face mesh and texture, for `mesh_render.FaceMeshRenderer`.
 

@@ -202,7 +202,8 @@ int b2r_abi_version(void);
 const char* b2r_strerror(int code);
 int b2r_last_cuda_error(void);
 /* sizeof() of the ABI structs, for bindings to verify their mirror: 0 B2RScene, 1 B2RStatus, 2 B2RWorkspace,
- * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin, 8 B2RMeshRender, 10 B2RGnMlp; 0 for anything else
+ * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin, 8 B2RMeshRender, 10 B2RGnMlp, 11 B2RRegs,
+ * 12 B2RRegsGrads; 0 for anything else
  * (7 and 9 are unused and report 0). */
 size_t b2r_sizeof(int which);
 
@@ -413,11 +414,76 @@ int b2r_gn_mlp_forward(const B2RGnMlp* m, float* out, float* saved, void* stream
 int b2r_gn_mlp_backward(const B2RGnMlp* m, const float* saved, const float* dL_dout, float* dL_dx, float* grads,
                         void* scratch, size_t scratch_bytes, void* stream);
 
+/* ExAvatar's per-frame human regularisers (avatar/main/model.py:217-257 with avatar/common/nets/loss.py:97-197 and
+ * smpl_x.get_arm) as ten means, out[10] = {gaussian_mean_reg, gaussian_mean_hand_reg, gaussian_scale_reg, lap_mean,
+ * lap_scale, lap_rgb, hand_rgb_reg, arm_rgb_reg, joint_offset_reg, joint_offset_sym_reg}, each equal to the mean of the
+ * reference's map with its constant factor (1e5 for lap_mean / lap_scale, 0.01 hand_rgb_reg, 0.1 arm_rgb_reg).
+ * Per-vertex inputs are (P,3) float, scale_offset (P); the tables are constants of the model (built once by the caller):
+ *   lap      nbr_idx / nbr_w (P,10): LaplacianReg's neighbour table; lapT_* its transpose as a CSR over the entries of
+ *            non-zero weight, each vertex's entries in ascending source order (the backward's adjoint gather).
+ *   weights  (5,P): the weight columns of gaussian_mean_reg, gaussian_scale_reg, lap_mean, lap_scale, lap_rgb.
+ *   hand     (P): bit 0 is_rhand, bit 1 is_lhand; n_hand = #(rhand | lhand) rows, n_rhand = #rhand = #lhand.
+ *   arm      arm_idx (n_arm): the is_arm rows ascending; arm_slot (P): position in arm_idx or -1.
+ *   joints   joint_target (J,3), joint_weight (J), sym_pairs (n_pairs,2) = (right, left) joint ids; J <= 256.
+ * The normals of `mesh` come from the b2r_vertex_normals kernel over faces / vf_offsets / vf_entries (no flip).  An arm
+ * row is upper when n_y > 0.5f, else lower; a lower row's target is the mean rgb of the k upper rows nearest in fp32
+ * distance among those with |fl(l_x - u_x)| < 0.01f, k = min(50, smallest such count), distance ties to the lower
+ * vertex index; k = 0 or no lower row gives NaN for arm_rgb_reg.  scale_reg (P,3) or NULL replaces `scale` in
+ * gaussian_scale_reg (the warm-up's scale_wo_clamp).  `scratch` >= b2r_regs_scratch_bytes(P, n_arm) is kept from the
+ * forward until the backward.  The backward reads dL_dout[10] on the device and writes every element of each gradient
+ * in B2RRegsGrads (scale_reg required iff given); mesh gets none.  No float atomics (bit-identical runs), no
+ * allocation, no sync: both calls can be captured in a CUDA graph. */
+typedef struct B2RRegs {
+  int32_t P, J, n_arm, n_pairs, n_hand, n_rhand, reserved[2];
+  const float* mesh;                /* (P,3) mesh_neutral_pose */
+  const float* mean_offset;         /* (P,3) */
+  const float* mean_offset_offset;  /* (P,3) */
+  const float* scale_offset;        /* (P) */
+  const float* scale;               /* (P,3) */
+  const float* scale_refined;       /* (P,3) */
+  const float* rgb;                 /* (P,3) */
+  const float* rgb_refined;         /* (P,3) */
+  const float* scale_reg;           /* (P,3) or NULL */
+  const float* joint_offset;        /* (J,3) */
+  const int32_t* faces;             /* (F,3) and the vertex -> face CSR of b2r_vertex_normals */
+  const int32_t* vf_offsets;
+  const int32_t* vf_entries;
+  const int32_t* nbr_idx;
+  const float* nbr_w;
+  const int32_t* lapT_offsets;      /* (P+1) */
+  const int32_t* lapT_src;
+  const float* lapT_w;
+  const float* weights;
+  const uint8_t* hand;
+  const int32_t* arm_idx;
+  const int32_t* arm_slot;
+  const float* joint_target;
+  const float* joint_weight;
+  const int32_t* sym_pairs;
+} B2RRegs;
+
+typedef struct B2RRegsGrads {
+  float* mean_offset;
+  float* mean_offset_offset;
+  float* scale_offset;
+  float* scale;
+  float* scale_refined;
+  float* rgb;
+  float* rgb_refined;
+  float* scale_reg;    /* required iff B2RRegs.scale_reg is given */
+  float* joint_offset;
+} B2RRegsGrads;
+
+size_t b2r_regs_scratch_bytes(int32_t P, int32_t n_arm);
+int b2r_regs_forward(const B2RRegs* r, float* out, void* scratch, size_t scratch_bytes, void* stream);
+int b2r_regs_backward(const B2RRegs* r, const float* dL_dout, const B2RRegsGrads* grads, const void* scratch,
+                      size_t scratch_bytes, void* stream);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_* and b2r_gn_mlp_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_* and b2r_regs_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
