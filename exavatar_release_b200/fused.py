@@ -38,13 +38,13 @@ from typing import Dict, Optional
 import torch
 from torch import nn
 
-from .plan import RENDERS, MergedFivePlan, _views_of, merged_bucket_layout, merged_pass_a_views
+from .plan import ASSETS, RENDERS, MergedFivePlan
 from .rasterizer import GaussianRasterizationSettings, _f32c
 from .renderer import render_settings
 
-_KEYS = ("mean_3d", "opacity", "scale", "rotation", "rgb")
-_SH_KEYS = ("mean_3d", "opacity", "scale", "rotation", "shs")  # a scene coloured from SH inside the kernels
-_GRAD_OF = {"mean_3d": "means3D", "opacity": "opacities", "scale": "scales", "rotation": "rotations", "rgb": "colors"}
+_KEYS = tuple(ASSETS)
+_SH_KEYS = tuple(k for k in ASSETS if k != "rgb") + ("shs",)  # a scene coloured from SH inside the kernels
+_GRAD_OF = {k: g for k, (g, _) in ASSETS.items()}
 
 
 class _FrameFn(torch.autograd.Function):
@@ -56,17 +56,15 @@ class _FrameFn(torch.autograd.Function):
         if plan.M > 0:
             scene["sh_degree"] = sh_degree
         mod._frame_no += 1
+        plan.set_scene(scene)  # an SH scene: both passes read the caller's coefficient tensor itself (eager)
         if mod.use_graph:
             mod._graph_forward(settings, settings_h, scene, human, refined)
         else:
-            plan.set_scene(scene)  # an SH scene: both passes read the caller's coefficient tensor itself
             plan.forward_frame(None, settings, settings_h, scene, human, refined)  # no descriptor cache: cameras change
-        outs = []
-        for r in RENDERS:  # fresh tensors: the plan's image buffers are overwritten by the next frame
-            pk = "A" if r in plan.VIEWS["A"] else "B"
-            color, depth, alpha = plan.passes[pk].img[plan.VIEWS[pk].index(r)]
-            outs += [color.clone(), depth.clone(), alpha.clone()]
-        radii_a, radii_b = plan.passes["A"].radii.clone(), plan.passes["B"].radii.clone()
+        # fresh tensors: the plan's buffers are overwritten by the next frame
+        outs = [t.clone() for r in RENDERS for t in plan.image(r)]
+        # the radii of a combined render are those of every row of its pass
+        radii_a, radii_b = (plan.render_outputs(r)[2].clone() for r in ("scene_human", "scene_human_refined"))
         ctx.mod = mod
         ctx.shapes = [t.shape for t in tensors]
         ctx.m2d_shape = scene_m2d.shape
@@ -82,15 +80,10 @@ class _FrameFn(torch.autograd.Function):
         gc = {r: (None if g[3 * i] is None else _f32c(g[3 * i], "grad_color")) for i, r in enumerate(RENDERS)}
         gd = {r: (None if g[3 * i + 1] is None else _f32c(g[3 * i + 1], "grad_depth")) for i, r in enumerate(RENDERS)}
         ga = {r: (None if g[3 * i + 2] is None else _f32c(g[3 * i + 2], "grad_alpha")) for i, r in enumerate(RENDERS)}
-        dev = plan.device
-        if mod.use_graph:
-            flat_a, flat_b = mod._graph_backward(gc, gd, ga)  # fresh copies of the resident gradient buffers
+        if mod.use_graph:  # views of fresh copies of the resident gradient buffers
+            _, (va, vb) = plan.grad_buffers(mod._graph_backward(gc, gd, ga))
         else:
-            flat_a = torch.empty(mod._flat_a_numel, dtype=torch.float32, device=dev)
-            flat_b = torch.empty(plan.PER * plan.Ph, dtype=torch.float32, device=dev)
-        va = merged_pass_a_views(flat_a, plan.Ps, plan.Ph, plan.M)
-        _, vb = _views_of(flat_b, plan.Ph)
-        if not mod.use_graph:
+            _, (va, vb) = plan.grad_buffers()
             plan.backward_frame(gc, va, vb, g_depths=gd, g_alphas=ga, densify=mod.densify)
         Ps = plan.Ps
         out = [None, None, None, None, va["means2D"][:Ps].reshape(ctx.m2d_shape)]
@@ -118,13 +111,11 @@ class TrainingFrameRenderer(nn.Module):
         self.plan = MergedFivePlan(P_scene, P_human, self.img_shape[1], self.img_shape[0], dup_capacity, device,
                                    sh_coeffs=sh_coeffs)
         self._scene_keys = _SH_KEYS if self.plan.M > 0 else _KEYS
-        lay = merged_bucket_layout(self.plan.Ps, self.plan.Ph, self.plan.M)
-        self._flat_a_numel = lay["A"][1] + lay["A_shs"][1]  # pass A's gradients (+ the scene's dL/dSH)
         self.densify = None  # optional {'grad_accum','count','radius_max'} (P_scene) tensors updated by the backward
         self._frame_no = 0
         self.use_graph = bool(use_graph)
         if self.use_graph:
-            dev, (H, W), plan = self.plan.device, self.img_shape, self.plan
+            dev, (H, W) = self.plan.device, self.img_shape
             # resident camera / background block the captured kernels read: view (16) | full projection (16) | campos (3) |
             # bg (3) | bg of the human-only renders (3)
             self._cam = torch.zeros(41, dtype=torch.float32, device=dev)
@@ -132,8 +123,8 @@ class TrainingFrameRenderer(nn.Module):
             # dL/ddepth and dL/dalpha inputs only when asked for: their backward variant is the slower one
             self._gin_d = {r: torch.zeros(1, H, W, dtype=torch.float32, device=dev) for r in RENDERS} if graph_depth_alpha else None
             self._gin_a = {r: torch.zeros(1, H, W, dtype=torch.float32, device=dev) for r in RENDERS} if graph_depth_alpha else None
-            self._flat_a = torch.zeros(self._flat_a_numel, dtype=torch.float32, device=dev)
-            self._flat_b = torch.zeros(plan.PER * plan.Ph, dtype=torch.float32, device=dev)
+            # resident gradient buffers the captured backward writes, and their views
+            self._flats, self._grad_views = self.plan.grad_buffers()
             # (tanfovx, tanfovy, scale_modifier, densify buffers, sh_degree) -> (settings, settings_h, forward graph,
             # backward graph)
             self._graphs = {}
@@ -155,12 +146,7 @@ class TrainingFrameRenderer(nn.Module):
         c[32:35].copy_(settings.campos.reshape(3))
         c[35:38].copy_(settings.bg.reshape(3))
         c[38:41].copy_(settings_h.bg.reshape(3))
-        pa, pb = plan.passes["A"], plan.passes["B"]
-        for k in _KEYS:
-            if k in scene:  # an SH scene has no `rgb`: its coefficients go to the plan's resident buffer below
-                pa.cat[k][: plan.Ps].copy_(scene[k].reshape(plan.Ps, -1))
-            pa.cat[k][plan.Ps:].copy_(human[k].reshape(plan.Ph, -1))
-            pb.cat[k][plan.Ps:].copy_(refined[k].reshape(plan.Ph, -1))
+        plan.load_rows(human, refined)  # set_scene already copied the scene rows into both passes
         if plan.M > 0:  # the captured kernels read the coefficients at a fixed address
             plan.use_scene_shs(scene["shs"], scene["sh_degree"], copy=True)
 
@@ -175,14 +161,9 @@ class TrainingFrameRenderer(nn.Module):
                plan.sh_degree if plan.M > 0 else None)
         if key not in self._graphs:
             st, st_h = self._resident_settings(settings, settings_h)
-            pa, pb = plan.passes["A"], plan.passes["B"]
-            va = merged_pass_a_views(self._flat_a, plan.Ps, plan.Ph, plan.M)
-            _, vb = _views_of(self._flat_b, plan.Ph)
-            scene_keys = [k for k in _KEYS if k != "rgb" or plan.M == 0]
+            va, vb = self._grad_views
 
             def fwd():
-                for k in scene_keys:  # the scene rows of pass B come from pass A's copy
-                    pb.cat[k][: plan.Ps].copy_(pa.cat[k][: plan.Ps])
                 plan.forward_frame(("graph", key), st, st_h, None, None, None, copy_inputs=False)
 
             def bwd(densify):
@@ -220,7 +201,7 @@ class TrainingFrameRenderer(nn.Module):
                 else:
                     dst[r].copy_(src[r].reshape(dst[r].shape))
         self._cur[3].replay()
-        return self._flat_a.clone(), self._flat_b.clone()
+        return tuple(f.clone() for f in self._flats)
 
     def overflowed(self) -> bool:
         return self.plan.overflowed()

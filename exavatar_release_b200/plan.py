@@ -13,7 +13,6 @@ bucket that is all-reduced once per step (SURVEY.md section 8e).
 from __future__ import annotations
 
 import ctypes as C
-import os
 from typing import Dict, Optional
 
 import torch
@@ -21,14 +20,28 @@ import torch
 from . import _lib as L
 from .rasterizer import _f32c, _make_scene, _ptr
 
+# the per-Gaussian asset tensors of a render: asset key -> (name of its gradient, floats per Gaussian)
+ASSETS = {"mean_3d": ("means3D", 3), "opacity": ("opacities", 1), "scale": ("scales", 3), "rotation": ("rotations", 4),
+          "rgb": ("colors", 3)}
+
+
+def _backward_args(images, grads, accumulate: bool = False, first_row: int = 0, densify=None, densify_rows: int = 0):
+    """B2RBackwardArgs of (dL/dcolor, dL/ddepth, dL/dalpha) `images` and the named gradient outputs `grads` (keys
+    means3D, means2D, shs, colors, opacities, scales, rotations, cov3D; missing -> not written).  `densify`:
+    {'grad_accum', 'count', 'radius_max'} updated for rows [0, densify_rows) (0: all)."""
+    outs = [grads.get(k) for k in ("means3D", "means2D", "shs", "colors", "opacities", "scales", "rotations", "cov3D")]
+    dens = [(densify or {}).get(k) for k in ("grad_accum", "count", "radius_max")]
+    flags = (L.B2R_BWD_ACCUMULATE if accumulate else 0) | L.B2R_BWD_SCRATCH_ZEROED
+    return L.B2RBackwardArgs(*map(_ptr, images), *map(_ptr, outs), flags, int(first_row), *map(_ptr, dens),
+                             int(densify_rows) if densify is not None else 0)
+
 
 class _Workspace:
     """The resident buffers of one projection + binning of P Gaussians with a fixed duplicate capacity, and the
-    B2RWorkspace pointing at them: ctx (status block first), duplicate ids, forward scratch, backward scratch and,
-    with `checkpoints`, the forward composite's segment table + blend-state checkpoints."""
+    B2RWorkspace pointing at them: ctx (status block first), duplicate ids, forward scratch, backward scratch and the
+    forward composite's segment table + blend-state checkpoints."""
 
-    def __init__(self, P: int, width: int, height: int, dup_capacity: int, device, checkpoints: bool = True,
-                 split: bool = False):
+    def __init__(self, P: int, width: int, height: int, dup_capacity: int, device, split: bool = False):
         self.lib = L.load()
         self.P, self.W, self.H = int(P), int(width), int(height)
         self.device = dev = torch.device(device)
@@ -44,23 +57,21 @@ class _Workspace:
         self.bwd_bytes = self.lib.b2r_backward_scratch_bytes(P)
         # zero once: every backward leaves it zero again (B2R_BWD_SCRATCH_ZEROED), so no memset node per render
         self.bwd_scratch = torch.zeros(self.bwd_bytes, dtype=torch.uint8, device=dev)
-        self.ckpt_bytes = self.lib.b2r_checkpoint_bytes(width, height, self.capacity) if checkpoints else 0
-        self.ckpt = torch.empty(max(self.ckpt_bytes, 1), dtype=torch.uint8, device=dev) if checkpoints else None
+        # segment table + blend-state checkpoints of the forward composite: the backward replays 512-entry list
+        # segments as independent work items
+        self.ckpt_bytes = self.lib.b2r_checkpoint_bytes(width, height, self.capacity)
+        self.ckpt = torch.empty(max(self.ckpt_bytes, 1), dtype=torch.uint8, device=dev)
         self.ws = L.B2RWorkspace(self.ctx_buf.data_ptr(), self.ctx_bytes, self.ids.data_ptr(), self.capacity,
-                                 self.scratch.data_ptr(), self.scratch_bytes, None, 0,
-                                 self.ckpt.data_ptr() if checkpoints else None, self.ckpt_bytes)
+                                 self.scratch.data_ptr(), self.scratch_bytes, None, 0, self.ckpt.data_ptr(),
+                                 self.ckpt_bytes)
 
     def status(self) -> dict:
         return L.read_status(self.ctx_buf)
 
 
 class FramePlan(_Workspace):
-    def __init__(self, P: int, width: int, height: int, dup_capacity: int, device, sh_coeffs: int = 0,
-                 segmented: bool = True):
-        # segment table + blend-state checkpoints of the forward composite (lets the backward replay 512-entry list
-        # segments as independent work items); `segmented=False` reproduces the round-1 whole-list backward
-        segmented = segmented and os.environ.get("B2R_SEGMENTED", "1") != "0"  # A/B switch for measurements
-        super().__init__(P, width, height, dup_capacity, device, checkpoints=segmented)
+    def __init__(self, P: int, width: int, height: int, dup_capacity: int, device, sh_coeffs: int = 0):
+        super().__init__(P, width, height, dup_capacity, device)
         self.M = int(sh_coeffs)
         f = lambda *s: torch.empty(s, dtype=torch.float32, device=self.device)
         self.color, self.depth, self.alpha = f(3, height, width), f(1, height, width), f(1, height, width)
@@ -98,12 +109,7 @@ class FramePlan(_Workspace):
         projection kernel -- ExAvatar's `track_stats` + `radius_max` update (module.py:155-157, model.py:283-285).
         first_row: Gaussians [0, first_row) are a detached prefix (cat(scene.detach(), human), model.py:117-125): the
         `grads` tensors then have P - first_row rows and receive the gradient of the remaining Gaussians only."""
-        a = L.B2RBackwardArgs(_ptr(g_color), _ptr(g_depth), _ptr(g_alpha), _ptr(grads.get("means3D")),
-                              _ptr(grads.get("means2D")), _ptr(grads.get("shs")), _ptr(grads.get("colors")),
-                              _ptr(grads.get("opacities")), _ptr(grads.get("scales")), _ptr(grads.get("rotations")),
-                              _ptr(grads.get("cov3D")), (L.B2R_BWD_ACCUMULATE if accumulate else 0) | L.B2R_BWD_SCRATCH_ZEROED, int(first_row),
-                              _ptr((densify or {}).get("grad_accum")), _ptr((densify or {}).get("count")),
-                              _ptr((densify or {}).get("radius_max")))
+        a = _backward_args((g_color, g_depth, g_alpha), grads, accumulate, first_row, densify)
         with torch.cuda.device(self.device):
             st = torch.cuda.current_stream(self.device).cuda_stream
             L.check(self.lib.b2r_backward(C.byref(sc), C.byref(self.ws), C.byref(a), self.bwd_scratch.data_ptr(),
@@ -183,7 +189,27 @@ def _views_of(flat: torch.Tensor, P: int, sh_coeffs: int = 0):
 RENDERS = ("scene", "human", "scene_human", "human_refined", "scene_human_refined")
 
 
-class FiveRenderPlan:
+class _FiveRenders:
+    """What the two five-render plans share: the row width of their gradient buckets, the densification sums at the
+    tail of the flat bucket (`_stats`) and the status of their workspaces (`_ws`: name -> _Workspace)."""
+    PER = 3 + 3 + 1 + 3 + 4 + 3  # floats per Gaussian in a bucket
+
+    def stats(self) -> Dict[str, torch.Tensor]:
+        """Per-step sums of ExAvatar's densification statistics (module.py:155-157), stored at the tail of the flat
+        bucket so the step's ONE sum all-reduce covers them; zero them at the start of a step (`zero_stats`)."""
+        return {"grad_accum": self._stats[: self.Ps], "count": self._stats[self.Ps:]}
+
+    def zero_stats(self) -> None:
+        self._stats.zero_()
+
+    def dups(self) -> Dict[str, int]:
+        return {k: w.status()["num_dups"] for k, w in self._ws.items()}
+
+    def overflowed(self) -> bool:
+        return any(w.status()["overflow"] for w in self._ws.values())
+
+
+class FiveRenderPlan(_FiveRenders):
     """One ExAvatar training frame = five rasteriser calls with one camera (avatar/main/model.py:81-162):
 
         scene                      -> gradients to the scene Gaussians
@@ -203,7 +229,6 @@ class FiveRenderPlan:
     tensor a multi-GPU step all-reduces once (SURVEY.md section 8e).  `MergedFivePlan` below produces the same results
     from two projection / binning passes instead of five (SURVEY.md section 8f-3).
     """
-    PER = 3 + 3 + 1 + 3 + 4 + 3  # floats per Gaussian in a bucket
 
     def __init__(self, P_scene: int, P_human: int, width: int, height: int, caps: Optional[Dict[str, int]], device):
         self.Ps, self.Ph = int(P_scene), int(P_human)
@@ -211,7 +236,7 @@ class FiveRenderPlan:
         caps = caps or {r: 8_000_000 for r in RENDERS}
         sizes = {"scene": self.Ps, "human": self.Ph, "scene_human": self.Ps + self.Ph, "human_refined": self.Ph,
                  "scene_human_refined": self.Ps + self.Ph}
-        self.plans = {r: FramePlan(sizes[r], width, height, caps[r], device) for r in RENDERS}
+        self._ws = self.plans = {r: FramePlan(sizes[r], width, height, caps[r], device) for r in RENDERS}
         self.streams = {r: torch.cuda.Stream(self.device) for r in RENDERS}
         self.first_row = {"scene": 0, "human": 0, "scene_human": self.Ps, "human_refined": 0, "scene_human_refined": self.Ps}
         out_rows = {"scene": self.Ps, "human": self.Ph, "scene_human": self.Ph, "human_refined": self.Ph,
@@ -231,8 +256,7 @@ class FiveRenderPlan:
                 o += tail
         self._reduced = self.PER * (self.Ps + 2 * self.Ph) + tail
         f = lambda w: torch.empty(self.Ps + self.Ph, w, dtype=torch.float32, device=device)
-        widths = {"mean_3d": 3, "opacity": 1, "scale": 3, "rotation": 4, "rgb": 3}
-        self.cat = {r: {k: f(w) for k, w in widths.items()} for r in ("scene_human", "scene_human_refined")}
+        self.cat = {r: {k: f(w) for k, (_, w) in ASSETS.items()} for r in ("scene_human", "scene_human_refined")}
 
     def describe(self) -> str:
         return "five independent renders (project+bin+sort+composite each) on five CUDA streams per frame"
@@ -294,24 +318,10 @@ class FiveRenderPlan:
     def flat_bucket(self) -> torch.Tensor:
         return self.all_flat[: self._reduced]
 
-    def stats(self) -> Dict[str, torch.Tensor]:
-        """Per-step sums of ExAvatar's densification statistics (module.py:155-157), stored at the tail of the flat
-        bucket so the step's ONE sum all-reduce covers them; zero them at the start of a step (`zero_stats`)."""
-        return {"grad_accum": self._stats[: self.Ps], "count": self._stats[self.Ps:]}
-
-    def zero_stats(self) -> None:
-        self._stats.zero_()
-
-    def dups(self) -> Dict[str, int]:
-        return {r: p.status()["num_dups"] for r, p in self.plans.items()}
-
     def consumed(self) -> Dict[str, list]:
         st = [self.plans[r].status() for r in RENDERS]
         return {"fwd": [s["consumed_fwd"] / s["consumed_fwd_div"] for s in st],
                 "bwd": [s["consumed_bwd"] / s["consumed_bwd_div"] for s in st]}
-
-    def overflowed(self) -> bool:
-        return any(p.status()["overflow"] for p in self.plans.values())
 
 
 class _Pass(_Workspace):
@@ -325,8 +335,7 @@ class _Pass(_Workspace):
         f = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
         self.img = [(f(3, H, W), f(1, H, W), f(1, H, W)) for _ in range(n_views)]
         self.state = [(f(H * W), torch.empty(H * W, dtype=torch.int32, device=dev)) for _ in range(n_views)]
-        widths = {"mean_3d": 3, "opacity": 1, "scale": 3, "rotation": 4, "rgb": 3}
-        self.cat = {k: f(P, w) for k, w in widths.items()}
+        self.cat = {k: f(P, w) for k, (_, w) in ASSETS.items()}
         self.streams = [torch.cuda.Stream(dev) for _ in range(n_views)]
         self.primed = False
 
@@ -342,25 +351,14 @@ def merged_bucket_layout(P_scene: int, P_human: int, sh_coeffs: int = 0) -> Dict
         total  the whole buffer
 
     sh_coeffs = 0 is the layout of a plan without SH: A | B | stats."""
-    PER = FiveRenderPlan.PER
+    PER = _FiveRenders.PER
     Ps, Ph, M = int(P_scene), int(P_human), int(sh_coeffs)
     nA, nS, nB = PER * (Ps + Ph), 3 * M * Ps, PER * Ph
     return {"A": (0, nA), "A_shs": (nA, nS), "B": (nA + nS, nB), "stats": (nA + nS + nB, 2 * Ps),
             "total": (0, nA + nS + nB + 2 * Ps)}
 
 
-def merged_pass_a_views(flat: torch.Tensor, P_scene: int, P_human: int, sh_coeffs: int = 0) -> Dict[str, torch.Tensor]:
-    """Named views of a pass-A gradient buffer laid out as the A | A_shs regions of `merged_bucket_layout`:
-    `_views_of` views with P_scene + P_human rows, plus "shs" (P_scene, M, 3) when sh_coeffs > 0."""
-    lay = merged_bucket_layout(P_scene, P_human, sh_coeffs)
-    (oa, na), (os_, ns) = lay["A"], lay["A_shs"]
-    _, views = _views_of(flat[oa:oa + na], int(P_scene) + int(P_human))
-    if sh_coeffs > 0:
-        views["shs"] = flat[os_:os_ + ns].view(int(P_scene), int(sh_coeffs), 3)
-    return views
-
-
-class MergedFivePlan:
+class MergedFivePlan(_FiveRenders):
     """ExAvatar's five renders per training frame (avatar/main/model.py:81-162) from TWO projection + binning passes
     instead of five (SURVEY.md section 8f-3, kernel half):
 
@@ -380,13 +378,12 @@ class MergedFivePlan:
     kernels (SURVEY.md section 8f-4) and the human sets from RGB -- both passes are mixed-source scenes
     (B2RScene.sh_rows = P_scene) reading ONE coefficient buffer (`use_scene_shs`).  The scene assets then carry `shs` +
     `sh_degree` instead of `rgb`, and `grads("scene")` holds `shs` instead of `colors`."""
-    PER = FiveRenderPlan.PER
     VIEWS = {"A": ("scene", "human", "scene_human"), "B": ("human_refined", "scene_human_refined")}
-    SKIP = os.environ.get("B2R_SKIP_TILES", "1") != "0"  # A/B switch of the skipped human-free tiles
     # Pass B projects, bins and sorts only the refined rows and takes the scene entries of its lists from pass A (the
-    # split pass of the C ABI); its views need the skipped tiles for that.  B2R_REFINED_PASS=full: the whole
-    # cat(scene, refined) again (A/B switch for measurements).
-    SPLIT = SKIP and os.environ.get("B2R_REFINED_PASS", "split") != "full"
+    # split pass of the C ABI).  SPLIT = False: the whole cat(scene, refined) again, the reference the tests compare the
+    # split pass against.  Read per frame; pass B's scratch is sized by its value at construction (the split pass needs
+    # more, so a split-built plan may be switched to the whole pass).
+    SPLIT = True
 
     def __init__(self, P_scene: int, P_human: int, width: int, height: int, caps: Optional[Dict[str, int]], device,
                  sh_coeffs: int = 0):
@@ -396,17 +393,16 @@ class MergedFivePlan:
         self.M = int(sh_coeffs)
         self.device = torch.device(device)
         caps = caps or {"A": 8_000_000, "B": 8_000_000}
-        self.passes = {k: _Pass(self.P, self.W, self.H, caps[k], len(v), self.device, split=(k == "B" and self.SPLIT))
-                       for k, v in self.VIEWS.items()}
+        self._ws = self.passes = {k: _Pass(self.P, self.W, self.H, caps[k], len(v), self.device,
+                                           split=(k == "B" and self.SPLIT)) for k, v in self.VIEWS.items()}
         self.pass_streams = {k: torch.cuda.Stream(self.device) for k in self.passes}
         # one flat gradient buffer: [pass A: scene rows | human rows][scene dL/dSH][pass B: refined rows][stats]
         lay = merged_bucket_layout(self.Ps, self.Ph, self.M)
         self.all_flat = torch.zeros(lay["total"][1], dtype=torch.float32, device=device)
         o, n = lay["stats"]
         self._stats = self.all_flat[o:o + n]  # per-step densification sums ride in the all-reduced buffer (stats())
-        self.views_A = merged_pass_a_views(self.all_flat, self.Ps, self.Ph, self.M)
         o, n = lay["B"]
-        _, self.views_B = _views_of(self.all_flat[o:o + n], self.Ph)
+        _, (self.views_A, self.views_B) = self.grad_buffers((self.all_flat[:o], self.all_flat[o:o + n]))
         # the scene's SH coefficients: the caller's tensor (eager) or this resident copy (`use_scene_shs`)
         self.shs = torch.zeros(self.Ps, self.M, 3, dtype=torch.float32, device=device) if self.M > 0 else None
         self._shs_src, self.sh_degree = self.shs, 0
@@ -424,12 +420,23 @@ class MergedFivePlan:
 
     def set_scene(self, scene_assets: Dict[str, torch.Tensor]) -> None:
         for ps in self.passes.values():
-            for k, buf in ps.cat.items():
-                if k == "rgb" and self.M > 0:
-                    continue  # SH scene: the colour rows of the scene are never read
-                buf[: self.Ps].copy_(scene_assets[k].reshape(self.Ps, -1))
+            self._copy_rows(ps, scene_assets, scene=True)
         if self.M > 0:
             self.use_scene_shs(scene_assets["shs"], scene_assets["sh_degree"])
+
+    def load_rows(self, human: Dict[str, torch.Tensor], refined: Dict[str, torch.Tensor]) -> None:
+        """Copies the human and refined rows behind the scene prefix of pass A and pass B, on the current stream: what
+        `forward_frame(copy_inputs=False)` leaves out, so that a captured graph reads fixed addresses and the copies
+        from the caller's tensors stay outside it."""
+        for ps, rows in zip(self.passes.values(), (human, refined)):
+            self._copy_rows(ps, rows)
+
+    def _copy_rows(self, ps, assets, scene: bool = False) -> None:
+        """Copies the scene's rows (`scene`) into the prefix of pass `ps`, or the human or refined set's behind it."""
+        lo, n = (0, self.Ps) if scene else (self.Ps, self.Ph)
+        for k, buf in ps.cat.items():
+            if not (scene and k == "rgb" and self.M > 0):  # SH scene: the colour rows of the scene are never read
+                buf[lo:lo + n].copy_(assets[k].reshape(n, -1))
 
     def use_scene_shs(self, shs: torch.Tensor, sh_degree: int, copy: bool = False) -> None:
         """The scene's (P_scene, M, 3) SH coefficients and active degree for the next frames.  Both passes read ONE
@@ -480,7 +487,7 @@ class MergedFivePlan:
         # Tiles no human Gaussian reaches: a combined view equals the scene-only view there and carries no gradient; a
         # human-only view shows the bare background there.  Both are pre-filled (`_forward_view`) and skipped by the
         # kernels.
-        skip = self.Ps if (self.SKIP and name != "scene") else 0
+        skip = self.Ps if name != "scene" else 0
         return L.B2RView(lo, hi, _ptr(bg), fT.data_ptr(), nc.data_ptr(), ps.ck[v].data_ptr(), ps.ckpt_bytes, skip, 0)
 
     # ---- the steps of a frame; each enqueues on the stream `s` it is given, which is also the current stream ----
@@ -491,8 +498,7 @@ class MergedFivePlan:
         descriptor and views stay in `_current[pk]` until the next frame."""
         ps = self.passes[pk]
         if src is not None:
-            for k, buf in ps.cat.items():
-                buf[self.Ps:].copy_(src[k].reshape(self.Ph, -1))
+            self._copy_rows(ps, src)
         sc = self._scene_desc((key, pk), ps, settings)
         sc.flags = L.B2R_FLAG_CTX_CLEAN if ps.primed else 0  # every pass leaves its ctx counters zero
         ps.primed = True
@@ -532,13 +538,15 @@ class MergedFivePlan:
         if name == "scene":
             scene_done.record(s)
 
-    def _backward_view(self, s, pk, v, g_color, g_depth=None, g_alpha=None) -> None:
-        """Backward composite of view v of pass pk: its screen-space gradients are added into the pass's scratch."""
+    def _backward_view(self, s, pk, v, g_color, g_depth, g_alpha) -> None:
+        """Backward composite of view v of pass pk: its screen-space gradients are added into the pass's scratch.  No
+        dL/dcolor: zeros.  The gradient images are kept alive while the launch may be queued."""
         ps = self.passes[pk]
         sc, views = self._current[pk]
-        a = L.B2RBackwardArgs(_ptr(g_color), _ptr(g_depth), _ptr(g_alpha))
-        a.flags = L.B2R_BWD_SCRATCH_ZEROED
-        a.first_row = self.first_row[self.VIEWS[pk][v]]
+        if g_color is None:
+            g_color = torch.zeros(3, self.H, self.W, dtype=torch.float32, device=self.device)
+        self._keep.append((g_color, g_depth, g_alpha))
+        a = _backward_args((g_color, g_depth, g_alpha), {}, first_row=self.first_row[self.VIEWS[pk][v]])
         L.check(self.lib.b2r_backward_composite(C.byref(sc), C.byref(ps.ws), C.byref(views[v]), C.byref(a),
                                                 ps.bwd_scratch.data_ptr(), ps.bwd_bytes, s.cuda_stream),
                 "b2r_backward_composite")
@@ -547,27 +555,24 @@ class MergedFivePlan:
         """The one backward projection of pass pk, from the scratch its views filled into the gradient views `g`."""
         ps = self.passes[pk]
         sc, _ = self._current[pk]
-        a = L.B2RBackwardArgs(None, None, None, _ptr(g["means3D"]), _ptr(g["means2D"]),
-                              _ptr(g.get("shs")) if pk == "A" else None, _ptr(g["colors"]),
-                              _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), None)
-        a.flags = (L.B2R_BWD_ACCUMULATE if accumulate else 0) | L.B2R_BWD_SCRATCH_ZEROED
-        a.first_row = 0 if pk == "A" else self.Ps  # pass B: the scene prefix (SH rows included) is detached
-        if pk == "A" and densify is not None:
-            a.densify_grad_accum, a.densify_count = _ptr(densify.get("grad_accum")), _ptr(densify.get("count"))
-            a.densify_radius_max = _ptr(densify.get("radius_max"))
-            a.densify_rows = self.Ps
+        # pass B: the scene prefix (SH rows included) is detached; the densification statistics are the scene rows'
+        a = _backward_args((None, None, None), g, accumulate, first_row=0 if pk == "A" else self.Ps,
+                           densify=densify if pk == "A" else None, densify_rows=self.Ps)
         L.check(self.lib.b2r_backward_project(C.byref(sc), C.byref(ps.ws), C.byref(a), ps.bwd_scratch.data_ptr(),
                                               ps.bwd_bytes, s.cuda_stream), "b2r_backward_project")
 
-    def frame(self, key, settings, settings_human_bg, scene, human, refined, g_colors: Dict[str, torch.Tensor],
-              accumulate: bool, densify: Optional[Dict[str, torch.Tensor]] = None, serial: bool = False, probe=None) -> None:
-        """Forward + backward of the five renders.  Each pass runs on its own stream and forks one stream per view, on
-        which the view's backward composite follows its forward composite; the pass joins its views, then runs its
-        backward projection.  `serial`: everything on the caller's stream.  `probe(label)` (serial mode): called after
-        every stage -- bench.py reads the in-library profiler there to get per-view kernel times."""
+    def _walk(self, key=None, settings=None, settings_human_bg=None, rows=None, g_images=None, grads=None,
+              accumulate: bool = False, densify=None, serial: bool = False, probe=None) -> None:
+        """Enqueues a frame pass by pass.  With `settings`: its forward -- each pass starts (`rows[pass]`: the rows to
+        copy behind its scene prefix, or None) and composites its views.  With `grads` (pass -> gradient views): its
+        backward -- each view composites the gradients g_images = (g_colors, g_depths, g_alphas) of its render (dicts,
+        None or a missing entry: no such gradient; a view with none at all is skipped), then each pass runs its backward
+        projection into grads[pass].  Each pass runs on its own stream and forks one stream per view, on which the
+        view's backward composite follows its forward composite; the pass joins its views before its backward
+        projection.  `serial`: everything on the caller's stream, and `probe(label)` is called after every stage."""
         probe = probe if (probe is not None and serial) else (lambda label: None)
         cur = torch.cuda.current_stream(self.device)
-        bg_h = self._human_bg(settings_human_bg)
+        bg_h = self._human_bg(settings_human_bg) if settings is not None else None
         scene_done, a_binned = torch.cuda.Event(), torch.cuda.Event()
         for pk, names in self.VIEWS.items():
             ps = self.passes[pk]
@@ -575,87 +580,83 @@ class MergedFivePlan:
             if not serial:
                 st.wait_stream(cur)
             with torch.cuda.stream(st):
-                self._start_pass(st, pk, key, settings, human if pk == "A" else refined, bg_h, a_binned)
-                probe(f"{pk}:bin")
+                if settings is not None:
+                    self._start_pass(st, pk, key, settings, rows[pk], bg_h, a_binned)
+                    probe(f"{pk}:bin")
                 for v, n in enumerate(names):
+                    g = [(d or {}).get(n) for d in g_images] if grads is not None else [None] * 3
+                    backward = any(x is not None for x in g)
+                    if settings is None and not backward:
+                        continue  # this render was not used downstream
                     vs = st if serial else ps.streams[v]
                     if not serial:
                         vs.wait_stream(st)
                     with torch.cuda.stream(vs):
-                        self._forward_view(vs, pk, v, bg_h, scene_done)
-                        probe(f"{pk}:{n}:fwd")
-                        self._backward_view(vs, pk, v, g_colors[n])
-                        probe(f"{pk}:{n}:bwd")
+                        if settings is not None:
+                            self._forward_view(vs, pk, v, bg_h, scene_done)
+                            probe(f"{pk}:{n}:fwd")
+                        if backward:
+                            self._backward_view(vs, pk, v, *g)
+                            probe(f"{pk}:{n}:bwd")
                 if not serial:
                     for v in range(len(names)):
                         st.wait_stream(ps.streams[v])
-                self._backward_project(st, pk, self.views_A if pk == "A" else self.views_B, accumulate, densify)
-                probe(f"{pk}:project_bwd")
+                if grads is not None:
+                    self._backward_project(st, pk, grads[pk], accumulate, densify)
+                    probe(f"{pk}:project_bwd")
         if not serial:
             for pk in self.passes:
                 cur.wait_stream(self.pass_streams[pk])
 
+    def frame(self, key, settings, settings_human_bg, scene, human, refined, g_colors: Dict[str, torch.Tensor],
+              accumulate: bool, densify: Optional[Dict[str, torch.Tensor]] = None, serial: bool = False, probe=None) -> None:
+        """Forward + backward of the five renders.  `serial`: everything on the caller's stream.  `probe(label)` (serial
+        mode): called after every stage -- bench.py reads the in-library profiler there to get per-view kernel times."""
+        self._walk(key, settings, settings_human_bg, {"A": human, "B": refined}, (g_colors, None, None),
+                   {"A": self.views_A, "B": self.views_B}, accumulate, densify, serial, probe)
+
     # ---- the same frame in two halves (forward now, backward when the caller's gradients exist): fused.py ----
     def forward_frame(self, key, settings, settings_human_bg, scene, human, refined, copy_inputs: bool = True) -> None:
-        """Forward of the five renders; images in `render_outputs()`, per-pixel state and checkpoints stay in the plan
-        until `backward_frame` (so the plan must not start another frame in between).  copy_inputs=False: the caller
-        already wrote the human / refined rows into `passes[*].cat` (a captured graph keeps the copies outside)."""
-        cur = torch.cuda.current_stream(self.device)
-        bg_h = self._human_bg(settings_human_bg)
-        scene_done, a_binned = torch.cuda.Event(), torch.cuda.Event()
-        for pk, names in self.VIEWS.items():
-            ps = self.passes[pk]
-            st = self.pass_streams[pk]
-            st.wait_stream(cur)
-            with torch.cuda.stream(st):
-                src = (human if pk == "A" else refined) if copy_inputs else None
-                self._start_pass(st, pk, key, settings, src, bg_h, a_binned)
-                for v in range(len(names)):
-                    vs = ps.streams[v]
-                    vs.wait_stream(st)
-                    with torch.cuda.stream(vs):
-                        self._forward_view(vs, pk, v, bg_h, scene_done)
-                for v in range(len(names)):
-                    st.wait_stream(ps.streams[v])
-        for pk in self.passes:
-            cur.wait_stream(self.pass_streams[pk])
+        """Forward of the five renders; images in `image()` / `render_outputs()`, per-pixel state and checkpoints stay
+        in the plan until `backward_frame` (so the plan must not start another frame in between).  copy_inputs=False:
+        the caller already wrote the human / refined rows (`load_rows`)."""
+        rows = {"A": human, "B": refined} if copy_inputs else {"A": None, "B": None}
+        self._walk(key, settings, settings_human_bg, rows)
 
     def backward_frame(self, g_colors: Dict[str, Optional[torch.Tensor]], grads_A: Dict[str, torch.Tensor],
                        grads_B: Dict[str, torch.Tensor], g_depths: Optional[Dict[str, torch.Tensor]] = None,
                        g_alphas: Optional[Dict[str, torch.Tensor]] = None, accumulate: bool = False,
                        densify: Optional[Dict[str, torch.Tensor]] = None) -> None:
         """Backward of the frame `forward_frame` rendered.  g_colors[name] = dL/dimage of a render, or None when the render
-        was not used downstream.  grads_A / grads_B: `_views_of`-style dicts with P / P_human rows (pass A: scene rows then
-        human rows; pass B: refined rows)."""
-        cur = torch.cuda.current_stream(self.device)
-        for pk, names in self.VIEWS.items():
-            ps = self.passes[pk]
-            st = self.pass_streams[pk]
-            st.wait_stream(cur)
-            with torch.cuda.stream(st):
-                for v, n in enumerate(names):
-                    gc, gd, ga = g_colors.get(n), (g_depths or {}).get(n), (g_alphas or {}).get(n)
-                    if gc is None and gd is None and ga is None:
-                        continue  # this render was not used downstream
-                    vs = ps.streams[v]
-                    vs.wait_stream(st)
-                    with torch.cuda.stream(vs):
-                        if gc is None:
-                            gc = torch.zeros(3, self.H, self.W, dtype=torch.float32, device=self.device)
-                        self._backward_view(vs, pk, v, gc, gd, ga)
-                        self._keep.append((gc, gd, ga))
-                for v in range(len(names)):
-                    st.wait_stream(ps.streams[v])
-                self._backward_project(st, pk, grads_A if pk == "A" else grads_B, accumulate, densify)
-        for pk in self.passes:
-            cur.wait_stream(self.pass_streams[pk])
+        was not used downstream.  grads_A / grads_B: pass A's and pass B's gradient views (`grad_buffers`)."""
+        self._walk(g_images=(g_colors, g_depths, g_alphas), grads={"A": grads_A, "B": grads_B}, accumulate=accumulate,
+                   densify=densify)
+
+    def grad_buffers(self, flats=None):
+        """((flat_a, flat_b), (views_a, views_b)): pass A's and pass B's gradient buffers -- `flats`, or a fresh
+        uninitialised pair -- and their named views, what `backward_frame` takes as grads_A / grads_B.  flat_a is laid
+        out as the A | A_shs regions of `merged_bucket_layout` (scene rows then human rows, plus the scene's dL/dSH
+        (P_scene, M, 3) as "shs" when M > 0), flat_b as its B region (refined rows)."""
+        lay = merged_bucket_layout(self.Ps, self.Ph, self.M)
+        (_, na), (_, ns), (_, nb) = lay["A"], lay["A_shs"], lay["B"]
+        if flats is None:
+            flats = tuple(torch.empty(n, dtype=torch.float32, device=self.device) for n in (na + ns, nb))
+        _, views_a = _views_of(flats[0][:na], self.P)
+        if self.M > 0:
+            views_a["shs"] = flats[0][na:].view(self.Ps, self.M, 3)
+        _, views_b = _views_of(flats[1], self.Ph)
+        return flats, (views_a, views_b)
+
+    def image(self, render: str):
+        """(color (3,H,W), depth (1,H,W), alpha (1,H,W)) of one of the five renders of the last frame (valid until the
+        next)."""
+        pk = "A" if render in self.VIEWS["A"] else "B"
+        return self.passes[pk].img[self.VIEWS[pk].index(render)]
 
     def render_outputs(self, render: str):
-        pk = "A" if render in self.VIEWS["A"] else "B"
-        ps = self.passes[pk]
-        color, _, alpha = ps.img[self.VIEWS[pk].index(render)]
+        color, _, alpha = self.image(render)
         lo, hi = self.ranges[render]
-        return color, alpha, ps.radii[lo:hi]
+        return color, alpha, self.passes["A" if render in self.VIEWS["A"] else "B"].radii[lo:hi]
 
     def reduce(self):
         """(scene, human, human_refined) flat gradient buckets of the step.  Nothing to fold: the backward projection of
@@ -678,16 +679,6 @@ class MergedFivePlan:
     def flat_bucket(self) -> torch.Tensor:
         return self.all_flat
 
-    def stats(self) -> Dict[str, torch.Tensor]:
-        """Per-step sums of the densification statistics at the tail of the flat bucket (see FiveRenderPlan.stats)."""
-        return {"grad_accum": self._stats[: self.Ps], "count": self._stats[self.Ps:]}
-
-    def zero_stats(self) -> None:
-        self._stats.zero_()
-
-    def dups(self) -> Dict[str, int]:
-        return {k: ps.status()["num_dups"] for k, ps in self.passes.items()}
-
     def consumed(self) -> Dict[str, list]:
         fwd, bwd = [], []
         for pk, names in self.VIEWS.items():  # the views of a pass add into the same counters: per-launch averages
@@ -695,6 +686,3 @@ class MergedFivePlan:
             fwd += [s["consumed_fwd"] / L.CONSUMED_FWD_DIV / len(names)] * len(names)
             bwd += [s["consumed_bwd"] / L.CONSUMED_BWD_DIV / len(names)] * len(names)
         return {"fwd": fwd, "bwd": bwd}
-
-    def overflowed(self) -> bool:
-        return any(ps.status()["overflow"] for ps in self.passes.values())

@@ -3,7 +3,7 @@ only the refined rows and builds a list only in the tiles they reach, as the mer
 to scene ids with its own sorted entries on the (depth_bits, id) key (b2r_forward_project_split / b2r_forward_bin_split).
 
 CPU: a numpy restatement of that filter + merge against the joint sort.  GPU: the split pass against the whole pass
-(B2R_REFINED_PASS=full) at full C4 size -- lists, images, alpha and radii bit-equal, gradients within the tolerance of
+(MergedFivePlan.SPLIT = False) at full C4 size -- lists, images, alpha and radii bit-equal, gradients within the tolerance of
 the backward's reordered float sums."""
 import ctypes as C
 import math
