@@ -296,7 +296,7 @@ def _set_columns(w: torch.Tensor, cols: Sequence[int], v: torch.Tensor):
 class _GnMlp(torch.autograd.Function):
     @staticmethod
     def forward(ctx, spec, *tensors):
-        n_in, n_heads, row_blocks, const_blocks, row_cols, const_cols, _ = spec
+        n_in, n_heads, row_blocks, const_blocks, row_cols, const_cols, _, grad_mode = spec
         inputs = tensors[:n_in]
         params = tensors[n_in:]
         w0, b0 = params[0], params[1]
@@ -323,7 +323,8 @@ class _GnMlp(torch.autograd.Function):
         for l in range(3):
             m.w[l], m.b[l], m.gamma[l], m.beta[l] = (_ptr(t) for t in lay[l])
         out = torch.empty((P, H), dtype=torch.float32, device=dev)
-        train = any(ctx.needs_input_grad)
+        # needs_input_grad follows requires_grad only, also under torch.no_grad(); the grad mode of the call decides
+        train = grad_mode and any(ctx.needs_input_grad)
         saved = torch.empty((3, P, HIDDEN), dtype=torch.float32, device=dev) if train else None
         lib = L.load()
         with torch.cuda.device(dev):
@@ -340,7 +341,7 @@ class _GnMlp(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dout):
-        n_in, n_heads, row_blocks, const_blocks, row_cols, const_cols, row_widths = ctx.spec
+        n_in, n_heads, row_blocks, const_blocks, row_cols, const_cols, row_widths, _ = ctx.spec
         (saved,) = ctx.saved_tensors
         x, lay, wh, bh, c = ctx.keep
         m = ctx.m
@@ -436,7 +437,7 @@ def gn_mlp(inputs: Sequence[torch.Tensor], trunk: nn.Sequential, heads: Optional
     if P < 1:
         raise ValueError("gn_mlp: no rows")
     spec = (len(inputs), len(head_lins), tuple(row_blocks), tuple(const_blocks), tuple(row_cols), tuple(const_cols),
-            tuple(int(inputs[i].shape[1]) for i in row_blocks))
+            tuple(int(inputs[i].shape[1]) for i in row_blocks), torch.is_grad_enabled())
     return _GnMlp.apply(spec, *inputs, *params)
 
 

@@ -340,7 +340,7 @@ def _relu_edge_rows(ins, t64, rel=2e-5):
     -- the op's or torch's -- may put such a y on the other side of the ReLU, which moves every weight gradient by that
     row's whole contribution (about 1e-3 of the max at this size); the gradient comparisons leave these rows out.
     Exact zeros stay in: both sides agree there (relu'(0) = 0)."""
-    P = ins[0].shape[0]
+    P = next(t.shape[0] for t in ins if t.dim() == 2)
     x = torch.cat([(t if t.dim() == 2 else t.reshape(1, -1).expand(P, -1)).double() for t in ins], 1)
     edge = torch.zeros(P, dtype=torch.bool, device=x.device)
     for l in range(3):
@@ -357,7 +357,7 @@ def _relu_edge_rows(ins, t64, rel=2e-5):
 
 def _torch_module_forward(ins, trunk, heads):
     """ExAvatar's own evaluation in fp32: the modules on the concatenated input (constant blocks repeated)."""
-    P = ins[0].shape[0]
+    P = next(t.shape[0] for t in ins if t.dim() == 2)
     x = torch.cat([t if t.dim() == 2 else t.reshape(1, -1).repeat(P, 1).detach() for t in ins], 1)
     feat = trunk(x)
     return torch.cat([h(feat) for h in heads], 1) if heads else feat
