@@ -1,6 +1,7 @@
-"""Builds libb200raster.so (the C-ABI library of include/b200raster.h) in-tree with nvcc for the H100 (sm_90a).
+"""Builds libb200raster.so (the C-ABI library of include/b200raster.h) in-tree with nvcc for the H100 (sm_90a), and the
+compiled torch binding of the public call on top of it (_b2r_torch.so).
 
-The .so is a build product (git-ignored); nvcc cross-compiles it without a GPU.
+The .so files are build products (git-ignored); nvcc cross-compiles the library without a GPU.
 """
 from __future__ import annotations
 
@@ -57,14 +58,22 @@ def _stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False, ptxas_info: bool = False) -> str:
+    """Builds libb200raster.so and the compiled torch binding of the public call (`build_torch_ext`) when either is
+    missing or stale; force=True rebuilds both."""
     # B2R_LIB_OUT + B2R_NVCC_EXTRA: a tuning variant of the same library next to the product one (load it with B2R_LIB)
     global LIB
     variant = os.environ.get("B2R_LIB_OUT")
     if variant:
         LIB = os.path.abspath(variant)
         force = True
-    if not force and not _stale():
-        return LIB
+    if force or _stale():
+        _build_lib(force, verbose, ptxas_info, variant)
+    if not variant:  # the binding links the in-tree library only
+        build_torch_ext(force, verbose)
+    return LIB
+
+
+def _build_lib(force: bool, verbose: bool, ptxas_info: bool, variant) -> None:
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     extra = os.environ.get("B2R_NVCC_EXTRA", "").split()  # e.g. -DB2_DRAIN_UNROLL=8 for tuning experiments
     # one object per translation unit, compiled in parallel (no relocatable device code: kernels never call across
@@ -94,7 +103,6 @@ def build(force: bool = False, verbose: bool = False, ptxas_info: bool = False) 
     if verbose:
         print(" ".join(cmd), flush=True)
     subprocess.check_call(cmd)
-    return LIB
 
 
 TORCH_EXT = os.path.join(PKG, "_b2r_torch.so")
@@ -102,10 +110,11 @@ TORCH_SRC = os.path.join(PKG, "csrc_torch", "b2r_torch.cpp")
 
 
 def build_torch_ext(force: bool = False, verbose: bool = False) -> str:
-    """The compiled torch binding of the eager path (csrc_torch/b2r_torch.cpp): host code only, g++ against the torch
-    headers of this interpreter, linked to libb200raster.so next to it (rpath $ORIGIN).  In-tree like the CUDA library."""
-    lib = build()
-    deps = [TORCH_SRC, os.path.join(PKG, "..", "include", "b200raster.h"), os.path.abspath(__file__)]
+    """The compiled torch binding of the public call (csrc_torch/b2r_torch.cpp): host code only, g++ against the torch
+    headers of this interpreter, linked to the in-tree libb200raster.so next to it (rpath $ORIGIN), which `build()`
+    makes first.  Rebuilt when older than its source, the C ABI header, this file or the library."""
+    lib = os.path.join(PKG, "libb200raster.so")
+    deps = [TORCH_SRC, os.path.join(PKG, "..", "include", "b200raster.h"), os.path.abspath(__file__), lib]
     if not force and os.path.exists(TORCH_EXT) and os.path.getmtime(TORCH_EXT) > max(os.path.getmtime(d) for d in deps):
         return TORCH_EXT
     import sysconfig
@@ -130,4 +139,3 @@ def build_torch_ext(force: bool = False, verbose: bool = False) -> str:
 
 if __name__ == "__main__":
     build(force=True, verbose=True, ptxas_info="--ptxas" in sys.argv)
-    build_torch_ext(force=True, verbose=True)

@@ -7,8 +7,9 @@
 // allocation, the saved context, the backward call -- as a C++ torch::autograd::Function over the SAME C ABI
 // (include/b200raster.h, libb200raster.so).  No kernels here and no second implementation of anything on the device.
 //
-// Scope: the rasteriser call with adaptive capacity.  rasterizer.py keeps the Python route for debug=True (snapshot
-// dump on failure), fixed-capacity / CUDA-graph capture and statistics requests.
+// Scope: every rasteriser call -- adaptive capacity, fixed capacity (no polling, capturable in a CUDA graph) and
+// debug=True (synchronises after each call).  rasterizer.py only maps the public arguments onto `rasterize` and dumps
+// the inputs of a failed debug call.
 #include <torch/extension.h>
 
 #include <c10/cuda/CUDAGuard.h>
@@ -16,9 +17,12 @@
 #include <cuda_runtime.h>
 
 #include <chrono>
+#include <deque>
 #include <map>
 #include <memory>
 #include <mutex>
+#include <stdexcept>
+#include <string>
 #include <tuple>
 
 #include "b200raster.h"
@@ -52,8 +56,32 @@ DeviceState& state_of(int device) {
   return *s;
 }
 
+// ctx buffers of the 64 most recent fixed-capacity calls: nothing is polled in that mode, so `overflowed()` reads their
+// status blocks after the step.  Never destroyed, so no tensor is freed at exit after the CUDA allocator is gone.
+struct RecentContexts {
+  std::mutex mu;
+  std::deque<at::Tensor> bufs;
+};
+
+RecentContexts& recent() {
+  static RecentContexts* r = new RecentContexts();
+  return *r;
+}
+
+// Library errors leave as std::runtime_error (RuntimeError in Python), not through TORCH_CHECK: on the H100 a c10::Error
+// thrown here, with the call's CUDA buffers live, took the process down (SIGSEGV) instead of reaching the caller.
 void check(int rc, const char* what) {
-  TORCH_CHECK(rc == B2R_OK, "b200raster: ", what, " failed: ", b2r_strerror(rc), " (cuda error ", b2r_last_cuda_error(), ")");
+  if (rc != B2R_OK)
+    throw std::runtime_error(std::string("b200raster: ") + what + " failed: " + b2r_strerror(rc) + " (cuda error " +
+                             std::to_string(b2r_last_cuda_error()) + ")");
+}
+
+// debug=True (B2R_FLAG_DEBUG): wait for the call, so that a fault surfaces here rather than at a later API call
+void sync_if_debug(uint32_t flags, cudaStream_t stream, const char* what) {
+  if (!(flags & B2R_FLAG_DEBUG)) return;
+  const cudaError_t e = cudaStreamSynchronize(stream);
+  if (e != cudaSuccess)
+    throw std::runtime_error(std::string("b200raster: ") + what + " failed on the device: " + cudaGetErrorString(e));
 }
 
 // spin until the scan kernel has published {num_dups, token}
@@ -112,8 +140,8 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
                                const c10::optional<at::Tensor>& rots_in, const c10::optional<at::Tensor>& cov_in, int64_t H,
                                int64_t W, double tanfovx, double tanfovy, const at::Tensor& bg_in, double scale_modifier,
                                const at::Tensor& view_in, const at::Tensor& proj_in, int64_t sh_degree,
-                               const at::Tensor& campos_in, bool tile_cull, bool speculative, double headroom,
-                               bool segmented) {
+                               const at::Tensor& campos_in, bool speculative, double headroom, int64_t fixed_capacity,
+                               bool debug) {
     const bool need_grad = means3D_in.requires_grad() || means2D.requires_grad() || (present(sh_in) && sh_in->requires_grad()) ||
                            (present(colors_in) && colors_in->requires_grad()) || opac_in.requires_grad() ||
                            (present(scales_in) && scales_in->requires_grad()) ||
@@ -146,57 +174,68 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
     }
     const at::Tensor bg = f32c(bg_in.to(dev), "bg"), view = f32c(view_in.to(dev), "viewmatrix");
     const at::Tensor proj = f32c(proj_in.to(dev), "projmatrix"), campos = f32c(campos_in.to(dev), "campos");
-    const uint32_t flags = tile_cull ? 0u : B2R_FLAG_NO_TILE_CULL;
+    const uint32_t flags = debug ? B2R_FLAG_DEBUG : 0u;
     const B2RScene sc = make_scene(P, H, W, sh_degree, flags, scale_modifier, tanfovx, tanfovy, bg, view, proj, campos,
                                    means3D, shs, colors, opac, scales, rots, cov);
     const size_t ctx_bytes = b2r_ctx_bytes((int32_t)P, (int32_t)W, (int32_t)H);
     at::Tensor ctx_buf = at::empty({(int64_t)ctx_bytes}, u8);
     B2RForwardOutputs out{color.data_ptr<float>(), depth.data_ptr<float>(), alpha.data_ptr<float>(), radii.data_ptr<int32_t>()};
 
-    DeviceState& st = state_of(dev.index());
     at::Tensor ids, ck;
-    uint64_t cap = 0, num = 0;
-    auto workspace = [&](uint64_t capacity, uint64_t token) {
+    uint64_t cap = 0;
+    auto workspace = [&](uint64_t capacity, uint64_t* mirror, uint64_t token) {
       cap = capacity;
       ids = at::empty({(int64_t)std::max<uint64_t>(cap, 1)}, i32);
       const size_t sbytes = b2r_scratch_bytes((int32_t)P, (int32_t)W, (int32_t)H, cap);
       at::Tensor scratch = at::empty({(int64_t)sbytes}, u8);  // recycled by the caching allocator in stream order
       size_t ckb = 0;
       ck = at::Tensor();
-      if (need_grad && segmented) {
+      if (need_grad) {  // segment table + blend-state checkpoints: the backward replays list segments independently
         ckb = b2r_checkpoint_bytes((int32_t)W, (int32_t)H, cap);
         ck = at::empty({(int64_t)ckb}, u8);
       }
       B2RWorkspace ws{ctx_buf.data_ptr(), ctx_bytes, (uint32_t*)ids.data_ptr<int32_t>(), cap, scratch.data_ptr(), sbytes,
-                      const_cast<uint64_t*>(st.mirror), token, ck.defined() ? ck.data_ptr() : nullptr, ckb};
+                      mirror, token, ck.defined() ? ck.data_ptr() : nullptr, ckb};
       return ws;
     };
-    {
+    if (fixed_capacity >= 0) {
+      // no pinned allocation (state_of), lock or poll: the call is capturable in a CUDA graph.  An overflow truncates
+      // the lists (never corrupts them) and is reported by `overflowed()` from the status block.
+      const B2RWorkspace ws = workspace((uint64_t)fixed_capacity, nullptr, 0);
+      check(b2r_forward(&sc, &ws, &out, stream), "b2r_forward");
+      RecentContexts& r = recent();
+      std::lock_guard<std::mutex> g(r.mu);
+      r.bufs.push_back(ctx_buf);
+      if (r.bufs.size() > 64) r.bufs.pop_front();
+    } else {
+      DeviceState& st = state_of(dev.index());
+      uint64_t* mirror = const_cast<uint64_t*>(st.mirror);
       std::lock_guard<std::mutex> g(st.mu);
       const auto key = std::make_tuple(P, W, H);
       const auto it = st.predicted.find(key);
+      uint64_t num = 0;
       if (speculative && it != st.predicted.end()) {
         uint64_t token = ++st.token;
-        B2RWorkspace ws = workspace((uint64_t)((double)it->second * headroom) + 4096, token);
+        B2RWorkspace ws = workspace((uint64_t)((double)it->second * headroom) + 4096, mirror, token);
         check(b2r_forward(&sc, &ws, &out, stream), "b2r_forward");
         num = wait_mirror(st, token, stream);
         if (num > cap) {  // misprediction: the whole forward again with the exact size
           token = ++st.token;
-          ws = workspace(num, token);
+          ws = workspace(num, mirror, token);
           check(b2r_forward(&sc, &ws, &out, stream), "b2r_forward");
           num = wait_mirror(st, token, stream);
         }
       } else {
         const uint64_t token = ++st.token;
-        B2RWorkspace ws0{ctx_buf.data_ptr(), ctx_bytes, nullptr, 0, nullptr, 0, const_cast<uint64_t*>(st.mirror), token,
-                         nullptr, 0};
+        B2RWorkspace ws0{ctx_buf.data_ptr(), ctx_bytes, nullptr, 0, nullptr, 0, mirror, token, nullptr, 0};
         check(b2r_forward_project(&sc, &ws0, radii.data_ptr<int32_t>(), stream), "b2r_forward_project");
         num = wait_mirror(st, token, stream);
-        B2RWorkspace ws = workspace(num, token);
+        B2RWorkspace ws = workspace(num, mirror, token);
         check(b2r_forward_render(&sc, &ws, &out, stream), "b2r_forward_render");
       }
       st.predicted[key] = num;
     }
+    sync_if_debug(flags, stream, "b2r_forward");
     // what must survive until backward (SURVEY.md section 8b "Ownership"); undefined tensors are saved as such
     ctx->save_for_backward({means3D, shs, colors, opac, scales, rots, cov, bg, view, proj, campos, ctx_buf, ids, ck});
     ctx->saved_data["H"] = H;
@@ -270,6 +309,7 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
     a.dL_drotations = d_rots.data_ptr<float>();
     a.dL_dcov3D = d_cov.data_ptr<float>();
     check(b2r_backward(&sc, &ws, &a, scratch.data_ptr(), sbytes, stream), "b2r_backward");
+    sync_if_debug(sc.flags, stream, "b2r_backward");
     int64_t m2_numel = 1;
     for (auto v : m2_shape) m2_numel *= v;
     out[0] = d_means3D;
@@ -289,17 +329,28 @@ std::vector<at::Tensor> rasterize(const at::Tensor& means3D, const at::Tensor& m
                                   const c10::optional<at::Tensor>& scales, const c10::optional<at::Tensor>& rots,
                                   const c10::optional<at::Tensor>& cov, int64_t H, int64_t W, double tanfovx, double tanfovy,
                                   const at::Tensor& bg, double scale_modifier, const at::Tensor& view, const at::Tensor& proj,
-                                  int64_t sh_degree, const at::Tensor& campos, bool tile_cull, bool speculative,
-                                  double headroom, bool segmented) {
+                                  int64_t sh_degree, const at::Tensor& campos, bool speculative, double headroom,
+                                  int64_t fixed_capacity, bool debug) {
   return RasterizeFn::apply(means3D, means2D, sh, colors, opac, scales, rots, cov, H, W, tanfovx, tanfovy, bg, scale_modifier,
-                            view, proj, sh_degree, campos, tile_cull, speculative, headroom, segmented);
+                            view, proj, sh_degree, campos, speculative, headroom, fixed_capacity, debug);
 }
 
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.def("rasterize", &rasterize, "GaussianRasterizer forward with autograd (compiled host path over libb200raster.so)");
+  m.def("rasterize", &rasterize, "GaussianRasterizer forward with autograd (compiled host path over libb200raster.so); "
+        "fixed_capacity < 0: adaptive duplicate capacity");
   m.def("abi_version", []() { return b2r_abi_version(); });
+  m.def("recent_contexts", []() {  // ctx buffers of the recent fixed-capacity calls, oldest first
+    RecentContexts& r = recent();
+    std::lock_guard<std::mutex> g(r.mu);
+    return std::vector<at::Tensor>(r.bufs.begin(), r.bufs.end());
+  });
+  m.def("clear_recent", []() {
+    RecentContexts& r = recent();
+    std::lock_guard<std::mutex> g(r.mu);
+    r.bufs.clear();
+  });
   m.def("get_predicted", [](int64_t device, int64_t P, int64_t W, int64_t H) -> int64_t {  // -1: shape not seen yet
     DeviceState& st = state_of((int)device);
     std::lock_guard<std::mutex> g(st.mu);

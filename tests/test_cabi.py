@@ -226,9 +226,10 @@ def test_error_codes_of_the_abi_v3_entry_points_without_touching_cuda():
     assert lib.b2r_launch_count() == launches
 
 
-def test_compiled_torch_binding_builds_and_loads():
-    """csrc_torch/b2r_torch.cpp (the eager call's host path as a C++ autograd Function) builds in-tree against this
-    interpreter's torch, links to libb200raster.so and reports the same ABI version.  No compute here (no GPU)."""
+def test_compiled_torch_binding_builds_loads_and_refuses_cpu_tensors():
+    """csrc_torch/b2r_torch.cpp (the public call's host as a C++ autograd Function) builds in-tree against this
+    interpreter's torch, links to libb200raster.so, reports the same ABI version and refuses CPU tensors with adaptive
+    and with fixed capacity.  No compute here (no GPU)."""
     from exavatar_release_b200 import build_ext, rasterizer
     path = build_ext.build_torch_ext()
     assert os.path.exists(path)
@@ -236,6 +237,7 @@ def test_compiled_torch_binding_builds_and_loads():
     assert ext and ext.abi_version() == L.ABI_VERSION
     import torch
     a = torch.zeros(4, 3)
-    with pytest.raises(RuntimeError, match="CUDA tensor"):  # no CPU fallback in the compiled route either
-        ext.rasterize(a, a, None, a, torch.zeros(4, 1), a, torch.zeros(4, 4), None, 16, 16, 1.0, 1.0, torch.zeros(3), 1.0,
-                      torch.eye(4), torch.eye(4), 0, torch.zeros(3), True, True, 1.25, True)
+    for fixed_capacity in (-1, 1000):  # no CPU fallback in either capacity mode
+        with pytest.raises(RuntimeError, match="CUDA tensor"):
+            ext.rasterize(a, a, None, a, torch.zeros(4, 1), a, torch.zeros(4, 4), None, 16, 16, 1.0, 1.0, torch.zeros(3),
+                          1.0, torch.eye(4), torch.eye(4), 0, torch.zeros(3), True, 1.25, fixed_capacity, False)

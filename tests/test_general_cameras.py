@@ -450,35 +450,36 @@ def _mixed(cam, seed_tag, n_plain, n_clamp):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("route", ["compiled", "python"])
+@pytest.mark.parametrize("capacity", ["adaptive", "fixed"])
 @pytest.mark.parametrize("mode", ["rgb", "cov"])
-def test_public_rasterizer_matches_oracle(dev, monkeypatch, route, mode):
-    """GaussianRasterizer (compiled C++ binding or the Python autograd Function) with scale / rotation or
-    cov3D_precomp at a general camera, against the oracle."""
+def test_public_rasterizer_matches_oracle(dev, capacity, mode):
+    """GaussianRasterizer with scale / rotation or cov3D_precomp at a general camera, against the oracle; with the
+    adaptive duplicate capacity and with a fixed one (`set_fixed_capacity`, the graph-capturable call)."""
     from exavatar_release_b200 import rasterizer as rz
-    if route == "python":
-        monkeypatch.setattr(rz, "_COMPILED", False)
-    else:
-        assert rz._compiled_binding(), "the compiled binding (_b2r_torch.so) must be built"
     cam = "c203x131"
     st, a = _mixed(cam, "public", 1500, 300)
     if mode == "cov":
         a = _with_cov(a, _seed(cam, "cov"))
     H, W = st.image_height, st.image_width
-    case = f"gencam/public/{route}/{mode}"
+    case = f"gencam/public/{capacity}/{mode}"
     oc, orad, od, oa, octx = O.forward(st, a["mean_3d"], a["opacity"], **_oracle_kw(a, mode))
     pm, gm = O.fragility(octx)
     P = a["mean_3d"].shape[0]
     L = {k: v.to(dev).requires_grad_() for k, v in a.items() if k != "_pcam"}
     m2 = torch.zeros(P, 3, device=dev, requires_grad=True)
-    color, radii, depth, alpha = rz.GaussianRasterizer(settings_on(st, dev, rz.GaussianRasterizationSettings))(
-        means3D=L["mean_3d"], means2D=m2, opacities=L["opacity"], **_oracle_kw(L, mode))
+    rz.set_fixed_capacity(octx.num_dups + 4096 if capacity == "fixed" else None)
+    try:
+        color, radii, depth, alpha = rz.GaussianRasterizer(settings_on(st, dev, rz.GaussianRasterizationSettings))(
+            means3D=L["mean_3d"], means2D=m2, opacities=L["opacity"], **_oracle_kw(L, mode))
+        gi, gd, ga = grad_images(H, W, _seed(case))
+        ((color * gi.to(dev)).sum() + (depth * gd.to(dev)).sum() + (alpha * ga.to(dev)).sum()).backward()
+        assert not rz.overflowed()
+    finally:
+        rz.set_fixed_capacity(None)
     assert np.array_equal(radii.cpu().numpy(), orad)
     compare(case, "color", color.detach().cpu().numpy(), oc, pm[None], kind="image")
     compare(case, "depth", depth.detach().cpu().numpy(), od, pm[None], kind="image")
     compare(case, "alpha", alpha.detach().cpu().numpy(), oa, pm[None], kind="image")
-    gi, gd, ga = grad_images(H, W, _seed(case))
-    ((color * gi.to(dev)).sum() + (depth * gd.to(dev)).sum() + (alpha * ga.to(dev)).sum()).backward()
     og = O.backward(octx, gi.numpy(), gd.numpy()[0], ga.numpy()[0])
     pairs = [("means3D", L["mean_3d"].grad), ("means2D", m2.grad), ("opacities", L["opacity"].grad),
              ("colors", L["rgb"].grad)]

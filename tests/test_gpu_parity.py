@@ -279,12 +279,12 @@ def test_cov3d_precomp_path(dev):
 
 
 @pytest.mark.parametrize("case", ["rgb", "sh", "cov", "depth_alpha_only", "noncontiguous"])
-def test_compiled_binding_equals_python_route(dev, monkeypatch, case):
-    """The C++ autograd Function (csrc_torch/b2r_torch.cpp) and the Python one (_RasterizeGaussians) are two hosts of the
-    same kernels: identical forward outputs bit for bit, gradients equal up to the order of the backward's atomic sums,
-    None exactly where the other route returns None."""
+def test_public_call_equals_frame_plan(dev, case):
+    """The public call (the compiled binding, csrc_torch/b2r_torch.cpp) and FramePlan (the C ABI through plan.py) are two
+    hosts of the same kernels: identical forward outputs bit for bit, gradients equal up to the order of the backward's
+    atomic sums.  The public call returns a gradient for exactly the inputs it was given."""
+    from exavatar_release_b200.plan import FramePlan
     rz = RZ()
-    assert rz._compiled_binding(), "the compiled binding (_b2r_torch.so) must be built: python -m exavatar_release_b200.build_ext"
     wl = "T2" if case == "sh" else "T1"
     st = workload_settings(wl, yaw=9.0, device=dev, settings_cls=rz.GaussianRasterizationSettings)
     if case == "sh":
@@ -294,45 +294,50 @@ def test_compiled_binding_equals_python_route(dev, monkeypatch, case):
         assert not st.viewmatrix.is_contiguous()
     a0 = make_assets(wl, seed=3)
     P = a0["mean_3d"].shape[0]
+    H, W = st.image_height, st.image_width
     if case == "cov":
         g = torch.Generator().manual_seed(5)
         A = torch.randn(P, 3, 3, generator=g) * 0.05
         S = A @ A.transpose(1, 2) + 1e-4 * torch.eye(3)
         a0 = dict(a0, cov=torch.stack([S[:, 0, 0], S[:, 0, 1], S[:, 0, 2], S[:, 1, 1], S[:, 1, 2], S[:, 2, 2]], 1))
+    given = {"sh": ("shs", "scale", "rotation"), "cov": ("rgb", "cov")}.get(case, ("rgb", "scale", "rotation"))
+    given = ("mean_3d", "opacity") + given
+    # asset key -> (keyword of the public call, gradient name of FramePlan.backward)
+    names = {"mean_3d": ("means3D", "means3D"), "opacity": ("opacities", "opacities"), "shs": ("shs", "shs"),
+             "rgb": ("colors_precomp", "colors"), "scale": ("scales", "scales"), "rotation": ("rotations", "rotations"),
+             "cov": ("cov3D_precomp", "cov3D")}
     gi = make_grad_image(wl, 4).to(dev)
+    g_color, g_depth, g_alpha = gi, None, None
+    if case == "depth_alpha_only":
+        g_color, g_depth, g_alpha = None, gi[:1], gi[1:2]
+    elif case == "rgb":
+        g_depth = 0.3 * gi[:1]
 
-    def run(compiled):
-        monkeypatch.setattr(rz, "_COMPILED", rz._compiled_binding() if compiled else False)
-        a = {k: v.to(dev).requires_grad_() for k, v in a0.items()}
-        m2 = torch.zeros(P, 3, device=dev, requires_grad=True)
-        kw = dict(means3D=a["mean_3d"], means2D=m2, opacities=a["opacity"])
-        if case == "sh":
-            kw.update(shs=a["shs"], scales=a["scale"], rotations=a["rotation"])
-        elif case == "cov":
-            kw.update(colors_precomp=a["rgb"], cov3D_precomp=a["cov"])
-        else:
-            kw.update(colors_precomp=a["rgb"], scales=a["scale"], rotations=a["rotation"])
-        out = rz.GaussianRasterizer(st)(**kw)
-        color, radii, depth, alpha = out
-        if case == "depth_alpha_only":
-            loss = (depth * gi[:1]).sum() + (alpha * gi[1:2]).sum()
-        elif case == "rgb":
-            loss = (color * gi).sum() + 0.3 * (depth * gi[:1]).sum()
-        else:
-            loss = (color * gi).sum()
-        loss.backward()
-        return [t.detach() for t in out], {k: v.grad for k, v in a.items()}, m2.grad
+    a = {k: v.to(dev).requires_grad_() for k, v in a0.items()}
+    m2 = torch.zeros(P, 3, device=dev, requires_grad=True)
+    out = rz.GaussianRasterizer(st)(means2D=m2, **{names[k][0]: a[k] for k in given})
+    sum((t * gt).sum() for t, gt in zip((out[0], out[2], out[3]), (g_color, g_depth, g_alpha)) if gt is not None).backward()
 
-    o_c, g_c, m_c = run(True)
-    o_p, g_p, m_p = run(False)
-    for x, y in zip(o_c, o_p):
-        assert torch.equal(x, y)
+    x = {k: v.to(dev) for k, v in a0.items()}
+    get = lambda k: x[k] if k in given else None
+    plan = FramePlan(P, W, H, rz.last_duplicate_count(dev, P, W, H), dev, sh_coeffs=a0["shs"].shape[1] if case == "sh" else 0)
+    sc, keep = rz._make_scene(st, x["mean_3d"], get("shs"), get("rgb"), x["opacity"], get("scale"), get("rotation"),
+                              get("cov"), 0)
+    plan.forward(sc)
+    grads = {names[k][1]: torch.zeros_like(x[k]) for k in given}
+    grads["means2D"] = torch.zeros(P, 3, device=dev)
+    plan.backward(sc, torch.zeros_like(gi) if g_color is None else g_color, grads, g_depth=g_depth, g_alpha=g_alpha)
+    torch.cuda.synchronize()
+    assert not plan.status()["overflow"]
+    for x_, y in zip(out, (plan.color, plan.radii, plan.depth, plan.alpha)):
+        assert torch.equal(x_.detach(), y)
     close = lambda x, y: torch.allclose(x, y, rtol=1e-4, atol=1e-5 * float(y.abs().max()) + 1e-12)
-    for k in g_p:
-        assert (g_c[k] is None) == (g_p[k] is None), k
-        if g_p[k] is not None:
-            assert g_c[k].shape == g_p[k].shape and close(g_c[k], g_p[k]), k
-    assert close(m_c, m_p)
+    for k in a:
+        assert (a[k].grad is None) == (k not in given), k
+        if k in given:
+            y = grads[names[k][1]]
+            assert a[k].grad.shape == y.shape and close(a[k].grad, y), k
+    assert close(m2.grad, grads["means2D"])
 
 
 def test_compiled_binding_handles_an_empty_call(dev):
@@ -372,20 +377,21 @@ def test_five_live_contexts_then_one_backward(dev):
         assert torch.allclose(m2.grad, m2b.grad, rtol=1e-4, atol=1e-4 * float(m2b.grad.abs().max()))
 
 
-@pytest.mark.parametrize("route", ["compiled", "python"])
-def test_forward_is_deterministic_and_capacity_modes_agree(dev, monkeypatch, route):
+@pytest.mark.parametrize("wl", ["T1", "T2"])
+def test_forward_is_deterministic_and_capacity_modes_agree(dev, monkeypatch, wl):
+    """RGB (T1) and degree-3 SH (T2) colour sources."""
     rz = RZ()
-    if route == "python":
-        monkeypatch.setattr(rz, "_COMPILED", False)
-    else:
-        assert rz._compiled_binding(), "the compiled binding (_b2r_torch.so) must be built: python -m exavatar_release_b200.build_ext"
-    st = workload_settings("T1", yaw=12.0, device=dev, settings_cls=rz.GaussianRasterizationSettings)
-    a = {k: v.to(dev) for k, v in make_assets("T1", seed=0).items()}
+    st = workload_settings(wl, yaw=12.0, device=dev, settings_cls=rz.GaussianRasterizationSettings)
+    a = {k: v.to(dev) for k, v in make_assets(wl, seed=0).items()}
     P = a["mean_3d"].shape[0]
+    colour = dict(colors_precomp=a["rgb"])
+    if wl == "T2":
+        st = st._replace(sh_degree=3)
+        colour = dict(shs=a["shs"])
 
     def render():
         return rz.GaussianRasterizer(st)(means3D=a["mean_3d"], means2D=torch.zeros(P, 3, device=dev), opacities=a["opacity"],
-                                         colors_precomp=a["rgb"], scales=a["scale"], rotations=a["rotation"])
+                                         scales=a["scale"], rotations=a["rotation"], **colour)
 
     monkeypatch.setattr(rz, "CAPACITY_MODE", "exact")
     ref = render()
@@ -397,13 +403,101 @@ def test_forward_is_deterministic_and_capacity_modes_agree(dev, monkeypatch, rou
     for x, y in zip(ref, spec):
         assert torch.equal(x, y)
     # a misprediction (capacity far too small) must be repaired transparently
-    rz._state(dev).predicted[(P, st.image_width, st.image_height)] = 10
-    if route == "compiled":
-        rz._compiled_binding().set_predicted(dev.index, P, st.image_width, st.image_height, 10)
+    rz._compiled_binding().set_predicted(dev.index, P, st.image_width, st.image_height, 10)
     monkeypatch.setattr(rz, "CAPACITY_HEADROOM", 1.0)
     small = render()
     for x, y in zip(ref, small):
         assert torch.equal(x, y)
+
+
+def test_fixed_capacity_call_is_graph_capturable(dev):
+    """Under set_fixed_capacity the public call polls nothing: forward + loss.backward() are captured in one CUDA graph
+    whose replay gives the eager adaptive call's image bit for bit and its gradients.  An undersized capacity is reported
+    by overflowed() (the lists are truncated, never corrupt); set_fixed_capacity(None) restores the adaptive policy."""
+    rz = RZ()
+    st = workload_settings("T1", yaw=12.0, device=dev, settings_cls=rz.GaussianRasterizationSettings)
+    a0 = {k: v.to(dev) for k, v in make_assets("T1", seed=6).items()}
+    P, W, H = a0["mean_3d"].shape[0], st.image_width, st.image_height
+    gi = make_grad_image("T1", 6).to(dev)
+    leaves = {k: v.clone().requires_grad_() for k, v in a0.items()}
+    m2 = torch.zeros(P, 3, device=dev, requires_grad=True)
+
+    def step(rows=P):
+        for t in (*leaves.values(), m2):
+            t.grad = None
+        color = rz.GaussianRasterizer(st)(means3D=leaves["mean_3d"][:rows], means2D=m2[:rows],
+                                          opacities=leaves["opacity"][:rows], colors_precomp=leaves["rgb"][:rows],
+                                          scales=leaves["scale"][:rows], rotations=leaves["rotation"][:rows])[0]
+        (color * gi).sum().backward()
+        return color
+
+    ref = step().detach().clone()
+    ref_grads = [t.grad.clone() for t in (*leaves.values(), m2)]
+    dups = rz.last_duplicate_count(dev, P, W, H)
+    Q = P - 7  # a shape no adaptive call has rendered yet
+    try:
+        rz.set_fixed_capacity(int(dups * 1.25) + 4096)
+        side = torch.cuda.Stream(dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(2):
+                step()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            color = step()
+        graph.replay()
+        torch.cuda.synchronize(dev)
+        assert torch.equal(color, ref)
+        for t, g in zip((*leaves.values(), m2), ref_grads):
+            assert torch.allclose(t.grad, g, rtol=1e-4, atol=1e-5 * float(g.abs().max()) + 1e-12)
+        assert not rz.overflowed()
+
+        rz.set_fixed_capacity(dups // 2)
+        with torch.no_grad():
+            rz.GaussianRasterizer(st)(means3D=a0["mean_3d"][:Q], means2D=m2[:Q], opacities=a0["opacity"][:Q],
+                                      colors_precomp=a0["rgb"][:Q], scales=a0["scale"][:Q], rotations=a0["rotation"][:Q])
+        assert rz.overflowed()
+        with pytest.raises(KeyError):  # a fixed-capacity call records no duplicate count
+            rz.last_duplicate_count(dev, Q, W, H)
+    finally:
+        rz.set_fixed_capacity(None)
+    assert not rz.overflowed()
+    step(Q)
+    assert rz.last_duplicate_count(dev, Q, W, H) > dups // 2
+    assert torch.equal(step(), ref)
+
+
+def test_debug_call(dev, tmp_path, monkeypatch):
+    """debug=True: a valid call gives the outputs and gradients of debug=False; an invalid one (sh_degree 4 with 16
+    coefficients, rejected on the host before any launch) raises and leaves snapshot_fw.dump with its inputs."""
+    rz = RZ()
+    st = workload_settings("T2", yaw=5.0, device=dev, settings_cls=rz.GaussianRasterizationSettings)._replace(sh_degree=3)
+    a0 = {k: v.to(dev) for k, v in make_assets("T2", seed=1).items()}
+    gi = make_grad_image("T2", 1).to(dev)
+
+    def run(settings):
+        a = {k: v.clone().requires_grad_() for k, v in a0.items()}
+        out = rz.GaussianRasterizer(settings)(means3D=a["mean_3d"], means2D=torch.zeros_like(a["mean_3d"]),
+                                              opacities=a["opacity"], shs=a["shs"], scales=a["scale"],
+                                              rotations=a["rotation"])
+        (out[0] * gi).sum().backward()
+        return [t.detach() for t in out], [a[k].grad for k in ("mean_3d", "opacity", "shs", "scale", "rotation")]
+
+    out, grads = run(st)
+    out_d, grads_d = run(st._replace(debug=True))
+    for x, y in zip(out_d, out):
+        assert torch.equal(x, y)
+    for x, y in zip(grads_d, grads):
+        assert torch.allclose(x, y, rtol=1e-4, atol=1e-5 * float(y.abs().max()) + 1e-12)
+
+    monkeypatch.chdir(tmp_path)
+    with pytest.raises(RuntimeError, match="b2r_forward"):
+        run(st._replace(sh_degree=4, debug=True))
+    dump = torch.load(tmp_path / "snapshot_fw.dump")
+    assert len(dump) == 7 and dump[1] is not None and dump[2] is None and dump[6] is None
+    assert torch.equal(dump[0], a0["mean_3d"].cpu()) and torch.equal(dump[1], a0["shs"].cpu())
 
 
 def test_properties_at_full_size(dev):
