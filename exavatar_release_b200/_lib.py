@@ -103,6 +103,22 @@ class B2RRegsGrads(C.Structure):
                                    "rgb_refined", "scale_reg", "joint_offset")]
 
 
+class B2RRig(C.Structure):
+    """ExAvatar's SMPL-X rig (b2r_rig_forward / b2r_rig_backward): the per-call inputs and the model's tables."""
+    _fields_ = [
+        ("V", C.c_int32), ("V1", C.c_int32), ("P", C.c_int32), ("J", C.c_int32), ("NB", C.c_int32), ("NE", C.c_int32),
+        ("n_body", C.c_int32), ("reserved", C.c_int32),
+        *[(n, _fp) for n in ("shape_param", "joint_offset", "full_pose", "expr", "template_", "shapedirs", "expr_dirs",
+                             "posedirs_t", "pose_offset0", "lbs_weights", "jreg_offsets", "jreg_cols", "jreg_vals",
+                             "jregT_offsets", "jregT_rows", "jregT_vals", "parents", "rot_neutral", "rot_zero",
+                             "rot_inv", "sub1", "sub2", "upT_offsets", "upT_rows", "upT_w", "mask")],
+    ]
+
+
+class B2RRigGrads(C.Structure):
+    _fields_ = [(n, _fp) for n in ("shape_param", "joint_offset", "full_pose", "expr")]
+
+
 class B2RForwardOutputs(C.Structure):
     _fields_ = [("color", _fp), ("depth", _fp), ("alpha", _fp), ("radii", _fp)]
 
@@ -186,6 +202,9 @@ SYMBOLS = [
     ("b2r_regs_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32]),
     ("b2r_regs_forward", C.c_int, [C.POINTER(B2RRegs), _fp, _fp, C.c_size_t, _fp]),
     ("b2r_regs_backward", C.c_int, [C.POINTER(B2RRegs), _fp, C.POINTER(B2RRegsGrads), _fp, C.c_size_t, _fp]),
+    ("b2r_rig_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    ("b2r_rig_forward", C.c_int, [C.POINTER(B2RRig), _fp, _fp, _fp, _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
+    ("b2r_rig_backward", C.c_int, [C.POINTER(B2RRig), _fp, _fp, _fp, C.POINTER(B2RRigGrads), _fp, C.c_size_t, _fp]),
     ("b2r_profile_enable", None, [C.c_int]),
     ("b2r_profile_read", C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int]),
     ("b2r_launch_count", C.c_uint64, []),
@@ -217,10 +236,10 @@ def load():
     if lib.b2r_abi_version() != ABI_VERSION:
         raise RuntimeError("b200raster: ABI version mismatch between the Python binding and libb200raster.so")
     # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8, B2RGnMlp 10 (9 unused too), B2RRegs 11,
-    # B2RRegsGrads 12
+    # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14
     for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
                      (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp), (11, B2RRegs),
-                     (12, B2RRegsGrads)):
+                     (12, B2RRegsGrads), (13, B2RRig), (14, B2RRigGrads)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

@@ -39,9 +39,11 @@ NVCC_FLAGS = [
 # (mesh_render.face_render_reference), so the per-pixel face is identical to it instead of "equal except at ulp ties".
 # regularizers.cu: the arm window |fl(l_x - u_x)| < 0.01f and the fp32 distances that pick the 50 nearest upper-arm rows
 # are the reference's expressions rounded operation by operation, so the selection (ties included) is the reference's.
+# smplx_rig.cu: the subdivision midpoints are fl(fl(a + b) * 0.5f) like pytorch3d's SubdivideMeshes, and the rig's
+# outputs feed every human render, so no product or sum is contracted.
 PER_FILE_FLAGS = {"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
                   "geometry.cu": ["--fmad=false"], "mesh_raster.cu": ["--fmad=false"],
-                  "regularizers.cu": ["--fmad=false"]}
+                  "regularizers.cu": ["--fmad=false"], "smplx_rig.cu": ["--fmad=false"]}
 
 
 def sources():

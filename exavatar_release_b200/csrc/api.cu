@@ -118,6 +118,22 @@ int validate_regs(const B2RRegs* r) {
   return B2R_OK;
 }
 
+// smplx_rig.cu: one thread per joint in a 128-thread CTA (J <= 64), NB / NE <= 128 (four coefficients per lane), the
+// pose_6d of the body joints needs 1 + n_body + 3 face joints <= J, and every table and input is required
+int validate_rig(const B2RRig* r) {
+  if (!r) return B2R_E_INVALID;
+  if (r->V < 1 || r->V1 < r->V || r->P < r->V1 || r->P >= (1 << 28) || r->J < 2 || r->J > 64 || r->NB < 1 ||
+      r->NB > 128 || r->NE < 1 || r->NE > 128 || r->n_body < 1 || r->n_body + 4 > r->J)
+    return B2R_E_INVALID;
+  if (!r->shape_param || !r->joint_offset || !r->full_pose || !r->expr) return B2R_E_INVALID;
+  if (!r->template_ || !r->shapedirs || !r->expr_dirs || !r->posedirs_t || !r->pose_offset0 || !r->lbs_weights ||
+      !r->jreg_offsets || !r->jreg_cols || !r->jreg_vals || !r->jregT_offsets || !r->jregT_rows || !r->jregT_vals ||
+      !r->parents || !r->rot_neutral || !r->rot_zero || !r->rot_inv || (r->V1 > r->V && !r->sub1) ||
+      (r->P > r->V1 && !r->sub2) || !r->upT_offsets || !r->upT_rows || !r->upT_w || !r->mask)
+    return B2R_E_INVALID;
+  return B2R_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -150,6 +166,8 @@ size_t b2r_sizeof(int which) {
     case 10: return sizeof(B2RGnMlp);  // 9 stays unused
     case 11: return sizeof(B2RRegs);
     case 12: return sizeof(B2RRegsGrads);
+    case 13: return sizeof(B2RRig);
+    case 14: return sizeof(B2RRigGrads);
     default: return 0;
   }
 }
@@ -472,6 +490,28 @@ int b2r_regs_backward(const B2RRegs* r, const float* dL_dout, const B2RRegsGrads
     return B2R_E_INVALID;
   if (scratch_bytes < regs_scratch_bytes(r->P, r->n_arm)) return B2R_E_WORKSPACE;
   return launch_regs_backward(*r, dL_dout, *grads, scratch, (cudaStream_t)stream);
+}
+
+size_t b2r_rig_scratch_bytes(int32_t V, int32_t J, int32_t NB, int32_t NE) { return rig_scratch_bytes(V, J, NB, NE); }
+
+int b2r_rig_forward(const B2RRig* r, float* mesh, float* mesh_wo, float* joint_mats, float* pose_offset,
+                    float* expr_offset, float* pose_6d, void* scratch, size_t scratch_bytes, void* stream) {
+  const int rc = validate_rig(r);
+  if (rc) return rc;
+  if (!mesh || !mesh_wo || !joint_mats || !pose_offset || !expr_offset || !pose_6d || !scratch) return B2R_E_INVALID;
+  if (scratch_bytes < rig_scratch_bytes(r->V, r->J, r->NB, r->NE)) return B2R_E_WORKSPACE;
+  return launch_rig_forward(*r, mesh, mesh_wo, joint_mats, pose_offset, expr_offset, pose_6d, scratch,
+                            (cudaStream_t)stream);
+}
+
+int b2r_rig_backward(const B2RRig* r, const float* dL_dmesh, const float* dL_djoint_mats, const float* dL_dexpr_offset,
+                     const B2RRigGrads* grads, void* scratch, size_t scratch_bytes, void* stream) {
+  const int rc = validate_rig(r);
+  if (rc) return rc;
+  if (!grads || !grads->shape_param || !grads->joint_offset || !grads->full_pose || !grads->expr || !scratch)
+    return B2R_E_INVALID;
+  if (scratch_bytes < rig_scratch_bytes(r->V, r->J, r->NB, r->NE)) return B2R_E_WORKSPACE;
+  return launch_rig_backward(*r, dL_dmesh, dL_djoint_mats, dL_dexpr_offset, *grads, scratch, (cudaStream_t)stream);
 }
 
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {

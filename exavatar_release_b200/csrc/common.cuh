@@ -540,6 +540,11 @@ size_t regs_scratch_bytes(int P, int n_arm);
 int launch_regs_forward(const B2RRegs& r, float* out, void* scratch, cudaStream_t st);
 int launch_regs_backward(const B2RRegs& r, const float* dout, const B2RRegsGrads& g, const void* scratch,
                          cudaStream_t st);
+size_t rig_scratch_bytes(int V, int J, int NB, int NE);
+int launch_rig_forward(const B2RRig& r, float* mesh, float* mesh_wo, float* joint_mats, float* pose_offset,
+                       float* expr_offset, float* pose_6d, void* scratch, cudaStream_t st);
+int launch_rig_backward(const B2RRig& r, const float* dmesh, const float* djm, const float* dexpr, const B2RRigGrads& g,
+                        void* scratch, cudaStream_t st);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

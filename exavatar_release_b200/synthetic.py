@@ -128,16 +128,23 @@ def make_population_assets(workload, seed=0, device="cpu", focal_ratio=1.465):
     return to(scene), to(human), to(refined)
 
 
-def _subdivide(verts, faces):
-    """One midpoint subdivision (each triangle into four, no smoothing), the input vertices kept first -- the order
-    ExAvatar's `lr_idx_to_hr_idx` relies on (module.py:511-514)."""
+def subdivide_edges(faces, num_vertices):
+    """One midpoint subdivision's topology: the unique edges (v0 < v1, lexicographic order, pytorch3d's edges_packed
+    order) whose midpoints become vertices num_vertices, num_vertices + 1, ..., and the four faces of each triangle."""
     e = np.sort(np.stack([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]], 1).reshape(-1, 2), axis=1)
     uniq, inv = np.unique(e, axis=0, return_inverse=True)
-    mid = (len(verts) + inv.reshape(-1, 3)).astype(np.int64)  # new vertex of edge (a,b), (b,c), (c,a)
+    mid = (num_vertices + inv.reshape(-1, 3)).astype(np.int64)  # new vertex of edge (a,b), (b,c), (c,a)
     ab, bc, ca = mid[:, 0], mid[:, 1], mid[:, 2]
     a, b, c = faces[:, 0], faces[:, 1], faces[:, 2]
     nf = np.stack([np.stack([a, ab, ca], 1), np.stack([b, bc, ab], 1), np.stack([c, ca, bc], 1),
                    np.stack([ab, bc, ca], 1)], 1).reshape(-1, 3)
+    return uniq, nf
+
+
+def _subdivide(verts, faces):
+    """One midpoint subdivision (each triangle into four, no smoothing), the input vertices kept first -- the order
+    ExAvatar's `lr_idx_to_hr_idx` relies on (module.py:511-514)."""
+    uniq, nf = subdivide_edges(faces, len(verts))
     return np.concatenate([verts, 0.5 * (verts[uniq[:, 0]] + verts[uniq[:, 1]])]), nf
 
 
@@ -155,6 +162,7 @@ def make_human_mesh(seed=0, rings=97, segments=108):
         queries   (P,3)  verts + N(0, 1 mm) offsets (`mean_3d`)
         self_map  (P,)   head cap and both flanks, about 30 % (is_rhand | is_lhand | is_face)
         flip      (P,)   the cavity's vertices (is_cavity)
+        base_faces (F0,3) the faces of the base mesh (`smpl_x.face`)
     """
     th = np.pi * np.arange(1, rings + 1) / (rings + 1)
     ph = 2 * np.pi * np.arange(segments) / segments
@@ -193,7 +201,49 @@ def make_human_mesh(seed=0, rings=97, segments=108):
     queries = verts + 0.001 * g.standard_normal(verts.shape)
     f32 = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))  # noqa: E731
     return {"targets": f32(verts[:V]), "verts": f32(verts), "faces": torch.from_numpy(fs), "queries": f32(queries),
-            "self_map": torch.from_numpy(self_map), "flip": torch.from_numpy(flip)}
+            "self_map": torch.from_numpy(self_map), "flip": torch.from_numpy(flip),
+            "base_faces": torch.from_numpy(faces)}
+
+
+# SMPL-X's kinematic tree (55 joints: pelvis, 21 body, jaw, two eyes, 15 per hand), parents before children
+SMPLX_PARENTS = (-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 15, 15, 15, 20, 25, 26, 20,
+                 28, 29, 20, 31, 32, 20, 34, 35, 20, 37, 38, 21, 40, 41, 21, 43, 44, 21, 46, 47, 21, 49, 50, 21, 52, 53)
+
+
+def make_smplx_model(mesh, seed=0, num_betas=100, num_expr=50):
+    """A seeded SMPL-X-shaped body model on `make_human_mesh`'s base mesh, for `smplx_rig.SmplxRig`: the tensors
+    ExAvatar reads from `smplx_layer` and `smpl_x`, as float32 / int64 / bool CPU tensors.
+        v_template (V,3), face_offset (V,3) a few mm, shapedirs (V,3,NB) and expr_dirs (V,3,NE) dense, posedirs
+        (9 (J-1), 3V) dense, J_regressor (J,V) row-normalised over 8 vertices per joint, lbs_weights (V,J) four joints
+        per vertex, parents (J,) SMPLX_PARENTS, pose_mean (3J) non-zero on the hands, neutral_body_pose (21,3)
+        ExAvatar's 大 pose, faces (F0,3) the base faces, and the masks is_rhand / is_lhand / is_face_expr (P,) of
+        `make_regs_labels`."""
+    g = np.random.default_rng(5000 + seed)
+    v = mesh["targets"].numpy().astype(np.float64)
+    V, J = len(v), len(SMPLX_PARENTS)
+    f32 = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))  # noqa: E731
+    jreg = np.zeros((J, V))
+    for j in range(J):
+        cols = np.sort(g.choice(V, 8, replace=False))
+        w = g.uniform(0.5, 1.5, 8)
+        jreg[j, cols] = w / w.sum()
+    W = np.zeros((V, J))
+    for i in range(V):
+        cols = g.choice(J, 4, replace=False)
+        w = g.uniform(0.1, 1.0, 4)
+        W[i, cols] = w / w.sum()
+    pose_mean = np.zeros(3 * J)
+    pose_mean[25 * 3:] = 0.2 * g.standard_normal(30 * 3)  # the hands' mean pose (flat_hand_mean=False)
+    nbp = np.zeros((21, 3))
+    nbp[0], nbp[1] = [0, 0, 1], [0, 0, -1]
+    labels = make_regs_labels(mesh)
+    return {"v_template": f32(v), "face_offset": f32(0.003 * g.standard_normal((V, 3))),
+            "shapedirs": f32(0.01 * g.standard_normal((V, 3, num_betas))),
+            "expr_dirs": f32(0.002 * g.standard_normal((V, 3, num_expr))),
+            "posedirs": f32(0.002 * g.standard_normal((9 * (J - 1), 3 * V))),
+            "J_regressor": f32(jreg), "lbs_weights": f32(W), "parents": torch.tensor(SMPLX_PARENTS, dtype=torch.int64),
+            "pose_mean": f32(pose_mean), "neutral_body_pose": f32(nbp), "faces": mesh["base_faces"].clone(),
+            "is_rhand": labels["is_rhand"], "is_lhand": labels["is_lhand"], "is_face_expr": labels["is_face_expr"]}
 
 
 def make_regs_labels(mesh, hand_fraction=0.03, arm_half_width=0.05, arm_ny=(0.3, 0.7)):

@@ -479,11 +479,77 @@ int b2r_regs_forward(const B2RRegs* r, float* out, void* scratch, size_t scratch
 int b2r_regs_backward(const B2RRegs* r, const float* dL_dout, const B2RRegsGrads* grads, const void* scratch,
                       size_t scratch_bytes, void* stream);
 
+/* ExAvatar's SMPL-X rig (HumanGaussian.forward, avatar/common/nets/module.py:517-518, 533, 537, 549): the 大-pose and
+ * zero-pose body-model forwards with identity information, the inverse-neutral and the frame's forward kinematics, the
+ * pose-corrective and expression offsets, and two midpoint subdivisions -- one forward and one backward call.
+ * Sizes: V base vertices, V1 after one subdivision, P after two; J joints (22 + 3 <= n_body + 4 <= J <= 64, parents
+ * topological: parents[0] = -1, 0 <= parents[i] < i), NB shape and NE expression coefficients (<= 128 each); the pose
+ * feature has 9 (J-1) entries.  Per-call inputs (float, device): shape_param (NB), joint_offset (J,3) before the root
+ * is zeroed (its row 0 is ignored), full_pose (J,3) axis-angle in the model's joint order, expr (NE).  Tables (constants
+ * of the model, built once by the caller):
+ *   template      (V,3)  v_template + face_offset, rounded as one fp32 add;  shapedirs (V,3,NB), expr_dirs (V,3,NE)
+ *   posedirs_t    (V,3,9(J-1)) posedirs per vertex row;  pose_offset0 (V,3) the 大 pose's corrective offsets
+ *   lbs_weights   (V,J);  jreg_* J_regressor as a per-joint CSR (offsets J+1, cols, vals) and jregT_* its transpose
+ *                 per vertex (offsets V+1, rows ascending, vals)
+ *   rot_neutral / rot_zero / rot_inv  (J,9) double: the rotations of the 大-pose, zero-pose and inverse-neutral chains
+ *   sub1 (V1-V,2), sub2 (P-V1,2): each new vertex is the midpoint fl(fl(a + b) * 0.5f) of two of the level below
+ *   upT_*         the composed two-level subdivision transposed per base vertex (offsets V+1, rows ascending, weights)
+ *   mask          (P) uint8: rows of pose_offset kept (is_rhand | is_lhand | is_face_expr); the others are written 0.
+ * Forward outputs: mesh (P,3) mesh_neutral_pose, mesh_wo (V,3) before subdivision, joint_mats (J,4,4), pose_offset
+ * (P,3), expr_offset (P,3), pose_6d (6 n_body): the first two rows of each body joint's rotation.  `scratch` >=
+ * b2r_rig_scratch_bytes(V, J, NB, NE) is kept from the forward until the backward.  The backward reads the gradients of
+ * mesh, joint_mats and expr_offset (any may be NULL: zero) and writes every element of the four B2RRigGrads buffers;
+ * the root row of joint_offset's gradient is exactly 0.  Parents that are not topological are found on the device:
+ * no chain is walked and joint_mats, the meshes and the joint and pose gradients are NaN.  No float atomics (bit-identical runs), no allocation, no sync:
+ * both calls can be captured in a CUDA graph. */
+typedef struct B2RRig {
+  int32_t V, V1, P, J, NB, NE, n_body, reserved;
+  const float* shape_param;
+  const float* joint_offset;
+  const float* full_pose;
+  const float* expr;
+  const float* template_;
+  const float* shapedirs;
+  const float* expr_dirs;
+  const float* posedirs_t;
+  const float* pose_offset0;
+  const float* lbs_weights;
+  const int32_t* jreg_offsets;
+  const int32_t* jreg_cols;
+  const float* jreg_vals;
+  const int32_t* jregT_offsets;
+  const int32_t* jregT_rows;
+  const float* jregT_vals;
+  const int32_t* parents;
+  const double* rot_neutral;
+  const double* rot_zero;
+  const double* rot_inv;
+  const int32_t* sub1;
+  const int32_t* sub2;
+  const int32_t* upT_offsets;
+  const int32_t* upT_rows;
+  const float* upT_w;
+  const uint8_t* mask;
+} B2RRig;
+
+typedef struct B2RRigGrads {
+  float* shape_param;
+  float* joint_offset;
+  float* full_pose;
+  float* expr;
+} B2RRigGrads;
+
+size_t b2r_rig_scratch_bytes(int32_t V, int32_t J, int32_t NB, int32_t NE);
+int b2r_rig_forward(const B2RRig* r, float* mesh, float* mesh_wo, float* joint_mats, float* pose_offset,
+                    float* expr_offset, float* pose_6d, void* scratch, size_t scratch_bytes, void* stream);
+int b2r_rig_backward(const B2RRig* r, const float* dL_dmesh, const float* dL_djoint_mats, const float* dL_dexpr_offset,
+                     const B2RRigGrads* grads, void* scratch, size_t scratch_bytes, void* stream);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_* and b2r_regs_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_* and b2r_rig_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
