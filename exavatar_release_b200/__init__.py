@@ -7,7 +7,8 @@ renders of a training frame, avatar/main/model.py:117-162, as one autograd call)
 posed by one rig), `l1_ssim` (the L1 + SSIM terms of the loss block, model.py:196-215), `nearest_rows` and
 `VertexNormals` (the nearest-vertex rows and mesh normals in front of the posing, module.py:501-504,541-546),
 `FaceMeshRenderer` (the textured face render, model.py:170-175), `HumanRegularizers` (the regulariser block,
-model.py:217-257), `SmplxRig` (the SMPL-X rig of HumanGaussian.forward, module.py:517-518,533,537,549), synthetic
+model.py:217-257), `SmplxRig` (the SMPL-X rig of HumanGaussian.forward, module.py:517-518,533,537,549), `Adam` (ExAvatar's optimizer
+step in one launch, base.py:83-85), synthetic
 workloads and the frame-sharding helper used by bench.py.
 """
 from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians  # noqa: F401
@@ -18,6 +19,7 @@ from .geometry import VertexNormals, nearest_rows  # noqa: F401
 from .mesh_render import FaceMeshRenderer  # noqa: F401
 from .regularizers import HumanRegularizers  # noqa: F401
 from .smplx_rig import SmplxRig, cat_full_pose  # noqa: F401
+from .optim import Adam  # noqa: F401
 
 
 def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loaded on first use
@@ -29,4 +31,4 @@ def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loa
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "GaussianRenderer",
            "render_settings", "TrainingFrameRenderer", "skin_gaussians", "l1_ssim", "nearest_rows", "VertexNormals",
-           "FaceMeshRenderer", "HumanRegularizers", "SmplxRig", "cat_full_pose"]
+           "FaceMeshRenderer", "HumanRegularizers", "SmplxRig", "cat_full_pose", "Adam"]

@@ -119,6 +119,16 @@ class B2RRigGrads(C.Structure):
     _fields_ = [(n, _fp) for n in ("shape_param", "joint_offset", "full_pose", "expr")]
 
 
+class B2RAdamSegment(C.Structure):
+    """One tensor of an Adam step (b2r_adam_step): its four device pointers, numel, first chunk, the param's row layout
+    and the fp32 scalars."""
+    _fields_ = [
+        ("param", _fp), ("grad", _fp), ("exp_avg", _fp), ("exp_avg_sq", _fp), ("numel", C.c_int64),
+        ("first_chunk", C.c_int64), ("row_len", C.c_int64), ("row_stride", C.c_int64), ("lerp_weight", C.c_float), ("beta2", C.c_float), ("one_minus_beta2", C.c_float),
+        ("bc2_sqrt", C.c_float), ("eps", C.c_float), ("step_size", C.c_float),
+    ]
+
+
 class B2RForwardOutputs(C.Structure):
     _fields_ = [("color", _fp), ("depth", _fp), ("alpha", _fp), ("radii", _fp)]
 
@@ -205,6 +215,8 @@ SYMBOLS = [
     ("b2r_rig_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     ("b2r_rig_forward", C.c_int, [C.POINTER(B2RRig), _fp, _fp, _fp, _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
     ("b2r_rig_backward", C.c_int, [C.POINTER(B2RRig), _fp, _fp, _fp, C.POINTER(B2RRigGrads), _fp, C.c_size_t, _fp]),
+    ("b2r_adam_chunk_elems", C.c_int64, []),
+    ("b2r_adam_step", C.c_int, [_fp, C.c_int32, C.c_int64, _fp]),
     ("b2r_profile_enable", None, [C.c_int]),
     ("b2r_profile_read", C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int]),
     ("b2r_launch_count", C.c_uint64, []),
@@ -236,10 +248,10 @@ def load():
     if lib.b2r_abi_version() != ABI_VERSION:
         raise RuntimeError("b200raster: ABI version mismatch between the Python binding and libb200raster.so")
     # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8, B2RGnMlp 10 (9 unused too), B2RRegs 11,
-    # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14
+    # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14, B2RAdamSegment 15
     for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
                      (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp), (11, B2RRegs),
-                     (12, B2RRegsGrads), (13, B2RRig), (14, B2RRigGrads)):
+                     (12, B2RRegsGrads), (13, B2RRig), (14, B2RRigGrads), (15, B2RAdamSegment)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

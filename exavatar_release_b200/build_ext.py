@@ -41,9 +41,11 @@ NVCC_FLAGS = [
 # are the reference's expressions rounded operation by operation, so the selection (ties included) is the reference's.
 # smplx_rig.cu: the subdivision midpoints are fl(fl(a + b) * 0.5f) like pytorch3d's SubdivideMeshes, and the rig's
 # outputs feed every human render, so no product or sum is contracted.
+# adam.cu: the step is bit-identical to torch.optim.Adam's foreach kernels, which fuse exactly where their SASS has an
+# FFMA; the kernel writes those as __fmaf_rn and every other product and sum stays rounded on its own.
 PER_FILE_FLAGS = {"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
                   "geometry.cu": ["--fmad=false"], "mesh_raster.cu": ["--fmad=false"],
-                  "regularizers.cu": ["--fmad=false"], "smplx_rig.cu": ["--fmad=false"]}
+                  "regularizers.cu": ["--fmad=false"], "smplx_rig.cu": ["--fmad=false"], "adam.cu": ["--fmad=false"]}
 
 
 def sources():

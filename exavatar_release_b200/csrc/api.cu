@@ -168,6 +168,7 @@ size_t b2r_sizeof(int which) {
     case 12: return sizeof(B2RRegsGrads);
     case 13: return sizeof(B2RRig);
     case 14: return sizeof(B2RRigGrads);
+    case 15: return sizeof(B2RAdamSegment);
     default: return 0;
   }
 }
@@ -512,6 +513,16 @@ int b2r_rig_backward(const B2RRig* r, const float* dL_dmesh, const float* dL_djo
     return B2R_E_INVALID;
   if (scratch_bytes < rig_scratch_bytes(r->V, r->J, r->NB, r->NE)) return B2R_E_WORKSPACE;
   return launch_rig_backward(*r, dL_dmesh, dL_djoint_mats, dL_dexpr_offset, *grads, scratch, (cudaStream_t)stream);
+}
+
+int64_t b2r_adam_chunk_elems(void) { return B2R_ADAM_CHUNK; }
+
+int b2r_adam_step(const B2RAdamSegment* table, int32_t n_segments, int64_t n_chunks, void* stream) {
+  if (n_segments < 0 || n_chunks < 0 || n_chunks > 0x7fffffff) return B2R_E_INVALID;  // one CTA per chunk: grid.x
+  if (n_segments > 0 && !table) return B2R_E_INVALID;
+  if (n_chunks > 0 && n_segments == 0) return B2R_E_INVALID;
+  if (n_chunks == 0) return B2R_OK;
+  return launch_adam_step(table, n_segments, n_chunks, (cudaStream_t)stream);
 }
 
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {

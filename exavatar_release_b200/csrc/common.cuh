@@ -545,6 +545,7 @@ int launch_rig_forward(const B2RRig& r, float* mesh, float* mesh_wo, float* join
                        float* expr_offset, float* pose_6d, void* scratch, cudaStream_t st);
 int launch_rig_backward(const B2RRig& r, const float* dmesh, const float* djm, const float* dexpr, const B2RRigGrads& g,
                         void* scratch, cudaStream_t st);
+int launch_adam_step(const B2RAdamSegment* table, int n_segments, int64_t n_chunks, cudaStream_t st);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

@@ -9,7 +9,8 @@
 //
 // Scope: every rasteriser call -- adaptive capacity, fixed capacity (no polling, capturable in a CUDA graph) and
 // debug=True (synchronises after each call).  rasterizer.py only maps the public arguments onto `rasterize` and dumps
-// the inputs of a failed debug call.
+// the inputs of a failed debug call.  Also here: the host side of optim.Adam's step (`adam_step`), whose walk over
+// thousands of SMPL-X param groups per step costs milliseconds in Python.
 #include <torch/extension.h>
 
 #include <c10/cuda/CUDAGuard.h>
@@ -17,6 +18,8 @@
 #include <cuda_runtime.h>
 
 #include <chrono>
+#include <cmath>
+#include <cstring>
 #include <deque>
 #include <map>
 #include <memory>
@@ -24,6 +27,7 @@
 #include <stdexcept>
 #include <string>
 #include <tuple>
+#include <vector>
 
 #include "b200raster.h"
 
@@ -335,9 +339,133 @@ std::vector<at::Tensor> rasterize(const at::Tensor& means3D, const at::Tensor& m
                             view, proj, sh_degree, campos, speculative, headroom, fixed_capacity, debug);
 }
 
+// ---- optim.Adam's step: the walk over the param groups, the state, the scalars and the segment table ----------------
+
+// torch/optim/adam.py _multi_tensor_adam (capturable=False): the Python float expressions, in double (Python's `**` is
+// C pow), rounded to fp32 once by the foreach ops' scalar arguments.
+void adam_scalars(double lr, double beta1, double beta2, double eps, double step, B2RAdamSegment& s) {
+  const double bc1 = 1 - std::pow(beta1, step);
+  const double bc2 = 1 - std::pow(beta2, step);
+  s.lerp_weight = (float)(1 - beta1);
+  s.beta2 = (float)beta2;
+  s.one_minus_beta2 = (float)(1 - beta2);
+  s.bc2_sqrt = (float)std::pow(bc2, 0.5);
+  s.eps = (float)eps;
+  s.step_size = (float)((lr / bc1) * -1);
+}
+
+// The param as rows of row_len contiguous floats, row_stride apart: a contiguous tensor, or a view such as ExAvatar's
+// feature_dc = feature[:, 0:1, :] of a (P,16,3) tensor.  False for any other layout.
+bool row_layout(const at::Tensor& p, int64_t& row_len, int64_t& row_stride) {
+  const auto sz = p.sizes(), st = p.strides();
+  int i = (int)sz.size() - 1;
+  row_len = 1;
+  for (; i >= 0 && (sz[i] == 1 || st[i] == row_len); i--) row_len *= sz[i];
+  row_stride = row_len;
+  int64_t span = -1;
+  for (; i >= 0; i--) {
+    if (sz[i] == 1) continue;
+    if (span < 0) {
+      row_stride = st[i];
+    } else if (st[i] != span) {
+      return false;
+    }
+    span = st[i] * sz[i];
+  }
+  return row_stride >= row_len;
+}
+
+[[noreturn]] void value_error(const std::string& what) { throw py::value_error("Adam: " + what); }
+
+// One Adam step over every param with a gradient in `groups` (the optimizer's param_groups), with torch.optim.Adam's
+// lazy state in `state`: one pinned segment table, one async H2D copy, one launch on the current stream of `device`.
+void adam_step(const py::list& groups, const py::object& state, int64_t device, int64_t chunk) {
+  const at::Device dev(at::kCUDA, (c10::DeviceIndex)device);
+  std::vector<B2RAdamSegment> segs;
+  for (const py::handle gh : groups) {
+    const py::dict group = py::reinterpret_borrow<py::dict>(gh);
+    bool scalars = false;
+    double lr = 0, beta1 = 0, beta2 = 0, eps = 0;
+    for (const py::handle ph : py::reinterpret_borrow<py::list>(group["params"])) {
+      const at::Tensor p = ph.cast<at::Tensor>();
+      const at::Tensor& g = p.grad();
+      if (!g.defined()) continue;
+      if (g.is_sparse()) value_error("sparse gradients are not supported");
+      if (p.device() != dev || p.scalar_type() != at::kFloat)
+        value_error("parameters must be float32 tensors on the optimizer's CUDA device");
+      if (g.scalar_type() != at::kFloat || g.device() != dev || g.sizes() != p.sizes() || !g.is_contiguous())
+        value_error("a gradient must be a contiguous float32 tensor shaped and placed as its parameter");
+      if (!scalars) {
+        lr = group["lr"].cast<double>();
+        const py::tuple betas = group["betas"];
+        beta1 = betas[0].cast<double>();
+        beta2 = betas[1].cast<double>();
+        eps = group["eps"].cast<double>();
+        scalars = true;
+      }
+      py::object st = state[ph];  // a defaultdict: the first access creates the empty state
+      if (py::len(st) == 0) {     // torch.optim.Adam._init_group's lazy state (capturable=False, fused=False)
+        st["step"] = at::zeros({}, at::TensorOptions().dtype(at::kFloat));
+        st["exp_avg"] = at::zeros_like(p, at::MemoryFormat::Preserve);
+        st["exp_avg_sq"] = at::zeros_like(p, at::MemoryFormat::Preserve);
+      }
+      const at::Tensor step = st["step"].cast<at::Tensor>();
+      const at::Tensor m = st["exp_avg"].cast<at::Tensor>(), v = st["exp_avg_sq"].cast<at::Tensor>();
+      if (!step.device().is_cpu() || step.scalar_type() != at::kFloat || step.numel() != 1)
+        value_error("state 'step' must be a CPU float32 scalar tensor");
+      for (const at::Tensor* t : {&m, &v})
+        if (t->device() != dev || t->scalar_type() != at::kFloat || t->sizes() != p.sizes() || !t->is_contiguous())
+          value_error("exp_avg / exp_avg_sq must be contiguous float32 tensors shaped and placed as their parameter");
+      // as torch's _foreach_add_(steps, tensor(1.), alpha=1.): every step count of a param with a gradient advances
+      float* sp = step.data_ptr<float>();
+      *sp = *sp + 1.0f;
+      if (p.numel() == 0) continue;
+      B2RAdamSegment s{};
+      if (!row_layout(p, s.row_len, s.row_stride))
+        value_error("a parameter must be contiguous or rows of contiguous floats at one stride");
+      s.param = p.data_ptr<float>();
+      s.grad = g.data_ptr<float>();
+      s.exp_avg = m.data_ptr<float>();
+      s.exp_avg_sq = v.data_ptr<float>();
+      s.numel = p.numel();
+      adam_scalars(lr, beta1, beta2, eps, (double)*sp, s);
+      segs.push_back(s);
+    }
+  }
+  if (segs.empty()) return;
+  int64_t n_chunks = 0;
+  for (auto& s : segs) {
+    s.first_chunk = n_chunks;
+    n_chunks += (s.numel + chunk - 1) / chunk;
+  }
+  const int64_t bytes = (int64_t)(segs.size() * sizeof(B2RAdamSegment));
+  // the caching host allocator records the copy on the stream and keeps `host` from reuse until the copy has run
+  at::Tensor host = at::empty({bytes}, at::TensorOptions().dtype(at::kByte).pinned_memory(true));
+  std::memcpy(host.data_ptr(), segs.data(), (size_t)bytes);
+  c10::cuda::CUDAGuard guard(dev);
+  at::Tensor table = at::empty({bytes}, at::TensorOptions().dtype(at::kByte).device(dev));
+  table.copy_(host, /*non_blocking=*/true);
+  const cudaStream_t stream = c10::cuda::getCurrentCUDAStream(dev.index()).stream();
+  const int rc = b2r_adam_step((const B2RAdamSegment*)table.data_ptr(), (int32_t)segs.size(), n_chunks, stream);
+  if (rc != B2R_OK)
+    throw std::runtime_error(std::string("b200raster: b2r_adam_step failed: ") + b2r_strerror(rc) + " (cudaError " +
+                             std::to_string(b2r_last_cuda_error()) + ")");
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
+  m.def("adam_step", &adam_step, "optim.Adam.step: one launch over every param with a gradient (csrc/adam.cu)");
+  m.def("adam_scalars", [](double lr, double beta1, double beta2, double eps, double step) {
+    B2RAdamSegment s{};
+    adam_scalars(lr, beta1, beta2, eps, step, s);
+    return std::vector<float>{s.lerp_weight, s.beta2, s.one_minus_beta2, s.bc2_sqrt, s.eps, s.step_size};
+  }, "the fp32 scalars of one tensor's step: (lerp_weight, beta2, one_minus_beta2, bc2_sqrt, eps, step_size)");
+  m.def("adam_row_layout", [](const at::Tensor& p) {
+    int64_t row_len = 0, row_stride = 0;
+    const bool ok = row_layout(p, row_len, row_stride);
+    return std::make_tuple(ok, row_len, row_stride);
+  }, "(representable, row_len, row_stride) of a param for the Adam step");
   m.def("rasterize", &rasterize, "GaussianRasterizer forward with autograd (compiled host path over libb200raster.so); "
         "fixed_capacity < 0: adaptive duplicate capacity");
   m.def("abi_version", []() { return b2r_abi_version(); });

@@ -545,11 +545,39 @@ int b2r_rig_forward(const B2RRig* r, float* mesh, float* mesh_wo, float* joint_m
 int b2r_rig_backward(const B2RRig* r, const float* dL_dmesh, const float* dL_djoint_mats, const float* dL_dexpr_offset,
                      const B2RRigGrads* grads, void* scratch, size_t scratch_bytes, void* stream);
 
+/* One Adam step over many fp32 tensors in one launch: ExAvatar's torch.optim.Adam(params, lr, eps=1e-15)
+ * (avatar/common/base.py:83-85), element for element the arithmetic of torch's default foreach path (weight_decay 0,
+ * no amsgrad, no maximize).  `table` (device) holds one segment per tensor with a gradient; grad, exp_avg and
+ * exp_avg_sq are numel contiguous floats, and param is numel / row_len rows of row_len contiguous floats, row_stride
+ * floats apart (row_stride >= row_len; row_stride == row_len: contiguous).  The strided form is a view such as
+ * ExAvatar's feature_dc / feature_rest, slices of one (P,16,3) tensor.  param / exp_avg / exp_avg_sq are updated in
+ * place.  The segments split into chunks of b2r_adam_chunk_elems() elements: first_chunk is the sum of
+ * ceil(numel / chunk) over the segments before it, and n_chunks that sum over all of them (the launch has one CTA per
+ * chunk).  The scalars are torch's, evaluated in double on the host and rounded to fp32 once: lerp_weight 1-beta1,
+ * beta2, one_minus_beta2 1-beta2, bc2_sqrt (1-beta2^t)^0.5, eps, step_size (lr / (1-beta1^t)) * -1.  Tensors may start
+ * anywhere (float4 I/O when a segment is contiguous and all four pointers are 16-byte aligned).  No atomics, no
+ * allocation, no sync; n_chunks == 0 launches nothing. */
+typedef struct B2RAdamSegment {
+  float* param;
+  const float* grad;
+  float* exp_avg;
+  float* exp_avg_sq;
+  int64_t numel;
+  int64_t first_chunk;
+  int64_t row_len;
+  int64_t row_stride;
+  float lerp_weight, beta2, one_minus_beta2, bc2_sqrt, eps, step_size;
+} B2RAdamSegment;
+
+#define B2R_ADAM_CHUNK 16384
+int64_t b2r_adam_chunk_elems(void);
+int b2r_adam_step(const B2RAdamSegment* table, int32_t n_segments, int64_t n_chunks, void* stream);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_* and b2r_rig_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_* and b2r_adam_step kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
