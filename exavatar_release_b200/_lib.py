@@ -129,6 +129,16 @@ class B2RAdamSegment(C.Structure):
     ]
 
 
+class B2RLpips(C.Structure):
+    """ExAvatar's LPIPS-VGG terms (b2r_lpips_forward / b2r_lpips_backward): the images, the box and the weights in the
+    kernels' layouts."""
+    _fields_ = [
+        ("width", C.c_int32), ("height", C.c_int32), ("n_images", C.c_int32), ("reserved", C.c_int32),
+        ("img", _fp), ("target", _fp), ("bbox", _fp), ("w_fwd", _fp * 13), ("w_bwd", _fp * 13), ("bias", _fp * 13),
+        ("lin", _fp * 5),
+    ]
+
+
 class B2RForwardOutputs(C.Structure):
     _fields_ = [("color", _fp), ("depth", _fp), ("alpha", _fp), ("radii", _fp)]
 
@@ -217,6 +227,10 @@ SYMBOLS = [
     ("b2r_rig_backward", C.c_int, [C.POINTER(B2RRig), _fp, _fp, _fp, C.POINTER(B2RRigGrads), _fp, C.c_size_t, _fp]),
     ("b2r_adam_chunk_elems", C.c_int64, []),
     ("b2r_adam_step", C.c_int, [_fp, C.c_int32, C.c_int64, _fp]),
+    ("b2r_lpips_saved_bytes", C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    ("b2r_lpips_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32]),
+    ("b2r_lpips_forward", C.c_int, [C.POINTER(B2RLpips), _fp, _fp, C.c_size_t, _fp, C.c_size_t, _fp]),
+    ("b2r_lpips_backward", C.c_int, [C.POINTER(B2RLpips), _fp, C.c_size_t, _fp, _fp, _fp, C.c_size_t, _fp]),
     ("b2r_profile_enable", None, [C.c_int]),
     ("b2r_profile_read", C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int]),
     ("b2r_launch_count", C.c_uint64, []),
@@ -248,10 +262,11 @@ def load():
     if lib.b2r_abi_version() != ABI_VERSION:
         raise RuntimeError("b200raster: ABI version mismatch between the Python binding and libb200raster.so")
     # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8, B2RGnMlp 10 (9 unused too), B2RRegs 11,
-    # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14, B2RAdamSegment 15
+    # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14, B2RAdamSegment 15, B2RLpips 16
     for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
                      (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp), (11, B2RRegs),
-                     (12, B2RRegsGrads), (13, B2RRig), (14, B2RRigGrads), (15, B2RAdamSegment)):
+                     (12, B2RRegsGrads), (13, B2RRig), (14, B2RRigGrads), (15, B2RAdamSegment),
+                     (16, B2RLpips)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

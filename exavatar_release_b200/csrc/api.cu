@@ -71,6 +71,19 @@ bool valid_l1ssim_size(int32_t width, int32_t height) {
   return width > 0 && height > 0 && height <= 65535 * 16 && (int64_t)width * height <= (int64_t)1 << 31;
 }
 
+// sizes and the pointers both directions read: every weight a layer uses, the images; the box may be NULL.  The conv
+// grids put H / 8 tiles in grid.y, and NHWC offsets of 64 x W x H floats stay in size_t.
+int validate_lpips(const B2RLpips* p) {
+  if (!p || p->width < 16 || p->height < 16 || p->n_images < 1) return B2R_E_INVALID;
+  if (p->height > 65535 * 8 || (int64_t)p->width * p->height > (int64_t)1 << 28) return B2R_E_INVALID;
+  if (!p->img || !p->target || !p->w_fwd[0] || !p->bias[0]) return B2R_E_INVALID;
+  for (int l = 1; l < 13; l++)
+    if (!p->w_fwd[l] || !p->w_bwd[l] || !p->bias[l]) return B2R_E_INVALID;
+  for (int t = 0; t < 5; t++)
+    if (!p->lin[t]) return B2R_E_INVALID;
+  return B2R_OK;
+}
+
 // sizes and the pointers both directions read; the index tables' contents are the caller's (see b200raster.h)
 int validate_mesh_render(const B2RMeshRender* m) {
   if (!m) return B2R_E_INVALID;
@@ -169,6 +182,7 @@ size_t b2r_sizeof(int which) {
     case 13: return sizeof(B2RRig);
     case 14: return sizeof(B2RRigGrads);
     case 15: return sizeof(B2RAdamSegment);
+    case 16: return sizeof(B2RLpips);
     default: return 0;
   }
 }
@@ -523,6 +537,35 @@ int b2r_adam_step(const B2RAdamSegment* table, int32_t n_segments, int64_t n_chu
   if (n_chunks > 0 && n_segments == 0) return B2R_E_INVALID;
   if (n_chunks == 0) return B2R_OK;
   return launch_adam_step(table, n_segments, n_chunks, (cudaStream_t)stream);
+}
+
+size_t b2r_lpips_saved_bytes(int32_t width, int32_t height, int32_t n_images) {
+  return lpips_saved_bytes(width > 0 ? width : 1, height > 0 ? height : 1, n_images > 0 ? n_images : 1);
+}
+size_t b2r_lpips_scratch_bytes(int32_t width, int32_t height) {
+  return lpips_scratch_bytes(width > 0 ? width : 1, height > 0 ? height : 1);
+}
+
+int b2r_lpips_forward(const B2RLpips* p, float* out, void* saved, size_t saved_bytes, void* scratch,
+                      size_t scratch_bytes, void* stream) {
+  const int rc = validate_lpips(p);
+  if (rc) return rc;
+  if (!out || !saved || !scratch) return B2R_E_INVALID;
+  if (saved_bytes < lpips_saved_bytes(p->width, p->height, p->n_images) ||
+      scratch_bytes < lpips_scratch_bytes(p->width, p->height))
+    return B2R_E_WORKSPACE;
+  return launch_lpips_forward(*p, out, (float*)saved, scratch, (cudaStream_t)stream);
+}
+
+int b2r_lpips_backward(const B2RLpips* p, const void* saved, size_t saved_bytes, const float* dL_dout, float* dL_dimg,
+                       void* scratch, size_t scratch_bytes, void* stream) {
+  const int rc = validate_lpips(p);
+  if (rc) return rc;
+  if (!saved || !dL_dout || !dL_dimg || !scratch) return B2R_E_INVALID;
+  if (saved_bytes < lpips_saved_bytes(p->width, p->height, p->n_images) ||
+      scratch_bytes < lpips_scratch_bytes(p->width, p->height))
+    return B2R_E_WORKSPACE;
+  return launch_lpips_backward(*p, (const float*)saved, dL_dout, dL_dimg, scratch, (cudaStream_t)stream);
 }
 
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {

@@ -496,6 +496,40 @@ __device__ __forceinline__ void stage_rows(float* __restrict__ wstage, float* __
   }
 }
 
+// Crop box of ExAvatar's image losses (l1ssim.cu, lpips.cu), read on the device.
+struct Crop {
+  int x0, y0, x1, y1;  // [y0, y1) x [x0, x1), x1 >= x0, y1 >= y0
+  __device__ bool has(int x, int y) const { return x >= x0 && x < x1 && y >= y0 && y < y1; }
+  __device__ float count3() const { return 3.f * (float)(x1 - x0) * (float)(y1 - y0); }
+};
+
+// the reference's integer rules: int() truncates, the CLAMPED start is added to the width (a box with negative xmin
+// moves right instead of being clipped), the end is clamped to the image
+__device__ __forceinline__ int trunc_i(float v) { return __float2int_rz(fminf(fmaxf(v, -1e9f), 1e9f)); }
+__device__ __forceinline__ Crop read_crop(const float* bbox, int W, int H) {
+  Crop c{0, 0, W, H};
+  if (bbox) {
+    c.x0 = max(trunc_i(bbox[0]), 0);
+    c.y0 = max(trunc_i(bbox[1]), 0);
+    c.x1 = max(min(c.x0 + trunc_i(bbox[2]), W), c.x0);
+    c.y1 = max(min(c.y0 + trunc_i(bbox[3]), H), c.y0);
+  }
+  return c;
+}
+
+// TF32 tensor-core helpers (gn_mlp.cu, lpips.cu): round to TF32 with cvt.rna, d += a.b on one m16n8k8 tile
+__device__ __forceinline__ uint32_t to_tf32(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return r;
+}
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
 // launch wrappers (one per translation unit)
 int launch_project(const B2RScene& sc, const Ctx& cx, int32_t* radii, cudaStream_t st, int first_row = 0);
 int launch_binning(const B2RScene& sc, const Ctx& cx, bool rescan, cudaStream_t st);
@@ -546,6 +580,11 @@ int launch_rig_forward(const B2RRig& r, float* mesh, float* mesh_wo, float* join
 int launch_rig_backward(const B2RRig& r, const float* dmesh, const float* djm, const float* dexpr, const B2RRigGrads& g,
                         void* scratch, cudaStream_t st);
 int launch_adam_step(const B2RAdamSegment* table, int n_segments, int64_t n_chunks, cudaStream_t st);
+size_t lpips_saved_bytes(int W, int H, int N);
+size_t lpips_scratch_bytes(int W, int H);
+int launch_lpips_forward(const B2RLpips& p, float* out, float* saved, void* scratch, cudaStream_t st);
+int launch_lpips_backward(const B2RLpips& p, const float* saved, const float* dout, float* dimg, void* scratch,
+                          cudaStream_t st);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

@@ -35,26 +35,6 @@ struct L1SsimIn {
   const float* bbox;  // device {xmin, ymin, width, height} or null
 };
 
-struct Crop {
-  int x0, y0, x1, y1;  // [y0, y1) x [x0, x1), x1 >= x0, y1 >= y0
-  __device__ bool has(int x, int y) const { return x >= x0 && x < x1 && y >= y0 && y < y1; }
-  __device__ float count3() const { return 3.f * (float)(x1 - x0) * (float)(y1 - y0); }
-};
-
-// the reference's integer rules: int() truncates, the CLAMPED start is added to the width (a box with negative xmin
-// moves right instead of being clipped), the end is clamped to the image
-__device__ __forceinline__ int trunc_i(float v) { return __float2int_rz(fminf(fmaxf(v, -1e9f), 1e9f)); }
-__device__ __forceinline__ Crop read_crop(const float* bbox, int W, int H) {
-  Crop c{0, 0, W, H};
-  if (bbox) {
-    c.x0 = max(trunc_i(bbox[0]), 0);
-    c.y0 = max(trunc_i(bbox[1]), 0);
-    c.x1 = max(min(c.x0 + trunc_i(bbox[2]), W), c.x0);
-    c.y1 = max(min(c.y0 + trunc_i(bbox[3]), H), c.y0);
-  }
-  return c;
-}
-
 __host__ __device__ inline int ls_tiles_x(int W) { return (W + LS_T - 1) / LS_T; }
 __host__ __device__ inline int ls_tiles_y(int H) { return (H + LS_T - 1) / LS_T; }
 static size_t ls_map_bytes(int W, int H) { return align_up((size_t)9 * W * H * sizeof(float)); }

@@ -573,11 +573,44 @@ typedef struct B2RAdamSegment {
 int64_t b2r_adam_chunk_elems(void);
 int b2r_adam_step(const B2RAdamSegment* table, int32_t n_segments, int64_t n_chunks, void* stream);
 
+/* ExAvatar's LPIPS-VGG terms (avatar/common/nets/loss.py LPIPS over lpips.LPIPS(net='vgg'), version 0.1, eval mode) of
+ * n_images (3,H,W) images `img` against one (3,H,W) `target`.  `bbox` is a DEVICE float[4] {xmin, ymin, width, height}
+ * or NULL (the whole image), read on the device by b2r_l1ssim_forward's crop rules.  Per image: crop, x*2-1, lpips's
+ * ScalingLayer, VGG-16 features through relu5_3 (3x3 zero padding at the crop's border, 2x2 floor max pools), and the
+ * sum over the taps relu1_2, relu2_2, relu3_3, relu4_3, relu5_3 of mean_p sum_c lin[t]_c (n_c(img) - n_c(target))^2,
+ * n(f) = f / (|f| + 1e-10).  Convolutions run as TF32 (round to nearest) on the tensor cores with fp32 accumulation.
+ * Weights (fp32, device): w_fwd[0] is conv1_1's (64,3,3,3) torch tensor and w_bwd[0] is not read; for l >= 1 w_fwd[l]
+ * is (3,3,C_in,C_out) (torch's (C_out,C_in,3,3) permuted 2,3,1,0) and w_bwd[l] is (3,3,C_out,C_in) (flipped in both
+ * taps, permuted 2,3,0,1); bias[l] (C_out); lin[t] (C) of tap t.  Weight and activation pointers are 16-byte aligned.
+ * Forward writes out[n] (NaN when the crop is narrower or shorter than 16 px) and fills `saved`
+ * (>= b2r_lpips_saved_bytes(W, H, N): the 13 ReLU outputs per image and the target's normalised taps), which the
+ * backward reads.  Backward reads dL_dout[n] (device) and writes every element of dL_dimg (N,3,H,W): zero outside the
+ * crop, and zero everywhere for a crop under 16 px.  No gradient for the target or the weights.  `scratch` >=
+ * b2r_lpips_scratch_bytes(W, H) is free between the calls.  W, H >= 16.  Fixed-order reductions, no float atomics:
+ * bit-identical runs; every grid is sized from W x H, never from the box.  Neither call allocates or syncs. */
+typedef struct B2RLpips {
+  int32_t width, height, n_images, reserved;
+  const float* img;
+  const float* target;
+  const float* bbox;
+  const float* w_fwd[13];
+  const float* w_bwd[13];
+  const float* bias[13];
+  const float* lin[5];
+} B2RLpips;
+
+size_t b2r_lpips_saved_bytes(int32_t width, int32_t height, int32_t n_images);
+size_t b2r_lpips_scratch_bytes(int32_t width, int32_t height);
+int b2r_lpips_forward(const B2RLpips* p, float* out, void* saved, size_t saved_bytes, void* scratch,
+                      size_t scratch_bytes, void* stream);
+int b2r_lpips_backward(const B2RLpips* p, const void* saved, size_t saved_bytes, const float* dL_dout, float* dL_dimg,
+                       void* scratch, size_t scratch_bytes, void* stream);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_* and b2r_adam_step kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_adam_step and b2r_lpips_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */

@@ -106,7 +106,9 @@ def rig_ops(d, beta, jo, pose, expr):
     return mesh, mesh_wo.detach(), joint_mats, pose_offset, expr_offset, pose_6d
 
 
-def frames_per_second(a, dev):
+def frames_per_second(a, dev, extras=None):
+    """Arm 4.  `extras` (name -> fn(renders, target) -> loss term): instead of the two rig arms, one arm per entry, each
+    with the rig op and that term added to the frame's loss (tools/bench_lpips.py)."""
     from bench_human_nets import stack
     from bench_human_regs import INPUTS as REG_INPUTS
     from bench_human_regs import setup as regs_setup
@@ -172,11 +174,13 @@ def frames_per_second(a, dev):
             l1, ss = l1_ssim(o[r]["img"], target)
             loss = loss + 0.8 * l1 + 0.2 * (1 - ss)
         loss = loss + sum(regs(mesh.detach(), *[y[k] for k in REG_INPUTS]).values())
+        if extras is not None:
+            loss = loss + extras[which](o, target)
         loss.backward()
         for v in leaves:
             v.grad = None
 
-    arms = ("rig_ops", "rig_op")
+    arms = ("rig_ops", "rig_op") if extras is None else tuple(extras)
     for k in arms:
         for _ in range(3):
             frame(k)
