@@ -139,6 +139,22 @@ class B2RLpips(C.Structure):
     ]
 
 
+class B2RSceneAssets(C.Structure):
+    """ExAvatar's scene Gaussian assets (b2r_scene_assets_forward / b2r_scene_assets_backward): the parameters, their
+    row strides, the device degree buffer and the camera (NULL: shs mode)."""
+    _fields_ = [
+        ("P", C.c_int32), ("M", C.c_int32), ("dc_stride", C.c_int64), ("rest_stride", C.c_int64),
+        *[(n, _fp) for n in ("mean", "opacity_logit", "log_scale", "rotation6d", "feature_dc", "feature_rest",
+                             "active_sh_degree", "cam_R", "cam_t")],
+    ]
+
+
+class B2RSceneAssetsGrads(C.Structure):
+    _fields_ = [(n, _fp) for n in ("opacity", "scale", "dL_dopacity", "dL_dscale", "dL_drotation", "dL_dcolor",
+                                   "dL_dlogit", "dL_dlog_scale", "dL_drotation6d", "dL_dfeature_dc",
+                                   "dL_dfeature_rest", "dL_dmean")]
+
+
 class B2RForwardOutputs(C.Structure):
     _fields_ = [("color", _fp), ("depth", _fp), ("alpha", _fp), ("radii", _fp)]
 
@@ -231,6 +247,8 @@ SYMBOLS = [
     ("b2r_lpips_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32]),
     ("b2r_lpips_forward", C.c_int, [C.POINTER(B2RLpips), _fp, _fp, C.c_size_t, _fp, C.c_size_t, _fp]),
     ("b2r_lpips_backward", C.c_int, [C.POINTER(B2RLpips), _fp, C.c_size_t, _fp, _fp, _fp, C.c_size_t, _fp]),
+    ("b2r_scene_assets_forward", C.c_int, [C.POINTER(B2RSceneAssets), _fp, _fp, _fp, _fp, _fp]),
+    ("b2r_scene_assets_backward", C.c_int, [C.POINTER(B2RSceneAssets), C.POINTER(B2RSceneAssetsGrads), _fp]),
     ("b2r_profile_enable", None, [C.c_int]),
     ("b2r_profile_read", C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int]),
     ("b2r_launch_count", C.c_uint64, []),
@@ -262,11 +280,12 @@ def load():
     if lib.b2r_abi_version() != ABI_VERSION:
         raise RuntimeError("b200raster: ABI version mismatch between the Python binding and libb200raster.so")
     # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8, B2RGnMlp 10 (9 unused too), B2RRegs 11,
-    # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14, B2RAdamSegment 15, B2RLpips 16
+    # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14, B2RAdamSegment 15, B2RLpips 16, B2RSceneAssets 17,
+    # B2RSceneAssetsGrads 18
     for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
                      (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp), (11, B2RRegs),
                      (12, B2RRegsGrads), (13, B2RRig), (14, B2RRigGrads), (15, B2RAdamSegment),
-                     (16, B2RLpips)):
+                     (16, B2RLpips), (17, B2RSceneAssets), (18, B2RSceneAssetsGrads)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

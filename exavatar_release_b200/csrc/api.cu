@@ -71,6 +71,19 @@ bool valid_l1ssim_size(int32_t width, int32_t height) {
   return width > 0 && height > 0 && height <= 65535 * 16 && (int64_t)width * height <= (int64_t)1 << 31;
 }
 
+// sizes, strides and the pointers the mode reads (shs mode: no camera, mean or degree); the degree's value is checked
+// on the device
+int validate_scene_assets(const B2RSceneAssets* s) {
+  if (!s || s->P < 0 || s->M < 1 || s->M > B2R_SCENE_MAX_COEFFS) return B2R_E_INVALID;
+  if ((s->cam_R != nullptr) != (s->cam_t != nullptr)) return B2R_E_INVALID;
+  if (s->P == 0) return B2R_OK;
+  if (!s->opacity_logit || !s->log_scale || !s->rotation6d || !s->feature_dc) return B2R_E_INVALID;
+  if (s->dc_stride < 3) return B2R_E_INVALID;
+  if (s->M > 1 && (!s->feature_rest || s->rest_stride < 3 * (s->M - 1))) return B2R_E_INVALID;
+  if (s->cam_R && (!s->mean || !s->active_sh_degree)) return B2R_E_INVALID;
+  return B2R_OK;
+}
+
 // sizes and the pointers both directions read: every weight a layer uses, the images; the box may be NULL.  The conv
 // grids put H / 8 tiles in grid.y, and NHWC offsets of 64 x W x H floats stay in size_t.
 int validate_lpips(const B2RLpips* p) {
@@ -183,6 +196,8 @@ size_t b2r_sizeof(int which) {
     case 14: return sizeof(B2RRigGrads);
     case 15: return sizeof(B2RAdamSegment);
     case 16: return sizeof(B2RLpips);
+    case 17: return sizeof(B2RSceneAssets);
+    case 18: return sizeof(B2RSceneAssetsGrads);
     default: return 0;
   }
 }
@@ -566,6 +581,27 @@ int b2r_lpips_backward(const B2RLpips* p, const void* saved, size_t saved_bytes,
       scratch_bytes < lpips_scratch_bytes(p->width, p->height))
     return B2R_E_WORKSPACE;
   return launch_lpips_backward(*p, (const float*)saved, dL_dout, dL_dimg, scratch, (cudaStream_t)stream);
+}
+
+int b2r_scene_assets_forward(const B2RSceneAssets* s, float* opacity, float* scale, float* rotation, float* color,
+                             void* stream) {
+  const int rc = validate_scene_assets(s);
+  if (rc) return rc;
+  if (s->P > 0 && (!opacity || !scale || !rotation || !color)) return B2R_E_INVALID;
+  return launch_scene_assets_forward(*s, opacity, scale, rotation, color, (cudaStream_t)stream);
+}
+
+int b2r_scene_assets_backward(const B2RSceneAssets* s, const B2RSceneAssetsGrads* g, void* stream) {
+  const int rc = validate_scene_assets(s);
+  if (rc) return rc;
+  if (!g) return B2R_E_INVALID;
+  if (s->P > 0) {
+    if (!g->opacity || !g->scale || !g->dL_dlogit || !g->dL_dlog_scale || !g->dL_drotation6d || !g->dL_dfeature_dc)
+      return B2R_E_INVALID;
+    if (s->M > 1 && !g->dL_dfeature_rest) return B2R_E_INVALID;
+    if ((s->cam_R != nullptr) != (g->dL_dmean != nullptr)) return B2R_E_INVALID;  // d mean exactly in rgb mode
+  }
+  return launch_scene_assets_backward(*s, *g, (cudaStream_t)stream);
 }
 
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {

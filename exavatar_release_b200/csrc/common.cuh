@@ -585,6 +585,9 @@ size_t lpips_scratch_bytes(int W, int H);
 int launch_lpips_forward(const B2RLpips& p, float* out, float* saved, void* scratch, cudaStream_t st);
 int launch_lpips_backward(const B2RLpips& p, const float* saved, const float* dout, float* dimg, void* scratch,
                           cudaStream_t st);
+int launch_scene_assets_forward(const B2RSceneAssets& s, float* opacity, float* scale, float* rotation, float* color,
+                                cudaStream_t st);
+int launch_scene_assets_backward(const B2RSceneAssets& s, const B2RSceneAssetsGrads& g, cudaStream_t st);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

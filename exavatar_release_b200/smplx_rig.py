@@ -17,7 +17,8 @@ rounding only).
 `smplx_rig_reference` restates those reference lines in torch (float64 or float32, ExAvatar's own route by default:
 upsampled tables, Python FK loops, torch.inverse) for tests and measurements.
 
-pytorch3d's `axis_angle_to_matrix`, `matrix_to_axis_angle` and `matrix_to_rotation_6d` are restated here from
+pytorch3d's `axis_angle_to_matrix`, `matrix_to_axis_angle`, `matrix_to_rotation_6d` and `rotation_6d_to_matrix` (the
+scene Gaussians' rotations, scene_assets.py) are restated here from
 pytorch3d 0.7.5 (the quaternion route: axis_angle_to_quaternion with its small-angle branch |angle| < 1e-6, where
 sin(angle/2)/angle is replaced by 0.5 - angle^2/48, then quaternion_to_matrix; matrix_to_quaternion with the
 largest-denominator candidate and the 0.1 floor, then quaternion_to_axis_angle).  pytorch3d is not a dependency of
@@ -104,6 +105,16 @@ def matrix_to_axis_angle(m: torch.Tensor) -> torch.Tensor:
 
 def matrix_to_rotation_6d(m: torch.Tensor) -> torch.Tensor:
     return m[..., :2, :].clone().reshape(m.shape[:-2] + (6,))
+
+
+def rotation_6d_to_matrix(d6: torch.Tensor) -> torch.Tensor:
+    """Gram-Schmidt on the two 3-vectors of `d6`; the three orthonormal vectors are the matrix's ROWS."""
+    a1, a2 = d6[..., :3], d6[..., 3:]
+    b1 = torch.nn.functional.normalize(a1, dim=-1)
+    b2 = a2 - (b1 * a2).sum(-1, keepdim=True) * b1
+    b2 = torch.nn.functional.normalize(b2, dim=-1)
+    b3 = torch.cross(b1, b2, dim=-1)
+    return torch.stack((b1, b2, b3), dim=-2)
 
 
 def batch_rodrigues(rot_vecs: torch.Tensor) -> torch.Tensor:

@@ -606,11 +606,61 @@ int b2r_lpips_forward(const B2RLpips* p, float* out, void* saved, size_t saved_b
 int b2r_lpips_backward(const B2RLpips* p, const void* saved, size_t saved_bytes, const float* dL_dout, float* dL_dimg,
                        void* scratch, size_t scratch_bytes, void* stream);
 
+/* ExAvatar's scene Gaussian assets (avatar/common/nets/module.py:253-272, SceneGaussian.forward) from the stored
+ * parameters of P Gaussians with M SH coefficients (1 <= M <= B2R_SCENE_MAX_COEFFS): opacity = sigmoid(logit) (P,1),
+ * scale = exp(log_scale) (P,3), rotation = pytorch3d 0.7.5's matrix_to_quaternion(rotation_6d_to_matrix(rotation6d))
+ * (P,4), and one colour output:
+ *   shs mode (cam_R == NULL): shs (P,M,3) = cat(feature_dc, feature_rest, 1);
+ *   rgb mode (cam_R, cam_t set): rgb (P,3) = clamp_min(eval_sh(deg, sh, normalize(mean - campos)) + 0.5, 0) with
+ *   campos = -R^-1 t (R (3,3) row-major and t (3) on the device; the camera gets no gradient) and deg the DEVICE float
+ *   `active_sh_degree`, compared as ExAvatar's eval_sh compares it.  A degree outside 0..3, or one needing more than M
+ *   coefficients, writes NaN colours and NaN colour gradients; no coefficient beyond M is read.
+ * rotation6d, log_scale, opacity_logit and mean are contiguous rows; feature_dc's row p (3 floats) starts at
+ * feature_dc + p * dc_stride and feature_rest's (3 (M-1) contiguous floats) at feature_rest + p * rest_stride, so the
+ * (P,1,3) / (P,M-1,3) views of one (P,M,3) tensor are read in place.  feature_rest may be NULL when M == 1.
+ * Backward: g's upstream gradients may be NULL (zero); it writes d logit (P,1), d log_scale (P,3), d rotation6d (P,6),
+ * d feature_dc (P,1,3) and d feature_rest (P,M-1,3) contiguous (exact zeros above the degree in rgb mode) and, in rgb
+ * mode, the view-direction term of d mean (P,3).  Each output element is written once; no atomics, no allocation, no
+ * sync. */
+#define B2R_SCENE_MAX_COEFFS 16
+typedef struct B2RSceneAssets {
+  int32_t P, M;
+  int64_t dc_stride, rest_stride;
+  const float* mean;
+  const float* opacity_logit;
+  const float* log_scale;
+  const float* rotation6d;
+  const float* feature_dc;
+  const float* feature_rest;
+  const float* active_sh_degree;
+  const float* cam_R;
+  const float* cam_t;
+} B2RSceneAssets;
+
+typedef struct B2RSceneAssetsGrads {
+  const float* opacity;       /* the forward's opacity (P,1) */
+  const float* scale;         /* the forward's scale (P,3) */
+  const float* dL_dopacity;   /* (P,1) or NULL */
+  const float* dL_dscale;     /* (P,3) or NULL */
+  const float* dL_drotation;  /* (P,4) or NULL */
+  const float* dL_dcolor;     /* shs mode (P,M,3), rgb mode (P,3), or NULL */
+  float* dL_dlogit;
+  float* dL_dlog_scale;
+  float* dL_drotation6d;
+  float* dL_dfeature_dc;
+  float* dL_dfeature_rest;    /* NULL when M == 1 */
+  float* dL_dmean;            /* rgb mode only */
+} B2RSceneAssetsGrads;
+
+int b2r_scene_assets_forward(const B2RSceneAssets* s, float* opacity, float* scale, float* rotation, float* color,
+                             void* stream);
+int b2r_scene_assets_backward(const B2RSceneAssets* s, const B2RSceneAssetsGrads* g, void* stream);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_adam_step and b2r_lpips_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_adam_step, b2r_lpips_* and b2r_scene_assets_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */

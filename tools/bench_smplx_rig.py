@@ -106,9 +106,11 @@ def rig_ops(d, beta, jo, pose, expr):
     return mesh, mesh_wo.detach(), joint_mats, pose_offset, expr_offset, pose_6d
 
 
-def frames_per_second(a, dev, extras=None):
+def frames_per_second(a, dev, extras=None, scenes=None):
     """Arm 4.  `extras` (name -> fn(renders, target) -> loss term): instead of the two rig arms, one arm per entry, each
-    with the rig op and that term added to the frame's loss (tools/bench_lpips.py)."""
+    with the rig op and that term added to the frame's loss (tools/bench_lpips.py).  `scenes` (name -> fn(scene, cam)
+    -> scene asset dict, given the population's activated assets and the camera): one arm per entry, each with the rig
+    op and the scene's assets built by that function every frame (tools/bench_scene_assets.py)."""
     from bench_human_nets import stack
     from bench_human_regs import INPUTS as REG_INPUTS
     from bench_human_regs import setup as regs_setup
@@ -168,7 +170,7 @@ def frames_per_second(a, dev, extras=None):
              "rgb": (torch.tanh(rgb) + 1) / 2, "rgb_refined": (torch.tanh(rgb + rgb_off) + 1) / 2, "joint_offset": x[1]}
         hv = dict(human, mean_3d=posed, scale=y["scale"], rgb=y["rgb"])
         rv = dict(human, mean_3d=posed_r, scale=y["scale_refined"], rgb=y["rgb_refined"])
-        o = fr(lv, hv, rv, cam, bg)
+        o = fr(lv if scenes is None else scenes[which](scene, cam), hv, rv, cam, bg)
         loss = 0
         for r in RENDERS:
             l1, ss = l1_ssim(o[r]["img"], target)
@@ -180,7 +182,7 @@ def frames_per_second(a, dev, extras=None):
         for v in leaves:
             v.grad = None
 
-    arms = ("rig_ops", "rig_op") if extras is None else tuple(extras)
+    arms = tuple(scenes) if scenes is not None else ("rig_ops", "rig_op") if extras is None else tuple(extras)
     for k in arms:
         for _ in range(3):
             frame(k)
