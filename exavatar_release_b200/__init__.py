@@ -9,7 +9,9 @@ posed by one rig), `l1_ssim` (the L1 + SSIM terms of the loss block, model.py:19
 `FaceMeshRenderer` (the textured face render, model.py:170-175), `HumanRegularizers` (the regulariser block,
 model.py:217-257), `SmplxRig` (the SMPL-X rig of HumanGaussian.forward, module.py:517-518,533,537,549), `Adam` (ExAvatar's optimizer
 step in one launch, base.py:83-85), `LPIPS` (the LPIPS-VGG terms, model.py:199,206), `scene_assets` (the scene
-Gaussians' asset dict of SceneGaussian.forward, module.py:253-272), synthetic workloads and the frame-sharding helper used by bench.py.
+Gaussians' asset dict of SceneGaussian.forward, module.py:253-272), `decode_smplx_pose` (SMPLXParamDict.forward,
+module.py:673-684), `HumanAssets` (HumanGaussian's geometry and colour code around its networks, module.py:524-539,561-565
+and model.py:92-96), synthetic workloads and the frame-sharding helper used by bench.py.
 """
 from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians  # noqa: F401
 from .renderer import GaussianRenderer, render_settings  # noqa: F401
@@ -22,6 +24,7 @@ from .smplx_rig import SmplxRig, cat_full_pose  # noqa: F401
 from .optim import Adam  # noqa: F401
 from .scene_assets import scene_assets  # noqa: F401
 from .perceptual import LPIPS  # noqa: F401
+from .human_assets import HumanAssets, decode_smplx_pose  # noqa: F401
 
 
 def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loaded on first use
@@ -34,4 +37,4 @@ def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loa
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "GaussianRenderer",
            "render_settings", "TrainingFrameRenderer", "skin_gaussians", "l1_ssim", "nearest_rows", "VertexNormals",
            "FaceMeshRenderer", "HumanRegularizers", "SmplxRig", "cat_full_pose", "Adam",
-           "scene_assets", "LPIPS"]
+           "scene_assets", "LPIPS", "decode_smplx_pose", "HumanAssets"]

@@ -155,6 +155,29 @@ class B2RSceneAssetsGrads(C.Structure):
                                    "dL_dfeature_rest", "dL_dmean")]
 
 
+class B2RSmplxPose(C.Structure):
+    """One frame's seven 6D pose parameters (b2r_decode_pose_forward / b2r_decode_pose_backward): pointers and rows."""
+    _fields_ = [("param", _fp * 7), ("rows", C.c_int32 * 7), ("reserved", C.c_int32)]
+
+
+class B2RSmplxPoseGrads(C.Structure):
+    _fields_ = [("param", _fp * 7)]
+
+
+class B2RHumanAssets(C.Structure):
+    """HumanGaussian's geometry around its networks (b2r_human_geometry_forward / b2r_human_geometry_backward)."""
+    _fields_ = [
+        ("P", C.c_int32), ("warmup", C.c_int32), ("geo_stride", C.c_int64), ("geo_offset_stride", C.c_int64),
+        *[(n, _fp) for n in ("mesh", "pose_offset", "expr_offset", "geo", "geo_offset", "mask")],
+    ]
+
+
+class B2RHumanAssetsGrads(C.Structure):
+    _fields_ = [(n, _fp) for n in ("dL_dmean_3d", "dL_dmean_3d_refined", "dL_dscale", "dL_dscale_refined",
+                                   "dL_dmean_offset_offset", "dL_dscale_wo_clamp", "dL_dscale_refined_wo_clamp",
+                                   "dL_dmesh", "dL_dexpr_offset", "dL_dgeo", "dL_dgeo_offset")]
+
+
 class B2RForwardOutputs(C.Structure):
     _fields_ = [("color", _fp), ("depth", _fp), ("alpha", _fp), ("radii", _fp)]
 
@@ -249,6 +272,12 @@ SYMBOLS = [
     ("b2r_lpips_backward", C.c_int, [C.POINTER(B2RLpips), _fp, C.c_size_t, _fp, _fp, _fp, C.c_size_t, _fp]),
     ("b2r_scene_assets_forward", C.c_int, [C.POINTER(B2RSceneAssets), _fp, _fp, _fp, _fp, _fp]),
     ("b2r_scene_assets_backward", C.c_int, [C.POINTER(B2RSceneAssets), C.POINTER(B2RSceneAssetsGrads), _fp]),
+    ("b2r_decode_pose_forward", C.c_int, [C.POINTER(B2RSmplxPose), _fp, _fp]),
+    ("b2r_decode_pose_backward", C.c_int, [C.POINTER(B2RSmplxPose), _fp, C.POINTER(B2RSmplxPoseGrads), _fp]),
+    ("b2r_human_geometry_forward", C.c_int, [C.POINTER(B2RHumanAssets), _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
+    ("b2r_human_geometry_backward", C.c_int, [C.POINTER(B2RHumanAssets), C.POINTER(B2RHumanAssetsGrads), _fp]),
+    ("b2r_human_colors_forward", C.c_int, [C.c_int32, _fp, _fp, _fp, _fp, _fp]),
+    ("b2r_human_colors_backward", C.c_int, [C.c_int32, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     ("b2r_profile_enable", None, [C.c_int]),
     ("b2r_profile_read", C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int]),
     ("b2r_launch_count", C.c_uint64, []),
@@ -281,11 +310,12 @@ def load():
         raise RuntimeError("b200raster: ABI version mismatch between the Python binding and libb200raster.so")
     # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8, B2RGnMlp 10 (9 unused too), B2RRegs 11,
     # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14, B2RAdamSegment 15, B2RLpips 16, B2RSceneAssets 17,
-    # B2RSceneAssetsGrads 18
+    # B2RSceneAssetsGrads 18, B2RSmplxPose 19, B2RSmplxPoseGrads 20, B2RHumanAssets 21, B2RHumanAssetsGrads 22
     for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
                      (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp), (11, B2RRegs),
                      (12, B2RRegsGrads), (13, B2RRig), (14, B2RRigGrads), (15, B2RAdamSegment),
-                     (16, B2RLpips), (17, B2RSceneAssets), (18, B2RSceneAssetsGrads)):
+                     (16, B2RLpips), (17, B2RSceneAssets), (18, B2RSceneAssetsGrads), (19, B2RSmplxPose),
+                     (20, B2RSmplxPoseGrads), (21, B2RHumanAssets), (22, B2RHumanAssetsGrads)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

@@ -45,10 +45,12 @@ NVCC_FLAGS = [
 # FFMA; the kernel writes those as __fmaf_rn and every other product and sum stays rounded on its own.
 # scene_assets.cu: clamp_min's mask (x >= 0 with x = fl(fl(C0 sh) + 0.5) at degree 0) and the activations are torch's
 # fp32 expressions rounded operation by operation, so the mask agrees with torch's at equality.
+# human_assets.cu: every forward output is ExAvatar's fp32 torch expression rounded operation by operation (the mask
+# multiplies, exp / tanh as torch's kernels call them), bit-identical to it.
 PER_FILE_FLAGS = {"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
                   "geometry.cu": ["--fmad=false"], "mesh_raster.cu": ["--fmad=false"],
                   "regularizers.cu": ["--fmad=false"], "smplx_rig.cu": ["--fmad=false"], "adam.cu": ["--fmad=false"],
-                  "scene_assets.cu": ["--fmad=false"]}
+                  "scene_assets.cu": ["--fmad=false"], "human_assets.cu": ["--fmad=false"]}
 
 
 def sources():

@@ -84,6 +84,27 @@ int validate_scene_assets(const B2RSceneAssets* s) {
   return B2R_OK;
 }
 
+// row counts (1 <= J <= 64 joints, one thread each) and the parameters that have rows
+int validate_pose(const B2RSmplxPose* p) {
+  if (!p) return B2R_E_INVALID;
+  int J = 0;
+  for (int k = 0; k < B2R_POSE_PARAMS; ++k) {
+    if (p->rows[k] < 0 || p->rows[k] > B2R_POSE_MAX_JOINTS) return B2R_E_INVALID;
+    if (p->rows[k] > 0 && !p->param[k]) return B2R_E_INVALID;
+    J += p->rows[k];
+  }
+  return J >= 1 && J <= B2R_POSE_MAX_JOINTS ? B2R_OK : B2R_E_INVALID;
+}
+
+// sizes, row strides and every input pointer (an empty set reads nothing)
+int validate_human_assets(const B2RHumanAssets* h) {
+  if (!h || h->P < 0 || (h->warmup != 0 && h->warmup != 1)) return B2R_E_INVALID;
+  if (h->P == 0) return B2R_OK;
+  if (!h->mesh || !h->pose_offset || !h->expr_offset || !h->geo || !h->geo_offset || !h->mask) return B2R_E_INVALID;
+  if (h->geo_stride < 4 || h->geo_offset_stride < 4) return B2R_E_INVALID;
+  return B2R_OK;
+}
+
 // sizes and the pointers both directions read: every weight a layer uses, the images; the box may be NULL.  The conv
 // grids put H / 8 tiles in grid.y, and NHWC offsets of 64 x W x H floats stay in size_t.
 int validate_lpips(const B2RLpips* p) {
@@ -198,6 +219,10 @@ size_t b2r_sizeof(int which) {
     case 16: return sizeof(B2RLpips);
     case 17: return sizeof(B2RSceneAssets);
     case 18: return sizeof(B2RSceneAssetsGrads);
+    case 19: return sizeof(B2RSmplxPose);
+    case 20: return sizeof(B2RSmplxPoseGrads);
+    case 21: return sizeof(B2RHumanAssets);
+    case 22: return sizeof(B2RHumanAssetsGrads);
     default: return 0;
   }
 }
@@ -602,6 +627,57 @@ int b2r_scene_assets_backward(const B2RSceneAssets* s, const B2RSceneAssetsGrads
     if ((s->cam_R != nullptr) != (g->dL_dmean != nullptr)) return B2R_E_INVALID;  // d mean exactly in rgb mode
   }
   return launch_scene_assets_backward(*s, *g, (cudaStream_t)stream);
+}
+
+int b2r_decode_pose_forward(const B2RSmplxPose* p, float* full_pose, void* stream) {
+  const int rc = validate_pose(p);
+  if (rc) return rc;
+  if (!full_pose) return B2R_E_INVALID;
+  return launch_decode_pose_forward(*p, full_pose, (cudaStream_t)stream);
+}
+
+int b2r_decode_pose_backward(const B2RSmplxPose* p, const float* dL_dfull_pose, const B2RSmplxPoseGrads* grads,
+                             void* stream) {
+  const int rc = validate_pose(p);
+  if (rc) return rc;
+  if (!dL_dfull_pose || !grads) return B2R_E_INVALID;
+  for (int k = 0; k < B2R_POSE_PARAMS; ++k)
+    if (p->rows[k] > 0 && !grads->param[k]) return B2R_E_INVALID;
+  return launch_decode_pose_backward(*p, dL_dfull_pose, *grads, (cudaStream_t)stream);
+}
+
+int b2r_human_geometry_forward(const B2RHumanAssets* h, float* mean_3d, float* mean_3d_refined, float* scale,
+                               float* scale_refined, float* mean_offset_offset, float* scale_wo_clamp,
+                               float* scale_refined_wo_clamp, void* stream) {
+  const int rc = validate_human_assets(h);
+  if (rc) return rc;
+  if (h->P > 0) {
+    if (!mean_3d || !mean_3d_refined || !scale || !scale_refined || !mean_offset_offset) return B2R_E_INVALID;
+    if (h->warmup && (!scale_wo_clamp || !scale_refined_wo_clamp)) return B2R_E_INVALID;
+  }
+  return launch_human_geometry_forward(*h, mean_3d, mean_3d_refined, scale, scale_refined, mean_offset_offset,
+                                       scale_wo_clamp, scale_refined_wo_clamp, (cudaStream_t)stream);
+}
+
+int b2r_human_geometry_backward(const B2RHumanAssets* h, const B2RHumanAssetsGrads* g, void* stream) {
+  const int rc = validate_human_assets(h);
+  if (rc) return rc;
+  if (!g) return B2R_E_INVALID;
+  if (h->P > 0 && (!g->dL_dmesh || !g->dL_dexpr_offset || !g->dL_dgeo || !g->dL_dgeo_offset)) return B2R_E_INVALID;
+  return launch_human_geometry_backward(*h, *g, (cudaStream_t)stream);
+}
+
+int b2r_human_colors_forward(int32_t P, const float* rgb, const float* rgb_offset, float* rgb_out, float* rgb_refined,
+                             void* stream) {
+  if (P < 0 || (P > 0 && (!rgb || !rgb_offset || !rgb_out || !rgb_refined))) return B2R_E_INVALID;
+  return launch_human_colors_forward(P, rgb, rgb_offset, rgb_out, rgb_refined, (cudaStream_t)stream);
+}
+
+int b2r_human_colors_backward(int32_t P, const float* rgb, const float* rgb_offset, const float* dL_drgb_out,
+                              const float* dL_drgb_refined, float* dL_drgb, float* dL_drgb_offset, void* stream) {
+  if (P < 0 || (P > 0 && (!rgb || !rgb_offset || !dL_drgb || !dL_drgb_offset))) return B2R_E_INVALID;
+  return launch_human_colors_backward(P, rgb, rgb_offset, dL_drgb_out, dL_drgb_refined, dL_drgb, dL_drgb_offset,
+                                      (cudaStream_t)stream);
 }
 
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {

@@ -588,6 +588,14 @@ int launch_lpips_backward(const B2RLpips& p, const float* saved, const float* do
 int launch_scene_assets_forward(const B2RSceneAssets& s, float* opacity, float* scale, float* rotation, float* color,
                                 cudaStream_t st);
 int launch_scene_assets_backward(const B2RSceneAssets& s, const B2RSceneAssetsGrads& g, cudaStream_t st);
+int launch_decode_pose_forward(const B2RSmplxPose& p, float* full_pose, cudaStream_t st);
+int launch_decode_pose_backward(const B2RSmplxPose& p, const float* dfull, const B2RSmplxPoseGrads& g, cudaStream_t st);
+int launch_human_geometry_forward(const B2RHumanAssets& h, float* mean, float* mean_r, float* scale, float* scale_r,
+                                  float* mmo, float* scale_wo, float* scale_r_wo, cudaStream_t st);
+int launch_human_geometry_backward(const B2RHumanAssets& h, const B2RHumanAssetsGrads& g, cudaStream_t st);
+int launch_human_colors_forward(int P, const float* rgb, const float* off, float* out, float* out_r, cudaStream_t st);
+int launch_human_colors_backward(int P, const float* rgb, const float* off, const float* g, const float* g_r,
+                                 float* d_rgb, float* d_off, cudaStream_t st);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

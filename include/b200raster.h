@@ -203,7 +203,9 @@ const char* b2r_strerror(int code);
 int b2r_last_cuda_error(void);
 /* sizeof() of the ABI structs, for bindings to verify their mirror: 0 B2RScene, 1 B2RStatus, 2 B2RWorkspace,
  * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin, 8 B2RMeshRender, 10 B2RGnMlp, 11 B2RRegs,
- * 12 B2RRegsGrads; 0 for anything else
+ * 12 B2RRegsGrads, 13 B2RRig, 14 B2RRigGrads, 15 B2RAdamSegment, 16 B2RLpips, 17 B2RSceneAssets,
+ * 18 B2RSceneAssetsGrads, 19 B2RSmplxPose, 20 B2RSmplxPoseGrads, 21 B2RHumanAssets, 22 B2RHumanAssetsGrads; 0 for
+ * anything else
  * (7 and 9 are unused and report 0). */
 size_t b2r_sizeof(int which);
 
@@ -656,11 +658,86 @@ int b2r_scene_assets_forward(const B2RSceneAssets* s, float* opacity, float* sca
                              void* stream);
 int b2r_scene_assets_backward(const B2RSceneAssets* s, const B2RSceneAssetsGrads* g, void* stream);
 
+/* ExAvatar's SMPLXParamDict.forward (avatar/common/nets/module.py:673-684) for one frame: each of the seven 6D pose
+ * parameters (root, body, jaw, leye, reye, lhand, rhand) through pytorch3d 0.7.5's
+ * matrix_to_axis_angle(rotation_6d_to_matrix(x)) -- Gram-Schmidt with the 1e-12 floor, the first largest q_abs with
+ * the 0.1 floor, the sign standardisation, atan2 and the |angle| < 1e-6 branch -- evaluated in fp64 from the fp32
+ * rows and rounded once.  param[k] holds rows[k] contiguous 6-float rows; full_pose (J,3), J = sum rows[k] (1 <= J <=
+ * B2R_POSE_MAX_JOINTS), takes them in order (ExAvatar's cat_full_pose order).  Backward: autograd's derivative through
+ * the branches the forward took (zero through sqrt where its argument is <= 0, through the selected branch of each
+ * `where`, norm's zero at a zero vector; finite at the identity), written to grads->param[k] (rows[k] x 6,
+ * contiguous).  One CTA of one thread per joint each way; no atomics, no allocation, no sync. */
+#define B2R_POSE_PARAMS 7
+#define B2R_POSE_MAX_JOINTS 64
+typedef struct B2RSmplxPose {
+  const float* param[B2R_POSE_PARAMS];
+  int32_t rows[B2R_POSE_PARAMS];
+  int32_t reserved;
+} B2RSmplxPose;
+
+typedef struct B2RSmplxPoseGrads {
+  float* param[B2R_POSE_PARAMS];
+} B2RSmplxPoseGrads;
+
+int b2r_decode_pose_forward(const B2RSmplxPose* p, float* full_pose, void* stream);
+int b2r_decode_pose_backward(const B2RSmplxPose* p, const float* dL_dfull_pose, const B2RSmplxPoseGrads* grads,
+                             void* stream);
+
+/* HumanGaussian's geometry around its networks (avatar/common/nets/module.py:524-539 with get_mean_offset_offset's
+ * mask, :489-493, and model.py:92-96's warm-up clamp), per Gaussian p of P, in ExAvatar's fp32 operations and order:
+ *   m = mesh + geo[0:3];  mmo = geo_offset[0:3] * (1 - mask);  mean_3d = m + expr_offset;
+ *   mean_3d_refined = (m + (mmo + pose_offset)) + expr_offset;  scale = exp(geo[3]) x3;
+ *   scale_refined = exp(geo[3] + geo_offset[3]) x3;  mean_offset_offset = mmo.
+ * warmup != 0: scale_wo_clamp / scale_refined_wo_clamp receive the unclamped scales and scale / scale_refined
+ * torch.clamp(x, max=0.001) (NaN stays NaN; the gradient passes where x <= 0.001).  mesh, pose_offset, expr_offset are
+ * (P,3) contiguous; geo / geo_offset rows are 4 contiguous floats, geo_stride / geo_offset_stride floats apart (the
+ * column views of a wider head output are read in place); mask (P) holds 0 or 1.  Outputs (P,3) contiguous.
+ * Backward: upstream gradients may be NULL (zero); it writes d mesh, d expr_offset (P,3) and d geo, d geo_offset (P,4)
+ * contiguous; pose_offset gets none (ExAvatar detaches the pose there).  One thread per Gaussian, each output element
+ * written once: no atomics, no allocation, no sync. */
+typedef struct B2RHumanAssets {
+  int32_t P, warmup;
+  int64_t geo_stride, geo_offset_stride;
+  const float* mesh;
+  const float* pose_offset;
+  const float* expr_offset;
+  const float* geo;
+  const float* geo_offset;
+  const float* mask;
+} B2RHumanAssets;
+
+typedef struct B2RHumanAssetsGrads {
+  const float* dL_dmean_3d;               /* each (P,3) or NULL */
+  const float* dL_dmean_3d_refined;
+  const float* dL_dscale;
+  const float* dL_dscale_refined;
+  const float* dL_dmean_offset_offset;
+  const float* dL_dscale_wo_clamp;        /* warmup only */
+  const float* dL_dscale_refined_wo_clamp;
+  float* dL_dmesh;                        /* (P,3) */
+  float* dL_dexpr_offset;                 /* (P,3) */
+  float* dL_dgeo;                         /* (P,4) */
+  float* dL_dgeo_offset;                  /* (P,4) */
+} B2RHumanAssetsGrads;
+
+int b2r_human_geometry_forward(const B2RHumanAssets* h, float* mean_3d, float* mean_3d_refined, float* scale,
+                               float* scale_refined, float* mean_offset_offset, float* scale_wo_clamp,
+                               float* scale_refined_wo_clamp, void* stream);
+int b2r_human_geometry_backward(const B2RHumanAssets* h, const B2RHumanAssetsGrads* g, void* stream);
+
+/* HumanGaussian's colours (module.py:561): rgb_out = (tanh(rgb) + 1) / 2, rgb_refined = (tanh(rgb + rgb_offset) + 1) / 2,
+ * (P,3) contiguous fp32, in torch's operations.  Backward: dL_drgb_out / dL_drgb_refined may be NULL (zero); writes
+ * dL_drgb and dL_drgb_offset (P,3). */
+int b2r_human_colors_forward(int32_t P, const float* rgb, const float* rgb_offset, float* rgb_out, float* rgb_refined,
+                             void* stream);
+int b2r_human_colors_backward(int32_t P, const float* rgb, const float* rgb_offset, const float* dL_drgb_out,
+                              const float* dL_drgb_refined, float* dL_drgb, float* dL_drgb_offset, void* stream);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_adam_step, b2r_lpips_* and b2r_scene_assets_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_adam_step, b2r_lpips_*, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
