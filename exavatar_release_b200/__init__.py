@@ -7,7 +7,8 @@ renders of a training frame, avatar/main/model.py:117-162, as one autograd call)
 posed by one rig), `l1_ssim` (the L1 + SSIM terms of the loss block, model.py:196-215), `nearest_rows` and
 `VertexNormals` (the nearest-vertex rows and mesh normals in front of the posing, module.py:501-504,541-546),
 `FaceMeshRenderer` (the textured face render, model.py:170-175), `HumanRegularizers` (the regulariser block,
-model.py:217-257), `SmplxRig` (the SMPL-X rig of HumanGaussian.forward, module.py:517-518,533,537,549), `Adam` (ExAvatar's optimizer
+model.py:217-257), `SmplxRig` (the SMPL-X rig of HumanGaussian.forward, module.py:517-518,533,537,549, and with
+`.body_mesh` the frame's body mesh of get_smplx_outputs, model.py:37-58), `Adam` (ExAvatar's optimizer
 step in one launch, base.py:83-85), `LPIPS` (the LPIPS-VGG terms, model.py:199,206), `scene_assets` (the scene
 Gaussians' asset dict of SceneGaussian.forward, module.py:253-272), `decode_smplx_pose` (SMPLXParamDict.forward,
 module.py:673-684), `HumanAssets` (HumanGaussian's geometry and colour code around its networks, module.py:524-539,561-565

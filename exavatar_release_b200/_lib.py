@@ -119,6 +119,17 @@ class B2RRigGrads(C.Structure):
     _fields_ = [(n, _fp) for n in ("shape_param", "joint_offset", "full_pose", "expr")]
 
 
+class B2RSmplxBody(C.Structure):
+    """The frame's SMPL-X body mesh (b2r_smplx_body_forward / b2r_smplx_body_backward): the rig's tables, pose_mean,
+    the five per-call inputs and the optional camera."""
+    _fields_ = [("rig", B2RRig), *[(n, _fp) for n in ("pose_mean", "shape_param", "joint_offset", "full_pose", "expr",
+                                                      "trans", "cam_R", "cam_t")]]
+
+
+class B2RSmplxBodyGrads(C.Structure):
+    _fields_ = [(n, _fp) for n in ("shape_param", "joint_offset", "full_pose", "expr", "trans")]
+
+
 class B2RAdamSegment(C.Structure):
     """One tensor of an Adam step (b2r_adam_step): its four device pointers, numel, first chunk, the param's row layout
     and the fp32 scalars."""
@@ -264,6 +275,10 @@ SYMBOLS = [
     ("b2r_rig_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     ("b2r_rig_forward", C.c_int, [C.POINTER(B2RRig), _fp, _fp, _fp, _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
     ("b2r_rig_backward", C.c_int, [C.POINTER(B2RRig), _fp, _fp, _fp, C.POINTER(B2RRigGrads), _fp, C.c_size_t, _fp]),
+    ("b2r_smplx_body_scratch_bytes", C.c_size_t, [C.c_int32, C.c_int32]),
+    ("b2r_smplx_body_forward", C.c_int, [C.POINTER(B2RSmplxBody), _fp, _fp, C.c_size_t, _fp]),
+    ("b2r_smplx_body_backward", C.c_int, [C.POINTER(B2RSmplxBody), _fp, C.POINTER(B2RSmplxBodyGrads), _fp, C.c_size_t,
+                                          _fp]),
     ("b2r_adam_chunk_elems", C.c_int64, []),
     ("b2r_adam_step", C.c_int, [_fp, C.c_int32, C.c_int64, _fp]),
     ("b2r_lpips_saved_bytes", C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
@@ -310,12 +325,14 @@ def load():
         raise RuntimeError("b200raster: ABI version mismatch between the Python binding and libb200raster.so")
     # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8, B2RGnMlp 10 (9 unused too), B2RRegs 11,
     # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14, B2RAdamSegment 15, B2RLpips 16, B2RSceneAssets 17,
-    # B2RSceneAssetsGrads 18, B2RSmplxPose 19, B2RSmplxPoseGrads 20, B2RHumanAssets 21, B2RHumanAssetsGrads 22
+    # B2RSceneAssetsGrads 18, B2RSmplxPose 19, B2RSmplxPoseGrads 20, B2RHumanAssets 21, B2RHumanAssetsGrads 22,
+    # B2RSmplxBody 23, B2RSmplxBodyGrads 24
     for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
                      (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp), (11, B2RRegs),
                      (12, B2RRegsGrads), (13, B2RRig), (14, B2RRigGrads), (15, B2RAdamSegment),
                      (16, B2RLpips), (17, B2RSceneAssets), (18, B2RSceneAssetsGrads), (19, B2RSmplxPose),
-                     (20, B2RSmplxPoseGrads), (21, B2RHumanAssets), (22, B2RHumanAssetsGrads)):
+                     (20, B2RSmplxPoseGrads), (21, B2RHumanAssets), (22, B2RHumanAssetsGrads), (23, B2RSmplxBody),
+                     (24, B2RSmplxBodyGrads)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

@@ -181,6 +181,13 @@ int validate_rig(const B2RRig* r) {
   return B2R_OK;
 }
 
+// smplx_rig.cu's body mesh: the rig's checks on its tables with the body's inputs, the camera both or neither
+int validate_body(const B2RSmplxBody* b) {
+  if (!b || !b->pose_mean || !b->trans || (b->cam_R != nullptr) != (b->cam_t != nullptr)) return B2R_E_INVALID;
+  const B2RSmplxBody o = with_body_inputs(*b);
+  return validate_rig(&o.rig);
+}
+
 }  // namespace
 
 extern "C" {
@@ -223,6 +230,8 @@ size_t b2r_sizeof(int which) {
     case 20: return sizeof(B2RSmplxPoseGrads);
     case 21: return sizeof(B2RHumanAssets);
     case 22: return sizeof(B2RHumanAssetsGrads);
+    case 23: return sizeof(B2RSmplxBody);
+    case 24: return sizeof(B2RSmplxBodyGrads);
     default: return 0;
   }
 }
@@ -567,6 +576,30 @@ int b2r_rig_backward(const B2RRig* r, const float* dL_dmesh, const float* dL_djo
     return B2R_E_INVALID;
   if (scratch_bytes < rig_scratch_bytes(r->V, r->J, r->NB, r->NE)) return B2R_E_WORKSPACE;
   return launch_rig_backward(*r, dL_dmesh, dL_djoint_mats, dL_dexpr_offset, *grads, scratch, (cudaStream_t)stream);
+}
+
+size_t b2r_smplx_body_scratch_bytes(int32_t V, int32_t J) {
+  (void)J;  // the joint buffers are sized for 64 joints
+  return smplx_body_scratch_bytes(V);
+}
+
+int b2r_smplx_body_forward(const B2RSmplxBody* b, float* mesh, void* scratch, size_t scratch_bytes, void* stream) {
+  const int rc = validate_body(b);
+  if (rc) return rc;
+  if (!mesh || !scratch) return B2R_E_INVALID;
+  if (scratch_bytes < smplx_body_scratch_bytes(b->rig.V)) return B2R_E_WORKSPACE;
+  return launch_smplx_body_forward(*b, mesh, scratch, (cudaStream_t)stream);
+}
+
+int b2r_smplx_body_backward(const B2RSmplxBody* b, const float* dL_dmesh, const B2RSmplxBodyGrads* grads,
+                            void* scratch, size_t scratch_bytes, void* stream) {
+  const int rc = validate_body(b);
+  if (rc) return rc;
+  if (!grads || !grads->shape_param || !grads->joint_offset || !grads->full_pose || !grads->expr || !grads->trans ||
+      !scratch)
+    return B2R_E_INVALID;
+  if (scratch_bytes < smplx_body_scratch_bytes(b->rig.V)) return B2R_E_WORKSPACE;
+  return launch_smplx_body_backward(*b, dL_dmesh, *grads, scratch, (cudaStream_t)stream);
 }
 
 int64_t b2r_adam_chunk_elems(void) { return B2R_ADAM_CHUNK; }

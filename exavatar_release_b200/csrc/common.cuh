@@ -579,6 +579,19 @@ int launch_rig_forward(const B2RRig& r, float* mesh, float* mesh_wo, float* join
                        float* expr_offset, float* pose_6d, void* scratch, cudaStream_t st);
 int launch_rig_backward(const B2RRig& r, const float* dmesh, const float* djm, const float* dexpr, const B2RRigGrads& g,
                         void* scratch, cudaStream_t st);
+// the body with its B2RRig's four input pointers set to the body's (the rig's validation and shape pass read them)
+inline B2RSmplxBody with_body_inputs(const B2RSmplxBody& b) {
+  B2RSmplxBody o = b;
+  o.rig.shape_param = b.shape_param;
+  o.rig.joint_offset = b.joint_offset;
+  o.rig.full_pose = b.full_pose;
+  o.rig.expr = b.expr;
+  return o;
+}
+size_t smplx_body_scratch_bytes(int V);
+int launch_smplx_body_forward(const B2RSmplxBody& b, float* mesh, void* scratch, cudaStream_t st);
+int launch_smplx_body_backward(const B2RSmplxBody& b, const float* dmesh, const B2RSmplxBodyGrads& g, void* scratch,
+                               cudaStream_t st);
 int launch_adam_step(const B2RAdamSegment* table, int n_segments, int64_t n_chunks, cudaStream_t st);
 size_t lpips_saved_bytes(int W, int H, int N);
 size_t lpips_scratch_bytes(int W, int H);

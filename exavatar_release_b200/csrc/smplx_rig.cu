@@ -30,6 +30,9 @@
 //                         partials of shapedirs^T dv_shaped.
 //   rig_bwd_reduce_kernel ONE CTA: d shape_param from those partials in a fixed order.
 //
+// The second half of the file is the frame's SMPL-X body mesh of get_smplx_outputs (b2r_smplx_body_*) over the same
+// tables, reusing the shape pass, the chain steps and their adjoints.
+//
 // Compiled with --fmad=false (build_ext.py): each product and sum is rounded on its own, so the midpoints are
 // fl(fl(a + b) * 0.5f) as in pytorch3d's SubdivideMeshes, and the vertex sums have one order whatever the compiler does.
 #include <math.h>
@@ -254,6 +257,20 @@ struct RigBackSm {
   double dG[2][RIG_JMAX * 12], dtl[2][RIG_JMAX * 3], dj[2][RIG_JMAX * 3], dR[RIG_JMAX * 9], dAt[RIG_JMAX * 3];
 };
 
+// the depth of each joint in the tree and the deepest level; parents that are not topological set `bad`, every depth
+// to 0 and maxd to -1 (no level is walked)
+__device__ void chain_depths(const int* __restrict__ parents, int J, int* depth, int& maxd, int& bad) {
+  int m = 0, b = 0;
+  for (int i = 0; i < J; i++) {
+    const int p = parents[i];
+    b |= i == 0 ? p != -1 : (p < 0 || p >= i);
+    depth[i] = b ? 0 : (p < 0 ? 0 : depth[p] + 1);
+    m = max(m, depth[i]);
+  }
+  maxd = b ? -1 : m;
+  bad = b;
+}
+
 // joints, frame rotations, depths, then the four chains; leaves sm.G, sm.jnp, sm.jzp filled
 __device__ void rig_chains(const B2RRig& r, const float* __restrict__ vs, RigChainSm& sm, bool from_vs,
                            const double* __restrict__ jn_saved) {
@@ -273,17 +290,7 @@ __device__ void rig_chains(const B2RRig& r, const float* __restrict__ vs, RigCha
     const double a[3] = {(double)r.full_pose[3 * tid], (double)r.full_pose[3 * tid + 1], (double)r.full_pose[3 * tid + 2]};
     aa_to_matrix(a, sm.rf + 9 * tid);
   }
-  if (tid == 0) {
-    int m = 0, bad = 0;
-    for (int i = 0; i < J; i++) {
-      const int p = r.parents[i];
-      bad |= i == 0 ? p != -1 : (p < 0 || p >= i);
-      sm.depth[i] = bad ? 0 : (p < 0 ? 0 : sm.depth[p] + 1);
-      m = max(m, sm.depth[i]);
-    }
-    sm.maxd = bad ? -1 : m;
-    sm.bad = bad;
-  }
+  if (tid == 0) chain_depths(r.parents, J, sm.depth, sm.maxd, sm.bad);
   __syncthreads();
   const int grp = tid / RIG_JMAX, i = tid % RIG_JMAX;
   for (int d = 0; d <= sm.maxd; d++) {
@@ -672,6 +679,459 @@ int launch_rig_backward(const B2RRig& r, const float* dmesh, const float* djm, c
   {
     ProfScope p(K_MISC, st);
     launch_k(rig_bwd_reduce_kernel, 1, RIG_CMAX, 0, st, true, r, s, g.shape_param);
+  }
+  return check_launch();
+}
+
+// =====================================================================================================================
+// The frame's SMPL-X body mesh (get_smplx_outputs, avatar/main/model.py:37-58): smplx's SMPLX.forward + lbs with the
+// frame's shape, expression, raw joint_offset, full_pose + pose_mean and transl, then optionally R^-1 (mesh - t).
+//
+// Forward:
+//   rig_shape_kernel        (the rig's) vs = template + shapedirs . beta, ev = expr_dirs . expr; v_shaped = vs + ev.
+//   body_chain_kernel       ONE CTA, fp64: J = J_regressor . v_shaped + joint_offset (every row) over the per-joint
+//                           CSR; smplx's batch_rodrigues of full_pose + pose_mean; the pose feature (R - I of joints
+//                           1..J-1); FK level by level; the rel transforms A; R^-1 by cofactors when a camera is given.
+//   body_lbs_kernel         one warp per vertex: v_posed = v_shaped + feature . posedirs (kept for the backward),
+//                           mesh = (W A) (v_posed, 1) + trans, then R^-1 (mesh - t).
+// Backward:
+//   body_bwd_vertex_kernel  fixed grid, one warp per vertex: g = R^-T dmesh; dv_posed = (W A)_R^T g; fp64 per-CTA
+//                           partials of dA = W^T (g (v_posed, 1)^T), d feature = posedirs^T dv_posed and d trans.
+//   body_bwd_reduce_kernel  one warp per partial entry: the CTAs' partials in a fixed order.
+//   body_bwd_chain_kernel   ONE CTA: the chain recomputed from the saved joints, its adjoint in reverse level order,
+//                           d rotation + d feature through batch_rodrigues' derivative (with its 1e-8 shift), d joints.
+//   body_bwd_shape_kernel   fixed grid, one warp per vertex: dv_shaped = dv_posed + J_regressor^T dJ; fp64 per-CTA
+//                           partials of shapedirs^T and expr_dirs^T dv_shaped.
+//   body_bwd_coeff_kernel   ONE CTA: d shape_param and d expr from those partials in a fixed order.
+
+constexpr int BODY_THREADS = 128;  // backward vertex kernel: four warps, so their fp64 partials fit static shared memory
+constexpr int BODY_WARPS = BODY_THREADS / 32;
+constexpr int BODY_PART_BLOCKS = 256;  // fixed, like RIG_PART_BLOCKS: the partials' bits never depend on the device
+constexpr int BODY_PART_A = 12 * RIG_JMAX;  // dA (J,3,4)
+constexpr int BODY_PART_F = 9 * RIG_JMAX;   // d feature (9 (J-1)), padded to whole lanes
+constexpr int BODY_FEAT_PER_LANE = BODY_PART_F / 32;
+constexpr int BODY_PART_W = BODY_PART_A + BODY_PART_F + 4;  // + d trans (3), padded
+constexpr double BODY_RODRIGUES_SHIFT = 1e-8;               // lbs.batch_rodrigues: |r + 1e-8|
+
+struct BodyLayout {
+  size_t vs, ev, vp, dvs, feat, an, rinv, jn, djn, part_v, red, part_b, part_e, total;
+};
+
+inline BodyLayout body_layout(int V) {
+  const size_t v = V > 0 ? (size_t)V : 1;
+  BodyLayout L;
+  size_t o = 0;
+  L.vs = o; o += align_up(v * 3 * sizeof(float));
+  L.ev = o; o += align_up(v * 3 * sizeof(float));
+  L.vp = o; o += align_up(v * 3 * sizeof(float));
+  L.dvs = o; o += align_up(v * 3 * sizeof(float));
+  L.feat = o; o += align_up((size_t)9 * RIG_JMAX * sizeof(float));
+  L.an = o; o += align_up((size_t)12 * RIG_JMAX * sizeof(float));
+  L.rinv = o; o += align_up((size_t)9 * sizeof(float));
+  L.jn = o; o += align_up((size_t)3 * RIG_JMAX * sizeof(double));
+  L.djn = o; o += align_up((size_t)3 * RIG_JMAX * sizeof(double));
+  L.part_v = o; o += align_up((size_t)BODY_PART_BLOCKS * BODY_PART_W * sizeof(double));
+  L.red = o; o += align_up((size_t)BODY_PART_W * sizeof(double));
+  L.part_b = o; o += align_up((size_t)RIG_PART_BLOCKS * RIG_CMAX * sizeof(double));
+  L.part_e = o; o += align_up((size_t)RIG_PART_BLOCKS * RIG_CMAX * sizeof(double));
+  L.total = o;
+  return L;
+}
+
+struct BodyPtrs {
+  float *vs, *ev, *vp, *dvs, *feat, *an, *rinv;
+  double *jn, *djn, *part_v, *red, *part_b, *part_e;
+};
+
+inline BodyPtrs body_ptrs(const B2RSmplxBody& b, void* scratch) {
+  const BodyLayout L = body_layout(b.rig.V);
+  char* s = (char*)scratch;
+  BodyPtrs p;
+  p.vs = (float*)(s + L.vs);
+  p.ev = (float*)(s + L.ev);
+  p.vp = (float*)(s + L.vp);
+  p.dvs = (float*)(s + L.dvs);
+  p.feat = (float*)(s + L.feat);
+  p.an = (float*)(s + L.an);
+  p.rinv = (float*)(s + L.rinv);
+  p.jn = (double*)(s + L.jn);
+  p.djn = (double*)(s + L.djn);
+  p.part_v = (double*)(s + L.part_v);
+  p.red = (double*)(s + L.red);
+  p.part_b = (double*)(s + L.part_b);
+  p.part_e = (double*)(s + L.part_e);
+  return p;
+}
+
+// smplx lbs.batch_rodrigues in fp64: angle = |r + 1e-8| (the shift on each component), d = r / angle, K = [d]x,
+// R = I + sin(angle) K + (1 - cos(angle)) K K
+__device__ __forceinline__ void rodrigues_terms(const double r[3], double e[3], double& angle, double K[9],
+                                                double KK[9]) {
+  for (int c = 0; c < 3; c++) e[c] = r[c] + BODY_RODRIGUES_SHIFT;
+  angle = sqrt(e[0] * e[0] + e[1] * e[1] + e[2] * e[2]);
+  const double d0 = r[0] / angle, d1 = r[1] / angle, d2 = r[2] / angle;
+  K[0] = 0.0; K[1] = -d2; K[2] = d1;
+  K[3] = d2; K[4] = 0.0; K[5] = -d0;
+  K[6] = -d1; K[7] = d0; K[8] = 0.0;
+  for (int a = 0; a < 3; a++)
+    for (int b = 0; b < 3; b++) KK[3 * a + b] = K[3 * a] * K[b] + K[3 * a + 1] * K[3 + b] + K[3 * a + 2] * K[6 + b];
+}
+
+__device__ void rodrigues(const double r[3], double R[9]) {
+  double e[3], angle, K[9], KK[9];
+  rodrigues_terms(r, e, angle, K, KK);
+  const double s = sin(angle), c1 = 1.0 - cos(angle);
+  for (int t = 0; t < 9; t++) R[t] = ((t % 4) == 0 ? 1.0 : 0.0) + s * K[t] + c1 * KK[t];
+}
+
+// dr = (dR/dr)^T dR through the shift: angle > 0 unless r = -1e-8 (1, 1, 1) exactly; there the norm's gradient is 0
+__device__ void rodrigues_bwd(const double r[3], const double dR[9], double dr[3]) {
+  double e[3], angle, K[9], KK[9];
+  rodrigues_terms(r, e, angle, K, KK);
+  const double s = sin(angle), co = cos(angle), c1 = 1.0 - co;
+  double ds = 0.0, dc1 = 0.0, dK[9];
+  for (int t = 0; t < 9; t++) {
+    ds += dR[t] * K[t];
+    dc1 += dR[t] * KK[t];
+  }
+  for (int a = 0; a < 3; a++)  // d(K K) = dK K + K dK: dK += c1 (dR K^T + K^T dR)
+    for (int b = 0; b < 3; b++) {
+      double acc = 0.0;
+      for (int t = 0; t < 3; t++) acc += dR[3 * a + t] * K[3 * b + t] + K[3 * t + a] * dR[3 * t + b];
+      dK[3 * a + b] = s * dR[3 * a + b] + c1 * acc;
+    }
+  const double dd[3] = {dK[7] - dK[5], dK[2] - dK[6], dK[3] - dK[1]};
+  double dangle = ds * co + dc1 * s;
+  for (int c = 0; c < 3; c++) {
+    dr[c] = dd[c] / angle;
+    dangle -= dd[c] * r[c] / (angle * angle);
+  }
+  const double inv = angle > 0.0 ? dangle / angle : 0.0;
+  for (int c = 0; c < 3; c++) dr[c] += inv * e[c];
+}
+
+struct BodyChainSm {
+  double jn[RIG_JMAX * 3], rot[RIG_JMAX * 9], G[RIG_JMAX * 12];
+  int depth[RIG_JMAX];
+  int maxd;
+  int bad;
+};
+
+struct BodyBackSm {
+  BodyChainSm c;
+  double dG[RIG_JMAX * 12], dtl[RIG_JMAX * 3], dj[RIG_JMAX * 3], dR[RIG_JMAX * 9];
+};
+static_assert(sizeof(BodyBackSm) <= 48 * 1024, "the backward's single CTA fits static shared memory");
+
+// the joints (from v_shaped, or the forward's saved ones), the rotations of full_pose + pose_mean, the depths, then FK
+__device__ void body_chain(const B2RSmplxBody& b, const BodyPtrs& s, BodyChainSm& sm, bool from_vs) {
+  const B2RRig& r = b.rig;
+  const int tid = threadIdx.x, J = r.J;
+  if (tid < J) {
+    if (from_vs) {
+      double acc[3] = {0.0, 0.0, 0.0};
+      for (int q = r.jreg_offsets[tid]; q < r.jreg_offsets[tid + 1]; q++) {
+        const int v = r.jreg_cols[q];
+        const double w = (double)r.jreg_vals[q];
+        for (int c = 0; c < 3; c++) acc[c] += w * (double)(s.vs[3 * v + c] + s.ev[3 * v + c]);
+      }
+      for (int c = 0; c < 3; c++) sm.jn[3 * tid + c] = acc[c] + (double)b.joint_offset[3 * tid + c];
+    } else {
+      for (int c = 0; c < 3; c++) sm.jn[3 * tid + c] = s.jn[3 * tid + c];
+    }
+    double a[3];
+    for (int c = 0; c < 3; c++) a[c] = (double)b.full_pose[3 * tid + c] + (double)b.pose_mean[3 * tid + c];
+    rodrigues(a, sm.rot + 9 * tid);
+  }
+  if (tid == 0) chain_depths(r.parents, J, sm.depth, sm.maxd, sm.bad);
+  __syncthreads();
+  for (int d = 0; d <= sm.maxd; d++) {
+    if (tid < J && sm.depth[tid] == d) chain_step(tid, r.parents, sm.rot, sm.jn, sm.G);
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(RIG_JMAX) body_chain_kernel(const B2RSmplxBody b, const BodyPtrs s) {
+  __shared__ BodyChainSm sm;
+  body_chain(b, s, sm, true);
+  const int tid = threadIdx.x;
+  if (tid == 0 && b.cam_R) {  // R^-1 by cofactors (rasterizer._inv3's expressions), fp32
+    const float* R = b.cam_R;
+    const float a = R[0], bb = R[1], c = R[2], d = R[3], e = R[4], f = R[5], g = R[6], h = R[7], i = R[8];
+    const float adj[9] = {e * i - f * h, c * h - bb * i, bb * f - c * e, f * g - d * i, a * i - c * g,
+                          c * d - a * f, d * h - e * g, bb * g - a * h, a * e - bb * d};
+    const float det = a * (e * i - f * h) - bb * (d * i - f * g) + c * (d * h - e * g);
+    for (int t = 0; t < 9; t++) s.rinv[t] = adj[t] / det;
+  }
+  if (tid >= b.rig.J) return;
+  for (int c = 0; c < 3; c++) s.jn[3 * tid + c] = sm.jn[3 * tid + c];
+  double A[12];
+  chain_rel(tid, sm.jn, sm.G, A);
+  for (int t = 0; t < 12; t++) s.an[12 * tid + t] = sm.bad ? nanf("") : (float)A[t];
+  if (tid >= 1)
+    for (int t = 0; t < 9; t++) s.feat[9 * (tid - 1) + t] = (float)(sm.rot[9 * tid + t] - ((t % 4) == 0 ? 1.0 : 0.0));
+}
+
+__global__ void __launch_bounds__(RIG_THREADS) body_lbs_kernel(const B2RSmplxBody b, const BodyPtrs s,
+                                                               float* __restrict__ mesh) {
+  __shared__ float feat[9 * RIG_JMAX];
+  __shared__ float an[12 * RIG_JMAX];
+  const B2RRig& r = b.rig;
+  const int K = 9 * (r.J - 1);
+  for (int t = threadIdx.x; t < K; t += RIG_THREADS) feat[t] = s.feat[t];
+  for (int t = threadIdx.x; t < 12 * r.J; t += RIG_THREADS) an[t] = s.an[t];
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const int v = blockIdx.x * RIG_WARPS + (threadIdx.x >> 5);
+  if (v >= r.V) return;
+  float po[3];
+  for (int c = 0; c < 3; c++) {
+    const float* D = r.posedirs_t + ((size_t)v * 3 + c) * K;
+    float a = 0.f;
+    for (int k = lane; k < K; k += 32) a += feat[k] * D[k];
+    po[c] = rig_warp_sum(a);
+  }
+  float T[12];
+  for (int t = 0; t < 12; t++) T[t] = 0.f;
+  for (int j = lane; j < r.J; j += 32) {
+    const float w = r.lbs_weights[(size_t)v * r.J + j];
+    for (int t = 0; t < 12; t++) T[t] += w * an[12 * j + t];
+  }
+  for (int t = 0; t < 12; t++) T[t] = rig_warp_sum(T[t]);
+  if (lane == 0) {
+    float x[3], m[3];
+    for (int c = 0; c < 3; c++) {
+      x[c] = po[c] + (s.vs[3 * v + c] + s.ev[3 * v + c]);  // v_posed = pose_offsets + v_shaped
+      s.vp[3 * v + c] = x[c];
+    }
+    for (int c = 0; c < 3; c++) m[c] = (T[4 * c] * x[0] + T[4 * c + 1] * x[1] + T[4 * c + 2] * x[2] + T[4 * c + 3]) +
+                                       b.trans[c];
+    if (b.cam_R) {
+      float d[3];
+      for (int c = 0; c < 3; c++) d[c] = m[c] - b.cam_t[c];
+      for (int c = 0; c < 3; c++) m[c] = s.rinv[3 * c] * d[0] + s.rinv[3 * c + 1] * d[1] + s.rinv[3 * c + 2] * d[2];
+    }
+    for (int c = 0; c < 3; c++) mesh[3 * v + c] = m[c];
+  }
+}
+
+__global__ void __launch_bounds__(BODY_THREADS) body_bwd_vertex_kernel(const B2RSmplxBody b, const BodyPtrs s,
+                                                                       const float* __restrict__ dmesh) {
+  __shared__ float an[12 * RIG_JMAX];
+  __shared__ double wpart[BODY_WARPS][BODY_PART_W];
+  const B2RRig& r = b.rig;
+  for (int t = threadIdx.x; t < 12 * r.J; t += BODY_THREADS) an[t] = s.an[t];
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int K = 9 * (r.J - 1);
+  float ri[9];
+  for (int t = 0; t < 9; t++) ri[t] = b.cam_R ? s.rinv[t] : ((t % 4) == 0 ? 1.f : 0.f);
+  double aA[2][12], aF[BODY_FEAT_PER_LANE], aT[3] = {0.0, 0.0, 0.0};
+#pragma unroll
+  for (int k = 0; k < 2; k++)
+#pragma unroll
+    for (int t = 0; t < 12; t++) aA[k][t] = 0.0;
+#pragma unroll
+  for (int i = 0; i < BODY_FEAT_PER_LANE; i++) aF[i] = 0.0;
+  for (int v = blockIdx.x * BODY_WARPS + warp; v < r.V; v += BODY_PART_BLOCKS * BODY_WARPS) {
+    float go[3], g[3], x[3];
+    for (int c = 0; c < 3; c++) {
+      go[c] = dmesh ? dmesh[3 * v + c] : 0.f;
+      x[c] = s.vp[3 * v + c];
+    }
+    for (int c = 0; c < 3; c++) g[c] = b.cam_R ? ri[c] * go[0] + ri[3 + c] * go[1] + ri[6 + c] * go[2] : go[c];
+    if (lane == 0)
+      for (int c = 0; c < 3; c++) aT[c] += (double)g[c];
+    float T[9];
+    for (int t = 0; t < 9; t++) T[t] = 0.f;
+#pragma unroll
+    for (int k = 0; k < 2; k++) {
+      const int j = lane + 32 * k;
+      if (j >= r.J) continue;
+      const float w = r.lbs_weights[(size_t)v * r.J + j];
+#pragma unroll
+      for (int a = 0; a < 3; a++) {
+        const double wg = (double)w * (double)g[a];
+#pragma unroll
+        for (int c = 0; c < 3; c++) aA[k][4 * a + c] += wg * (double)x[c];
+        aA[k][4 * a + 3] += wg;
+      }
+      for (int a = 0; a < 3; a++)
+        for (int c = 0; c < 3; c++) T[3 * a + c] += w * an[12 * j + 4 * a + c];
+    }
+    for (int t = 0; t < 9; t++) T[t] = rig_warp_sum(T[t]);
+    float dvp[3];
+    for (int c = 0; c < 3; c++) dvp[c] = T[c] * g[0] + T[3 + c] * g[1] + T[6 + c] * g[2];
+    if (lane == 0)
+      for (int c = 0; c < 3; c++) s.dvs[3 * v + c] = dvp[c];
+    const float* D = r.posedirs_t + (size_t)v * 3 * K;
+#pragma unroll
+    for (int i = 0; i < BODY_FEAT_PER_LANE; i++) {
+      const int k = lane + 32 * i;
+      if (k < K)
+        aF[i] += ((double)D[k] * (double)dvp[0] + (double)D[K + k] * (double)dvp[1]) + (double)D[2 * K + k] * (double)dvp[2];
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 2; k++)
+#pragma unroll
+    for (int t = 0; t < 12; t++) wpart[warp][12 * (lane + 32 * k) + t] = aA[k][t];
+#pragma unroll
+  for (int i = 0; i < BODY_FEAT_PER_LANE; i++) wpart[warp][BODY_PART_A + lane + 32 * i] = aF[i];
+  if (lane == 0)
+    for (int c = 0; c < 4; c++) wpart[warp][BODY_PART_A + BODY_PART_F + c] = c < 3 ? aT[c] : 0.0;
+  __syncthreads();
+  for (int t = threadIdx.x; t < BODY_PART_W; t += BODY_THREADS) {
+    double a = 0.0;
+    for (int w = 0; w < BODY_WARPS; w++) a += wpart[w][t];
+    s.part_v[(size_t)blockIdx.x * BODY_PART_W + t] = a;
+  }
+}
+
+__global__ void __launch_bounds__(RIG_THREADS) body_bwd_reduce_kernel(const BodyPtrs s) {
+  const int t = blockIdx.x * RIG_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (t >= BODY_PART_W) return;
+  double a = 0.0;
+  for (int blk = lane; blk < BODY_PART_BLOCKS; blk += 32) a += s.part_v[(size_t)blk * BODY_PART_W + t];
+  for (int o = 16; o; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);  // a fixed butterfly: the same bits each run
+  if (lane == 0) s.red[t] = a;
+}
+
+__global__ void __launch_bounds__(RIG_JMAX) body_bwd_chain_kernel(const B2RSmplxBody b, const BodyPtrs s,
+                                                                  const B2RSmplxBodyGrads gr) {
+  __shared__ BodyBackSm sm;
+  const B2RRig& r = b.rig;
+  const int tid = threadIdx.x, J = r.J;
+  body_chain(b, s, sm.c, false);
+  if (tid < J) {
+    const double* dA = s.red + 12 * tid;
+    double dAR[9], dAt[3];
+    for (int a = 0; a < 3; a++) {
+      for (int c = 0; c < 3; c++) dAR[3 * a + c] = dA[4 * a + c];
+      dAt[a] = dA[4 * a + 3];
+    }
+    chain_own(tid, sm.c.jn, sm.c.G, dAR, dAt, nullptr, sm.dG, sm.dj);
+  }
+  if (tid < 3) gr.trans[tid] = (float)s.red[BODY_PART_A + BODY_PART_F + tid];
+  __syncthreads();
+  for (int d = sm.c.maxd; d >= 0; d--) {
+    if (tid < J && sm.c.depth[tid] == d)
+      chain_back_step(tid, J, r.parents, sm.c.rot, sm.c.jn, sm.c.G, sm.dG, sm.dtl, sm.dj, sm.dR);
+    __syncthreads();
+  }
+  if (tid >= J) return;
+  double dR[9], a[3], da[3];
+  for (int t = 0; t < 9; t++) dR[t] = sm.dR[9 * tid + t] + (tid >= 1 ? s.red[BODY_PART_A + 9 * (tid - 1) + t] : 0.0);
+  for (int c = 0; c < 3; c++) a[c] = (double)b.full_pose[3 * tid + c] + (double)b.pose_mean[3 * tid + c];
+  rodrigues_bwd(a, dR, da);
+  for (int c = 0; c < 3; c++) {
+    const double dj = sm.c.bad ? nan("") : sm.dj[3 * tid + c];
+    s.djn[3 * tid + c] = dj;
+    gr.joint_offset[3 * tid + c] = (float)dj;
+    gr.full_pose[3 * tid + c] = sm.c.bad ? nanf("") : (float)da[c];
+  }
+}
+
+__global__ void __launch_bounds__(RIG_THREADS) body_bwd_shape_kernel(const B2RSmplxBody b, const BodyPtrs s) {
+  __shared__ double djn[3 * RIG_JMAX];
+  __shared__ double wpart[RIG_WARPS][2 * RIG_CMAX];
+  const B2RRig& r = b.rig;
+  for (int t = threadIdx.x; t < 3 * r.J; t += RIG_THREADS) djn[t] = s.djn[t];
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double aB[4] = {0.0, 0.0, 0.0, 0.0}, aE[4] = {0.0, 0.0, 0.0, 0.0};
+  for (int v = blockIdx.x * RIG_WARPS + warp; v < r.V; v += RIG_PART_BLOCKS * RIG_WARPS) {
+    double d[3];
+    for (int c = 0; c < 3; c++) d[c] = (double)s.dvs[3 * v + c];
+    for (int q = r.jregT_offsets[v]; q < r.jregT_offsets[v + 1]; q++) {  // every lane, same order
+      const int k = r.jregT_rows[q];
+      const double w = (double)r.jregT_vals[q];
+      for (int c = 0; c < 3; c++) d[c] += w * djn[3 * k + c];
+    }
+    for (int k = 0; k < 4; k++) {
+      const int n = lane + 32 * k;
+      if (n < r.NB) {
+        double a = 0.0;
+        for (int c = 0; c < 3; c++) a += (double)r.shapedirs[((size_t)v * 3 + c) * r.NB + n] * d[c];
+        aB[k] += a;
+      }
+      if (n < r.NE) {
+        double a = 0.0;
+        for (int c = 0; c < 3; c++) a += (double)r.expr_dirs[((size_t)v * 3 + c) * r.NE + n] * d[c];
+        aE[k] += a;
+      }
+    }
+  }
+  for (int k = 0; k < 4; k++) {
+    wpart[warp][lane + 32 * k] = aB[k];
+    wpart[warp][RIG_CMAX + lane + 32 * k] = aE[k];
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < 2 * RIG_CMAX; t += RIG_THREADS) {
+    double a = 0.0;
+    for (int w = 0; w < RIG_WARPS; w++) a += wpart[w][t];
+    (t < RIG_CMAX ? s.part_b : s.part_e)[(size_t)blockIdx.x * RIG_CMAX + t % RIG_CMAX] = a;
+  }
+}
+
+__global__ void __launch_bounds__(2 * RIG_CMAX) body_bwd_coeff_kernel(const B2RSmplxBody b, const BodyPtrs s,
+                                                                      const B2RSmplxBodyGrads gr) {
+  const int t = threadIdx.x, n = t % RIG_CMAX;
+  const bool shape = t < RIG_CMAX;
+  if (n >= (shape ? b.rig.NB : b.rig.NE)) return;
+  const double* part = shape ? s.part_b : s.part_e;
+  double a = 0.0;
+  for (int blk = 0; blk < RIG_PART_BLOCKS; blk++) a += part[(size_t)blk * RIG_CMAX + n];
+  (shape ? gr.shape_param : gr.expr)[n] = (float)a;
+}
+
+size_t smplx_body_scratch_bytes(int V) { return body_layout(V).total; }
+
+int launch_smplx_body_forward(const B2RSmplxBody& body, float* mesh, void* scratch, cudaStream_t st) {
+  const B2RSmplxBody b = with_body_inputs(body);
+  const BodyPtrs s = body_ptrs(b, scratch);
+  RigPtrs shape = {};  // the rig's shape pass writes v_shaped's two parts into the body's scratch
+  shape.vs = s.vs;
+  shape.ev = s.ev;
+  const int vblocks = (b.rig.V + RIG_WARPS - 1) / RIG_WARPS;
+  {
+    ProfScope p(K_MISC, st);
+    launch_k(rig_shape_kernel, vblocks, RIG_THREADS, 0, st, true, b.rig, shape);
+  }
+  {
+    ProfScope p(K_MISC, st);
+    launch_k(body_chain_kernel, 1, RIG_JMAX, 0, st, true, b, s);
+  }
+  {
+    ProfScope p(K_MISC, st);
+    launch_k(body_lbs_kernel, vblocks, RIG_THREADS, 0, st, true, b, s, mesh);
+  }
+  return check_launch();
+}
+
+int launch_smplx_body_backward(const B2RSmplxBody& body, const float* dmesh, const B2RSmplxBodyGrads& g, void* scratch,
+                               cudaStream_t st) {
+  const B2RSmplxBody b = with_body_inputs(body);
+  const BodyPtrs s = body_ptrs(b, scratch);
+  {
+    ProfScope p(K_MISC, st);
+    launch_k(body_bwd_vertex_kernel, BODY_PART_BLOCKS, BODY_THREADS, 0, st, true, b, s, dmesh);
+  }
+  {
+    ProfScope p(K_MISC, st);
+    launch_k(body_bwd_reduce_kernel, (BODY_PART_W + RIG_WARPS - 1) / RIG_WARPS, RIG_THREADS, 0, st, true, s);
+  }
+  {
+    ProfScope p(K_MISC, st);
+    launch_k(body_bwd_chain_kernel, 1, RIG_JMAX, 0, st, true, b, s, g);
+  }
+  {
+    ProfScope p(K_MISC, st);
+    launch_k(body_bwd_shape_kernel, RIG_PART_BLOCKS, RIG_THREADS, 0, st, true, b, s);
+  }
+  {
+    ProfScope p(K_MISC, st);
+    launch_k(body_bwd_coeff_kernel, 1, 2 * RIG_CMAX, 0, st, true, b, s, g);
   }
   return check_launch();
 }

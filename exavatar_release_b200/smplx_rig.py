@@ -17,6 +17,12 @@ rounding only).
 `smplx_rig_reference` restates those reference lines in torch (float64 or float32, ExAvatar's own route by default:
 upsampled tables, Python FK loops, torch.inverse) for tests and measurements.
 
+`rig.body_mesh(...)` is the frame's SMPL-X body mesh of `Model.get_smplx_outputs` (avatar/main/model.py:37-58, and
+animate.py:81-82 without the camera) over the same tables, in one forward and one backward call; `smplx_body_reference`
+restates it in torch.
+
+    mesh = rig.body_mesh(shape_param, joint_offset, full_pose, expr, trans, cam_R, cam_t)   # (V,3)
+
 pytorch3d's `axis_angle_to_matrix`, `matrix_to_axis_angle`, `matrix_to_rotation_6d` and `rotation_6d_to_matrix` (the
 scene Gaussians' rotations, scene_assets.py) are restated here from
 pytorch3d 0.7.5 (the quaternion route: axis_angle_to_quaternion with its small-angle branch |angle| < 1e-6, where
@@ -248,6 +254,48 @@ class _Rig(torch.autograd.Function):
         return (None, *[g.reshape(s) for g, s in zip(grads, ctx.shapes)])
 
 
+class _Body(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, rig, shape_param, joint_offset, full_pose, expr, trans, cam_R, cam_t):
+        lib = L.load()
+        dev = rig.device
+        ins = [rig._input(t, n, name) for t, n, name in ((shape_param, rig.NB, "shape_param"),
+                                                          (joint_offset, 3 * rig.J, "joint_offset"),
+                                                          (full_pose, 3 * rig.J, "full_pose"),
+                                                          (expr, rig.NE, "expr"), (trans, 3, "trans"))]
+        if (cam_R is None) != (cam_t is None):
+            raise ValueError("SmplxRig.body_mesh: give both cam_R and cam_t, or neither")
+        cam = [] if cam_R is None else [rig._input(cam_R, 9, "cam_R"), rig._input(cam_t, 3, "cam_t")]
+        mesh = torch.empty((rig.V, 3), dtype=torch.float32, device=dev)
+        scratch = torch.empty(rig.body_scratch_bytes, dtype=torch.uint8, device=dev)
+        st = rig._body_struct(ins, cam)
+        with torch.cuda.device(dev):
+            L.check(lib.b2r_smplx_body_forward(C.byref(st), _ptr(mesh), _ptr(scratch), rig.body_scratch_bytes,
+                                               torch.cuda.current_stream(dev).cuda_stream), "b2r_smplx_body_forward")
+        ctx.rig = rig
+        ctx.n_cam = len(cam)
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(*ins, *cam, scratch)
+        ctx.shapes = (shape_param.shape, joint_offset.shape, full_pose.shape, expr.shape, trans.shape)
+        return mesh
+
+    @staticmethod
+    def backward(ctx, g_mesh):
+        *ins, scratch = ctx.saved_tensors
+        ins, cam = ins[:5], ins[5:]
+        rig = ctx.rig
+        dev = rig.device
+        lib = L.load()
+        grads = [torch.empty(n, dtype=torch.float32, device=dev) for n in (rig.NB, 3 * rig.J, 3 * rig.J, rig.NE, 3)]
+        gs = L.B2RSmplxBodyGrads(*[_ptr(g) for g in grads])
+        up = None if g_mesh is None else g_mesh.to(torch.float32).contiguous()
+        st = rig._body_struct(ins, cam)
+        with torch.cuda.device(dev):
+            L.check(lib.b2r_smplx_body_backward(C.byref(st), _ptr(up), C.byref(gs), _ptr(scratch), scratch.numel(),
+                                                torch.cuda.current_stream(dev).cuda_stream), "b2r_smplx_body_backward")
+        return (None, *[g.reshape(s) for g, s in zip(grads, ctx.shapes)], None, None)
+
+
 class SmplxRig:
     """ExAvatar's SMPL-X rig (module.py:517-518, 533, 537, 549) as one sync-free CUDA op.
 
@@ -265,6 +313,8 @@ class SmplxRig:
     axis-angle in the model's order (`cat_full_pose`) and expr (NE), float32 CUDA tensors, and returns `RigOutputs`.
     Divergence from the reference: the pose and expression offsets are contracted at V and then subdivided (ExAvatar
     subdivides the tables and contracts at P); the joints and the four chains run in fp64.
+
+    `body_mesh` is the frame's body mesh of get_smplx_outputs over the same tables (its own scratch per call).
     """
 
     def __init__(self, *, v_template, shapedirs, expr_dirs, posedirs, J_regressor, parents, lbs_weights, pose_mean,
@@ -309,7 +359,9 @@ class SmplxRig:
         self.upT_offsets, self.upT_rows, self.upT_w = (dev(offs, torch.int32), dev(row, torch.int32),
                                                        dev(w, torch.float32))
         self.mask = dev(m["mask"], torch.uint8)
+        self.pose_mean = dev(m["pose_mean"], torch.float32)  # body_mesh only
         self.scratch_bytes = int(L.load().b2r_rig_scratch_bytes(V, J, self.NB, self.NE))
+        self.body_scratch_bytes = int(L.load().b2r_smplx_body_scratch_bytes(V, J))
         self._template = L.B2RRig(
             V=V, V1=self.V1, P=self.P, J=J, NB=self.NB, NE=self.NE, n_body=self.n_body,
             **{k: _ptr(getattr(self, a)) for k, a in (
@@ -339,6 +391,28 @@ class SmplxRig:
     def reference(self, *args, **kw) -> RigOutputs:
         """smplx_rig_reference with this rig's model."""
         return smplx_rig_reference(self.model, *args, **kw)
+
+    def _body_struct(self, ins, cam) -> "L.B2RSmplxBody":
+        st = L.B2RSmplxBody(rig=self._template, pose_mean=_ptr(self.pose_mean))
+        st.shape_param, st.joint_offset, st.full_pose, st.expr, st.trans = (_ptr(t) for t in ins)
+        if cam:
+            st.cam_R, st.cam_t = (_ptr(t) for t in cam)
+        return st
+
+    def body_mesh(self, shape_param, joint_offset, full_pose, expr, trans, cam_R=None, cam_t=None) -> torch.Tensor:
+        """The frame's SMPL-X body mesh (V,3) float32: ExAvatar's get_smplx_outputs (model.py:37-58), i.e. smplx's
+        SMPLX.forward + lbs (body_models.py:1122-1300, lbs.py:155-250) with face_offset, the raw joint_offset and transl,
+        then R^-1 (mesh - t) in world coordinates.  Without a camera the mesh stays in camera coordinates (animate.py).
+
+        shape_param (NB), joint_offset (J,3) as given -- every row moves the joints, the root included (ExAvatar passes
+        human_gaussian.joint_offset without get_joint_offset here) --, full_pose (J,3) in `cat_full_pose` order
+        (`decode_smplx_pose(...)["full_pose"]` as is; the model's pose_mean is added), expr (NE), trans (3), and the
+        optional cam_R (3,3) / cam_t (3): float32 CUDA tensors on the rig's device.  Gradients flow to the five inputs;
+        the camera gets none.  The layer's landmarks, extra joints and `joints` output, which both callers discard, are
+        not computed.  Divergence from the reference: v_shaped is (template + shapedirs . beta) + expr_dirs . expr in
+        fp32 (smplx contracts the 150 coefficients in one einsum), the joints, rotations and chain run in fp64, and
+        R^-1 is taken by cofactors instead of torch.inverse, so nothing synchronises the host."""
+        return _Body.apply(self, shape_param, joint_offset, full_pose, expr, trans, cam_R, cam_t)
 
 
 def validate_model(*, v_template, shapedirs, expr_dirs, posedirs, J_regressor, parents, lbs_weights, pose_mean,
@@ -453,3 +527,30 @@ def smplx_rig_reference(model: dict, shape_param, joint_offset, full_pose, expr,
         raise ValueError(f"smplx_rig_reference: route must be 'upsample' or 'contract', got {route!r}")
     pose_6d = matrix_to_rotation_6d(Rf[1:1 + n_body]).reshape(-1).detach()
     return RigOutputs(mesh, mesh_wo.detach(), joint_mats, pose_offset, expr_offset, pose_6d)
+
+
+def smplx_body_reference(model: dict, shape_param, joint_offset, full_pose, expr, trans, cam_R=None, cam_t=None, *,
+                         dtype=torch.float64, device=None) -> torch.Tensor:
+    """get_smplx_outputs (avatar/main/model.py:37-58) restated in torch, differentiable in the five inputs: smplx's
+    SMPLX.forward + lbs for one frame with face_offset, the raw joint_offset and transl (body_models.py:1233 adds
+    pose_mean; lbs.py:155-250 with smplx's batch_rodrigues and batch_rigid_transform), then torch.inverse(R) (mesh - t)
+    when a camera is given.  `model` is validate_model's dict (SmplxRig.model); the tables are cast to `dtype`, so
+    dtype=torch.float32 is ExAvatar's own fp32 route.  The product never calls this."""
+    dev = torch.device(device) if device is not None else shape_param.device
+    cv = lambda t: t.to(device=dev, dtype=dtype)  # noqa: E731
+    V, J = model["V"], model["J"]
+    beta, jo, pose, e, tr = (cv(t).reshape(-1) for t in (shape_param, joint_offset, full_pose, expr, trans))
+    jo, pose = jo.view(J, 3), pose.view(J, 3)
+    tmpl = cv(model["v_template"]) + cv(model["face_offset"])
+    dirs = torch.cat([cv(model["shapedirs"]), cv(model["expr_dirs"])], dim=-1)
+    v_shaped = tmpl + torch.einsum("l,mkl->mk", torch.cat([beta, e]), dirs)
+    Jr = cv(model["J_regressor"]) @ v_shaped + jo
+    rot = batch_rodrigues(pose + cv(model["pose_mean"]).view(J, 3))
+    eye = torch.eye(3, dtype=dtype, device=dev)
+    v_posed = v_shaped + ((rot[1:] - eye).reshape(1, -1) @ cv(model["posedirs"])).view(V, 3)
+    _, A = rigid_transform(rot, Jr, model["parents"].tolist())
+    T = (cv(model["lbs_weights"]) @ A.reshape(J, 16)).view(V, 4, 4)
+    mesh = (T @ torch.cat([v_posed, torch.ones_like(v_posed[:, :1])], 1)[:, :, None])[:, :3, 0] + tr
+    if cam_R is not None:
+        mesh = torch.matmul(torch.inverse(cv(cam_R)), (mesh - cv(cam_t).view(1, 3)).permute(1, 0)).permute(1, 0)
+    return mesh

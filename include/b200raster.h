@@ -204,8 +204,8 @@ int b2r_last_cuda_error(void);
 /* sizeof() of the ABI structs, for bindings to verify their mirror: 0 B2RScene, 1 B2RStatus, 2 B2RWorkspace,
  * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin, 8 B2RMeshRender, 10 B2RGnMlp, 11 B2RRegs,
  * 12 B2RRegsGrads, 13 B2RRig, 14 B2RRigGrads, 15 B2RAdamSegment, 16 B2RLpips, 17 B2RSceneAssets,
- * 18 B2RSceneAssetsGrads, 19 B2RSmplxPose, 20 B2RSmplxPoseGrads, 21 B2RHumanAssets, 22 B2RHumanAssetsGrads; 0 for
- * anything else
+ * 18 B2RSceneAssetsGrads, 19 B2RSmplxPose, 20 B2RSmplxPoseGrads, 21 B2RHumanAssets, 22 B2RHumanAssetsGrads,
+ * 23 B2RSmplxBody, 24 B2RSmplxBodyGrads; 0 for anything else
  * (7 and 9 are unused and report 0). */
 size_t b2r_sizeof(int which);
 
@@ -547,6 +547,44 @@ int b2r_rig_forward(const B2RRig* r, float* mesh, float* mesh_wo, float* joint_m
 int b2r_rig_backward(const B2RRig* r, const float* dL_dmesh, const float* dL_djoint_mats, const float* dL_dexpr_offset,
                      const B2RRigGrads* grads, void* scratch, size_t scratch_bytes, void* stream);
 
+/* The frame's SMPL-X body mesh (ExAvatar's get_smplx_outputs, avatar/main/model.py:37-58: smplx's SMPLX.forward and
+ * lbs.lbs, then the world transform) for one frame, over the rig's tables.  `rig` is the model's B2RRig as
+ * b2r_rig_forward takes it (its four input pointers are not read; the body's are).  Per-call inputs (float, device):
+ * shape_param (NB), joint_offset (J,3) used as given, every row including the root, full_pose (J,3) axis-angle in the
+ * model's joint order, expr (NE), trans (3); pose_mean (J,3) is the model's.  With v_shaped = template + shapedirs .
+ * shape_param + expr_dirs . expr, J = J_regressor . v_shaped + joint_offset, rot = smplx batch_rodrigues(full_pose +
+ * pose_mean) (angle = |r + 1e-8|), v_posed = v_shaped + (rot[1:] - I) . posedirs, the forward writes mesh (V,3) =
+ * LBS(v_posed, batch_rigid_transform(rot, J)) + trans and, when cam_R (3,3) row-major and cam_t (3) are given (both or
+ * neither), R^-1 (mesh - t) with R^-1 by cofactors.  Landmarks and joints are not computed.  `scratch` >=
+ * b2r_smplx_body_scratch_bytes(V, J) is kept from the forward until the backward.  The backward reads dL_dmesh (NULL:
+ * zero) and writes every element of the five B2RSmplxBodyGrads buffers; the camera gets no gradient.  Parents that are
+ * not topological give NaN meshes and joint / pose gradients.  No float atomics (bit-identical runs), no allocation, no
+ * sync: both calls can be captured in a CUDA graph. */
+typedef struct B2RSmplxBody {
+  B2RRig rig;
+  const float* pose_mean;
+  const float* shape_param;
+  const float* joint_offset;
+  const float* full_pose;
+  const float* expr;
+  const float* trans;
+  const float* cam_R;
+  const float* cam_t;
+} B2RSmplxBody;
+
+typedef struct B2RSmplxBodyGrads {
+  float* shape_param;
+  float* joint_offset;
+  float* full_pose;
+  float* expr;
+  float* trans;
+} B2RSmplxBodyGrads;
+
+size_t b2r_smplx_body_scratch_bytes(int32_t V, int32_t J);
+int b2r_smplx_body_forward(const B2RSmplxBody* b, float* mesh, void* scratch, size_t scratch_bytes, void* stream);
+int b2r_smplx_body_backward(const B2RSmplxBody* b, const float* dL_dmesh, const B2RSmplxBodyGrads* grads,
+                            void* scratch, size_t scratch_bytes, void* stream);
+
 /* One Adam step over many fp32 tensors in one launch: ExAvatar's torch.optim.Adam(params, lr, eps=1e-15)
  * (avatar/common/base.py:83-85), element for element the arithmetic of torch's default foreach path (weight_decay 0,
  * no amsgrad, no maximize).  `table` (device) holds one segment per tensor with a gradient; grad, exp_avg and
@@ -737,7 +775,7 @@ int b2r_human_colors_backward(int32_t P, const float* rgb, const float* rgb_offs
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_adam_step, b2r_lpips_*, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */

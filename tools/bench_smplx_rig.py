@@ -106,13 +106,16 @@ def rig_ops(d, beta, jo, pose, expr):
     return mesh, mesh_wo.detach(), joint_mats, pose_offset, expr_offset, pose_6d
 
 
-def frames_per_second(a, dev, extras=None, scenes=None, poses=None):
+def frames_per_second(a, dev, extras=None, scenes=None, poses=None, meshes=None):
     """Arm 4.  `extras` (name -> fn(renders, target) -> loss term): instead of the two rig arms, one arm per entry, each
     with the rig op and that term added to the frame's loss (tools/bench_lpips.py).  `scenes` (name -> fn(scene, cam)
     -> scene asset dict, given the population's activated assets and the camera): one arm per entry, each with the rig
     op and the scene's assets built by that function every frame (tools/bench_scene_assets.py).  `poses` (name -> fn()
     -> (J,3) axis-angle pose): one arm per entry, each with the rig op fed the pose that function decodes every frame
-    from the frame's 6D parameters (tools/bench_human_assets.py)."""
+    from the frame's 6D parameters (tools/bench_human_assets.py).  `meshes` (name -> fn(rig, shape_param, joint_offset,
+    full_pose, expr, trans, cam_R, cam_t) -> (V,3) mesh or None): one arm per entry, each with the rig op and the
+    frame's SMPL-X body mesh of get_smplx_outputs computed by that function every frame, its result unused as in
+    ExAvatar's training step (tools/bench_smplx_body.py)."""
     from bench_human_nets import stack
     from bench_human_regs import INPUTS as REG_INPUTS
     from bench_human_regs import setup as regs_setup
@@ -159,6 +162,8 @@ def frames_per_second(a, dev, extras=None, scenes=None, poses=None):
             out = rig(x[0], x[1], poses[which](), x[3])
         else:
             out = rig_ops(d, *x) if which == "rig_ops" else rig(*x)
+        if meshes is not None:
+            meshes[which](rig, *x, trans, R, tc)
         mesh, mesh_wo, joint_mats, pose_offset, expr_offset, pose = out
         f = tri(tp, tpf)
         net = lambda k, ins: gn_mlp(ins, *nets[k])  # noqa: E731
@@ -188,7 +193,7 @@ def frames_per_second(a, dev, extras=None, scenes=None, poses=None):
             v.grad = None
 
     arms = (tuple(scenes) if scenes is not None else tuple(poses) if poses is not None else
-            ("rig_ops", "rig_op") if extras is None else tuple(extras))
+            tuple(meshes) if meshes is not None else ("rig_ops", "rig_op") if extras is None else tuple(extras))
     for k in arms:
         for _ in range(3):
             frame(k)
