@@ -17,10 +17,7 @@ plus the wait for the sync at its end; the gradient assignment between steps is 
 algorithmic bytes (28 B per element: p, g, m, v read, p, m, v written), achieved bandwidth and share of 3.35 TB/s (the
 H100 SXM data sheet's HBM3 figure).  Prints the card name and power limit with the numbers.
 """
-import argparse
-import json
 import os
-import statistics
 import sys
 import time
 
@@ -31,10 +28,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_frame_sh import card  # noqa: E402
+from benchkit import HBM_BYTES_PER_S, arg_parser, card, cuda_device, emit, stats  # noqa: E402
 from exavatar_release_b200.optim import Adam  # noqa: E402
 
-HBM_TBPS = 3.35
 FRAME_PARAMS = {"root_pose": (6,), "body_pose": (21, 6), "jaw_pose": (6,), "leye_pose": (6,), "reye_pose": (6,),
                 "lhand_pose": (15, 6), "rhand_pose": (15, 6), "expr": (50,), "trans": (3,)}
 
@@ -152,28 +148,20 @@ def run(n_frames, a, dev):
             nbytes = 28 * elems
             prof[k].update(elements=elems, algorithmic_bytes=nbytes, kernel_ms=kms,
                            achieved_TBps=nbytes / (kms * 1e-3) / 1e12 if kms else None,
-                           share_of_hbm=nbytes / (kms * 1e-3) / (HBM_TBPS * 1e12) if kms else None)
-    med = lambda v: {"median": statistics.median(v), "min": min(v), "max": max(v)}  # noqa: E731
-    return {"groups": len(spec), "host_step_ms": {k: med(v) for k, v in host.items()},
-            "step_to_sync_ms": {k: med(v) for k, v in step_ms.items()}, "profile": prof, "agreement": agree}
+                           share_of_hbm=nbytes / (kms * 1e-3) / HBM_BYTES_PER_S if kms else None)
+    return {"groups": len(spec), "host_step_ms": {k: stats(v) for k, v in host.items()},
+            "step_to_sync_ms": {k: stats(v) for k, v in step_ms.items()}, "profile": prof, "agreement": agree}
 
 
 def main():
-    ap = argparse.ArgumentParser()
+    ap = arg_parser(__doc__, iters=None)
     ap.add_argument("--steps", type=int, default=20, help="optimizer steps per timed window")
-    ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--scene", type=int, default=130_000)
-    ap.add_argument("--frames", type=int, nargs="+", default=[1, 100, 1000])
-    ap.add_argument("--json", default=None)
+    ap.add_argument("--frames", type=int, nargs="+", default=[1, 100, 1000], help="SMPL-X frames in the layout")
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_adam: needs a CUDA device (there is no CPU measurement)")
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_adam")
     res = {"card": card(), "scene": a.scene, "by_frames": {n: run(n, a, dev) for n in a.frames}}
-    print(json.dumps(res, indent=1))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(res, f, indent=1)
+    emit(res, a.json)
 
 
 if __name__ == "__main__":

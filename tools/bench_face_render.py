@@ -10,12 +10,8 @@ pytorch3d's MeshRasterizer itself cannot be installed offline and is not measure
 in one process (host clock around N frames + device sync): median (min-max).  Kernel times come from a separate
 torch.profiler run.  Prints the card name and power limit with the numbers.
 """
-import argparse
-import json
 import os
-import statistics
 import sys
-import time
 
 import torch
 
@@ -23,36 +19,17 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_frame_sh import card  # noqa: E402
+from benchkit import alternate, arg_parser, card, cuda_device, emit, graph_replay, stats  # noqa: E402
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
 from exavatar_release_b200.mesh_render import FaceMeshRenderer, face_render_reference  # noqa: E402
 from exavatar_release_b200.synthetic import make_face_mesh, make_human_mesh  # noqa: E402
 
 
-def timed(fn, n):
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(n):
-        fn()
-    torch.cuda.synchronize()
-    return (time.perf_counter() - t0) / n
-
-
-def stats(v, scale=1.0, nd=3):
-    return {"median": round(statistics.median(v) * scale, nd), "min": round(min(v) * scale, nd),
-            "max": round(max(v) * scale, nd)}
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=20, help="frames per timed window")
-    ap.add_argument("--rounds", type=int, default=5)
+    ap = arg_parser(__doc__, iters=20)
     ap.add_argument("--profile-iters", type=int, default=5)
-    ap.add_argument("--json", default=None)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_face_render: needs a CUDA device (no CPU timing)")
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_face_render")
     H, W = 512, 512
     face = make_face_mesh()
     verts = make_human_mesh()["verts"][face["vertex_idx"]].to(dev)
@@ -89,27 +66,11 @@ def main():
     result["covered_pixels"] = int((p2f >= 0).sum())
     result["image_max_abs_diff"] = float((img - ref).abs().max())
 
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        for _ in range(3):
-            frame_op()
-    torch.cuda.current_stream(dev).wait_stream(side)
-    torch.cuda.synchronize()
-    clear()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        frame_op()  # the graph owns the .grad it accumulates into; replays overwrite it
-
-    arms = {"reference": lambda: (frame_ref(), clear()), "op": lambda: (frame_op(), clear()), "op_graph": graph.replay}
-    for fn in arms.values():
-        for _ in range(3):
-            fn()
-    times = {k: [] for k in arms}
-    for _ in range(a.rounds):
-        for k, fn in arms.items():
-            times[k].append(timed(fn, a.iters))
-    result["ms"] = {k: stats(v, 1e3) for k, v in times.items()}
+    # the graph owns the .grad it accumulates into; replays overwrite it
+    arms = {"reference": lambda: (frame_ref(), clear()), "op": lambda: (frame_op(), clear()),
+            "op_graph": graph_replay(frame_op, 3, reset=clear)}
+    times = alternate(arms, a.iters, a.rounds, 3)
+    result["ms"] = {k: stats(v, 1e3, 3) for k, v in times.items()}
 
     from torch.profiler import ProfilerActivity, profile
     for k in ("op", "reference"):
@@ -125,10 +86,7 @@ def main():
         result["kernels"][k] = {"device_us_per_frame": round(sum(v[0] for v in per.values()), 1),
                                 "launches_per_frame": round(sum(v[1] for v in per.values()), 1),
                                 "top": {n[:90]: [round(v[0], 1), v[1]] for n, v in top[:8]}}
-    print(json.dumps(result))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(result, f, indent=1)
+    emit(result, a.json)
 
 
 if __name__ == "__main__":

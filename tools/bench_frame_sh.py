@@ -12,20 +12,19 @@ and use_graph=True, arms alternated round by round in one process (host clock ar
 in-library CUDA-event profiler (profiling run of its own) gives K1 (project) and K6 (project_bwd) per merged pass.
 Prints the card name and power limit with the numbers.
 """
-import argparse
 import ctypes as C
-import json
 import os
 import statistics
-import subprocess
 import sys
-import time
+from functools import partial
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 
+from benchkit import alternate, arg_parser, card, cuda_device, emit, stats  # noqa: E402
 from exavatar_release_b200 import TrainingFrameRenderer  # noqa: E402
 from exavatar_release_b200 import _lib as L  # noqa: E402
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
@@ -38,30 +37,13 @@ ARMS = {"a_caller_rgb": False, "b_in_kernel_sh": True}
 L_NUM = 9  # B2R_NUM_KERNELS: kernel ids 0 project (K1) ... 7 project_bwd (K6)
 
 
-def card():
-    info = {"name": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clk = (s.strip() for s in q.split(","))
-        info.update(name=name, power_limit=power, max_sm_clock=clk)
-    except Exception as e:  # noqa: BLE001 -- a missing nvidia-smi leaves the torch name
-        info["power_limit"] = f"unknown ({type(e).__name__})"
-    return info
-
-
 def main():
-    ap = argparse.ArgumentParser()
+    ap = arg_parser(__doc__, iters=None, frames=30)
     ap.add_argument("--workload", default="C4")
-    ap.add_argument("--frames", type=int, default=30, help="frames per timed window")
     ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--rounds", type=int, default=5, help="alternated (a, b) windows per mode")
     ap.add_argument("--profile-frames", type=int, default=10)
-    ap.add_argument("--json", default=None, help="also write the result record here")
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_frame_sh: needs a CUDA device (no CPU timing)")
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_frame_sh")
     lib = L.load()
     wl = WORKLOADS[a.workload]
     H, W = wl.height, wl.width
@@ -99,6 +81,10 @@ def main():
         for t in leaves:
             t.grad = None
 
+    def window(fr, sh):
+        for i in range(a.frames):
+            step(fr, sh, cams[i % len(cams)])
+
     result = {"workload": wl.name, "sh_degree": deg, "P_scene": Ps, "P_human": Ph, "caps": caps, "card": card(),
               "fps": {}, "kernel_ms": {}}
     for mode, use_graph in (("eager", False), ("graph", True)):
@@ -107,19 +93,10 @@ def main():
         for arm, sh in ARMS.items():
             for i in range(a.warmup):
                 step(frs[arm], sh, cams[i % len(cams)])
-        torch.cuda.synchronize()
-        fps = {arm: [] for arm in ARMS}
-        for _ in range(a.rounds):
-            for arm, sh in ARMS.items():
-                torch.cuda.synchronize()
-                t0 = time.perf_counter()
-                for i in range(a.frames):
-                    step(frs[arm], sh, cams[i % len(cams)])
-                torch.cuda.synchronize()
-                fps[arm].append(a.frames / (time.perf_counter() - t0))
-            assert not any(f.overflowed() for f in frs.values())
-        result["fps"][mode] = {arm: {"median": round(statistics.median(v), 1), "min": round(min(v), 1),
-                                     "max": round(max(v), 1)} for arm, v in fps.items()}
+        # one call per window: each window walks the cameras from the first
+        windows = alternate({arm: partial(window, frs[arm], sh) for arm, sh in ARMS.items()}, 1, a.rounds, 0)
+        assert not any(f.overflowed() for f in frs.values())
+        result["fps"][mode] = {arm: stats([a.frames / s for s in v], nd=1) for arm, v in windows.items()}
         del frs
         torch.cuda.empty_cache()
 
@@ -157,10 +134,7 @@ def main():
         result["kernel_ms"][arm] = {k: round(statistics.median(v), 4) for k, v in sorted(acc.items())}
         del plan
         torch.cuda.empty_cache()
-    print(json.dumps(result))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(result, f, indent=1)
+    emit(result, a.json)
 
 
 if __name__ == "__main__":

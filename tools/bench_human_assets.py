@@ -11,19 +11,14 @@ and every asset output.  Arms:
                 in ExAvatar's fp32 operations, with line 564's per-frame matrix_to_quaternion of P identity matrices;
   2. op:        `decode_smplx_pose` + `HumanAssets.geometry` / `.colors`, eager;
   3. op_graph:  arm 2 captured once in a CUDA graph and replayed;
-  4. frame_*:   C4 training frames/s of tools/bench_smplx_rig.py's frame with the rig's pose decoded every frame from
+  4. frame_*:   C4 training frames/s of tools/c4_frame.py's frame with the rig's pose decoded every frame from
                 the frame's 6D parameters by arm 1's route (frame_decode_exavatar) or by the op (frame_decode_op).
 Arms alternate window by window in one process (host clock around N calls + device sync): median (min-max).  Host
 syncs per call are counted with torch's sync debug mode ("warn"); device time and launches per call come from a
 separate torch.profiler run.  Prints the card name and power limit with the numbers.
 """
-import argparse
-import json
 import os
-import statistics
 import sys
-import time
-import warnings
 
 import torch
 
@@ -31,7 +26,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_frame_sh import card  # noqa: E402
+from benchkit import alternate, arg_parser, card, cuda_device, emit, graph_replay, host_syncs, kernel_events, stats  # noqa: E402
+from c4_frame import FrameArm, frames_per_second  # noqa: E402
 from exavatar_release_b200 import HumanAssets, decode_smplx_pose  # noqa: E402
 from exavatar_release_b200.human_assets import (POSE_KEYS, POSE_ROWS, constant_rotation_reference,  # noqa: E402
                                                 decode_smplx_pose_reference, human_colors_reference,
@@ -73,15 +69,8 @@ KEYS = ("mean_3d", "mean_3d_refined", "scale", "scale_refined", "mean_offset_off
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=20, help="calls per timed window")
-    ap.add_argument("--rounds", type=int, default=5)
-    ap.add_argument("--frames", type=int, default=10, help="training frames per timed window")
-    ap.add_argument("--json", default=None)
-    a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_human_assets: needs a CUDA device (there is no CPU measurement)")
-    dev = torch.device("cuda:0")
+    a = arg_parser(__doc__, iters=20, frames=10).parse_args()
+    dev = cuda_device("bench_human_assets")
     g = torch.Generator().manual_seed(1)
     mask = torch.zeros(P, dtype=torch.bool)
     mask[torch.randperm(P, generator=g)[:P // 3]] = True
@@ -115,73 +104,30 @@ def main():
 
     pg = {k: v.detach().clone().requires_grad_() for k, v in params.items()}
     xg = [t.detach().clone().requires_grad_(t.requires_grad) for t in ins]
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            run_op(pg, xg)
-    torch.cuda.current_stream().wait_stream(s)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        run_op(pg, xg)
-    arms = {"exavatar": run_exavatar, "op": run_op, "op_graph": graph.replay}
-    for fn in arms.values():
-        fn()
-    torch.cuda.synchronize()
-    times = {k: [] for k in arms}
-    for _ in range(a.rounds):
-        for k, fn in arms.items():
-            torch.cuda.synchronize()
-            t = time.perf_counter()
-            for _ in range(a.iters):
-                fn()
-            torch.cuda.synchronize()
-            times[k].append((time.perf_counter() - t) / a.iters * 1e3)
-
-    syncs = {}
-    for k in ("exavatar", "op"):
-        torch.cuda.synchronize()
-        with warnings.catch_warnings(record=True) as caught:
-            warnings.simplefilter("always")
-            torch.cuda.set_sync_debug_mode("warn")
-            try:
-                arms[k]()
-            finally:
-                torch.cuda.set_sync_debug_mode(0)
-        syncs[k] = sum("synchroniz" in str(m.message).lower() for m in caught)
+    arms = {"exavatar": run_exavatar, "op": run_op, "op_graph": graph_replay(lambda: run_op(pg, xg), 2)}
+    times = alternate(arms, a.iters, a.rounds, 1)
+    syncs = {k: host_syncs(arms[k]) for k in ("exavatar", "op")}
 
     prof = {}
-    from torch.profiler import ProfilerActivity, profile
     for k, fn in arms.items():
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as p:
-            fn()
-            torch.cuda.synchronize()
-        ev = [e for e in p.events() if e.device_type.name == "CUDA" and "Memcpy" not in e.name
-              and "Memset" not in e.name]
-        prof[k] = {"device_ms": sum(e.device_time for e in ev) / 1e3, "launches": len(ev),
-                   "kernels": sorted({e.name for e in ev if "human" in e.name or "decode_pose" in e.name})}
+        ev, prof[k] = kernel_events(fn)
+        prof[k]["kernels"] = sorted({e.name for e in ev if "human" in e.name or "decode_pose" in e.name})
 
-    from bench_smplx_rig import frames_per_second
     fp = pose_params(dev, seed=2)
 
-    def decode(form):
-        def fn():
+    def decode_arm(decode):
+        def pose_rig(rig, d, x):
             for v in fp.values():
                 v.grad = None
-            return decode_smplx_pose_reference(fp)["full_pose"] if form == "exavatar" else \
-                decode_smplx_pose(fp)["full_pose"]
-        return fn
+            return rig(x[0], x[1], decode(fp)["full_pose"], x[3])
+        return FrameArm(rig=pose_rig)
 
     res = {"card": card(), "P": P, "joints": 55,
-           "ms_per_call": {k: {"median": statistics.median(v), "min": min(v), "max": max(v)} for k, v in times.items()},
+           "ms_per_call": {k: stats(v, 1e3) for k, v in times.items()},
            "host_syncs_per_call": syncs, "profile": prof, "exavatar_vs_op": agree,
-           "frames_per_s": frames_per_second(a, dev, poses={"decode_exavatar": decode("exavatar"),
-                                                            "decode_op": decode("op")})}
-    print(json.dumps(res, indent=1))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(res, f, indent=1)
+           "frames_per_s": frames_per_second(a, dev, {"decode_exavatar": decode_arm(decode_smplx_pose_reference),
+                                                      "decode_op": decode_arm(decode_smplx_pose)})}
+    emit(res, a.json)
 
 
 if __name__ == "__main__":

@@ -16,12 +16,9 @@ queries with a 30 % self-map, 335 232 faces).  Arms:
 Arms alternate window by window in one process (host clock around N calls + device sync): median (min-max).  Kernel
 times come from a separate torch.profiler run.  Prints the card name and power limit with the numbers.
 """
-import argparse
-import json
 import os
-import statistics
 import sys
-import time
+from functools import partial
 
 import torch
 import torch.nn.functional as F
@@ -30,7 +27,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_frame_sh import card  # noqa: E402
+from benchkit import alternate, arg_parser, card, cuda_device, emit, graph_replay, stats  # noqa: E402
 from exavatar_release_b200 import TrainingFrameRenderer  # noqa: E402
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
 from exavatar_release_b200.geometry import VertexNormals, nearest_rows, nearest_rows_reference  # noqa: E402
@@ -57,31 +54,11 @@ def torch_normals(xyz, faces_np, is_cavity):
     return n * (1 - cav) + (-n) * cav
 
 
-def timed(fn, n):
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(n):
-        fn()
-    torch.cuda.synchronize()
-    return (time.perf_counter() - t0) / n
-
-
-def stats(v, scale=1.0, nd=3):
-    return {"median": round(statistics.median(v) * scale, nd), "min": round(min(v) * scale, nd),
-            "max": round(max(v) * scale, nd)}
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=20, help="calls per timed window")
-    ap.add_argument("--frames", type=int, default=10, help="training frames per timed window")
-    ap.add_argument("--rounds", type=int, default=5)
+    ap = arg_parser(__doc__, iters=20, frames=10)
     ap.add_argument("--profile-iters", type=int, default=5)
-    ap.add_argument("--json", default=None)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_human_geometry: needs a CUDA device (no CPU timing)")
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_human_geometry")
     m = make_human_mesh()
     P, V = m["verts"].shape[0], m["targets"].shape[0]
     q, t, x = m["queries"].to(dev), m["targets"].to(dev), m["verts"].to(dev)
@@ -106,26 +83,9 @@ def main():
         nearest_rows(q, t, sm)
         vn(x)
 
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        for _ in range(3):
-            arm_op()
-    torch.cuda.current_stream(dev).wait_stream(side)
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        arm_op()
-
-    arms = {"torch": arm_torch, "op": arm_op, "op_graph": graph.replay}
-    for fn in arms.values():
-        for _ in range(3):
-            fn()
-    times = {k: [] for k in arms}
-    for _ in range(a.rounds):
-        for k, fn in arms.items():
-            times[k].append(timed(fn, a.iters))
-    result["ms"] = {k: stats(v, 1e3) for k, v in times.items()}
+    arms = {"torch": arm_torch, "op": arm_op, "op_graph": graph_replay(arm_op, 3)}
+    times = alternate(arms, a.iters, a.rounds, 3)
+    result["ms"] = {k: stats(v, 1e3, 3) for k, v in times.items()}
 
     from torch.profiler import ProfilerActivity, profile
     for k in ("torch", "op"):
@@ -184,20 +144,10 @@ def main():
         for v in leaves:
             v.grad = None
 
-    farms = ("torch", "op")
-    for k in farms:
-        for _ in range(3):
-            frame(k)
-    fps = {k: [] for k in farms}
-    for _ in range(a.rounds):
-        for k in farms:
-            fps[k].append(a.frames / timed(lambda: [frame(k) for _ in range(a.frames)], 1))
+    times = alternate({k: partial(frame, k) for k in ("torch", "op")}, a.frames, a.rounds, 3)
     assert not fr.overflowed()
-    result["frame_fps"] = {"frame_" + k: stats(v, 1.0, 1) for k, v in fps.items()}
-    print(json.dumps(result))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(result, f, indent=1)
+    result["frame_fps"] = {"frame_" + k: stats([1 / s for s in v], 1.0, 1) for k, v in times.items()}
+    emit(result, a.json)
 
 
 if __name__ == "__main__":

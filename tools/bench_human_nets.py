@@ -20,12 +20,10 @@ times come from a separate torch.profiler run of arm 2.  Achieved TFLOP/s counts
 ExAvatar's form (pose unfolded) and with the pose folded; 3xTF32 issues three tensor-core MMAs per counted product, so
 the tensor cores do three times the counted work.  Prints the card name and power limit with the numbers.
 """
-import argparse
-import json
 import os
 import statistics
 import sys
-import time
+from functools import partial
 
 import torch
 import torch.nn as nn
@@ -35,7 +33,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_frame_sh import card  # noqa: E402
+from benchkit import alternate, arg_parser, card, cuda_device, emit, graph_replay, stats  # noqa: E402
 from exavatar_release_b200 import TrainingFrameRenderer  # noqa: E402
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
 from exavatar_release_b200.geometry import VertexNormals, nearest_rows  # noqa: E402
@@ -63,11 +61,6 @@ def macs_per_row(folded):
              "rgb_offset": TRI + NORMAL + (0 if folded else POSE)}
     heads = {"geo": 4, "geo_offset": 4, "rgb": 3, "rgb_offset": 3}
     return sum(k * 128 + 2 * 128 * 128 + 128 * heads[n] for n, k in first.items())
-
-
-def stats(v, scale=1.0, nd=3):
-    return {"median": round(statistics.median(v) * scale, nd), "min": round(min(v) * scale, nd),
-            "max": round(max(v) * scale, nd)}
 
 
 def frames_per_second(args, dev, nets, tp, tpf, pose):
@@ -142,35 +135,17 @@ def frames_per_second(args, dev, nets, tp, tpf, pose):
         for v in leaves:
             v.grad = None
 
-    arms = ("torch", "op")
-    for k in arms:
-        for _ in range(3):
-            frame(k)
-    times = {k: [] for k in arms}
-    for _ in range(args.rounds):
-        for k in arms:
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            for _ in range(args.frames):
-                frame(k)
-            torch.cuda.synchronize()
-            times[k].append(args.frames / (time.perf_counter() - t0))
+    times = alternate({k: partial(frame, k) for k in ("torch", "op")}, args.frames, args.rounds, 3)
     if fr.overflowed():
         raise SystemExit("bench_human_nets: a render overflowed its list capacity")
-    return {f"frame_{k}": stats(v, 1.0, 1) for k, v in times.items()}
+    return {f"frame_{k}": stats([1 / s for s in v], 1.0, 1) for k, v in times.items()}
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=10, help="steps per timed window")
-    ap.add_argument("--rounds", type=int, default=5)
-    ap.add_argument("--frames", type=int, default=10, help="training frames per timed window")
-    ap.add_argument("--json", default=None)
+    ap = arg_parser(__doc__, iters=10, frames=10)
     ap.add_argument("--trace-dir", default=None)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_human_nets: needs a CUDA device")
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_human_nets")
     torch.manual_seed(0)
     g = torch.Generator(device=dev).manual_seed(0)
     pos = (torch.rand((P, 3), generator=g, device=dev) - 0.5) * torch.tensor([0.9, 1.9, 0.4], device=dev)
@@ -218,31 +193,14 @@ def main():
     for _ in range(3):
         zero(); torch_step()  # noqa: E702
         zero(); op_step()  # noqa: E702
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            zero()
-            op_step()
-    torch.cuda.current_stream().wait_stream(s)
-    zero()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        op_step()
-    graph.replay()
+    op = lambda: (zero(), op_step())  # noqa: E731
+    replay = graph_replay(op, 2)
+    replay()
     torch.cuda.synchronize()
 
-    arms = {"torch": lambda: (zero(), torch_step()), "op": lambda: (zero(), op_step()), "op_graph": graph.replay}
-    times = {k: [] for k in arms}
-    for _ in range(args.rounds):
-        for k, fn in arms.items():
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            for _ in range(args.iters):
-                fn()
-            torch.cuda.synchronize()
-            times[k].append((time.perf_counter() - t0) / args.iters)
-    res = {"card": card(), "P": P, "step_ms": {k: stats(v, 1e3) for k, v in times.items()}}
+    arms = {"torch": lambda: (zero(), torch_step()), "op": op, "op_graph": replay}
+    times = alternate(arms, args.iters, args.rounds, 0)
+    res = {"card": card(), "P": P, "step_ms": {k: stats(v, 1e3, 3) for k, v in times.items()}}
     for folded in (False, True):
         flop = 3 * 2 * macs_per_row(folded) * P  # forward + backward (dX and dW)
         key = "tflops_folded" if folded else "tflops_exavatar_form"
@@ -267,11 +225,7 @@ def main():
         os.makedirs(args.trace_dir, exist_ok=True)
         prof.export_chrome_trace(os.path.join(args.trace_dir, "human_nets_trace.json"))
     res["frame_fps"] = frames_per_second(args, dev, nets, tp, tpf, pose)
-    print(json.dumps(res, indent=1))
-    if args.json:
-        os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
-        with open(args.json, "w") as f:
-            json.dump(res, f, indent=1)
+    emit(res, args.json)
 
 
 if __name__ == "__main__":

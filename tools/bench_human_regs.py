@@ -15,17 +15,13 @@ The block at C4 size (the synthetic 167 618-vertex mesh with make_regs_labels' l
                 `l1_ssim` of the five renders, then the regularisers and the backward: without the block
                 (frame_no_regs), with the block of arm 1 (frame_regs_ops) and with the op (frame_regs_op).
 Arms alternate window by window in one process (host clock around N calls + device sync): median (min-max).  Host
-syncs per block are counted under torch.cuda.set_sync_debug_mode("warn"); device time and launch count per block come
+syncs per block are counted with torch's sync debug mode ("warn"); device time and launch count per block come
 from a separate torch.profiler run.  Prints the card name and power limit with the numbers.
 """
-import argparse
-import json
 import math
 import os
-import statistics
 import sys
-import time
-import warnings
+from functools import partial
 
 import numpy as np
 import torch
@@ -35,7 +31,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_frame_sh import card  # noqa: E402
+from benchkit import alternate, arg_parser, card, cuda_device, emit, graph_replay, host_syncs, kernel_events, stats  # noqa: E402
 from bench_human_nets import stack  # noqa: E402
 from exavatar_release_b200 import HumanRegularizers, TrainingFrameRenderer  # noqa: E402
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
@@ -232,34 +228,15 @@ def frames_per_second(a, dev, d, regs):
         for v in leaves:
             v.grad = None
 
-    arms = ("no_regs", "regs_ops", "regs_op")
-    for k in arms:
-        for _ in range(3):
-            frame(k)
-    times = {k: [] for k in arms}
-    for _ in range(a.rounds):
-        for k in arms:
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            for _ in range(a.frames):
-                frame(k)
-            torch.cuda.synchronize()
-            times[k].append(a.frames / (time.perf_counter() - t0))
+    times = alternate({k: partial(frame, k) for k in ("no_regs", "regs_ops", "regs_op")}, a.frames, a.rounds, 3)
     if fr.overflowed():
         raise SystemExit("bench_human_regs: a render overflowed its list capacity")
-    return {f"frame_{k}": {"median": statistics.median(v), "min": min(v), "max": max(v)} for k, v in times.items()}
+    return {f"frame_{k}": stats([1 / s for s in v]) for k, v in times.items()}
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=20, help="block calls per timed window")
-    ap.add_argument("--rounds", type=int, default=5)
-    ap.add_argument("--frames", type=int, default=10, help="training frames per timed window")
-    ap.add_argument("--json", default=None)
-    a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_human_regs: needs a CUDA device (there is no CPU measurement)")
-    dev = torch.device("cuda:0")
+    a = arg_parser(__doc__, iters=20, frames=10).parse_args()
+    dev = cuda_device("bench_human_regs")
     d, regs, x = setup(dev)
 
     def run_ops():
@@ -275,60 +252,14 @@ def main():
 
     # the graph arm owns its leaves, so no autograd node of the eager arms is kept alive into the capture
     xg = {k: v.detach().clone().requires_grad_() for k, v in x.items()}
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            run_op(xg)
-    torch.cuda.current_stream().wait_stream(s)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        run_op(xg)
-    arms = {"ops": run_ops, "op": run_op, "op_graph": graph.replay}
-    for fn in arms.values():
-        fn()
-    torch.cuda.synchronize()
-    times = {k: [] for k in arms}
-    for _ in range(a.rounds):
-        for k, fn in arms.items():
-            torch.cuda.synchronize()
-            t = time.perf_counter()
-            for _ in range(a.iters):
-                fn()
-            torch.cuda.synchronize()
-            times[k].append((time.perf_counter() - t) / a.iters * 1e3)
-
-    syncs = {}
-    for k in ("ops", "op"):
-        torch.cuda.synchronize()
-        with warnings.catch_warnings(record=True) as w:
-            warnings.simplefilter("always")
-            torch.cuda.set_sync_debug_mode("warn")
-            try:
-                arms[k]()
-            finally:
-                torch.cuda.set_sync_debug_mode(0)
-        syncs[k] = sum("synchroniz" in str(m.message).lower() for m in w)
-
-    prof = {}
-    from torch.profiler import ProfilerActivity, profile
-    for k, fn in arms.items():
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as p:
-            fn()
-            torch.cuda.synchronize()
-        ev = [e for e in p.events() if e.device_type.name == "CUDA" and "Memcpy" not in e.name
-              and "Memset" not in e.name]
-        prof[k] = {"device_ms": sum(e.device_time for e in ev) / 1e3, "launches": len(ev)}
-
+    arms = {"ops": run_ops, "op": run_op, "op_graph": graph_replay(lambda: run_op(xg), 2)}
+    times = alternate(arms, a.iters, a.rounds, 1)
     res = {"card": card(), "P": d["P"],
-           "block_ms": {k: {"median": statistics.median(v), "min": min(v), "max": max(v)} for k, v in times.items()},
-           "host_syncs_per_block": syncs, "profile": prof, "values_ops_vs_op": agree,
+           "block_ms": {k: stats(v, 1e3) for k, v in times.items()},
+           "host_syncs_per_block": {k: host_syncs(arms[k]) for k in ("ops", "op")},
+           "profile": {k: kernel_events(fn)[1] for k, fn in arms.items()}, "values_ops_vs_op": agree,
            "frames_per_s": frames_per_second(a, dev, d, regs)}
-    print(json.dumps(res, indent=1))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(res, f, indent=1)
+    emit(res, a.json)
 
 
 if __name__ == "__main__":

@@ -14,13 +14,10 @@ backward into the five renders.  Arms:
 Arms alternate window by window in one process (host clock around N calls + device sync): median (min-max).  Kernel
 times come from a separate torch.profiler run.  Prints the card name and power limit with the numbers.
 """
-import argparse
-import json
 import math
 import os
-import statistics
 import sys
-import time
+from functools import partial
 
 import torch
 import torch.nn.functional as F
@@ -29,7 +26,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_frame_sh import card  # noqa: E402
+from benchkit import alternate, arg_parser, card, cuda_device, emit, graph_replay, stats  # noqa: E402
 from exavatar_release_b200 import TrainingFrameRenderer  # noqa: E402
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
 from exavatar_release_b200.losses import l1_ssim  # noqa: E402
@@ -117,32 +114,12 @@ def make_data(H, W, dev):
             "faces": faces}
 
 
-def timed(fn, n):
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(n):
-        fn()
-    torch.cuda.synchronize()
-    return (time.perf_counter() - t0) / n
-
-
-def stats(v, scale=1.0, nd=3):
-    return {"median": round(statistics.median(v) * scale, nd), "min": round(min(v) * scale, nd),
-            "max": round(max(v) * scale, nd)}
-
-
 def main():
-    ap = argparse.ArgumentParser()
+    ap = arg_parser(__doc__, iters=50, frames=30)
     ap.add_argument("--workload", default="C4")
-    ap.add_argument("--iters", type=int, default=50, help="block calls per timed window")
-    ap.add_argument("--frames", type=int, default=30, help="training frames per timed window")
-    ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--profile-iters", type=int, default=10)
-    ap.add_argument("--json", default=None)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_l1_ssim: needs a CUDA device (no CPU timing)")
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_l1_ssim")
     wl = WORKLOADS[a.workload]
     H, W = wl.height, wl.width
     d = make_data(H, W, dev)
@@ -162,26 +139,9 @@ def main():
     def graph_body():
         return torch.autograd.grad(block_op(static_in, d), list(static_in.values()))
 
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        for _ in range(3):
-            graph_body()
-    torch.cuda.current_stream(dev).wait_stream(side)
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        graph_body()
-
-    arms = {"ops": lambda: step("ops"), "op": lambda: step("op"), "op_graph": graph.replay}
-    for fn in arms.values():
-        for _ in range(5):
-            fn()
-    times = {k: [] for k in arms}
-    for _ in range(a.rounds):
-        for k, fn in arms.items():
-            times[k].append(timed(fn, a.iters))
-    result["block_ms"] = {k: stats(v, 1e3) for k, v in times.items()}
+    arms = {"ops": lambda: step("ops"), "op": lambda: step("op"), "op_graph": graph_replay(graph_body, 3)}
+    times = alternate(arms, a.iters, a.rounds, 5)
+    result["block_ms"] = {k: stats(v, 1e3, 3) for k, v in times.items()}
 
     # kernel times of one block call (fwd + bwd), profiler run of its own
     from torch.profiler import ProfilerActivity, profile
@@ -216,20 +176,19 @@ def main():
         for t in fleaves:
             t.grad = None
 
+    def window(block):
+        for i in range(a.frames):
+            frame(block, i)
+
     farms = {"frame_only": None, "frame_ops": "ops", "frame_op": "op"}
     for b in farms.values():
         for i in range(5):
             frame(b, i)
-    fps = {k: [] for k in farms}
-    for _ in range(a.rounds):
-        for k, b in farms.items():
-            fps[k].append(1.0 / timed(lambda: [frame(b, i) for i in range(a.frames)], 1) * a.frames)
+    # one call per window: each window walks the cameras from the first
+    windows = alternate({k: partial(window, b) for k, b in farms.items()}, 1, a.rounds, 0)
     assert not fr.overflowed()
-    result["frame_fps"] = {k: stats(v, 1.0, 1) for k, v in fps.items()}
-    print(json.dumps(result))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(result, f, indent=1)
+    result["frame_fps"] = {k: stats([a.frames / s for s in v], 1.0, 1) for k, v in windows.items()}
+    emit(result, a.json)
 
 
 if __name__ == "__main__":

@@ -10,7 +10,7 @@ depend on their values).  Arms:
                 the render and the target through VGG in each call -- and one backward;
   2. op:        `LPIPS` on the pair (N = 2, one target pass), eager;
   3. op_graph:  arm 2 captured once in a CUDA graph and replayed;
-  4. frame_*:   C4 training frames/s of tools/bench_smplx_rig.py's frame (rig op, networks, skinning, the five renders,
+  4. frame_*:   C4 training frames/s of tools/c4_frame.py's frame (rig op, networks, skinning, the five renders,
                 l1_ssim, regularisers) with 0.2 x the two LPIPS terms of scene_human / scene_human_refined added: none,
                 arm 1's form, or the op.
 Arms alternate window by window in one process (host clock around N calls + device sync): median (min-max).  Per-kernel
@@ -19,13 +19,8 @@ device time per call comes from a separate torch.profiler run, and achieved TFLO
 backward runs as a GEMM) over that device time, against the 495 TFLOP/s dense TF32 data-sheet figure.  Prints the card
 name and power limit with the numbers.
 """
-import argparse
-import json
 import os
-import statistics
 import sys
-import time
-import warnings
 
 import torch
 import torch.nn.functional as F
@@ -35,11 +30,11 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 
-from bench_frame_sh import card  # noqa: E402
+from benchkit import alternate, arg_parser, card, cuda_device, emit, graph_replay, host_syncs, kernel_events, stats  # noqa: E402
+from c4_frame import BOX, FrameArm, frames_per_second  # noqa: E402
 from exavatar_release_b200.perceptual import LPIPS, SCALE, SHIFT, SLICES  # noqa: E402
 
 H = W = 512
-BOX = (102.4, 60.8, 307.5, 396.2)  # ~60 % of the image (tools/bench_l1_ssim.py)
 TF32_PEAK = 495e12
 
 
@@ -87,15 +82,8 @@ class ExAvatarLpips(torch.nn.Module):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=10, help="calls per timed window")
-    ap.add_argument("--rounds", type=int, default=5)
-    ap.add_argument("--frames", type=int, default=10, help="training frames per timed window")
-    ap.add_argument("--json", default=None)
-    a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_lpips: needs a CUDA device (there is no CPU measurement)")
-    dev = torch.device("cuda:0")
+    a = arg_parser(__doc__, iters=10, frames=10).parse_args()
+    dev = cuda_device("bench_lpips")
     from make_lpips_golden import lpips_weights
     feats, lins = lpips_weights()
     op = LPIPS(feats, lins, dev)
@@ -124,42 +112,14 @@ def main():
     agree = {"grad_max_abs_diff": float((xe.grad - xo.grad).abs().max()), "grad_max_abs": float(xe.grad.abs().max())}
 
     xg = pair.clone().requires_grad_()
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            xg.grad = None
-            run_op(xg)
-    torch.cuda.current_stream().wait_stream(s)
-    graph = torch.cuda.CUDAGraph()
-    xg.grad = None
-    with torch.cuda.graph(graph):
-        run_op(xg)
-    arms = {"exavatar": run_exavatar, "op": run_op, "op_graph": graph.replay}
-    for fn in arms.values():
-        fn()
-    torch.cuda.synchronize()
-    times = {k: [] for k in arms}
-    for _ in range(a.rounds):
-        for k, fn in arms.items():
-            torch.cuda.synchronize()
-            t = time.perf_counter()
-            for _ in range(a.iters):
-                fn()
-            torch.cuda.synchronize()
-            times[k].append((time.perf_counter() - t) / a.iters * 1e3)
 
-    syncs = {}
-    for k in ("exavatar", "op"):
-        torch.cuda.synchronize()
-        with warnings.catch_warnings(record=True) as caught:
-            warnings.simplefilter("always")
-            torch.cuda.set_sync_debug_mode("warn")
-            try:
-                arms[k]()
-            finally:
-                torch.cuda.set_sync_debug_mode(0)
-        syncs[k] = sum("synchroniz" in str(m.message).lower() for m in caught)
+    def run_op_xg():
+        xg.grad = None
+        run_op(xg)
+
+    arms = {"exavatar": run_exavatar, "op": run_op, "op_graph": graph_replay(run_op_xg, 2)}
+    times = alternate(arms, a.iters, a.rounds, 1)
+    syncs = {k: host_syncs(arms[k]) for k in ("exavatar", "op")}
 
     x0, y0 = int(BOX[0]), int(BOX[1])
     cw, ch = min(x0 + int(BOX[2]), W) - x0, min(y0 + int(BOX[3]), H) - y0
@@ -167,26 +127,17 @@ def main():
     flops = {"exavatar": 2 * (4 * fwd + 2 * (fwd - c11)), "op": 2 * (3 * fwd + 2 * (fwd - c11))}
     flops["op_graph"] = flops["op"]
     prof = {}
-    from torch.profiler import ProfilerActivity, profile
     for k, fn in arms.items():
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as p:
-            fn()
-            torch.cuda.synchronize()
-        ev = [e for e in p.events() if e.device_type.name == "CUDA" and "Memcpy" not in e.name
-              and "Memset" not in e.name]
+        ev, prof[k] = kernel_events(fn)
         per = {}
         for e in ev:
             n = e.name if len(e.name) <= 90 else e.name[:87] + "..."
             per.setdefault(n, [0.0, 0])
             per[n][0] += e.device_time / 1e3
             per[n][1] += 1
-        dms = sum(e.device_time for e in ev) / 1e3
-        prof[k] = {"device_ms": dms, "launches": len(ev), "tflops": flops[k] / (dms * 1e-3) / 1e12,
-                   "share_of_tf32_peak": flops[k] / (dms * 1e-3) / TF32_PEAK,
-                   "kernels_ms": {n: round(v[0], 4) for n, v in sorted(per.items(), key=lambda kv: -kv[1][0])[:12]}}
-
-    from bench_smplx_rig import frames_per_second
+        dms = prof[k]["device_ms"]
+        prof[k].update(tflops=flops[k] / (dms * 1e-3) / 1e12, share_of_tf32_peak=flops[k] / (dms * 1e-3) / TF32_PEAK,
+                       kernels_ms={n: round(v[0], 4) for n, v in sorted(per.items(), key=lambda kv: -kv[1][0])[:12]})
 
     def lp_exavatar(o, target):
         return sum(0.2 * ref(o[r]["img"][None], target[None], bbox).sum()
@@ -195,15 +146,12 @@ def main():
     def lp_op(o, target):
         return 0.2 * op(torch.stack((o["scene_human"]["img"], o["scene_human_refined"]["img"])), target, bbox).sum()
 
-    frames = frames_per_second(a, dev, {"lpips_none": lambda o, t: 0.0, "lpips_exavatar": lp_exavatar,
-                                        "lpips_op": lp_op})
+    frames = frames_per_second(a, dev, {"lpips_none": FrameArm(loss=lambda o, t: 0.0),
+                                        "lpips_exavatar": FrameArm(loss=lp_exavatar), "lpips_op": FrameArm(loss=lp_op)})
     res = {"card": card(), "size": [H, W], "crop": [ch, cw], "gflop_per_frame": {k: v / 1e9 for k, v in flops.items()},
-           "lpips_ms": {k: {"median": statistics.median(v), "min": min(v), "max": max(v)} for k, v in times.items()},
+           "lpips_ms": {k: stats(v, 1e3) for k, v in times.items()},
            "host_syncs_per_call": syncs, "profile": prof, "exavatar_vs_op": agree, "frames_per_s": frames}
-    print(json.dumps(res, indent=1))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(res, f, indent=1)
+    emit(res, a.json)
 
 
 if __name__ == "__main__":

@@ -25,7 +25,6 @@ import ctypes as C
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -33,22 +32,16 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 
+from benchkit import HBM_BYTES_PER_S, card, cuda_device  # noqa: E402
 from exavatar_release_b200 import _lib as L  # noqa: E402
 from exavatar_release_b200 import rasterizer as rz  # noqa: E402
 from exavatar_release_b200.plan import FramePlan  # noqa: E402
 from exavatar_release_b200.synthetic import WORKLOADS, make_assets, make_grad_image  # noqa: E402
 from util import workload_settings  # noqa: E402
 
-HBM_BPS = 3.35e12
 WIDTHS = {"means3D": 3, "means2D": 3, "colors": 3, "opacities": 1, "scales": 3, "rotations": 4}
-
-
-def card_now():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    name, power, clk, clk_max = (s.strip() for s in q.split(","))
-    return {"name": name, "power_limit": power, "sm_clock": clk, "max_sm_clock": clk_max}
 
 
 def algorithmic_bytes(rows, vis, vis_scene, accumulate):
@@ -64,9 +57,7 @@ def main():
                     help="the first run saves the gradient scratch here, later runs load it; every run saves the outputs "
                          "of one writing launch per pass as <label>_<pass>.pt")
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_project_bwd: needs a CUDA device (no CPU timing)")
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_project_bwd")
     wl = WORKLOADS["C4"]
     P, Ps = wl.n_avatar + wl.n_scene, wl.n_scene
     assets = {k: v.to(dev) for k, v in make_assets("C4", seed=0).items()}
@@ -137,8 +128,8 @@ def main():
         result["passes"][name] = {"first_row": first_row, "rows": rows, "visible": vis, "us_per_launch": round(us, 2),
                                   "us_min": round(min(times), 2), "us_max": round(max(times), 2),
                                   "algorithmic_bytes": nbytes, "GBps": round(nbytes / us / 1e3, 1),
-                                  "frac_of_3.35TBps": round(nbytes / (us * 1e-6) / HBM_BPS, 3)}
-    result["card"] = card_now()
+                                  "frac_of_3.35TBps": round(nbytes / (us * 1e-6) / HBM_BYTES_PER_S, 3)}
+    result["card"] = card()
     print(json.dumps(result), flush=True)
 
 

@@ -13,12 +13,9 @@ Timed eager and as a captured CUDA graph (CUDA events around --iters calls), arm
 in front of `TrainingFrameRenderer(use_graph=True)`, frames/s the same way.  Then a torch.profiler run of its own for
 the device time of each skinning kernel.  Prints the card name and power limit with the numbers.
 """
-import argparse
-import json
 import os
-import statistics
 import sys
-import time
+from functools import partial
 
 import torch
 
@@ -26,7 +23,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_frame_sh import card  # noqa: E402
+from benchkit import alternate, arg_parser, card, cuda_device, emit, graph_replay, stats  # noqa: E402
 from exavatar_release_b200 import TrainingFrameRenderer  # noqa: E402
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
 from exavatar_release_b200.plan import RENDERS  # noqa: E402
@@ -64,21 +61,11 @@ def pose(arm, x, xr, W, rows, A, tr, R, t, capturable):
     return (lbs_reference(x, w, A, tr, R, t, cam_R_inv=Rinv), lbs_reference(xr, w, A, tr, R, t, cam_R_inv=Rinv))
 
 
-def stats(v):
-    return {"median": round(statistics.median(v), 4), "min": round(min(v), 4), "max": round(max(v), 4)}
-
-
 def main():
-    ap = argparse.ArgumentParser()
+    ap = arg_parser(__doc__, iters=50, frames=30)
     ap.add_argument("--workload", default="C4")
-    ap.add_argument("--iters", type=int, default=50, help="pose fwd+bwd calls per timed window")
-    ap.add_argument("--frames", type=int, default=30, help="training frames per timed window")
-    ap.add_argument("--rounds", type=int, default=5)
-    ap.add_argument("--json", default=None)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_skin_pair: needs a CUDA device (no CPU timing)")
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_skin_pair")
     wl = WORKLOADS[a.workload]
     H, W_img = wl.height, wl.width
     scene, human, refined = make_population_assets(a.workload, seed=0, device=dev)
@@ -101,19 +88,8 @@ def main():
         return torch.autograd.grad(loss, (lv["x"], lv["xr"], lv["A"], lv["tr"]))
 
     # ---- pose forward + backward: eager and CUDA graph ----
-    graphs = {}
-    for arm in ARMS:
-        side = torch.cuda.Stream(dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            for _ in range(3):
-                pose_step(arm, capturable=True)
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize()
-        graphs[arm] = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graphs[arm]):
-            pose_step(arm, capturable=True)
-    runners = {"eager": lambda arm: pose_step(arm), "graph": lambda arm: graphs[arm].replay()}
+    graphs = {arm: graph_replay(partial(pose_step, arm, capturable=True), 3) for arm in ARMS}
+    runners = {"eager": lambda arm: pose_step(arm), "graph": lambda arm: graphs[arm]()}
     for mode, run in runners.items():
         for arm in ARMS:
             for _ in range(5):
@@ -129,7 +105,7 @@ def main():
                 e1.record()
                 torch.cuda.synchronize()
                 times[arm].append(e0.elapsed_time(e1) / a.iters)
-        result["pose_fwd_bwd_ms"][mode] = {arm: stats(v) for arm, v in times.items()}
+        result["pose_fwd_bwd_ms"][mode] = {arm: stats(v, nd=4) for arm, v in times.items()}
     del graphs
 
     # ---- device time per kernel (profiler run of its own) ----
@@ -174,25 +150,18 @@ def main():
         for x in leaves:
             x.grad = None
 
+    def window(arm):
+        for i in range(a.frames):
+            frame(arm, i)
+
     for arm in ARMS:
         for i in range(5):
             frame(arm, i)
-    torch.cuda.synchronize()
-    fps = {arm: [] for arm in ARMS}
-    for _ in range(a.rounds):
-        for arm in ARMS:
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            for i in range(a.frames):
-                frame(arm, i)
-            torch.cuda.synchronize()
-            fps[arm].append(a.frames / (time.perf_counter() - t0))
+    # one call per window: each window walks the cameras from the first
+    windows = alternate({arm: partial(window, arm) for arm in ARMS}, 1, a.rounds, 0)
     assert not any(f.overflowed() for f in frs.values())
-    result["frame_fps"]["use_graph"] = {arm: stats(v) for arm, v in fps.items()}
-    print(json.dumps(result))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(result, f, indent=1)
+    result["frame_fps"]["use_graph"] = {arm: stats([a.frames / s for s in v], nd=4) for arm, v in windows.items()}
+    emit(result, a.json)
 
 
 if __name__ == "__main__":

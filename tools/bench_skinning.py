@@ -13,7 +13,9 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 
+from benchkit import cuda_device, graph_replay  # noqa: E402
 from exavatar_release_b200 import rasterizer as RZ  # noqa: E402
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
 from exavatar_release_b200.renderer import lbs_reference, render_settings  # noqa: E402
@@ -27,7 +29,7 @@ def main():
     ap.add_argument("--iters", type=int, default=30)
     a = ap.parse_args()
     wl = WORKLOADS[a.workload]
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_skinning")
     H, W = wl.height, wl.width
     _, human, _ = make_population_assets(a.workload, seed=0, device=dev)
     P, J = human["mean_3d"].shape[0], 55
@@ -70,7 +72,7 @@ def main():
             fn(lv)
         torch.cuda.synchronize()
 
-        def timed(run):
+        def event_ms(run):
             ms = 0.0
             for _ in range(a.iters):
                 flush.zero_()
@@ -87,25 +89,15 @@ def main():
                 v.grad = None
             fn(lv)
 
-        out[name] = timed(eager)
+        out[name] = event_ms(eager)
         # the same work captured in a CUDA graph: removes the host cost of the extra PyTorch launches from the picture.
         # Fresh leaves: the gradient-accumulation nodes of the eager ones belong to the default stream, which a capture
         # may not wait on.
         lv = leaves()
-        side = torch.cuda.Stream(dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            eager()
-        torch.cuda.current_stream(dev).wait_stream(side)
+        replay = graph_replay(eager, 1)
+        replay()
         torch.cuda.synchronize()
-        for v in lv.values():
-            v.grad = None
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            fn(lv)
-        g.replay()
-        torch.cuda.synchronize()
-        out_graph[name] = timed(g.replay)
+        out_graph[name] = event_ms(replay)
     assert not RZ.overflowed()
     print(f"{a.workload}: human population P={P}, J={J}, {W}x{H}; forward+backward through the public API")
     for tag, o in (("eager", out), ("CUDA graph", out_graph)):

@@ -13,19 +13,15 @@ of a seeded weighted sum of the mesh.  Arms:
   2. op:        `SmplxRig.body_mesh`, eager;
   3. op_graph:  arm 2 captured once in a CUDA graph and replayed.
 Arms alternate window by window in one process (host clock around N calls + device sync): median (min-max).  Host
-syncs per call are counted under torch.cuda.set_sync_debug_mode("warn"); device time and launches per call come from a
+syncs per call are counted with torch's sync debug mode ("warn"); device time and launches per call come from a
 separate torch.profiler run, which also lists the op's kernels one by one.  The op's algorithmic bytes (the model
 tables it must read and the mesh I/O, from shapes) are reported over its kernels' device time as a share of the H100's
-3.35 TB/s data-sheet bandwidth.  Finally C4 training frames/s of tools/bench_smplx_rig.py's frame with the body mesh
-computed every frame in ExAvatar's form (mesh_exavatar), by the op (mesh_op) and not at all (mesh_none).  Prints the card name and power limit with the numbers.
+3.35 TB/s data-sheet bandwidth.  Finally C4 training frames/s of tools/c4_frame.py's frame with the body mesh computed
+every frame in ExAvatar's form (mesh_exavatar), by the op (mesh_op) and not at all (mesh_none).  Prints the card name
+and power limit with the numbers.
 """
-import argparse
-import json
 import os
-import statistics
 import sys
-import time
-import warnings
 
 import torch
 
@@ -33,12 +29,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_frame_sh import card  # noqa: E402
-from bench_smplx_rig import frames_per_second  # noqa: E402
+from benchkit import (HBM_BYTES_PER_S, alternate, arg_parser, card, cuda_device, emit, graph_replay,  # noqa: E402
+                      host_syncs, kernel_events, stats)
+from c4_frame import FrameArm, frames_per_second  # noqa: E402
 from exavatar_release_b200.smplx_rig import SmplxRig, batch_rodrigues, smplx_body_reference  # noqa: E402
 from exavatar_release_b200.synthetic import make_human_mesh, make_smplx_model  # noqa: E402
-
-HBM_BYTES_PER_S = 3.35e12  # H100 SXM data sheet
 
 
 def device_model(rig):
@@ -62,15 +57,8 @@ def algorithmic_bytes(rig):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=50, help="calls per timed window")
-    ap.add_argument("--rounds", type=int, default=5)
-    ap.add_argument("--frames", type=int, default=10, help="training frames per timed window")
-    ap.add_argument("--json", default=None)
-    a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_smplx_body: needs a CUDA device (there is no CPU measurement)")
-    dev = torch.device("cuda:0")
+    a = arg_parser(__doc__, iters=50, frames=10).parse_args()
+    dev = cuda_device("bench_smplx_body")
     rig = SmplxRig(**make_smplx_model(make_human_mesh()), device=dev)
     dm = device_model(rig)
     g = torch.Generator().manual_seed(0)
@@ -106,66 +94,25 @@ def main():
         agree = {k: float((fn().double() - ref64).abs().max()) for k, fn in (("exavatar", exavatar), ("op", op))}
         agree["max_abs"] = float(ref64.abs().max())
 
-    graphs = {}
-    for mode, wrap in (("fwd", fwd), ("fwd_bwd", fwd_bwd)):
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(2):
-                wrap(op)()
-        torch.cuda.current_stream().wait_stream(s)
-        gr = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(gr):
-            wrap(op)()
-        graphs[mode] = gr
+    modes = (("fwd", fwd), ("fwd_bwd", fwd_bwd))
+    graphs = {mode: graph_replay(wrap(op), 2) for mode, wrap in modes}
     arms = {}
-    for mode, wrap in (("fwd", fwd), ("fwd_bwd", fwd_bwd)):
+    for mode, wrap in modes:
         arms[f"exavatar_{mode}"] = wrap(exavatar)
         arms[f"op_{mode}"] = wrap(op)
-        arms[f"op_graph_{mode}"] = graphs[mode].replay
-    for fn in arms.values():
-        for _ in range(3):
-            fn()
-    torch.cuda.synchronize()
-    times = {k: [] for k in arms}
-    for _ in range(a.rounds):
-        for k, fn in arms.items():
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            for _ in range(a.iters):
-                fn()
-            torch.cuda.synchronize()
-            times[k].append((time.perf_counter() - t0) / a.iters * 1e3)
-
-    syncs = {}
-    for k in arms:
-        if "graph" in k:
-            continue
-        torch.cuda.synchronize()
-        with warnings.catch_warnings(record=True) as caught:
-            warnings.simplefilter("always")
-            torch.cuda.set_sync_debug_mode("warn")
-            try:
-                arms[k]()
-            finally:
-                torch.cuda.set_sync_debug_mode(0)
-        syncs[k] = sum("synchroniz" in str(m.message).lower() for m in caught)
+        arms[f"op_graph_{mode}"] = graphs[mode]
+    times = alternate(arms, a.iters, a.rounds, 3)
+    syncs = {k: host_syncs(fn) for k, fn in arms.items() if "graph" not in k}
 
     prof = {}
-    from torch.profiler import ProfilerActivity, profile
     for k, fn in arms.items():
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as p:
-            fn()
-            torch.cuda.synchronize()
-        ev = [e for e in p.events() if e.device_type.name == "CUDA" and "Memcpy" not in e.name
-              and "Memset" not in e.name]
+        ev, prof[k] = kernel_events(fn)
         own = {}
         for e in ev:
             if e.name.startswith("b2r::"):
                 name = e.name.split("(")[0][len("b2r::"):]
                 own[name] = own.get(name, 0.0) + e.device_time / 1e3
-        prof[k] = {"device_ms": sum(e.device_time for e in ev) / 1e3, "launches": len(ev), "op_kernels_ms": own}
+        prof[k]["op_kernels_ms"] = own
 
     nbytes = algorithmic_bytes(rig)
     bw = {}
@@ -182,18 +129,15 @@ def main():
         return smplx_body_reference(models[id(r)], beta, jo, pose, expr, trans, cam_R, cam_t, dtype=torch.float32,
                                     device=dev)
 
-    meshes = {"mesh_exavatar": mesh_exavatar,
-              "mesh_op": lambda r, *ins: r.body_mesh(*ins),
-              "mesh_none": lambda *ins: None}
+    meshes = {"mesh_exavatar": FrameArm(mesh=mesh_exavatar),
+              "mesh_op": FrameArm(mesh=lambda r, *ins: r.body_mesh(*ins)),
+              "mesh_none": FrameArm(mesh=lambda *ins: None)}
     res = {"card": card(), "V": rig.V, "J": rig.J,
-           "ms": {k: {"median": statistics.median(v), "min": min(v), "max": max(v)} for k, v in times.items()},
+           "ms": {k: stats(v, 1e3) for k, v in times.items()},
            "host_syncs_per_call": syncs, "profile": prof, "algorithmic_bytes": nbytes, "op_bandwidth": bw,
            "max_abs_error_vs_float64": agree,
-           "frames_per_s": frames_per_second(a, dev, meshes=meshes)}
-    print(json.dumps(res, indent=1))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(res, f, indent=1)
+           "frames_per_s": frames_per_second(a, dev, meshes)}
+    emit(res, a.json)
 
 
 if __name__ == "__main__":
