@@ -2,7 +2,8 @@
 
 Public surface (mirrors what /root/reference/avatar/common/nets/module.py:11 imports):
     GaussianRasterizationSettings, GaussianRasterizer
-plus the host-side mirror of the caller (`GaussianRenderer`, module.py:588-647), `TrainingFrameRenderer` (the five
+plus the host-side mirror of the caller (`GaussianRenderer`, module.py:588-647), `device_render_settings` (its render
+settings computed on the device from a CUDA camera, no host read), `TrainingFrameRenderer` (the five
 renders of a training frame, avatar/main/model.py:117-162, as one autograd call), `skin_gaussians` (both human sets
 posed by one rig), `l1_ssim` (the L1 + SSIM terms of the loss block, model.py:196-215), `nearest_rows` and
 `VertexNormals` (the nearest-vertex rows and mesh normals in front of the posing, module.py:501-504,541-546),
@@ -15,7 +16,7 @@ module.py:673-684), `HumanAssets` (HumanGaussian's geometry and colour code arou
 and model.py:92-96), synthetic workloads and the frame-sharding helper used by bench.py.
 """
 from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians  # noqa: F401
-from .renderer import GaussianRenderer, render_settings  # noqa: F401
+from .renderer import GaussianRenderer, device_render_settings, render_settings  # noqa: F401
 from .skinning import skin_gaussians  # noqa: F401
 from .losses import l1_ssim  # noqa: F401
 from .geometry import VertexNormals, nearest_rows  # noqa: F401
@@ -36,6 +37,6 @@ def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loa
 
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "GaussianRenderer",
-           "render_settings", "TrainingFrameRenderer", "skin_gaussians", "l1_ssim", "nearest_rows", "VertexNormals",
+           "render_settings", "device_render_settings", "TrainingFrameRenderer", "skin_gaussians", "l1_ssim", "nearest_rows", "VertexNormals",
            "FaceMeshRenderer", "HumanRegularizers", "SmplxRig", "cat_full_pose", "Adam",
            "scene_assets", "LPIPS", "decode_smplx_pose", "HumanAssets"]

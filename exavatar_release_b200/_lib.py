@@ -26,6 +26,8 @@ class B2RScene(C.Structure):
         ("P", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("sh_degree", C.c_int32),
         ("sh_coeffs", C.c_int32), ("flags", C.c_uint32),
         ("scale_modifier", C.c_float), ("tanfovx", C.c_float), ("tanfovy", C.c_float),
+        # (2) device tan(fov_x / 2), tan(fov_y / 2), or NULL (a zeroed struct): the by-value floats above are used
+        ("tanfov", _fp),
         ("bg", _fp), ("viewmatrix", _fp), ("projmatrix", _fp), ("campos", _fp),
         ("means3D", _fp), ("shs", _fp), ("colors_precomp", _fp), ("opacities", _fp),
         ("scales", _fp), ("rotations", _fp), ("cov3D_precomp", _fp),
@@ -248,6 +250,7 @@ SYMBOLS = [
     ("b2r_forward", C.c_int, [C.POINTER(B2RScene), C.POINTER(B2RWorkspace), C.POINTER(B2RForwardOutputs), _fp]),
     ("b2r_backward", C.c_int, [C.POINTER(B2RScene), C.POINTER(B2RWorkspace), C.POINTER(B2RBackwardArgs), _fp,
                                C.c_size_t, _fp]),
+    ("b2r_camera_setup", C.c_int, [_fp, _fp, _fp, C.c_int32, C.c_int32, _fp, _fp]),
     ("b2r_mark_visible", C.c_int, [C.c_int32, _fp, _fp, _fp, _fp]),
     ("b2r_skin_forward", C.c_int, [C.POINTER(B2RSkin), _fp]),
     ("b2r_skin_backward", C.c_int, [C.POINTER(B2RSkin), C.POINTER(_fp), C.POINTER(_fp), _fp, _fp, _fp, C.c_size_t, _fp]),

@@ -47,10 +47,13 @@ NVCC_FLAGS = [
 # fp32 expressions rounded operation by operation, so the mask agrees with torch's at equality.
 # human_assets.cu: every forward output is ExAvatar's fp32 torch expression rounded operation by operation (the mask
 # multiplies, exp / tanh as torch's kernels call them), bit-identical to it.
+# camera.cu: the camera block restates torch's fp32 expressions (reciprocal, atanf, tanf) and the fp32 sums of torch.mm
+# operation by operation.
 PER_FILE_FLAGS = {"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
                   "geometry.cu": ["--fmad=false"], "mesh_raster.cu": ["--fmad=false"],
                   "regularizers.cu": ["--fmad=false"], "smplx_rig.cu": ["--fmad=false"], "adam.cu": ["--fmad=false"],
-                  "scene_assets.cu": ["--fmad=false"], "human_assets.cu": ["--fmad=false"]}
+                  "scene_assets.cu": ["--fmad=false"], "human_assets.cu": ["--fmad=false"],
+                  "camera.cu": ["--fmad=false"]}
 
 
 def sources():

@@ -10,7 +10,8 @@ int validate_scene(const B2RScene* sc) {
   if (sc->P < 0 || sc->width <= 0 || sc->height <= 0) return B2R_E_INVALID;
   if (sc->P >= (1 << 29)) return B2R_E_INVALID;  // the splat record carries id in 29 bits (common.cuh Geom)
   if (sc->width > 65535 * TILE || sc->height > 32767 * TILE) return B2R_E_INVALID;
-  if (!(sc->tanfovx > 0.f) || !(sc->tanfovy > 0.f)) return B2R_E_INVALID;
+  // a device tan(fov) is checked by the kernels that read it (gaussian_math.cuh load_cam)
+  if (!sc->tanfov && (!(sc->tanfovx > 0.f) || !(sc->tanfovy > 0.f))) return B2R_E_INVALID;
   if (!sc->bg || !sc->viewmatrix || !sc->projmatrix || !sc->campos) return B2R_E_INVALID;
   if (sc->sh_rows < 0 || sc->sh_rows > sc->P) return B2R_E_INVALID;
   if (sc->P > 0) {
@@ -711,6 +712,12 @@ int b2r_human_colors_backward(int32_t P, const float* rgb, const float* rgb_offs
   if (P < 0 || (P > 0 && (!rgb || !rgb_offset || !dL_drgb || !dL_drgb_offset))) return B2R_E_INVALID;
   return launch_human_colors_backward(P, rgb, rgb_offset, dL_drgb_out, dL_drgb_refined, dL_drgb, dL_drgb_offset,
                                       (cudaStream_t)stream);
+}
+
+int b2r_camera_setup(const float* R, const float* t, const float* focal, int32_t width, int32_t height, float* out,
+                     void* stream) {
+  if (!R || !t || !focal || !out || width <= 0 || height <= 0) return B2R_E_INVALID;
+  return launch_camera_setup(R, t, focal, width, height, out, (cudaStream_t)stream);
 }
 
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream) {

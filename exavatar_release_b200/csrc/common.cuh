@@ -609,6 +609,7 @@ int launch_human_geometry_backward(const B2RHumanAssets& h, const B2RHumanAssets
 int launch_human_colors_forward(int P, const float* rgb, const float* off, float* out, float* out_r, cudaStream_t st);
 int launch_human_colors_backward(int P, const float* rgb, const float* off, const float* g, const float* g_r,
                                  float* d_rgb, float* d_off, cudaStream_t st);
+int launch_camera_setup(const float* R, const float* t, const float* focal, int W, int H, float* out, cudaStream_t st);
 
 // RAII bracket around one kernel launch: counts it and, when profiling is on, records CUDA events around it.
 enum KernelId { K_PROJECT = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_LARGE, K_COMPOSITE_FWD, K_COMPOSITE_BWD,

@@ -11,8 +11,15 @@ struct Cam {
   float campos[3];
   float fx, fy, tanfovx, tanfovy;
   int W, H;
+  bool valid;  // false: the device tan(fov) is not finite and > 0 -- the projection culls every Gaussian
 };
 
+// The one place the projection kernels read tan(fov): B2RScene.tanfov on the device when set, the by-value floats
+// otherwise (checked > 0 on the host).  The host cannot check a device value, so one that is not finite and > 0 marks
+// the camera invalid instead (the forward projection then culls every Gaussian, and nothing is visible to the backward).
+// DEVICE_TANFOV = false compiles the by-value read alone: the forward projection kernel is instantiated both ways,
+// because at its 64-register budget two loaded floats in place of two kernel parameters would spill.
+template <bool DEVICE_TANFOV = true>
 __device__ __forceinline__ Cam load_cam(const B2RScene& sc) {
   Cam c;
 #pragma unroll
@@ -26,8 +33,15 @@ __device__ __forceinline__ Cam load_cam(const B2RScene& sc) {
   c.H = sc.height;
   c.tanfovx = sc.tanfovx;
   c.tanfovy = sc.tanfovy;
-  c.fx = (float)sc.width / (2.f * sc.tanfovx);
-  c.fy = (float)sc.height / (2.f * sc.tanfovy);
+  c.valid = true;
+  if (DEVICE_TANFOV && sc.tanfov) {
+    const float tx = __ldg(sc.tanfov), ty = __ldg(sc.tanfov + 1);
+    c.valid = tx > 0.f && tx < INFINITY && ty > 0.f && ty < INFINITY;
+    c.tanfovx = tx;
+    c.tanfovy = ty;
+  }
+  c.fx = (float)sc.width / (2.f * c.tanfovx);
+  c.fy = (float)sc.height / (2.f * c.tanfovy);
   return c;
 }
 

@@ -54,8 +54,11 @@ __device__ __forceinline__ void sh_to_rgb(int deg, const float* __restrict__ sh,
 #endif
 // MIXED (B2RScene.sh_rows > 0): rows [0, sh_rows) take their colour from `shs`, the rest from `colors_precomp`.  A
 // separate instantiation, so the single-source kernel stays the code it was.
-template <bool MIXED>
-__global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2RScene sc, const Ctx cx, int32_t* __restrict__ radii,
+// DEVICE_TANFOV (B2RScene.tanfov set): tan(fov) and the focal lengths derived from it are loaded values instead of
+// kernel parameters, which the 64-register budget cannot hold without spilling; that instantiation runs with one CTA
+// per SM less (80 registers).  The by-value instantiations are the code they were.
+template <bool MIXED, bool DEVICE_TANFOV>
+__global__ void __launch_bounds__(256, DEVICE_TANFOV ? PROJ_MIN_BLOCKS - 1 : PROJ_MIN_BLOCKS) project_kernel(const B2RScene sc, const Ctx cx, int32_t* __restrict__ radii,
                                                       const int aggregate, const int first_row) {
   // CTA-level histogram in shared memory: atomics of different warps to the SAME global address serialise in L2
   // (the hot avatar tiles receive thousands), so each CTA adds to a tile's counter at most once.
@@ -79,7 +82,7 @@ __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2R
     __syncwarp();
     shrow = wstage + lane * S;
   }
-  const Cam cam = load_cam(sc);
+  const Cam cam = load_cam<DEVICE_TANFOV>(sc);
   bool visible = false;
   Geom g;
   g.g0 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -90,7 +93,7 @@ __global__ void __launch_bounds__(256, PROJ_MIN_BLOCKS) project_kernel(const B2R
     const float3 p = make_float3(__ldg(sc.means3D + 3 * (size_t)i), __ldg(sc.means3D + 3 * (size_t)i + 1),
                                  __ldg(sc.means3D + 3 * (size_t)i + 2));
     const float3 pv = xform4x3(p, cam.v);
-    if (pv.z > K_NEAR) {  // App. A.1 step 1
+    if (cam.valid && pv.z > K_NEAR) {  // App. A.1 step 1; an invalid device tan(fov) culls every Gaussian
       // Homogeneous position and pixel centre WITHOUT fma contraction, operation for operation as the oracle's C
       // expression (App. A.1 steps 2, 7).  One ulp of a pixel coordinate near 1000 is 6e-5 px; through a sharp splat's
       // exponent that is a 1e-4 relative change of alpha, enough to flip alpha >= 1/255 decisions the oracle's threshold
@@ -387,7 +390,8 @@ int launch_project(const B2RScene& sc, const Ctx& cx, int32_t* radii, cudaStream
     const int aggregate = cx.tiles <= 2048;  // beyond that the per-CTA sweeps over the tile table cost more than they save
     const size_t smem = (aggregate ? (size_t)cx.tiles * 4 : 0) +
                         (sc.shs ? (size_t)8 * 32 * ((sc.sh_coeffs * 3) | 1) * sizeof(float) : 0);
-    auto kern = sc.sh_rows > 0 ? project_kernel<true> : project_kernel<false>;
+    auto kern = sc.tanfov ? (sc.sh_rows > 0 ? project_kernel<true, true> : project_kernel<false, true>)
+                          : (sc.sh_rows > 0 ? project_kernel<true, false> : project_kernel<false, false>);
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);  // per device
     launch_k(kern, (sc.P - first_row + 255) / 256, 256, smem, st, true, sc, cx, radii, aggregate, first_row);
   }

@@ -105,13 +105,22 @@ at::Tensor f32c(const at::Tensor& t, const char* name) {
   TORCH_CHECK(t.is_cuda(), "b200raster: `", name, "` must be a CUDA tensor (got ", t.device(), "); there is no CPU fallback");
   return (t.scalar_type() == at::kFloat ? t : t.to(at::kFloat)).contiguous();
 }
+// The device tan(fov) pair: two contiguous fp32 values on the render's device.  Checked by shape only -- its values are
+// never read on the host (the kernels cull everything when they are not finite and > 0).
+at::Tensor device_tanfov(const at::Tensor& t, const c10::Device& dev) {
+  TORCH_CHECK(t.is_cuda() && t.device() == dev, "b200raster: `tanfov` must be a CUDA tensor on the render's device");
+  TORCH_CHECK(t.scalar_type() == at::kFloat && t.numel() == 2 && t.is_contiguous(),
+              "b200raster: `tanfov` must be 2 contiguous float32 values");
+  return t;
+}
 bool present(const c10::optional<at::Tensor>& t) { return t.has_value() && t->defined() && t->numel() > 0; }
 const float* fptr(const at::Tensor& t) { return t.defined() && t.numel() > 0 ? t.data_ptr<float>() : nullptr; }
 
 B2RScene make_scene(int64_t P, int64_t H, int64_t W, int64_t sh_degree, uint32_t flags, double scale_modifier, double tanfovx,
                     double tanfovy, const at::Tensor& bg, const at::Tensor& view, const at::Tensor& proj,
                     const at::Tensor& campos, const at::Tensor& means3D, const at::Tensor& shs, const at::Tensor& colors,
-                    const at::Tensor& opac, const at::Tensor& scales, const at::Tensor& rots, const at::Tensor& cov) {
+                    const at::Tensor& opac, const at::Tensor& scales, const at::Tensor& rots, const at::Tensor& cov,
+                    const at::Tensor& tanfov) {
   B2RScene sc{};
   sc.P = (int32_t)P;
   sc.width = (int32_t)W;
@@ -122,6 +131,7 @@ B2RScene make_scene(int64_t P, int64_t H, int64_t W, int64_t sh_degree, uint32_t
   sc.scale_modifier = (float)scale_modifier;
   sc.tanfovx = (float)tanfovx;
   sc.tanfovy = (float)tanfovy;
+  sc.tanfov = fptr(tanfov);  // device tan(fov) (2), never read on the host; undefined: the floats above
   sc.bg = fptr(bg);
   sc.viewmatrix = fptr(view);
   sc.projmatrix = fptr(proj);
@@ -145,7 +155,7 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
                                int64_t W, double tanfovx, double tanfovy, const at::Tensor& bg_in, double scale_modifier,
                                const at::Tensor& view_in, const at::Tensor& proj_in, int64_t sh_degree,
                                const at::Tensor& campos_in, bool speculative, double headroom, int64_t fixed_capacity,
-                               bool debug) {
+                               bool debug, const c10::optional<at::Tensor>& tanfov_in) {
     const bool need_grad = means3D_in.requires_grad() || means2D.requires_grad() || (present(sh_in) && sh_in->requires_grad()) ||
                            (present(colors_in) && colors_in->requires_grad()) || opac_in.requires_grad() ||
                            (present(scales_in) && scales_in->requires_grad()) ||
@@ -178,9 +188,10 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
     }
     const at::Tensor bg = f32c(bg_in.to(dev), "bg"), view = f32c(view_in.to(dev), "viewmatrix");
     const at::Tensor proj = f32c(proj_in.to(dev), "projmatrix"), campos = f32c(campos_in.to(dev), "campos");
+    const at::Tensor tanfov = tanfov_in.has_value() && tanfov_in->defined() ? device_tanfov(*tanfov_in, dev) : at::Tensor();
     const uint32_t flags = debug ? B2R_FLAG_DEBUG : 0u;
     const B2RScene sc = make_scene(P, H, W, sh_degree, flags, scale_modifier, tanfovx, tanfovy, bg, view, proj, campos,
-                                   means3D, shs, colors, opac, scales, rots, cov);
+                                   means3D, shs, colors, opac, scales, rots, cov, tanfov);
     const size_t ctx_bytes = b2r_ctx_bytes((int32_t)P, (int32_t)W, (int32_t)H);
     at::Tensor ctx_buf = at::empty({(int64_t)ctx_bytes}, u8);
     B2RForwardOutputs out{color.data_ptr<float>(), depth.data_ptr<float>(), alpha.data_ptr<float>(), radii.data_ptr<int32_t>()};
@@ -241,7 +252,7 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
     }
     sync_if_debug(flags, stream, "b2r_forward");
     // what must survive until backward (SURVEY.md section 8b "Ownership"); undefined tensors are saved as such
-    ctx->save_for_backward({means3D, shs, colors, opac, scales, rots, cov, bg, view, proj, campos, ctx_buf, ids, ck});
+    ctx->save_for_backward({means3D, shs, colors, opac, scales, rots, cov, bg, view, proj, campos, ctx_buf, ids, ck, tanfov});
     ctx->saved_data["H"] = H;
     ctx->saved_data["W"] = W;
     ctx->saved_data["tanfovx"] = tanfovx;
@@ -255,8 +266,8 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
   }
 
   static variable_list backward(AutogradContext* ctx, variable_list grads) {
-    // one entry per forward argument: 8 tensors, then 14 settings
-    variable_list out(22);
+    // one entry per forward argument: 8 tensors, then 15 settings
+    variable_list out(23);
     at::Tensor g_color = grads[0], g_depth = grads[2], g_alpha = grads[3];
     if (!g_color.defined() && !g_depth.defined() && !g_alpha.defined()) return out;
     const int64_t P = ctx->saved_data["P"].toInt();
@@ -277,7 +288,7 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
     const auto sv = ctx->get_saved_variables();
     const at::Tensor &means3D = sv[0], &shs = sv[1], &colors = sv[2], &opac = sv[3], &scales = sv[4], &rots = sv[5],
                      &cov = sv[6], &bg = sv[7], &view = sv[8], &proj = sv[9], &campos = sv[10], &ctx_buf = sv[11],
-                     &ids = sv[12], &ck = sv[13];
+                     &ids = sv[12], &ck = sv[13], &tanfov = sv[14];
     const int64_t H = ctx->saved_data["H"].toInt(), W = ctx->saved_data["W"].toInt();
     const auto dev = means3D.device();
     c10::cuda::CUDAGuard guard(dev);
@@ -285,7 +296,7 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
     const B2RScene sc = make_scene(P, H, W, ctx->saved_data["sh_degree"].toInt(), (uint32_t)ctx->saved_data["flags"].toInt(),
                                    ctx->saved_data["scale_modifier"].toDouble(), ctx->saved_data["tanfovx"].toDouble(),
                                    ctx->saved_data["tanfovy"].toDouble(), bg, view, proj, campos, means3D, shs, colors, opac,
-                                   scales, rots, cov);
+                                   scales, rots, cov, tanfov);
     const auto f32 = means3D.options().dtype(at::kFloat);
     const int64_t M = sc.sh_coeffs;
     at::Tensor d_means3D = at::empty({P, 3}, f32), d_means2D = at::empty({P, 3}, f32), d_colors = at::empty({P, 3}, f32);
@@ -334,9 +345,9 @@ std::vector<at::Tensor> rasterize(const at::Tensor& means3D, const at::Tensor& m
                                   const c10::optional<at::Tensor>& cov, int64_t H, int64_t W, double tanfovx, double tanfovy,
                                   const at::Tensor& bg, double scale_modifier, const at::Tensor& view, const at::Tensor& proj,
                                   int64_t sh_degree, const at::Tensor& campos, bool speculative, double headroom,
-                                  int64_t fixed_capacity, bool debug) {
+                                  int64_t fixed_capacity, bool debug, const c10::optional<at::Tensor>& tanfov) {
   return RasterizeFn::apply(means3D, means2D, sh, colors, opac, scales, rots, cov, H, W, tanfovx, tanfovy, bg, scale_modifier,
-                            view, proj, sh_degree, campos, speculative, headroom, fixed_capacity, debug);
+                            view, proj, sh_degree, campos, speculative, headroom, fixed_capacity, debug, tanfov);
 }
 
 // ---- optim.Adam's step: the walk over the param groups, the state, the scalars and the segment table ----------------
@@ -467,7 +478,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return std::make_tuple(ok, row_len, row_stride);
   }, "(representable, row_len, row_stride) of a param for the Adam step");
   m.def("rasterize", &rasterize, "GaussianRasterizer forward with autograd (compiled host path over libb200raster.so); "
-        "fixed_capacity < 0: adaptive duplicate capacity");
+        "fixed_capacity < 0: adaptive duplicate capacity; tanfov: (2) device tan(fov) in place of tanfovx / tanfovy",
+        py::arg("means3D"), py::arg("means2D"), py::arg("sh"), py::arg("colors"), py::arg("opac"), py::arg("scales"),
+        py::arg("rots"), py::arg("cov"), py::arg("H"), py::arg("W"), py::arg("tanfovx"), py::arg("tanfovy"), py::arg("bg"),
+        py::arg("scale_modifier"), py::arg("view"), py::arg("proj"), py::arg("sh_degree"), py::arg("campos"),
+        py::arg("speculative"), py::arg("headroom"), py::arg("fixed_capacity"), py::arg("debug"),
+        py::arg("tanfov") = py::none());
   m.def("abi_version", []() { return b2r_abi_version(); });
   m.def("recent_contexts", []() {  // ctx buffers of the recent fixed-capacity calls, oldest first
     RecentContexts& r = recent();

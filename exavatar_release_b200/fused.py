@@ -28,8 +28,10 @@ One frame may be in flight per instance: run backward (or drop the outputs) befo
 copy their inputs into the plan's resident buffers (assets, camera, dL/dimage) and replay.  The Python cost of a frame
 drops from ~2.9 ms (hundreds of stream switches, ctypes calls and small copies) to a few copies and two graph launches,
 so an otherwise EAGER training loop runs the raster part at graph speed.  Kernel arguments passed by value are frozen in
-the graphs, so a change of the intrinsics (tan fov) re-captures; every render's backward runs (a render left out of the
-loss contributes zeros).
+the graphs: with float settings (`render_settings`) a change of the intrinsics (tan fov) re-captures.  Settings from
+`renderer.device_render_settings` carry tan(fov) on the device; it is copied into the resident block with the matrices
+and the graphs read it from there, so one capture per SH degree serves every camera.  Every render's backward runs (a
+render left out of the loss contributes zeros).
 """
 from __future__ import annotations
 
@@ -39,7 +41,7 @@ import torch
 from torch import nn
 
 from .plan import ASSETS, RENDERS, MergedFivePlan
-from .rasterizer import GaussianRasterizationSettings, _f32c
+from .rasterizer import GaussianRasterizationSettings, _f32c, device_tanfov
 from .renderer import render_settings
 
 _KEYS = tuple(ASSETS)
@@ -117,26 +119,28 @@ class TrainingFrameRenderer(nn.Module):
         if self.use_graph:
             dev, (H, W) = self.plan.device, self.img_shape
             # resident camera / background block the captured kernels read: view (16) | full projection (16) | campos (3) |
-            # bg (3) | bg of the human-only renders (3)
-            self._cam = torch.zeros(41, dtype=torch.float32, device=dev)
+            # bg (3) | bg of the human-only renders (3) | tan(fov_x/2), tan(fov_y/2) of device settings (2)
+            self._cam = torch.zeros(43, dtype=torch.float32, device=dev)
             self._gin = {r: torch.zeros(3, H, W, dtype=torch.float32, device=dev) for r in RENDERS}
             # dL/ddepth and dL/dalpha inputs only when asked for: their backward variant is the slower one
             self._gin_d = {r: torch.zeros(1, H, W, dtype=torch.float32, device=dev) for r in RENDERS} if graph_depth_alpha else None
             self._gin_a = {r: torch.zeros(1, H, W, dtype=torch.float32, device=dev) for r in RENDERS} if graph_depth_alpha else None
             # resident gradient buffers the captured backward writes, and their views
             self._flats, self._grad_views = self.plan.grad_buffers()
-            # (tanfovx, tanfovy, scale_modifier, densify buffers, sh_degree) -> (settings, settings_h, forward graph,
-            # backward graph)
+            # (tanfovx, tanfovy or "device", scale_modifier, densify buffers, sh_degree) -> (settings, settings_h,
+            # forward graph, backward graph)
             self._graphs = {}
             self._cur = None
 
     # ---- use_graph=True ----
     def _resident_settings(self, settings, settings_h):
         c = self._cam
+        # device settings: the captured kernels read tan(fov) from the resident block, floats stay kernel arguments
+        tx, ty = (settings.tanfovx, settings.tanfovy) if device_tanfov(settings) is None else (c[41], c[42])
         mk = lambda bg: GaussianRasterizationSettings(
-            image_height=settings.image_height, image_width=settings.image_width, tanfovx=settings.tanfovx,
-            tanfovy=settings.tanfovy, bg=bg, scale_modifier=settings.scale_modifier, viewmatrix=c[0:16].view(4, 4),
-            projmatrix=c[16:32].view(4, 4), sh_degree=0, campos=c[32:35], prefiltered=False, debug=False)
+            image_height=settings.image_height, image_width=settings.image_width, tanfovx=tx, tanfovy=ty, bg=bg,
+            scale_modifier=settings.scale_modifier, viewmatrix=c[0:16].view(4, 4), projmatrix=c[16:32].view(4, 4),
+            sh_degree=0, campos=c[32:35], prefiltered=False, debug=False)
         return mk(c[35:38]), mk(c[38:41])
 
     def _load_inputs(self, settings, settings_h, scene, human, refined):
@@ -146,6 +150,9 @@ class TrainingFrameRenderer(nn.Module):
         c[32:35].copy_(settings.campos.reshape(3))
         c[35:38].copy_(settings.bg.reshape(3))
         c[38:41].copy_(settings_h.bg.reshape(3))
+        tanfov = device_tanfov(settings)
+        if tanfov is not None:
+            c[41:43].copy_(tanfov)
         plan.load_rows(human, refined)  # set_scene already copied the scene rows into both passes
         if plan.M > 0:  # the captured kernels read the coefficients at a fixed address
             plan.use_scene_shs(scene["shs"], scene["sh_degree"], copy=True)
@@ -156,7 +163,8 @@ class TrainingFrameRenderer(nn.Module):
         dn = self.densify or {}
         # the SH degree is a kernel argument frozen in the graphs: ExAvatar raises it on a schedule (module.py:152-153),
         # so each degree is captured once and replayed afterwards
-        key = (float(settings.tanfovx), float(settings.tanfovy), float(settings.scale_modifier),
+        fov = ("device",) if device_tanfov(settings) is not None else (float(settings.tanfovx), float(settings.tanfovy))
+        key = (*fov, float(settings.scale_modifier),
                tuple(0 if dn.get(k) is None else dn[k].data_ptr() for k in ("grad_accum", "count", "radius_max")),
                plan.sh_degree if plan.M > 0 else None)
         if key not in self._graphs:
@@ -211,6 +219,8 @@ class TrainingFrameRenderer(nn.Module):
         """Asset dicts as `GaussianRenderer.forward` takes them (mean_3d, opacity, scale, rotation, rgb; the scene asset
         carries shs + sh_degree instead of rgb when the renderer was built with sh_coeffs > 0); `bg_human` is the
         background of the two human-only renders (model.py:72), `bg` of the others (white by default, module.py:592).
+        `raster_settings` (default `render_settings(cam_param)`) may come from `renderer.device_render_settings`: the
+        frame then runs from camera to loss without a device->host read.
         Returns {render name: {img, depthmap, mask, radius, is_vis[, mean_2d]}} for the five renders of plan.RENDERS."""
         sh_scene = "shs" in scene_asset and "rgb" not in scene_asset
         if sh_scene != (self.plan.M > 0):

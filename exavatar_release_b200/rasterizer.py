@@ -34,6 +34,8 @@ from . import _lib as L
 class GaussianRasterizationSettings(NamedTuple):
     image_height: int
     image_width: int
+    # Python floats (the reference's signature), or 0-dim CUDA tensors (renderer.device_render_settings): those are read
+    # by the kernels on the device and never converted on the host
     tanfovx: float
     tanfovy: float
     bg: torch.Tensor
@@ -66,9 +68,28 @@ def _f32c(t: torch.Tensor, name: str) -> torch.Tensor:
     return t.contiguous()
 
 
+def device_tanfov(settings) -> Optional[torch.Tensor]:
+    """(2) fp32 CUDA tensor (tan(fov_x / 2), tan(fov_y / 2)) of settings whose tanfovx / tanfovy are 0-dim CUDA tensors,
+    None for float settings.  Adjacent fp32 elements of one block (device_render_settings, the resident block of a
+    captured frame) are used in place; other tensors are stacked on the device.  Nothing is read on the host."""
+    tx, ty = settings.tanfovx, settings.tanfovy
+    if not isinstance(tx, torch.Tensor) and not isinstance(ty, torch.Tensor):
+        return None
+    if not (isinstance(tx, torch.Tensor) and isinstance(ty, torch.Tensor)) or tx.numel() != 1 or ty.numel() != 1:
+        raise TypeError("b200raster: tanfovx / tanfovy must both be floats or both be one-element tensors")
+    if not (tx.is_cuda and ty.is_cuda):
+        raise RuntimeError("b200raster: tensor tanfovx / tanfovy must be CUDA tensors; there is no CPU fallback")
+    if (tx.dtype == ty.dtype == torch.float32 and tx.device == ty.device and ty.data_ptr() == tx.data_ptr() + 4
+            and tx.untyped_storage().data_ptr() == ty.untyped_storage().data_ptr()):
+        return tx.as_strided((2,), (1,))
+    return torch.stack((tx.reshape(()), ty.reshape(()))).float()
+
+
 def _make_scene(settings: GaussianRasterizationSettings, means3D, shs, colors, opac, scales, rots, cov, flags):
     dev = means3D.device
+    tanfov = device_tanfov(settings)
     keep = {
+        "tanfov": None if tanfov is None else tanfov.to(dev),
         "bg": _f32c(settings.bg.to(dev), "bg"),
         "view": _f32c(settings.viewmatrix.to(dev), "viewmatrix"),
         "proj": _f32c(settings.projmatrix.to(dev), "projmatrix"),
@@ -83,8 +104,10 @@ def _make_scene(settings: GaussianRasterizationSettings, means3D, shs, colors, o
     sc.sh_coeffs = 0 if shs is None or shs.numel() == 0 else int(shs.shape[1])
     sc.flags = flags
     sc.scale_modifier = float(settings.scale_modifier)
-    sc.tanfovx = float(settings.tanfovx)
-    sc.tanfovy = float(settings.tanfovy)
+    if tanfov is None:
+        sc.tanfovx = float(settings.tanfovx)
+        sc.tanfovy = float(settings.tanfovy)
+    sc.tanfov = _ptr(keep["tanfov"])
     sc.bg = _ptr(keep["bg"])
     sc.viewmatrix = _ptr(keep["view"])
     sc.projmatrix = _ptr(keep["proj"])
@@ -148,12 +171,14 @@ def last_duplicate_count(device: torch.device, P: int, W: int, H: int) -> int:
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
     st = raster_settings
     ext = _compiled_binding()
+    tanfov = device_tanfov(st)
+    tx, ty = (float(st.tanfovx), float(st.tanfovy)) if tanfov is None else (0.0, 0.0)
     try:
         return tuple(ext.rasterize(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                                   int(st.image_height), int(st.image_width), float(st.tanfovx), float(st.tanfovy), st.bg,
+                                   int(st.image_height), int(st.image_width), tx, ty, st.bg,
                                    float(st.scale_modifier), st.viewmatrix, st.projmatrix, int(st.sh_degree), st.campos,
                                    CAPACITY_MODE == "speculative", CAPACITY_HEADROOM,
-                                   -1 if FIXED_CAPACITY is None else FIXED_CAPACITY, bool(st.debug)))
+                                   -1 if FIXED_CAPACITY is None else FIXED_CAPACITY, bool(st.debug), tanfov))
     except Exception:
         if st.debug:  # reference behaviour with debug=True: dump the arguments, re-raise
             args = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)

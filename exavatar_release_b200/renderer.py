@@ -15,6 +15,7 @@ from __future__ import annotations
 import torch
 from torch import nn
 
+from . import _lib as L
 from .camera import get_fov, get_proj_matrix, get_view_matrix
 from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer
 from .sh import sh_to_rgb
@@ -53,6 +54,32 @@ def _device_camera(img_shape, cam_param):
         _CAM_CACHE.pop(next(iter(_CAM_CACHE)))
     _CAM_CACHE[key] = (ts, out)  # `ts` held on purpose: pins the storage the key refers to
     return out
+
+
+def device_render_settings(img_shape, cam_param, bg):
+    """`render_settings` for a camera given as CUDA tensors, computed on the device: one `b2r_camera_setup` launch writes
+    a fresh 37-float block view | full projection | campos | tan(fov_x/2) | tan(fov_y/2), and the returned settings'
+    viewmatrix, projmatrix, campos and tanfovx / tanfovy (0-dim tensors) are views of it.  Nothing is read back, so a
+    new camera every frame costs no host synchronisation, and `TrainingFrameRenderer(use_graph=True)` replays one
+    captured frame for every camera.  The arithmetic is module.py:604-613's as the reference evaluates it on the device
+    (include/b200raster.h); it is not bit-equal to `render_settings`, whose host mirror evaluates atan / tan with torch's
+    CPU kernels.  R (3,3), t (3) and focal (2) are read as fp32; princpt is ignored, as in the reference."""
+    R, t, focal = cam_param["R"], cam_param["t"], cam_param["focal"]
+    if not (R.is_cuda and t.is_cuda and focal.is_cuda):
+        raise RuntimeError("device_render_settings: cam_param R, t and focal must be CUDA tensors (use render_settings "
+                           "for a CPU camera)")
+    dev = R.device
+    R, t, focal = (x.to(dev, torch.float32).contiguous() for x in (R.reshape(9), t.reshape(3), focal.reshape(2)))
+    H, W = int(img_shape[0]), int(img_shape[1])
+    block = torch.empty(37, dtype=torch.float32, device=dev)
+    lib = L.load()
+    with torch.cuda.device(dev):
+        L.check(lib.b2r_camera_setup(R.data_ptr(), t.data_ptr(), focal.data_ptr(), W, H, block.data_ptr(),
+                                     torch.cuda.current_stream(dev).cuda_stream), "b2r_camera_setup")
+    return GaussianRasterizationSettings(image_height=H, image_width=W, tanfovx=block[35], tanfovy=block[36], bg=bg,
+                                         scale_modifier=1.0, viewmatrix=block[0:16].view(4, 4),
+                                         projmatrix=block[16:32].view(4, 4), sh_degree=0, campos=block[32:35],
+                                         prefiltered=False, debug=False)
 
 
 def render_settings(img_shape, cam_param, bg, settings_cls=GaussianRasterizationSettings):

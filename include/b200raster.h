@@ -57,7 +57,13 @@ typedef struct B2RScene {
   int32_t sh_coeffs;      /* M: coefficients per Gaussian in `shs` (0 when shs == NULL) */
   uint32_t flags;         /* B2R_FLAG_* */
   float scale_modifier;
-  float tanfovx, tanfovy;
+  float tanfovx, tanfovy;     /* read only when `tanfov` is NULL; then both must be > 0 */
+  /* (2) tan(fov_x / 2), tan(fov_y / 2) on the device -- e.g. floats 35..36 of a b2r_camera_setup block -- or NULL to use
+   * tanfovx / tanfovy above.  With it the host never needs the intrinsics' values, so a frame whose camera comes as
+   * device tensors is set up and rendered without a device->host read, and a CUDA graph captured once serves every
+   * camera.  The host cannot check device values: a value that is not finite and > 0 culls every Gaussian (radii 0,
+   * background images, zero gradients) instead of faulting. */
+  const float* tanfov;
   const float* bg;            /* (3) */
   const float* viewmatrix;    /* (16) world->view, [4c+r] */
   const float* projmatrix;    /* (16) full projection (proj*view), [4c+r] */
@@ -771,11 +777,26 @@ int b2r_human_colors_forward(int32_t P, const float* rgb, const float* rgb_offse
 int b2r_human_colors_backward(int32_t P, const float* rgb, const float* rgb_offset, const float* dL_drgb_out,
                               const float* dL_drgb_refined, float* dL_drgb, float* dL_drgb_offset, void* stream);
 
+/* The render settings of one camera on the device, in one single-thread launch: what ExAvatar's GaussianRenderer
+ * derives from cam_param (avatar/common/nets/module.py:604-613 with transforms.py:38-70), without reading R, t or focal
+ * on the host.  R (3,3) row-major, t (3), focal (2) = (fx, fy), fp32, device; width / height the image size.  `out`
+ * (37 floats, device) receives
+ *   [0..15]  viewmatrix  [R t; 0 0 0 1], [4c+r]            (B2RScene.viewmatrix)
+ *   [16..31] projmatrix  view * proj summed left to right   (B2RScene.projmatrix)
+ *   [32..34] campos      -R^T t in fp64, rounded once       (B2RScene.campos)
+ *   [35..36] tan(fov_x / 2), tan(fov_y / 2)                 (B2RScene.tanfov)
+ * fov = 2 atan(W / (2 f)) as torch evaluates it on the device (reciprocal of 2 f times W, atanf); tan(fov / 2) is tanf;
+ * the projection's entries are fp64 functions of the fp32 fov (math.tan), rounded once; znear 0.01, zfar 100; the
+ * principal point is ignored, as in the reference.  A focal length of 0 or NaN yields a tan(fov / 2) that is negative
+ * (fp32 pi / 2 lies past the pole) or NaN, which the renders treat as "cull everything" (B2RScene.tanfov). */
+int b2r_camera_setup(const float* R, const float* t, const float* focal, int32_t width, int32_t height, float* out,
+                     void* stream);
+
 /* present[i] = 1 iff Gaussian i passes the near-plane test (z_view > 0.2). */
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */

@@ -103,10 +103,21 @@ class FrameArm(NamedTuple):
     scene: Optional[Callable] = None  # (scene, cam) -> the scene's asset dict; default the scene leaves
     mesh: Optional[Callable] = None   # (rig, shape_param, joint_offset, full_pose, expr, trans, cam_R, cam_t), unused
     loss: Optional[Callable] = None   # (renders, target) -> a term added to the frame's loss; default none
+    camera: Optional[Callable] = None  # (img_shape, cam, bg) -> the renderer's raster settings; default render_settings
 
 
-def frames_per_second(a, dev, arms):
+def frames_per_second(a, dev, arms, use_graph=True):
     """C4 training frames/s of each arm (name -> FrameArm), arms alternated window by window: {"frame_<name>": stats}."""
+    frame, fr = make_frame(dev, use_graph)
+    times = alternate({k: partial(frame, arm) for k, arm in arms.items()}, a.frames, a.rounds, 3)
+    if fr.overflowed():
+        raise SystemExit("c4_frame: a render overflowed its list capacity")
+    return {f"frame_{k}": stats([1 / s for s in v]) for k, v in times.items()}
+
+
+def make_frame(dev, use_graph=True):
+    """(frame, renderer): `frame(arm)` runs one C4 training frame, forward and backward, with the stages of `arm`
+    (a FrameArm); `renderer` is its TrainingFrameRenderer."""
     dr, regs, _ = regs_setup(dev)
     m, P = dr["m"], dr["P"]
     c4 = WORKLOADS["C4"]
@@ -133,7 +144,8 @@ def frames_per_second(a, dev, arms):
     bg = torch.tensor([0.3, 0.7, 0.2], device=dev)
     target = torch.rand((3, H, W), generator=torch.Generator(device=dev).manual_seed(6), device=dev)
     fr = TrainingFrameRenderer(scene["mean_3d"].shape[0], P, (H, W), dev, {"A": 8_000_000, "B": 8_000_000},
-                               use_graph=True)
+                               use_graph=use_graph)
+    white = torch.ones(3, device=dev)
     leaves = [tp, tpf, trans, *x, *lv.values()] + [p for t, hs in nets.values() for mm in [t, *hs]
                                                    for p in mm.parameters()]
 
@@ -157,7 +169,8 @@ def frames_per_second(a, dev, arms):
              "rgb": (torch.tanh(rgb) + 1) / 2, "rgb_refined": (torch.tanh(rgb + rgb_off) + 1) / 2, "joint_offset": x[1]}
         hv = dict(human, mean_3d=posed, scale=y["scale"], rgb=y["rgb"])
         rv = dict(human, mean_3d=posed_r, scale=y["scale_refined"], rgb=y["rgb_refined"])
-        o = fr(arm.scene(scene, cam) if arm.scene else lv, hv, rv, cam, bg)
+        st = arm.camera((H, W), cam, white) if arm.camera else None
+        o = fr(arm.scene(scene, cam) if arm.scene else lv, hv, rv, cam, bg, raster_settings=st)
         loss = 0
         for r in RENDERS:
             l1, ss = l1_ssim(o[r]["img"], target)
@@ -169,7 +182,4 @@ def frames_per_second(a, dev, arms):
         for v in leaves:
             v.grad = None
 
-    times = alternate({k: partial(frame, arm) for k, arm in arms.items()}, a.frames, a.rounds, 3)
-    if fr.overflowed():
-        raise SystemExit("c4_frame: a render overflowed its list capacity")
-    return {f"frame_{k}": stats([1 / s for s in v]) for k, v in times.items()}
+    return frame, fr
