@@ -7,7 +7,8 @@ settings computed on the device from a CUDA camera, no host read), `TrainingFram
 renders of a training frame, avatar/main/model.py:117-162, as one autograd call), `skin_gaussians` (both human sets
 posed by one rig), `l1_ssim` (the L1 + SSIM terms of the loss block, model.py:196-215), `nearest_rows` and
 `VertexNormals` (the nearest-vertex rows and mesh normals in front of the posing, module.py:501-504,541-546),
-`FaceMeshRenderer` (the textured face render, model.py:170-175), `HumanRegularizers` (the regulariser block,
+`FaceMeshRenderer` (the textured face render, model.py:170-175), `ShadedMeshRenderer` (the animation scripts' shaded
+SMPL-X mesh panel, utils/vis.py:73-109), `HumanRegularizers` (the regulariser block,
 model.py:217-257), `SmplxRig` (the SMPL-X rig of HumanGaussian.forward, module.py:517-518,533,537,549, and with
 `.body_mesh` the frame's body mesh of get_smplx_outputs, model.py:37-58), `Adam` (ExAvatar's optimizer
 step in one launch, base.py:83-85), `LPIPS` (the LPIPS-VGG terms, model.py:199,206), `scene_assets` (the scene
@@ -20,7 +21,7 @@ from .renderer import GaussianRenderer, device_render_settings, render_settings 
 from .skinning import skin_gaussians  # noqa: F401
 from .losses import l1_ssim  # noqa: F401
 from .geometry import VertexNormals, nearest_rows  # noqa: F401
-from .mesh_render import FaceMeshRenderer  # noqa: F401
+from .mesh_render import FaceMeshRenderer, ShadedMeshRenderer  # noqa: F401
 from .regularizers import HumanRegularizers  # noqa: F401
 from .smplx_rig import SmplxRig, cat_full_pose  # noqa: F401
 from .optim import Adam  # noqa: F401
@@ -38,5 +39,5 @@ def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loa
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "GaussianRenderer",
            "render_settings", "device_render_settings", "TrainingFrameRenderer", "skin_gaussians", "l1_ssim", "nearest_rows", "VertexNormals",
-           "FaceMeshRenderer", "HumanRegularizers", "SmplxRig", "cat_full_pose", "Adam",
+           "FaceMeshRenderer", "ShadedMeshRenderer", "HumanRegularizers", "SmplxRig", "cat_full_pose", "Adam",
            "scene_assets", "LPIPS", "decode_smplx_pose", "HumanAssets"]

@@ -265,6 +265,8 @@ SYMBOLS = [
     ("b2r_mesh_render_scratch_bytes", C.c_size_t, [C.c_int32]),
     ("b2r_mesh_render_forward", C.c_int, [C.POINTER(B2RMeshRender), _fp, _fp, _fp, C.c_size_t, _fp]),
     ("b2r_mesh_render_backward", C.c_int, [C.POINTER(B2RMeshRender), _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
+    ("b2r_mesh_shade_forward", C.c_int, [C.POINTER(B2RMeshRender), _fp, _fp, C.c_float, C.c_float, _fp, _fp,
+                                         C.c_size_t, _fp]),
     ("b2r_triplane_forward", C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     ("b2r_triplane_backward", C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp, _fp, _fp, _fp, _fp, _fp,
                                         _fp]),

@@ -1,4 +1,6 @@
 // api.cu -- the extern "C" boundary declared in include/b200raster.h.
+#include <cmath>
+
 #include "common.cuh"
 
 using namespace b2r;
@@ -131,6 +133,16 @@ int validate_mesh_render(const B2RMeshRender* m) {
     if ((int64_t)m->C * m->tex_height * m->tex_width >= ((int64_t)1 << 31)) return B2R_E_INVALID;
     if (!m->mesh || !m->faces || !m->vertex_uv || !m->face_uv || !m->texture) return B2R_E_INVALID;
   }
+  return B2R_OK;
+}
+
+// the shaded render reads the geometry, camera and keys fields only (the texture fields are ignored)
+int validate_mesh_shade(const B2RMeshRender* m) {
+  if (!m) return B2R_E_INVALID;
+  if (m->V < 0 || m->F < 0 || m->F >= (1 << 29) || m->V >= (1 << 29)) return B2R_E_INVALID;
+  if (m->width <= 0 || m->height <= 0 || (int64_t)m->width * m->height >= ((int64_t)1 << 31)) return B2R_E_INVALID;
+  if (!m->cam_R || !m->cam_t || !m->focal || !m->princpt || !m->keys) return B2R_E_INVALID;
+  if (m->F > 0 && (m->V < 1 || !m->mesh || !m->faces)) return B2R_E_INVALID;
   return B2R_OK;
 }
 
@@ -494,6 +506,16 @@ int b2r_mesh_render_backward(const B2RMeshRender* mr, const int32_t* pix_to_face
   if (mr->V > 0 && (!dL_dmesh || !mr->vf_offsets || !mr->vf_entries)) return B2R_E_INVALID;
   if (scratch_bytes < mesh_render_scratch_bytes(mr->F)) return B2R_E_WORKSPACE;
   return launch_mesh_render_backward(*mr, pix_to_face, dL_dimage, dL_dmesh, scratch, (cudaStream_t)stream);
+}
+
+int b2r_mesh_shade_forward(const B2RMeshRender* mr, const float* normals, const float* bkg, float blend,
+                           float blend_complement, float* out, void* scratch, size_t scratch_bytes, void* stream) {
+  const int rc = validate_mesh_shade(mr);
+  if (rc) return rc;
+  if (mr->F > 0 && !normals) return B2R_E_INVALID;
+  if (!bkg || !out || !scratch || !std::isfinite(blend) || !std::isfinite(blend_complement)) return B2R_E_INVALID;
+  if (scratch_bytes < mesh_render_scratch_bytes(mr->F)) return B2R_E_WORKSPACE;
+  return launch_mesh_shade_forward(*mr, normals, bkg, blend, blend_complement, out, scratch, (cudaStream_t)stream);
 }
 
 int b2r_triplane_forward(int32_t P, int32_t C, int32_t height, int32_t width, const float* planes,

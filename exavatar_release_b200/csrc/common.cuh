@@ -560,6 +560,8 @@ int launch_mesh_render_forward(const B2RMeshRender& m, float* image, int32_t* pi
                                cudaStream_t st);
 int launch_mesh_render_backward(const B2RMeshRender& m, const int32_t* pix_to_face, const float* dimage, float* dmesh,
                                 void* scratch, cudaStream_t st);
+int launch_mesh_shade_forward(const B2RMeshRender& m, const float* normals, const float* bkg, float blend,
+                              float blend_complement, float* out, void* scratch, cudaStream_t st);
 int launch_triplane_forward(int P, int C, int H, int W, const float* planes, const float* planes_face,
                             const uint8_t* is_face, const int32_t* corners, const float* weights, float* feat,
                             cudaStream_t st);

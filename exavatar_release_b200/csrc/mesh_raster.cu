@@ -12,6 +12,9 @@
 //   mr_resolve_kernel  one thread per pixel: decode the key, recompute the barycentrics with the same device function,
 //                      interpolate uv, sample the texture (ATen's bilinear expression order), write the image and the
 //                      face id, and reset the key to ~0 -- the buffer is clean for the next call (no memset node).
+//   mr_shade_kernel    (b2r_mesh_shade_forward, the animation scripts' untextured mesh panel) one thread per pixel:
+//                      decode and reset the key like the resolve, interpolate position, vertex normal and the
+//                      all-ones texture, Phong-shade with pytorch3d's default point light, composite over `bkg`.
 //   mr_face_bwd_kernel one work item per face walks its box in raster order and sums, over the pixels whose face id is
 //                      that face, dL/d(x_ndc, y_ndc, z) of its three corners (the big boxes again by the whole warp, each
 //                      lane a fixed stride, combined by a fixed shuffle tree).  Every face's 9 values are written.
@@ -410,6 +413,75 @@ __global__ void __launch_bounds__(MR_THREADS) mr_vertex_bwd_kernel(const B2RMesh
   dmesh[3 * v + 2] = out[2];
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Shaded render (b2r_mesh_shade_forward): the mesh panel of ExAvatar's animation scripts (utils/vis.py render_mesh:
+// pytorch3d's SoftPhongShader with the default PointLights, white TexturesVertex, no specular, then the host composite).
+// mr_face_kernel's coverage, then one thread per pixel.  Shading runs in the op's camera coordinates (p_c = R p + t,
+// n_c = R n) with the light at (0, -1, 0): pytorch3d's light (0, 1, 0) seen from the xy-negated frame it renders in.
+// Negating x and y is exact, so every dot product is the one pytorch3d forms.
+// ---------------------------------------------------------------------------------------------------------------------
+
+// n_c = R n, each row left to right
+__device__ __forceinline__ void mr_rotate(const MRCam& c, float X, float Y, float Z, float& xc, float& yc, float& zc) {
+  xc = c.R[0] * X + c.R[1] * Y + c.R[2] * Z;
+  yc = c.R[3] * X + c.R[4] * Y + c.R[5] * Z;
+  zc = c.R[6] * X + c.R[7] * Y + c.R[8] * Z;
+}
+
+__global__ void __launch_bounds__(MR_THREADS) mr_shade_kernel(const B2RMeshRender m, const MRFace* __restrict__ recs,
+                                                              const float* __restrict__ normals,
+                                                              const float* __restrict__ bkg, const float blend,
+                                                              const float blend_c, float* __restrict__ out) {
+  const int p = blockIdx.x * MR_THREADS + threadIdx.x;
+  const int N = m.width * m.height;
+  if (p >= N) return;
+  const uint64_t key = m.keys[p];
+  m.keys[p] = ~0ull;
+  float c = 1.f;       // softmax_rgb_blend's white background where no face covers the pixel
+  float is_bkg = 1.f;  // vis.py: zbuf <= 0, and zbuf is -1 where no face covers the pixel
+  if (key != ~0ull) {
+    const int f = (int)(uint32_t)key;
+    if (__uint_as_float((uint32_t)(key >> 32)) > 0.f) is_bkg = 0.f;
+    const int col = p % m.width, r = p / m.width;
+    MRBary o;
+    mr_bary(recs[f], mr_pix_ndc(m.width - 1 - col, m.width, m.height), mr_pix_ndc(m.height - 1 - r, m.height, m.width),
+            o);
+    const MRCam cam = mr_load_cam(m);
+    // interpolate_face_attributes: position, normal and the all-ones texture, corners in order 0, 1, 2
+    float P[3], Nv[3], texel = 0.f;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+      const int v = m.faces[3 * f + k];
+      float q[3], n[3];
+      mr_to_cam(cam, m.mesh[3 * v], m.mesh[3 * v + 1], m.mesh[3 * v + 2], q[0], q[1], q[2]);
+      mr_rotate(cam, normals[3 * v], normals[3 * v + 1], normals[3 * v + 2], n[0], n[1], n[2]);
+#pragma unroll
+      for (int i = 0; i < 3; i++) {
+        P[i] = k ? P[i] + o.b[k] * q[i] : o.b[k] * q[i];
+        Nv[i] = k ? Nv[i] + o.b[k] * n[i] : o.b[k] * n[i];
+      }
+      texel = k ? texel + o.b[k] : o.b[k];
+    }
+    // _apply_lighting: F.normalize(normal), F.normalize(light - point), relu of their dot product
+    const float d[3] = {0.f - P[0], -1.f - P[1], 0.f - P[2]};
+    const float nl = fmaxf(sqrtf(Nv[0] * Nv[0] + Nv[1] * Nv[1] + Nv[2] * Nv[2]), 1e-6f);
+    const float dl = fmaxf(sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), 1e-6f);
+    float cosa = (Nv[0] / nl) * (d[0] / dl) + (Nv[1] / nl) * (d[1] / dl) + (Nv[2] / nl) * (d[2] / dl);
+    if (cosa < 0.f) cosa = 0.f;  // relu; a NaN stays NaN as in torch
+    // (ambient 1 * 0.5 + diffuse 1 * 0.3 * angle) * texel; the specular term is 0
+    c = (0.5f + 0.3f * cosa) * texel;
+  }
+  // vis.py:107-108 in float32, numpy's order: fg = c * blend + bkg / 255 * (1 - blend); fg (1 - is_bkg) 255 + bkg is_bkg
+  const float* bg = bkg + (size_t)3 * p;
+  float* o3 = out + (size_t)3 * p;
+#pragma unroll
+  for (int ch = 0; ch < 3; ch++) {
+    const float b = bg[ch];
+    const float fg = c * blend + (b / 255.f) * blend_c;
+    o3[ch] = (fg * (1.f - is_bkg)) * 255.f + b * is_bkg;
+  }
+}
+
 size_t mesh_render_scratch_bytes(int F) { return mr_layout(F).total; }
 
 int launch_mesh_render_forward(const B2RMeshRender& m, float* image, int32_t* pix_to_face, void* scratch,
@@ -425,6 +497,23 @@ int launch_mesh_render_forward(const B2RMeshRender& m, float* image, int32_t* pi
     ProfScope p(K_MISC, st);
     launch_k(mr_resolve_kernel, (N + MR_THREADS - 1) / MR_THREADS, MR_THREADS, 0, st, true, m, (const MRFace*)recs,
              image, pix_to_face);
+  }
+  return check_launch();
+}
+
+int launch_mesh_shade_forward(const B2RMeshRender& m, const float* normals, const float* bkg, float blend,
+                              float blend_complement, float* out, void* scratch, cudaStream_t st) {
+  const MRLayout L = mr_layout(m.F);
+  MRFace* recs = (MRFace*)((char*)scratch + L.faces);
+  if (m.F > 0) {
+    ProfScope p(K_MISC, st);
+    launch_k(mr_face_kernel, (m.F + MR_THREADS - 1) / MR_THREADS, MR_THREADS, 0, st, true, m, recs);
+  }
+  {
+    const int N = m.width * m.height;
+    ProfScope p(K_MISC, st);
+    launch_k(mr_shade_kernel, (N + MR_THREADS - 1) / MR_THREADS, MR_THREADS, 0, st, true, m, (const MRFace*)recs,
+             normals, bkg, blend, blend_complement, out);
   }
   return check_launch();
 }

@@ -34,10 +34,44 @@ restatement has not been checked against pytorch3d itself.
 
 `face_render_reference` is the literal torch restatement of 1-6 (float32 or float64, any device) the tests compare
 against; the product never calls it.
+
+Shaded render
+-------------
+`ShadedMeshRenderer` draws the middle panel of every video frame of ExAvatar's animation scripts (animate.py:83,
+animate_view_rot.py:98 -> `render_mesh`, avatar/common/utils/vis.py:73-109).  `render_mesh` uploads the face list,
+builds pytorch3d's `Meshes`, `PerspectiveCameras`, `MeshRasterizer(bin_size=0)`, `PointLights`, `SoftPhongShader` and
+`Materials` on every call, reads zbuf and the image back to the host and composites there.  The op runs the vertex
+normals, the coverage pass above and one shading + composite kernel on the device.  Restated from pytorch3d's
+implementation, which cannot be installed offline, so this restatement has not been checked against pytorch3d itself:
+
+  1. camera    the mesh is in camera coordinates: R = I, t = 0, only focal and princpt are read; the image size is
+               bkg's (H, W), which may be non-square.
+  2. coverage  steps 1-3 above, unchanged (bin_size=0 changes pytorch3d's speed, not its result).
+  3. normals   pytorch3d's verts_normals_packed of the xy-negated mesh equals D n, D = diag(-1, -1, 1), with n the
+               area-weighted normals of the mesh as given (b2r_vertex_normals, no flip).  Divergence: that kernel's
+               (x1 - x0) x (x2 - x0) summed per vertex in CSR order differs from pytorch3d's (v2 - v1) x (v0 - v1) and
+               float index_add in rounding only.
+  4. shading   SoftPhongShader with PointLights() (location (0, 1, 0), ambient 0.5, diffuse 0.3, specular 0.2),
+               Materials(specular 0, shininess 0) and all-ones TexturesVertex.  With b the corrected barycentrics and
+               each sum over the corners in order 0, 1, 2: P = sum b_k p_k, N = sum b_k n_k, texel = b0 + b1 + b2 (not
+               1 in fp32, and kept), c = (0.5 + 0.3 relu(N/max(|N|,1e-6) . (L - P)/max(|L - P|,1e-6))) texel.  The
+               kernel shades in ExAvatar's camera coordinates with L = (0, -1, 0): the dot product does not change
+               under D.  The specular term is 0.2 pow(., 0) 0 = 0.
+  5. blend     softmax_rgb_blend with one face per pixel (sigma = gamma = 1e-4, white background, znear 1, zfar 100)
+               gives (p c + d) / (p + d) with p >= 0.5 and d = 1e-10 while pz < 99.8, i.e. c to within an fp32
+               rounding; the op writes c.  Divergence: past depth ~99.8 pytorch3d fades the mesh towards white, which
+               needs its signed edge distance; that branch is not restated.
+  6. composite vis.py:105-108 in fp32, numpy's order: is_bkg = 1 where no face covers the pixel or pz <= 0,
+               fg = c blend + (bkg / 255) (1 - blend), out = (fg (1 - is_bkg)) 255 + bkg is_bkg, with blend and
+               (1 - blend), taken in double, rounded to fp32.  Background pixels are bkg bit for bit.
+
+`shaded_mesh_reference` restates 1-6 in torch (float32 or float64) for the tests; the product never calls it.
 """
 from __future__ import annotations
 
 import ctypes as C
+import math
+import numbers
 from typing import Dict, Optional, Tuple, Union
 
 import numpy as np
@@ -45,15 +79,16 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib as L
-from .geometry import VertexNormals
+from .geometry import NORMAL_EPS, VertexNormals
 from .rasterizer import _ptr
 
 EPS = 1e-8  # pytorch3d's kEpsilon
 
 
-def _cam_tensors(cam_param: Dict[str, torch.Tensor], device, fn: str):
+def _cam_tensors(cam_param: Dict[str, torch.Tensor], device, fn: str,
+                 keys: Tuple[Tuple[str, int], ...] = (("R", 9), ("t", 3), ("focal", 2), ("princpt", 2))):
     out = []
-    for k, n in (("R", 9), ("t", 3), ("focal", 2), ("princpt", 2)):
+    for k, n in keys:
         if k not in cam_param:
             raise ValueError(f"{fn}: cam_param has no `{k}`")
         v = cam_param[k]
@@ -116,7 +151,34 @@ def _int_table(name: str, a, fn: str) -> torch.Tensor:
     return t
 
 
-class FaceMeshRenderer:
+class _CoverageTables:
+    """What both mesh renderers hand to the coverage pass of csrc/mesh_raster.cu: the int32 face table and its CSR (a
+    `VertexNormals` in `self.topology`), the sizes, and the per-pixel key buffer its calls leave clean."""
+
+    def _keys_for(self, n: int) -> torch.Tensor:
+        if self._keys is None or self._keys.numel() < n:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError(f"{type(self).__name__}: run one call at this output size before capturing a CUDA "
+                                   "graph (the first call allocates the per-pixel key buffer)")
+            self._keys = torch.full((n,), -1, dtype=torch.int64, device=self.device)  # all bits set = no face
+        return self._keys
+
+    def _struct(self, x, texture, R, t, focal, princpt, H, W, keys) -> L.B2RMeshRender:
+        """texture None: the texture fields stay zero (the shaded render ignores them)."""
+        m = L.B2RMeshRender()
+        m.V, m.F, m.height, m.width = self.num_vertices, self.num_faces, H, W
+        m.mesh, m.faces = _ptr(x), _ptr(self.topology.faces)
+        if texture is not None:
+            m.Vt, m.C = int(self.vertex_uv.shape[0]), int(texture.shape[0])
+            m.tex_height, m.tex_width = int(texture.shape[1]), int(texture.shape[2])
+            m.vertex_uv, m.face_uv, m.texture = _ptr(self.vertex_uv), _ptr(self.face_uv), _ptr(texture)
+        m.cam_R, m.cam_t, m.focal, m.princpt = _ptr(R), _ptr(t), _ptr(focal), _ptr(princpt)
+        m.keys = _ptr(keys)
+        m.vf_offsets, m.vf_entries = _ptr(self.topology.offsets), _ptr(self.topology.entries)
+        return m
+
+
+class FaceMeshRenderer(_CoverageTables):
     """ExAvatar's `MeshRenderer(flame.vertex_uv, flame.face_uv)` + its call with `flame.face`, as a CUDA op.
 
         renderer = FaceMeshRenderer(flame.vertex_uv, flame.face_uv, flame.face, flame.vertex_num)     # once
@@ -160,25 +222,6 @@ class FaceMeshRenderer:
         self.num_faces = int(f.shape[0])
         self._keys: Optional[torch.Tensor] = None
 
-    def _keys_for(self, n: int) -> torch.Tensor:
-        if self._keys is None or self._keys.numel() < n:
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError("FaceMeshRenderer: run one call at this output size before capturing a CUDA graph "
-                                   "(the first call allocates the per-pixel key buffer)")
-            self._keys = torch.full((n,), -1, dtype=torch.int64, device=self.device)  # all bits set = no face
-        return self._keys
-
-    def _struct(self, x, texture, R, t, focal, princpt, H, W, keys) -> L.B2RMeshRender:
-        m = L.B2RMeshRender()
-        m.V, m.F, m.Vt, m.C = self.num_vertices, self.num_faces, int(self.vertex_uv.shape[0]), int(texture.shape[0])
-        m.tex_height, m.tex_width, m.height, m.width = int(texture.shape[1]), int(texture.shape[2]), H, W
-        m.mesh, m.faces, m.vertex_uv, m.face_uv = _ptr(x), _ptr(self.topology.faces), _ptr(self.vertex_uv), \
-            _ptr(self.face_uv)
-        m.texture, m.cam_R, m.cam_t, m.focal, m.princpt = _ptr(texture), _ptr(R), _ptr(t), _ptr(focal), _ptr(princpt)
-        m.keys = _ptr(keys)
-        m.vf_offsets, m.vf_entries = _ptr(self.topology.offsets), _ptr(self.topology.entries)
-        return m
-
     def render(self, uvmap: torch.Tensor, mesh: torch.Tensor, cam_param: Dict[str, torch.Tensor],
                render_shape: Tuple[int, int]) -> Tuple[torch.Tensor, torch.Tensor]:
         """The image (1,C,H,W) and the per-pixel face (H,W) int32 (-1: background; no gradient)."""
@@ -211,6 +254,86 @@ class FaceMeshRenderer:
     def __call__(self, uvmap: torch.Tensor, mesh: torch.Tensor, cam_param: Dict[str, torch.Tensor],
                  render_shape: Tuple[int, int]) -> torch.Tensor:
         return self.render(uvmap, mesh, cam_param, render_shape)[0]
+
+
+class ShadedMeshRenderer(_CoverageTables):
+    """The mesh panel of ExAvatar's animation scripts, `render_mesh(mesh, smpl_x.face, cam_param, bkg)`
+    (avatar/common/utils/vis.py:73-109; animate.py:83, animate_view_rot.py:98), as a CUDA op.
+
+        renderer = ShadedMeshRenderer(smpl_x.face, smpl_x.vertex_num)                 # once
+        panel = renderer(mesh, cam_param, bkg, blend_ratio=1.0)                        # per video frame
+
+    faces         (F,3) integer array or tensor of vertex indices in [0, num_vertices); uploaded once as int32 and
+                  range-checked with its vertex -> face table (construction may synchronise).
+    device        where the tables live; defaults to the current CUDA device.
+
+    A call takes mesh (V,3) or (1,V,3) float32 in camera coordinates, cam_param with focal (2) and princpt (2) (other
+    keys are ignored, as render_mesh ignores them), bkg (H,W,3) float32 in 0-255 (it sets the image size) and a finite
+    blend_ratio.  It returns a new (H,W,3) float32 tensor, HWC like render_mesh's numpy result, with no gradient: the
+    shaded mesh blended with bkg where a face covers the pixel, bkg bit for bit elsewhere (the module section
+    "Shaded render" has the semantics).  Normals, coverage, shading and composite run in three kernels with no
+    upload and no host synchronisation, so a captured CUDA graph replays with new mesh, focal, princpt and bkg
+    contents.  As with `FaceMeshRenderer`, calls of one renderer run on one stream and the first call at an output size
+    must not be inside a graph capture.
+    """
+
+    def __init__(self, faces: Union[np.ndarray, torch.Tensor], num_vertices: int, device=None):
+        fn = "ShadedMeshRenderer"
+        f = _int_table("faces", faces, fn)
+        if f.shape[0] >= 2 ** 29 or int(num_vertices) >= 2 ** 29:
+            raise ValueError(f"{fn}: {f.shape[0]} faces / {num_vertices} vertices exceed the op's limits")
+        self.topology = VertexNormals(f, num_vertices, device=device)  # faces range-checked, int32, + the CSR
+        self.device = self.topology.device
+        self.num_vertices = int(num_vertices)
+        self.num_faces = int(f.shape[0])
+        self.R = torch.eye(3, dtype=torch.float32, device=self.device).reshape(9)  # PerspectiveCameras without R / T
+        self.t = torch.zeros(3, dtype=torch.float32, device=self.device)
+        self._keys: Optional[torch.Tensor] = None
+
+    def __call__(self, mesh: torch.Tensor, cam_param: Dict[str, torch.Tensor], bkg: torch.Tensor,
+                 blend_ratio: float = 1.0) -> torch.Tensor:
+        fn = "ShadedMeshRenderer"
+        for name, v in (("mesh", mesh), ("bkg", bkg)):
+            if not v.is_cuda:
+                raise RuntimeError(f"{fn}: `{name}` must be a CUDA tensor (got {v.device}); there is no CPU path")
+        if mesh.dim() == 3 and mesh.shape[0] != 1:
+            raise ValueError(f"{fn}: only a batch of 1 is supported (mesh {tuple(mesh.shape)})")
+        if mesh.dim() not in (2, 3) or mesh.shape[-1] != 3 or mesh.shape[-2] != self.num_vertices:
+            raise ValueError(f"{fn}: mesh must be (1,{self.num_vertices},3) or ({self.num_vertices},3), got "
+                             f"{tuple(mesh.shape)}")
+        if bkg.dim() != 3 or bkg.shape[2] != 3:
+            raise ValueError(f"{fn}: bkg must be (H,W,3), got {tuple(bkg.shape)}")
+        H, W = int(bkg.shape[0]), int(bkg.shape[1])
+        if H < 1 or W < 1 or H * W >= 2 ** 31:
+            raise ValueError(f"{fn}: bad image size {(H, W)}")
+        for name, v in (("mesh", mesh), ("bkg", bkg)):
+            if v.dtype != torch.float32:
+                raise ValueError(f"{fn}: `{name}` must be float32, got {v.dtype}")
+            if v.device != self.device:
+                raise ValueError(f"{fn}: `{name}` is on {v.device}, the mesh tables on {self.device}")
+        if isinstance(blend_ratio, bool) or not isinstance(blend_ratio, numbers.Real) or \
+                not math.isfinite(blend_ratio):
+            raise ValueError(f"{fn}: blend_ratio must be a finite number, got {blend_ratio!r}")
+        focal, princpt = _cam_tensors(cam_param, self.device, fn, (("focal", 2), ("princpt", 2)))
+        x = mesh.detach().reshape(-1, 3).contiguous()
+        return self._shade(x, self.topology(x), focal, princpt, bkg.detach().contiguous(), float(blend_ratio))
+
+    def _shade(self, x, normals, focal, princpt, bkg, blend_ratio: float) -> torch.Tensor:
+        """b2r_mesh_shade_forward on checked, contiguous float32 tensors; `normals` (V,3) per vertex."""
+        lib = L.load()
+        H, W = int(bkg.shape[0]), int(bkg.shape[1])
+        m = self._struct(x, None, self.R, self.t, focal, princpt, H, W, self._keys_for(H * W))
+        nbytes = lib.b2r_mesh_render_scratch_bytes(self.num_faces)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        out = torch.empty((H, W, 3), dtype=torch.float32, device=self.device)
+        # vis.py's `render * blend_ratio + bkg / 255 * (1 - blend_ratio)`: numpy rounds the Python floats blend_ratio
+        # and (1 - blend_ratio), the latter taken in double, to float32; ctypes' c_float rounds the same way
+        with torch.cuda.device(self.device):
+            L.check(lib.b2r_mesh_shade_forward(C.byref(m), _ptr(normals), _ptr(bkg), blend_ratio, 1.0 - blend_ratio,
+                                               _ptr(out), _ptr(scratch), nbytes,
+                                               torch.cuda.current_stream(self.device).cuda_stream),
+                    "b2r_mesh_shade_forward")
+        return out
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -361,3 +484,60 @@ def face_render_reference(uvmap: torch.Tensor, mesh: torch.Tensor, faces, vertex
     img = torch.full((Cn, H * W), -1.0, dtype=dt, device=dev)
     img = img.index_put((torch.arange(Cn, device=dev)[:, None], fg[None]), val)
     return img.view(1, Cn, H, W), p2f.view(H, W)
+
+
+def _shade_reference(mesh: torch.Tensor, faces, cam_param: Dict[str, torch.Tensor], H: int, W: int,
+                     pix_to_face: Optional[torch.Tensor] = None, chunk: int = 1 << 22):
+    """Steps 1-5 of "Shaded render" in mesh's dtype, without grad: (colour c (H,W,3), zbuf (H,W) with -1 where no face
+    covers the pixel, pix_to_face (H,W) int64).  `pix_to_face` given: that map is used instead of step 2's."""
+    dev, dt = mesh.device, mesh.dtype
+    v = mesh.detach().reshape(-1, 3)
+    fa = torch.as_tensor(np.asarray(faces) if not isinstance(faces, torch.Tensor) else faces).to(dev).long()
+    cam = {"R": torch.eye(3, dtype=dt, device=dev), "t": torch.zeros(3, dtype=dt, device=dev),
+           "focal": cam_param["focal"], "princpt": cam_param["princpt"]}
+    x, y, z = _ndc(v, cam, H, W)
+    if pix_to_face is None:
+        p2f = _pixel_faces(x, y, z, fa, H, W, chunk)
+    else:
+        p2f = pix_to_face.reshape(-1).to(device=dev, dtype=torch.int64)
+    fg = torch.nonzero(p2f >= 0)[:, 0]
+    fc = fa[p2f[fg]]
+    colx, rowy = _pix_ndc(W, H, dt, dev), _pix_ndc(H, W, dt, dev)
+    b, pz = _bary(colx[fg % W], rowy[torch.div(fg, W, rounding_mode="floor")], x[fc], y[fc], z[fc])
+    # pytorch3d renders the xy-negated mesh: verts_normals_packed, interpolate_face_attributes, _apply_lighting there
+    vn = torch.stack([-v[:, 0], -v[:, 1], v[:, 2]], 1)
+    v0, v1, v2 = vn[fa[:, 0]], vn[fa[:, 1]], vn[fa[:, 2]]
+    fnorm = torch.cross(v2 - v1, v0 - v1, dim=1)
+    n = torch.zeros_like(vn)
+    for k in range(3):
+        n = n.index_add(0, fa[:, k], fnorm)
+    n = F.normalize(n, eps=NORMAL_EPS, dim=1)
+    P = b[:, 0, None] * vn[fc[:, 0]] + b[:, 1, None] * vn[fc[:, 1]] + b[:, 2, None] * vn[fc[:, 2]]
+    N = b[:, 0, None] * n[fc[:, 0]] + b[:, 1, None] * n[fc[:, 1]] + b[:, 2, None] * n[fc[:, 2]]
+    texel = b[:, 0] + b[:, 1] + b[:, 2]
+    light = torch.tensor([0.0, 1.0, 0.0], dtype=dt, device=dev)  # PointLights' default location
+    angle = torch.relu((F.normalize(N, eps=NORMAL_EPS, dim=1) * F.normalize(light - P, eps=NORMAL_EPS, dim=1)).sum(1))
+    c = torch.ones(H * W, dtype=dt, device=dev)  # softmax_rgb_blend's white background
+    c[fg] = (0.5 + 0.3 * angle) * texel
+    zbuf = torch.full((H * W,), -1.0, dtype=dt, device=dev)
+    zbuf[fg] = pz
+    return c.view(H, W, 1).expand(H, W, 3).contiguous(), zbuf.view(H, W), p2f.view(H, W)
+
+
+def shaded_mesh_reference(mesh: torch.Tensor, faces, cam_param: Dict[str, torch.Tensor], bkg: torch.Tensor,
+                          blend_ratio: float = 1.0, pix_to_face: Optional[torch.Tensor] = None, chunk: int = 1 << 22
+                          ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Steps 1-6 of "Shaded render" restated in torch, computed in mesh's dtype (float32 or float64) on mesh's device:
+    returns (out (H,W,3), pix_to_face (H,W) int64).  The normals are pytorch3d's form in the xy-negated frame
+    ((v2 - v1) x (v0 - v1) added per corner with index_add, F.normalize), not the op's b2r_vertex_normals; the
+    composite is vis.py's numpy expression with blend_ratio and (1 - blend_ratio) rounded to the dtype.
+    `pix_to_face` given: that map is used instead of step 2's.  The tests' reference; the product never calls it."""
+    dev, dt = mesh.device, mesh.dtype
+    H, W = int(bkg.shape[0]), int(bkg.shape[1])
+    c, zbuf, p2f = _shade_reference(mesh, faces, cam_param, H, W, pix_to_face, chunk)
+    bk = bkg.to(device=dev, dtype=dt)
+    is_bkg = (zbuf <= 0).to(dt)[:, :, None]
+    beta = torch.tensor(float(blend_ratio), dtype=dt, device=dev)
+    beta_c = torch.tensor(1.0 - float(blend_ratio), dtype=dt, device=dev)
+    fg = c * beta + _div(bk, 255.0) * beta_c
+    return (fg * (1 - is_bkg)) * 255 + bk * is_bkg, p2f

@@ -375,6 +375,29 @@ int b2r_mesh_render_forward(const B2RMeshRender* mr, float* image, int32_t* pix_
 int b2r_mesh_render_backward(const B2RMeshRender* mr, const int32_t* pix_to_face, const float* dL_dimage,
                              float* dL_dmesh, void* scratch, size_t scratch_bytes, void* stream);
 
+/* Shaded render of a triangle mesh over a background: the mesh panel of ExAvatar's animation scripts
+ * (avatar/common/utils/vis.py:73-109 render_mesh: pytorch3d's SoftPhongShader with PointLights(), white TexturesVertex,
+ * Materials(specular 0), then the host composite), restated from pytorch3d's implementation.  Reads the geometry, camera
+ * and keys fields of `mr` (V, F, height, width, mesh, faces, cam_R, cam_t, focal, princpt, keys) and ignores the
+ * texture and CSR fields; render_mesh's camera is R = I, t = 0.
+ *   coverage b2r_mesh_render_forward's, unchanged: the covering face of least pz per pixel, pz its depth.
+ *   shading  in camera coordinates (p_c = R p + t, n_c = R n, normals (V,3) per vertex, b2r_vertex_normals of mesh
+ *            without a flip): with b the perspective-corrected barycentrics and every sum over the corners 0, 1, 2 in
+ *            order, P = sum b_k p_k, N = sum b_k n_k, texel = b_0 + b_1 + b_2 (kept, not 1),
+ *            c = (0.5 + 0.3 relu(N / max(|N|, 1e-6) . D / max(|D|, 1e-6))) texel with D = (0, -1, 0) - P:
+ *            pytorch3d's light (0, 1, 0) in its xy-negated frame, ambient 0.5, diffuse 0.3, specular 0.
+ *            Uncovered: c = 1.  pytorch3d's softmax_rgb_blend returns c to within an fp32 rounding while pz < 99.8
+ *            (znear 1, zfar 100); its fade to white past that depth is not restated.
+ *   output   out (height, width, 3) HWC from bkg (height, width, 3) HWC, per channel in fp32 (vis.py:105-108):
+ *            fg = c blend + (bkg / 255) blend_complement, out = (fg (1 - is_bkg)) 255 + bkg is_bkg, is_bkg = 1 where
+ *            no face covers the pixel or pz <= 0.  blend = fp32(blend_ratio), blend_complement = fp32(1 - blend_ratio)
+ *            taken in double, as numpy gets them; both must be finite.
+ * `scratch` >= b2r_mesh_render_scratch_bytes(F).  keys as for b2r_mesh_render_forward: all ~0 on entry, left all ~0.
+ * Writes every element of out.  Two launches (mr_face_kernel, mr_shade_kernel); no allocation, no sync, no device
+ * read on the host, so a captured graph replays with new mesh, normals, camera and bkg contents. */
+int b2r_mesh_shade_forward(const B2RMeshRender* mr, const float* normals, const float* bkg, float blend,
+                           float blend_complement, float* out, void* scratch, size_t scratch_bytes, void* stream);
+
 /* Triplane features of the human Gaussians (avatar/common/nets/module.py:424-457 extract_tri_feature).  planes and
  * planes_face are (3,C,height,width); corners (P,3,4) int32 holds, per row and plane (xy, xz, yz), the texels
  * y * width + x of F.grid_sample's four bilinear corners in its order (nw, ne, sw, se), -1 for a corner outside the
@@ -796,7 +819,7 @@ int b2r_camera_setup(const float* R, const float* t, const float* focal, int32_t
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
