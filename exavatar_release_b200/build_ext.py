@@ -49,7 +49,9 @@ NVCC_FLAGS = [
 # multiplies, exp / tanh as torch's kernels call them), bit-identical to it.
 # camera.cu: the camera block restates torch's fp32 expressions (reciprocal, atanf, tanf) and the fp32 sums of torch.mm
 # operation by operation.
-PER_FILE_FLAGS = {"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
+# metrics.cu: the PNG round trip, the mask composite and the ScalingLayer are torch's fp32 expressions rounded operation
+# by operation, and SSIM's numerator and denominator are the same bits for identical images (exactly 1).
+PER_FILE_FLAGS = {"metrics.cu": ["--fmad=false"],"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
                   "geometry.cu": ["--fmad=false"], "mesh_raster.cu": ["--fmad=false"],
                   "regularizers.cu": ["--fmad=false"], "smplx_rig.cu": ["--fmad=false"], "adam.cu": ["--fmad=false"],
                   "scene_assets.cu": ["--fmad=false"], "human_assets.cu": ["--fmad=false"],

@@ -121,6 +121,19 @@ int validate_lpips(const B2RLpips* p) {
   return B2R_OK;
 }
 
+// metrics.cu: sizes (the second pool needs 31 px; SSIM tiles put H / 16 in grid.y and 3 N in grid.z, the convs 2 N;
+// per-image offsets of W x H x 4 floats stay in int32 pixel indices), the mask's channel count with the mask, and
+// every pointer the op reads
+int validate_neuman(const B2RNeumanScores* p) {
+  if (!p || p->width < 31 || p->height < 31 || p->n_images < 1 || p->n_images > 16384) return B2R_E_INVALID;
+  if (p->height > 65535 * 16 || (int64_t)p->width * p->height > (int64_t)1 << 28) return B2R_E_INVALID;
+  if (p->mask ? (p->mask_channels != 1 && p->mask_channels != 3) : p->mask_channels != 0) return B2R_E_INVALID;
+  if (!p->render || !p->target) return B2R_E_INVALID;
+  for (int l = 0; l < 5; l++)
+    if (!p->w[l] || !p->bias[l] || !p->lin[l]) return B2R_E_INVALID;
+  return B2R_OK;
+}
+
 // sizes and the pointers both directions read; the index tables' contents are the caller's (see b200raster.h)
 int validate_mesh_render(const B2RMeshRender* m) {
   if (!m) return B2R_E_INVALID;
@@ -245,6 +258,7 @@ size_t b2r_sizeof(int which) {
     case 22: return sizeof(B2RHumanAssetsGrads);
     case 23: return sizeof(B2RSmplxBody);
     case 24: return sizeof(B2RSmplxBodyGrads);
+    case 25: return sizeof(B2RNeumanScores);
     default: return 0;
   }
 }
@@ -662,6 +676,18 @@ int b2r_lpips_backward(const B2RLpips* p, const void* saved, size_t saved_bytes,
       scratch_bytes < lpips_scratch_bytes(p->width, p->height))
     return B2R_E_WORKSPACE;
   return launch_lpips_backward(*p, (const float*)saved, dL_dout, dL_dimg, scratch, (cudaStream_t)stream);
+}
+
+size_t b2r_neuman_scratch_bytes(int32_t width, int32_t height, int32_t n_images) {
+  return neuman_scratch_bytes(width > 31 ? width : 31, height > 31 ? height : 31, n_images > 0 ? n_images : 1);
+}
+
+int b2r_neuman_scores(const B2RNeumanScores* p, float* out, void* scratch, size_t scratch_bytes, void* stream) {
+  const int rc = validate_neuman(p);
+  if (rc) return rc;
+  if (!out || !scratch) return B2R_E_INVALID;
+  if (scratch_bytes < neuman_scratch_bytes(p->width, p->height, p->n_images)) return B2R_E_WORKSPACE;
+  return launch_neuman_scores(*p, out, scratch, (cudaStream_t)stream);
 }
 
 int b2r_scene_assets_forward(const B2RSceneAssets* s, float* opacity, float* scale, float* rotation, float* color,

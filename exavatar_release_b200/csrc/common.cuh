@@ -600,6 +600,8 @@ size_t lpips_scratch_bytes(int W, int H);
 int launch_lpips_forward(const B2RLpips& p, float* out, float* saved, void* scratch, cudaStream_t st);
 int launch_lpips_backward(const B2RLpips& p, const float* saved, const float* dout, float* dimg, void* scratch,
                           cudaStream_t st);
+size_t neuman_scratch_bytes(int W, int H, int N);
+int launch_neuman_scores(const B2RNeumanScores& p, float* out, void* scratch, cudaStream_t st);
 int launch_scene_assets_forward(const B2RSceneAssets& s, float* opacity, float* scale, float* rotation, float* color,
                                 cudaStream_t st);
 int launch_scene_assets_backward(const B2RSceneAssets& s, const B2RSceneAssetsGrads& g, cudaStream_t st);

@@ -211,7 +211,7 @@ int b2r_last_cuda_error(void);
  * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin, 8 B2RMeshRender, 10 B2RGnMlp, 11 B2RRegs,
  * 12 B2RRegsGrads, 13 B2RRig, 14 B2RRigGrads, 15 B2RAdamSegment, 16 B2RLpips, 17 B2RSceneAssets,
  * 18 B2RSceneAssetsGrads, 19 B2RSmplxPose, 20 B2RSmplxPoseGrads, 21 B2RHumanAssets, 22 B2RHumanAssetsGrads,
- * 23 B2RSmplxBody, 24 B2RSmplxBodyGrads; 0 for anything else
+ * 23 B2RSmplxBody, 24 B2RSmplxBodyGrads, 25 B2RNeumanScores; 0 for anything else
  * (7 and 9 are unused and report 0). */
 size_t b2r_sizeof(int which);
 
@@ -675,6 +675,35 @@ int b2r_lpips_forward(const B2RLpips* p, float* out, void* saved, size_t saved_b
 int b2r_lpips_backward(const B2RLpips* p, const void* saved, size_t saved_bytes, const float* dL_dout, float* dL_dimg,
                        void* scratch, size_t scratch_bytes, void* stream);
 
+/* The test-set scores of ExAvatar's NeuMan protocol (avatar/tools/eval_neuman.py) of n_images frames, each a (3,H,W)
+ * `render` against its own (3,H,W) `target` (fp32, device, contiguous (N,3,H,W)).  Per frame, both images take the
+ * 8-bit PNG round trip (v = fl(p 255); 0 if v is NaN or |v| >= 2^31, else clamp(rint(v), 0, 255); then / 255 in
+ * double, rounded to fp32) and, with a `mask` (N,mask_channels,H,W), 1 = human, mask_channels 1 or 3, the white
+ * background fl(fl(q m) + fl(1 - m)); mask NULL (mask_channels 0) keeps the background.  out[3n..3n+2] =
+ *   psnr   10 log10(1 / mse), fp64 accumulation rounded once (+inf for identical images);
+ *   ssim   torchmetrics' SSIM (11x11 Gaussian window, sigma 1.5, variances clamped at 0) over the (H-10)(W-10) window
+ *          centres per channel, with fp64 window sums;
+ *   lpips  lpips.LPIPS(net='alex') version 0.1 of x*2-1: ScalingLayer, alexnet().features[0:12] as TF32 (round to
+ *          nearest) implicit GEMMs with fp32 accumulation, the heads of relu1..relu5.
+ * Weights (fp32, device, 16-byte aligned): w[l] (K_l, C_out) with row (ky KS + kx) C_in + ci holding torch's
+ * weight[co, ci, ky, kx], C_in padded to 4 for conv 1 (channel 3 zero) and the rows padded with zeros to K_l =
+ * ceil(KS^2 C_in / 32) 32 (512, 1600, 1728, 3456, 2304); bias[l] (C_out = 64, 192, 384, 256, 256); lin[t] (C_out of
+ * conv t).  scratch >= b2r_neuman_scratch_bytes(W, H, N); its layout (the composited images, every tap) is documented
+ * in csrc/metrics.cu.  W, H >= 31 (the second pool is empty below).  Fixed-order reductions, no float atomics:
+ * bit-identical runs.  No allocation, no sync; forward only. */
+typedef struct B2RNeumanScores {
+  int32_t width, height, n_images, mask_channels;
+  const float* render;
+  const float* target;
+  const float* mask;
+  const float* w[5];
+  const float* bias[5];
+  const float* lin[5];
+} B2RNeumanScores;
+
+size_t b2r_neuman_scratch_bytes(int32_t width, int32_t height, int32_t n_images);
+int b2r_neuman_scores(const B2RNeumanScores* p, float* out, void* scratch, size_t scratch_bytes, void* stream);
+
 /* ExAvatar's scene Gaussian assets (avatar/common/nets/module.py:253-272, SceneGaussian.forward) from the stored
  * parameters of P Gaussians with M SH coefficients (1 <= M <= B2R_SCENE_MAX_COEFFS): opacity = sigmoid(logit) (P,1),
  * scale = exp(log_scale) (P,3), rotation = pytorch3d 0.7.5's matrix_to_quaternion(rotation_6d_to_matrix(rotation6d))
@@ -819,7 +848,7 @@ int b2r_camera_setup(const float* R, const float* t, const float* focal, int32_t
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_neuman_scores, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
