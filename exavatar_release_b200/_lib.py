@@ -2,11 +2,17 @@
 
 There is NO CPU fallback: if the shared library is missing or cannot be loaded, `load()` raises.  The library is built
 in-tree by `exavatar_release_b200.build_ext.build()` (nvcc, sm_90a).
+
+Every per-frame op reaches the library through `run` and checks its tensors with `cuda`, `float32` and `same_device`,
+so the stream, device and error rules of a call live here once.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+from typing import Optional
+
+import torch
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "libb200raster.so")
@@ -361,3 +367,39 @@ def check(rc: int, what: str):
         lib = load()
         msg = lib.b2r_strerror(rc).decode()
         raise RuntimeError(f"b200raster: {what} failed: {msg} (code {rc}, cudaError {lib.b2r_last_cuda_error()})")
+
+
+def ptr(t: Optional[torch.Tensor]):
+    """The device address of `t` for the C ABI; None (NULL) for an absent or empty tensor."""
+    return None if t is None or t.numel() == 0 else t.data_ptr()
+
+
+def run(name: str, device: torch.device, *args) -> None:
+    """Calls the launching entry point `name` with `args` on the current stream of `device`, with `device` current.
+    Every launching b2r_* entry takes its stream last.  Raises RuntimeError naming `name` unless it returns B2R_OK."""
+    lib = load()
+    with torch.cuda.device(device):
+        check(getattr(lib, name)(*args, torch.cuda.current_stream(device).cuda_stream), name)
+
+
+def cuda(fn: str, name: str, t, device: Optional[torch.device] = None) -> None:
+    """Raises RuntimeError unless `t` is a CUDA tensor (on `device`, when given): the ops have no CPU code."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        got = t.device if isinstance(t, torch.Tensor) else type(t).__name__
+        raise RuntimeError(f"{fn}: `{name}` must be a CUDA tensor (got {got}); there is no CPU fallback")
+    if device is not None and t.device != device:
+        raise RuntimeError(f"{fn}: `{name}` must be on {device}, got {t.device}")
+
+
+def float32(fn: str, name: str, t: torch.Tensor) -> None:
+    """Raises ValueError unless `t` is float32."""
+    if t.dtype != torch.float32:
+        raise ValueError(f"{fn}: `{name}` must be float32, got {t.dtype}")
+
+
+def same_device(fn: str, tensors, device: Optional[torch.device] = None) -> None:
+    """Raises ValueError unless the tensors that are not None, and the op's `device` when given, share one device."""
+    devices = {t.device for t in tensors if t is not None} | ({device} if device is not None else set())
+    if len(devices) != 1:
+        where = "the same device" if device is None else "the op's device"
+        raise ValueError(f"{fn}: all tensors must be on {where}")

@@ -49,6 +49,16 @@ def get_proj_matrix(focal, princpt, img_shape, z_near, z_far, z_sign):
     return m.to(focal.device)
 
 
+def _inv3(R: torch.Tensor) -> torch.Tensor:
+    """3x3 inverse by cofactors: a handful of elementwise kernels, no cuSOLVER call -- capturable in a CUDA graph
+    (`torch.inverse`, which the reference uses at module.py:556, synchronises)."""
+    a, b, c, d, e, f, g, h, i = R.reshape(9).unbind()
+    adj = torch.stack((e * i - f * h, c * h - b * i, b * f - c * e,
+                       f * g - d * i, a * i - c * g, c * d - a * f,
+                       d * h - e * g, b * g - a * h, a * e - b * d)).reshape(3, 3)
+    return adj / (a * (e * i - f * h) - b * (d * i - f * g) + c * (d * h - e * g))
+
+
 def look_at_cam_param(yaw_deg: float, img_shape, focal_ratio: float = 1.465, target_z: float = 4.24, device="cpu"):
     """Synthetic camera orbiting the subject (SURVEY section 8d: fx = fy = 1.465*H, subject at z = 4.24 m)."""
     H, W = img_shape

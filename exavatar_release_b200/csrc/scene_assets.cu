@@ -101,7 +101,7 @@ __device__ __forceinline__ float sh_basis(int k, float x, float y, float z, floa
   }
 }
 
-// -R^-1 t by cofactors (rasterizer._inv3's expressions)
+// -R^-1 t by cofactors (camera._inv3's expressions)
 __device__ __forceinline__ void cam_position(const float* __restrict__ R, const float* __restrict__ t, float* c) {
   const float a = __ldg(R + 0), b = __ldg(R + 1), cc = __ldg(R + 2), d = __ldg(R + 3), e = __ldg(R + 4),
               f = __ldg(R + 5), g = __ldg(R + 6), h = __ldg(R + 7), i = __ldg(R + 8);

@@ -855,7 +855,7 @@ __global__ void __launch_bounds__(RIG_JMAX) body_chain_kernel(const B2RSmplxBody
   __shared__ BodyChainSm sm;
   body_chain(b, s, sm, true);
   const int tid = threadIdx.x;
-  if (tid == 0 && b.cam_R) {  // R^-1 by cofactors (rasterizer._inv3's expressions), fp32
+  if (tid == 0 && b.cam_R) {  // R^-1 by cofactors (camera._inv3's expressions), fp32
     const float* R = b.cam_R;
     const float a = R[0], bb = R[1], c = R[2], d = R[3], e = R[4], f = R[5], g = R[6], h = R[7], i = R[8];
     const float adj[9] = {e * i - f * h, c * h - bb * i, bb * f - c * e, f * g - d * i, a * i - c * g,

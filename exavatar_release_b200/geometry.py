@@ -22,26 +22,22 @@ import numpy as np
 import torch
 
 from . import _lib as L
-from .rasterizer import _ptr
 
 NORMAL_EPS = 1e-6  # F.normalize's eps
 
 
 def _points(name: str, t: torch.Tensor, fn: str) -> torch.Tensor:
-    if not t.is_cuda:
-        raise RuntimeError(f"{fn}: `{name}` must be a CUDA tensor (got {t.device}); there is no CPU path")
+    L.cuda(fn, name, t)
     if t.dim() != 2 or t.shape[1] != 3:
         raise ValueError(f"{fn}: `{name}` must be (N,3), got {tuple(t.shape)}")
-    if t.dtype != torch.float32:
-        raise ValueError(f"{fn}: `{name}` must be float32, got {t.dtype}")
+    L.float32(fn, name, t)
     return t.detach().contiguous()
 
 
 def _mask_u8(name: str, m: Optional[torch.Tensor], P: int, fn: str, device) -> Optional[torch.Tensor]:
     if m is None:
         return None
-    if not m.is_cuda:
-        raise RuntimeError(f"{fn}: `{name}` must be a CUDA tensor (got {m.device}); there is no CPU path")
+    L.cuda(fn, name, m)
     if m.dtype not in (torch.bool, torch.uint8):
         raise ValueError(f"{fn}: `{name}` must be bool or uint8, got {m.dtype}")
     if m.numel() != P or m.dim() != 1:
@@ -71,13 +67,10 @@ def nearest_rows(queries: torch.Tensor, targets: torch.Tensor, self_map: Optiona
     if V < 1 and P > 0:
         raise ValueError(f"{fn}: no targets to search")
     m = _mask_u8("self_map", self_map, P, fn, q.device)
-    lib = L.load()
     rows = torch.empty(P, dtype=torch.int32, device=q.device)
-    nbytes = lib.b2r_nearest_scratch_bytes(P, V)
+    nbytes = L.load().b2r_nearest_scratch_bytes(P, V)
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
-    with torch.cuda.device(q.device):
-        L.check(lib.b2r_nearest_rows(P, _ptr(q), V, _ptr(t), _ptr(m), _ptr(rows), _ptr(scratch), nbytes,
-                                     torch.cuda.current_stream(q.device).cuda_stream), "b2r_nearest_rows")
+    L.run("b2r_nearest_rows", q.device, P, L.ptr(q), V, L.ptr(t), L.ptr(m), L.ptr(rows), L.ptr(scratch), nbytes)
     return rows
 
 
@@ -139,7 +132,7 @@ class VertexNormals:
             device = flip.device if flip is not None else torch.device("cuda", torch.cuda.current_device())
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError(f"VertexNormals: device must be CUDA (got {device}); there is no CPU path")
+            raise RuntimeError(f"VertexNormals: device must be CUDA (got {device}); there is no CPU fallback")
         if device.index is None:
             device = torch.device("cuda", torch.cuda.current_device())
         num_vertices = int(num_vertices)
@@ -149,8 +142,7 @@ class VertexNormals:
         if f.numel() and (int(f.min()) < 0 or int(f.max()) >= num_vertices):
             raise ValueError(f"VertexNormals: face indices must lie in [0, {num_vertices})")
         if flip is not None:
-            if not flip.is_cuda:
-                raise RuntimeError(f"VertexNormals: `flip` must be a CUDA tensor (got {flip.device})")
+            L.cuda("VertexNormals", "flip", flip)
             if flip.numel() != num_vertices or flip.dim() != 1:
                 raise ValueError(f"VertexNormals: flip must be ({num_vertices},), got {tuple(flip.shape)}")
             flip = (flip.to(device) != 0).to(torch.uint8).contiguous()
@@ -172,12 +164,9 @@ class VertexNormals:
             raise ValueError(f"{fn}: xyz has {x.shape[0]} rows for a mesh of {self.num_vertices} vertices")
         if x.device != self.device:
             raise ValueError(f"{fn}: xyz is on {x.device}, the mesh tables on {self.device}")
-        lib = L.load()
         out = torch.empty((self.num_vertices, 3), dtype=torch.float32, device=x.device)
-        with torch.cuda.device(x.device):
-            L.check(lib.b2r_vertex_normals(self.num_vertices, _ptr(x), _ptr(self.faces), _ptr(self.offsets),
-                                           _ptr(self.entries), _ptr(self.flip), _ptr(out),
-                                           torch.cuda.current_stream(x.device).cuda_stream), "b2r_vertex_normals")
+        L.run("b2r_vertex_normals", x.device, self.num_vertices, L.ptr(x), L.ptr(self.faces), L.ptr(self.offsets),
+              L.ptr(self.entries), L.ptr(self.flip), L.ptr(out))
         return out
 
 

@@ -28,7 +28,6 @@ import ctypes as C
 import torch
 
 from . import _lib as L
-from .rasterizer import _ptr
 from .smplx_rig import matrix_to_axis_angle, matrix_to_quaternion, rotation_6d_to_matrix
 
 # SMPLXParamDict's pose keys in cat_full_pose order and their rows in SMPL-X (root, 21 body, jaw, eyes, 15 per hand)
@@ -37,22 +36,16 @@ POSE_ROWS = (1, 21, 1, 1, 1, 15, 15)
 WARMUP_SCALE_MAX = 0.001  # model.py:94
 
 
-def _stream(dev):
-    return torch.cuda.current_stream(dev).cuda_stream
-
-
 class _DecodePose(torch.autograd.Function):
     @staticmethod
     def forward(ctx, *params):
-        lib = L.load()
         dev = params[0].device
         rows = [p.detach().reshape(-1, 6).contiguous() for p in params]
         st = L.B2RSmplxPose()
         for k, r in enumerate(rows):
-            st.param[k], st.rows[k] = _ptr(r), r.shape[0]
+            st.param[k], st.rows[k] = L.ptr(r), r.shape[0]
         full = torch.empty((sum(POSE_ROWS), 3), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_decode_pose_forward(C.byref(st), _ptr(full), _stream(dev)), "b2r_decode_pose_forward")
+        L.run("b2r_decode_pose_forward", dev, C.byref(st), L.ptr(full))
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(*rows)
         ctx.shapes = [p.shape for p in params]
@@ -64,23 +57,13 @@ class _DecodePose(torch.autograd.Function):
             return (None,) * len(POSE_KEYS)
         rows = ctx.saved_tensors
         dev = rows[0].device
-        lib = L.load()
         st, gs = L.B2RSmplxPose(), L.B2RSmplxPoseGrads()
         grads = [torch.empty_like(r) for r in rows]
         for k, (r, g) in enumerate(zip(rows, grads)):
-            st.param[k], st.rows[k], gs.param[k] = _ptr(r), r.shape[0], _ptr(g)
+            st.param[k], st.rows[k], gs.param[k] = L.ptr(r), r.shape[0], L.ptr(g)
         up = g_full.to(torch.float32).contiguous()
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_decode_pose_backward(C.byref(st), _ptr(up), C.byref(gs), _stream(dev)),
-                    "b2r_decode_pose_backward")
+        L.run("b2r_decode_pose_backward", dev, C.byref(st), L.ptr(up), C.byref(gs))
         return tuple(g.reshape(s) for g, s in zip(grads, ctx.shapes))
-
-
-def _check_cuda(fn, name, t, dev):
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or (dev is not None and t.device != dev):
-        raise RuntimeError(f"{fn}: `{name}` must be a CUDA tensor on {dev}; there is no CPU path")
-    if t.dtype != torch.float32:
-        raise ValueError(f"{fn}: `{name}` must be float32, got {t.dtype}")
 
 
 def decode_smplx_pose(smplx_param) -> dict:
@@ -93,7 +76,8 @@ def decode_smplx_pose(smplx_param) -> dict:
     params = [smplx_param[k] for k in POSE_KEYS]
     dev = params[0].device if isinstance(params[0], torch.Tensor) else None
     for k, p, n in zip(POSE_KEYS, params, POSE_ROWS):
-        _check_cuda("decode_smplx_pose", k, p, dev)
+        L.cuda("decode_smplx_pose", k, p, dev)
+        L.float32("decode_smplx_pose", k, p)
         if not (tuple(p.shape) == (n, 6) or (n == 1 and tuple(p.shape) == (6,))):
             want = f"({n},6)" + (" or (6,)" if n == 1 else "")
             raise ValueError(f"decode_smplx_pose: `{k}` must be {want} (SMPL-X's 55-joint order), "
@@ -128,19 +112,17 @@ def _rows4(t: torch.Tensor):
 class _Geometry(torch.autograd.Function):
     @staticmethod
     def forward(ctx, ha, warmup, mesh, pose_offset, expr_offset, geo, geo_offset):
-        lib = L.load()
         dev = ha.device
         P = ha.P
         g4, gs = _rows4(geo.detach())
         o4, os_ = _rows4(geo_offset.detach())
         ins = [t.detach().contiguous() for t in (mesh, pose_offset, expr_offset)]
         st = L.B2RHumanAssets(P=P, warmup=int(warmup), geo_stride=gs, geo_offset_stride=os_)
-        st.mesh, st.pose_offset, st.expr_offset = (_ptr(t) for t in ins)
-        st.geo, st.geo_offset, st.mask = _ptr(g4), _ptr(o4), _ptr(ha.mask)
+        st.mesh, st.pose_offset, st.expr_offset = (L.ptr(t) for t in ins)
+        st.geo, st.geo_offset, st.mask = L.ptr(g4), L.ptr(o4), L.ptr(ha.mask)
         outs = [torch.empty((P, 3), dtype=torch.float32, device=dev) for _ in range(7 if warmup else 5)]
-        ptrs = [_ptr(o) for o in outs] + [None, None] * (not warmup)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_human_geometry_forward(C.byref(st), *ptrs, _stream(dev)), "b2r_human_geometry_forward")
+        ptrs = [L.ptr(o) for o in outs] + [None, None] * (not warmup)
+        L.run("b2r_human_geometry_forward", dev, C.byref(st), *ptrs)
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(*ins, g4, o4)
         ctx.meta = (ha, st, geo.shape, geo_offset.shape)
@@ -151,29 +133,23 @@ class _Geometry(torch.autograd.Function):
         mesh, pose_offset, expr_offset, g4, o4 = ctx.saved_tensors
         ha, st, geo_shape, off_shape = ctx.meta
         dev = ha.device
-        lib = L.load()
         up = [None if g is None else g.to(torch.float32).contiguous() for g in grads]
         up += [None] * (7 - len(up))
         f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)  # noqa: E731
         d_mesh, d_expr, d_geo, d_off = f(ha.P, 3), f(ha.P, 3), f(ha.P, 4), f(ha.P, 4)
-        gs = L.B2RHumanAssetsGrads(*[_ptr(x) for x in (*up, d_mesh, d_expr, d_geo, d_off)])
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_human_geometry_backward(C.byref(st), C.byref(gs), _stream(dev)),
-                    "b2r_human_geometry_backward")
+        gs = L.B2RHumanAssetsGrads(*[L.ptr(x) for x in (*up, d_mesh, d_expr, d_geo, d_off)])
+        L.run("b2r_human_geometry_backward", dev, C.byref(st), C.byref(gs))
         return None, None, d_mesh, None, d_expr, d_geo.reshape(geo_shape), d_off.reshape(off_shape)
 
 
 class _Colors(torch.autograd.Function):
     @staticmethod
     def forward(ctx, rgb, rgb_offset):
-        lib = L.load()
         dev = rgb.device
         x, o = rgb.detach().contiguous(), rgb_offset.detach().contiguous()
         P = x.shape[0]
         out, out_r = torch.empty_like(x), torch.empty_like(x)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_human_colors_forward(P, _ptr(x), _ptr(o), _ptr(out), _ptr(out_r), _stream(dev)),
-                    "b2r_human_colors_forward")
+        L.run("b2r_human_colors_forward", dev, P, L.ptr(x), L.ptr(o), L.ptr(out), L.ptr(out_r))
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(x, o)
         return out, out_r
@@ -182,12 +158,10 @@ class _Colors(torch.autograd.Function):
     def backward(ctx, g, g_r):
         x, o = ctx.saved_tensors
         dev = x.device
-        lib = L.load()
         g, g_r = (None if t is None else t.to(torch.float32).contiguous() for t in (g, g_r))
         d_rgb, d_off = torch.empty_like(x), torch.empty_like(x)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_human_colors_backward(x.shape[0], _ptr(x), _ptr(o), _ptr(g), _ptr(g_r), _ptr(d_rgb),
-                                                  _ptr(d_off), _stream(dev)), "b2r_human_colors_backward")
+        L.run("b2r_human_colors_backward", dev, x.shape[0], L.ptr(x), L.ptr(o), L.ptr(g), L.ptr(g_r), L.ptr(d_rgb),
+              L.ptr(d_off))
         return d_rgb, d_off
 
 
@@ -199,7 +173,7 @@ class HumanAssets:
     def __init__(self, is_rhand, is_lhand, is_face_expr, device=None):
         device = torch.device(device if device is not None else "cuda")
         if device.type != "cuda":
-            raise RuntimeError(f"HumanAssets: device must be CUDA (got {device}); there is no CPU path")
+            raise RuntimeError(f"HumanAssets: device must be CUDA (got {device}); there is no CPU fallback")
         if device.index is None:
             device = torch.device("cuda", torch.cuda.current_device())
         masks = [torch.as_tensor(m).detach().reshape(-1) for m in (is_rhand, is_lhand, is_face_expr)]
@@ -224,7 +198,8 @@ class HumanAssets:
         for name, t, shape in (("mesh_neutral_pose", mesh_neutral_pose, (P, 3)), ("pose_offset", pose_offset, (P, 3)),
                                ("expr_offset", expr_offset, (P, 3)), ("geo", geo, (P, 4)),
                                ("geo_offset", geo_offset, (P, 4))):
-            _check_cuda("HumanAssets.geometry", name, t, dev)
+            L.cuda("HumanAssets.geometry", name, t, dev)
+            L.float32("HumanAssets.geometry", name, t)
             if tuple(t.shape) != shape:
                 raise ValueError(f"HumanAssets.geometry: `{name}` must be {shape}, got {tuple(t.shape)}")
         outs = _Geometry.apply(self, bool(warmup), mesh_neutral_pose, pose_offset, expr_offset, geo, geo_offset)
@@ -238,7 +213,8 @@ class HumanAssets:
         """module.py:561: ((tanh(rgb) + 1) / 2, (tanh(rgb + rgb_offset) + 1) / 2) from the (P,3) float32 CUDA network
         outputs; gradients reach both."""
         for name, t in (("rgb", rgb), ("rgb_offset", rgb_offset)):
-            _check_cuda("HumanAssets.colors", name, t, self.device)
+            L.cuda("HumanAssets.colors", name, t, self.device)
+            L.float32("HumanAssets.colors", name, t)
             if tuple(t.shape) != (self.P, 3):
                 raise ValueError(f"HumanAssets.colors: `{name}` must be ({self.P}, 3), got {tuple(t.shape)}")
         return _Colors.apply(rgb, rgb_offset)

@@ -27,7 +27,6 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib as L
-from .rasterizer import _ptr
 
 TRIPLANE_SHAPE_3D = 2.0       # cfg.triplane_shape_3d: the body triplane spans [-1, 1] m around the mean vertex
 TRIPLANE_FACE_SHAPE_3D = 0.3  # cfg.triplane_face_shape_3d
@@ -81,28 +80,23 @@ def bilinear_corners(grid: torch.Tensor, height: int, width: int) -> Tuple[torch
 
 
 def _plane_shape(name: str, t: torch.Tensor, fn: str) -> Tuple[int, int, int]:
-    if not t.is_cuda:
-        raise RuntimeError(f"{fn}: `{name}` must be a CUDA tensor (got {t.device}); there is no CPU path")
+    L.cuda(fn, name, t)
     if t.dim() != 4 or t.shape[0] != 3:
         raise ValueError(f"{fn}: `{name}` must be (3,C,H,W), got {tuple(t.shape)}")
-    if t.dtype != torch.float32:
-        raise ValueError(f"{fn}: `{name}` must be float32, got {t.dtype}")
+    L.float32(fn, name, t)
     return int(t.shape[1]), int(t.shape[2]), int(t.shape[3])
 
 
 class _Triplane(torch.autograd.Function):
     @staticmethod
     def forward(ctx, triplane, triplane_face, op):
-        lib = L.load()
         dev = triplane.device
         Cc, H, W = triplane.shape[1:]
         t = triplane.detach().contiguous()
         tf = triplane_face.detach().contiguous()
         feat = torch.empty((op.P, 3 * Cc), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_triplane_forward(op.P, Cc, H, W, _ptr(t), _ptr(tf), _ptr(op.is_face), _ptr(op.corners),
-                                             _ptr(op.weights), _ptr(feat), torch.cuda.current_stream(dev).cuda_stream),
-                    "b2r_triplane_forward")
+        L.run("b2r_triplane_forward", dev, op.P, Cc, H, W, L.ptr(t), L.ptr(tf), L.ptr(op.is_face), L.ptr(op.corners),
+              L.ptr(op.weights), L.ptr(feat))
         ctx.op = op
         ctx.shape = tuple(triplane.shape)
         return feat
@@ -110,16 +104,13 @@ class _Triplane(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dfeat):
         op = ctx.op
-        lib = L.load()
         g = dfeat.to(torch.float32).contiguous()
         dev = g.device
         _, Cc, H, W = ctx.shape
         d = torch.empty(ctx.shape, dtype=torch.float32, device=dev)
         df = torch.empty(ctx.shape, dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_triplane_backward(op.P, Cc, H, W, _ptr(g), _ptr(op.offsets), _ptr(op.rows),
-                                              _ptr(op.entry_w), _ptr(d), _ptr(df),
-                                              torch.cuda.current_stream(dev).cuda_stream), "b2r_triplane_backward")
+        L.run("b2r_triplane_backward", dev, op.P, Cc, H, W, L.ptr(g), L.ptr(op.offsets), L.ptr(op.rows),
+              L.ptr(op.entry_w), L.ptr(d), L.ptr(df))
         return d, df, None
 
 
@@ -145,8 +136,7 @@ class TriplaneFeatures:
     def __init__(self, pos_enc_mesh: torch.Tensor, is_face: torch.Tensor, shape_3d=TRIPLANE_SHAPE_3D,
                  face_shape_3d=TRIPLANE_FACE_SHAPE_3D, plane_size: Tuple[int, int] = (128, 128)):
         fn = "TriplaneFeatures"
-        if not pos_enc_mesh.is_cuda:
-            raise RuntimeError(f"{fn}: pos_enc_mesh must be a CUDA tensor (got {pos_enc_mesh.device})")
+        L.cuda(fn, "pos_enc_mesh", pos_enc_mesh)
         if pos_enc_mesh.dim() != 2 or pos_enc_mesh.shape[1] != 3 or pos_enc_mesh.dtype != torch.float32:
             raise ValueError(f"{fn}: pos_enc_mesh must be (P,3) float32, got {pos_enc_mesh.dtype} "
                              f"{tuple(pos_enc_mesh.shape)}")
@@ -319,17 +309,14 @@ class _GnMlp(torch.autograd.Function):
         wh = torch.cat(hw, 0).contiguous()
         bh = torch.cat(hb, 0).contiguous()
         H = int(wh.shape[0])
-        m = L.B2RGnMlp(P=P, K=len(row_cols), H=H, x=_ptr(x), w_head=_ptr(wh), b_head=_ptr(bh))
+        m = L.B2RGnMlp(P=P, K=len(row_cols), H=H, x=L.ptr(x), w_head=L.ptr(wh), b_head=L.ptr(bh))
         for l in range(3):
-            m.w[l], m.b[l], m.gamma[l], m.beta[l] = (_ptr(t) for t in lay[l])
+            m.w[l], m.b[l], m.gamma[l], m.beta[l] = (L.ptr(t) for t in lay[l])
         out = torch.empty((P, H), dtype=torch.float32, device=dev)
         # needs_input_grad follows requires_grad only, also under torch.no_grad(); the grad mode of the call decides
         train = grad_mode and any(ctx.needs_input_grad)
         saved = torch.empty((3, P, HIDDEN), dtype=torch.float32, device=dev) if train else None
-        lib = L.load()
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_gn_mlp_forward(C.byref(m), _ptr(out), _ptr(saved),
-                                           torch.cuda.current_stream(dev).cuda_stream), "b2r_gn_mlp_forward")
+        L.run("b2r_gn_mlp_forward", dev, C.byref(m), L.ptr(out), L.ptr(saved))
         if train:
             ctx.spec = spec
             ctx.keep = (x, lay, wh, bh, c)  # the struct's pointers stay valid while these live
@@ -354,9 +341,8 @@ class _GnMlp(torch.autograd.Function):
         grads = torch.empty(int(lib.b2r_gn_mlp_grads_count(K, H)), dtype=torch.float32, device=dev)
         nbytes = int(lib.b2r_gn_mlp_scratch_bytes(P))
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_gn_mlp_backward(C.byref(m), _ptr(saved), _ptr(g), _ptr(dx), _ptr(grads), _ptr(scratch),
-                                            nbytes, torch.cuda.current_stream(dev).cuda_stream), "b2r_gn_mlp_backward")
+        L.run("b2r_gn_mlp_backward", dev, C.byref(m), L.ptr(saved), L.ptr(g), L.ptr(dx), L.ptr(grads), L.ptr(scratch),
+              nbytes)
         o = 0
 
         def take(*shape):
@@ -424,13 +410,12 @@ def gn_mlp(inputs: Sequence[torch.Tensor], trunk: nn.Sequential, heads: Optional
     for h in head_lins:
         params += [h.weight, h.bias]
     dev = params[0].device
-    for t in params + inputs:
-        if not t.is_cuda:
-            raise RuntimeError(f"gn_mlp: every tensor must be on a CUDA device (got {t.device}); there is no CPU path")
+    named = [(f"parameter {k}", p) for k, p in enumerate(params)] + [(f"input {i}", t) for i, t in enumerate(inputs)]
+    for name, t in named:
+        L.cuda("gn_mlp", name, t)
         if t.device != dev:
             raise ValueError(f"gn_mlp: tensors on {t.device} and {dev}")
-        if t.dtype != torch.float32:
-            raise ValueError(f"gn_mlp: every tensor must be float32, got {t.dtype}")
+        L.float32("gn_mlp", name, t)
     for i in row_blocks:
         if int(inputs[i].shape[0]) != P:
             raise ValueError(f"gn_mlp: per-row input {i} has {inputs[i].shape[0]} rows, input {row_blocks[0]} has {P}")

@@ -22,7 +22,6 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib as L
-from .rasterizer import _ptr
 
 C1 = 0.01 ** 2
 C2 = 0.03 ** 2
@@ -61,20 +60,17 @@ def _image_shape(name: str, t: torch.Tensor) -> Tuple[int, int]:
 class _L1Ssim(torch.autograd.Function):
     @staticmethod
     def forward(ctx, img, target, bbox, mask, with_ssim):
-        lib = L.load()
         dev = img.device
         H, W = img.shape[-2:]
         x = img.detach().reshape(3, H, W).contiguous()
         y = target.detach().reshape(3, H, W).contiguous()
         m = None if mask is None else mask.detach().reshape(H, W).contiguous()
         b = None if bbox is None else bbox.detach().reshape(4).to(torch.float32).contiguous()
-        nbytes = lib.b2r_l1ssim_scratch_bytes(W, H)
+        nbytes = L.load().b2r_l1ssim_scratch_bytes(W, H)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         out = torch.empty(2, dtype=torch.float32, device=dev)  # out[1] is written (and returned) only with SSIM
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_l1ssim_forward(W, H, _ptr(x), _ptr(y), _ptr(m), _ptr(b), int(with_ssim), _ptr(out),
-                                           _ptr(scratch), nbytes, torch.cuda.current_stream(dev).cuda_stream),
-                    "b2r_l1ssim_forward")
+        L.run("b2r_l1ssim_forward", dev, W, H, L.ptr(x), L.ptr(y), L.ptr(m), L.ptr(b), int(with_ssim), L.ptr(out),
+              L.ptr(scratch), nbytes)
         ctx.save_for_backward(x, y, m, b, scratch)
         ctx.with_ssim = with_ssim
         ctx.img_shape = img.shape
@@ -85,15 +81,12 @@ class _L1Ssim(torch.autograd.Function):
         if not ctx.needs_input_grad[0]:
             return None, None, None, None, None
         x, y, m, b, scratch = ctx.saved_tensors
-        lib = L.load()
         dev = x.device
         H, W = x.shape[-2:]
         g = dout.to(torch.float32).contiguous()
         dimg = torch.empty((3, H, W), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_l1ssim_backward(W, H, _ptr(x), _ptr(y), _ptr(m), _ptr(b), int(ctx.with_ssim), _ptr(g),
-                                            _ptr(dimg), _ptr(scratch), scratch.numel(),
-                                            torch.cuda.current_stream(dev).cuda_stream), "b2r_l1ssim_backward")
+        L.run("b2r_l1ssim_backward", dev, W, H, L.ptr(x), L.ptr(y), L.ptr(m), L.ptr(b), int(ctx.with_ssim), L.ptr(g),
+              L.ptr(dimg), L.ptr(scratch), scratch.numel())
         return dimg.reshape(ctx.img_shape), None, None, None, None
 
 
@@ -122,14 +115,14 @@ def l1_ssim(img: torch.Tensor, target: torch.Tensor, bbox: Optional[torch.Tensor
     run in a fixed order: two runs give bit-identical results.  CUDA tensors only: there is no CPU fallback.
     """
     for name, v in (("img", img), ("target", target), ("bbox", bbox), ("mask", mask)):
-        if v is not None and not v.is_cuda:
-            raise RuntimeError(f"l1_ssim: `{name}` must be a CUDA tensor (got {v.device}); there is no CPU fallback")
+        if v is not None:
+            L.cuda("l1_ssim", name, v)
     H, W = _image_shape("img", img)
     if _image_shape("target", target) != (H, W):
         raise ValueError(f"l1_ssim: target {tuple(target.shape)} does not match img {tuple(img.shape)}")
     for name, v in (("img", img), ("target", target), ("mask", mask)):
-        if v is not None and v.dtype != torch.float32:
-            raise ValueError(f"l1_ssim: `{name}` must be float32, got {v.dtype}")
+        if v is not None:
+            L.float32("l1_ssim", name, v)
     if mask is not None and (mask.dim() not in (2, 3, 4) or tuple(mask.shape[-2:]) != (H, W) or mask.numel() != H * W):
         raise ValueError(f"l1_ssim: mask must be (H,W), (1,H,W) or (1,1,H,W) with H,W = {H},{W}, "
                          f"got {tuple(mask.shape)}")
@@ -139,8 +132,7 @@ def l1_ssim(img: torch.Tensor, target: torch.Tensor, bbox: Optional[torch.Tensor
     for name, v in (("target", target), ("mask", mask)):
         if v is not None and v.requires_grad:
             raise ValueError(f"l1_ssim: `{name}` requires grad, but the op returns a gradient for `img` only")
-    if len({t.device for t in (img, target, bbox, mask) if t is not None}) != 1:
-        raise ValueError("l1_ssim: all tensors must be on the same device")
+    L.same_device("l1_ssim", (img, target, bbox, mask))
     out = _L1Ssim.apply(img, target, bbox, mask, bool(ssim))
     return (out[0], out[1]) if ssim else (out[0], None)
 

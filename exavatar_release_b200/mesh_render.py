@@ -80,7 +80,6 @@ import torch.nn.functional as F
 
 from . import _lib as L
 from .geometry import NORMAL_EPS, VertexNormals
-from .rasterizer import _ptr
 
 EPS = 1e-8  # pytorch3d's kEpsilon
 
@@ -92,8 +91,7 @@ def _cam_tensors(cam_param: Dict[str, torch.Tensor], device, fn: str,
         if k not in cam_param:
             raise ValueError(f"{fn}: cam_param has no `{k}`")
         v = cam_param[k]
-        if not isinstance(v, torch.Tensor) or not v.is_cuda:
-            raise RuntimeError(f"{fn}: cam_param['{k}'] must be a CUDA tensor; there is no CPU path")
+        L.cuda(fn, f"cam_param['{k}']", v)
         if v.numel() != n:
             raise ValueError(f"{fn}: cam_param['{k}'] must hold {n} values (batch 1), got {tuple(v.shape)}")
         if v.device != device:
@@ -105,19 +103,16 @@ def _cam_tensors(cam_param: Dict[str, torch.Tensor], device, fn: str,
 class _FaceRender(torch.autograd.Function):
     @staticmethod
     def forward(ctx, mesh, texture, R, t, focal, princpt, renderer, H, W):
-        lib = L.load()
         dev = mesh.device
         x = mesh.detach().reshape(-1, 3).contiguous()
         Cn = int(texture.shape[0])
         keys = renderer._keys_for(H * W)
         m = renderer._struct(x, texture, R, t, focal, princpt, H, W, keys)
-        nbytes = lib.b2r_mesh_render_scratch_bytes(renderer.num_faces)
+        nbytes = L.load().b2r_mesh_render_scratch_bytes(renderer.num_faces)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         image = torch.empty((Cn, H, W), dtype=torch.float32, device=dev)
         p2f = torch.empty((H, W), dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_mesh_render_forward(C.byref(m), _ptr(image), _ptr(p2f), _ptr(scratch), nbytes,
-                                                torch.cuda.current_stream(dev).cuda_stream), "b2r_mesh_render_forward")
+        L.run("b2r_mesh_render_forward", dev, C.byref(m), L.ptr(image), L.ptr(p2f), L.ptr(scratch), nbytes)
         ctx.save_for_backward(x, texture, R, t, focal, princpt, p2f, scratch)
         ctx.renderer = renderer
         ctx.size = (H, W)
@@ -130,17 +125,14 @@ class _FaceRender(torch.autograd.Function):
         if not ctx.needs_input_grad[0] or gimg is None:
             return (None,) * 9
         x, texture, R, t, focal, princpt, p2f, scratch = ctx.saved_tensors
-        lib = L.load()
         dev = x.device
         H, W = ctx.size
         r = ctx.renderer
         g = gimg.reshape(texture.shape[0], H, W).to(torch.float32).contiguous()
         dmesh = torch.empty((r.num_vertices, 3), dtype=torch.float32, device=dev)
         m = r._struct(x, texture, R, t, focal, princpt, H, W, None)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_mesh_render_backward(C.byref(m), _ptr(p2f), _ptr(g), _ptr(dmesh), _ptr(scratch),
-                                                 scratch.numel(), torch.cuda.current_stream(dev).cuda_stream),
-                    "b2r_mesh_render_backward")
+        L.run("b2r_mesh_render_backward", dev, C.byref(m), L.ptr(p2f), L.ptr(g), L.ptr(dmesh), L.ptr(scratch),
+              scratch.numel())
         return (dmesh.reshape(ctx.mesh_shape),) + (None,) * 8
 
 
@@ -167,14 +159,14 @@ class _CoverageTables:
         """texture None: the texture fields stay zero (the shaded render ignores them)."""
         m = L.B2RMeshRender()
         m.V, m.F, m.height, m.width = self.num_vertices, self.num_faces, H, W
-        m.mesh, m.faces = _ptr(x), _ptr(self.topology.faces)
+        m.mesh, m.faces = L.ptr(x), L.ptr(self.topology.faces)
         if texture is not None:
             m.Vt, m.C = int(self.vertex_uv.shape[0]), int(texture.shape[0])
             m.tex_height, m.tex_width = int(texture.shape[1]), int(texture.shape[2])
-            m.vertex_uv, m.face_uv, m.texture = _ptr(self.vertex_uv), _ptr(self.face_uv), _ptr(texture)
-        m.cam_R, m.cam_t, m.focal, m.princpt = _ptr(R), _ptr(t), _ptr(focal), _ptr(princpt)
-        m.keys = _ptr(keys)
-        m.vf_offsets, m.vf_entries = _ptr(self.topology.offsets), _ptr(self.topology.entries)
+            m.vertex_uv, m.face_uv, m.texture = L.ptr(self.vertex_uv), L.ptr(self.face_uv), L.ptr(texture)
+        m.cam_R, m.cam_t, m.focal, m.princpt = L.ptr(R), L.ptr(t), L.ptr(focal), L.ptr(princpt)
+        m.keys = L.ptr(keys)
+        m.vf_offsets, m.vf_entries = L.ptr(self.topology.offsets), L.ptr(self.topology.entries)
         return m
 
 
@@ -227,8 +219,7 @@ class FaceMeshRenderer(_CoverageTables):
         """The image (1,C,H,W) and the per-pixel face (H,W) int32 (-1: background; no gradient)."""
         fn = "FaceMeshRenderer"
         for name, v in (("uvmap", uvmap), ("mesh", mesh)):
-            if not v.is_cuda:
-                raise RuntimeError(f"{fn}: `{name}` must be a CUDA tensor (got {v.device}); there is no CPU path")
+            L.cuda(fn, name, v)
         if uvmap.requires_grad:
             raise ValueError(f"{fn}: `uvmap` requires grad, but the op returns a gradient for `mesh` only")
         if uvmap.dim() == 4 and uvmap.shape[0] != 1 or mesh.dim() == 3 and mesh.shape[0] != 1:
@@ -240,8 +231,7 @@ class FaceMeshRenderer(_CoverageTables):
             raise ValueError(f"{fn}: mesh must be (1,{self.num_vertices},3) or ({self.num_vertices},3), got "
                              f"{tuple(mesh.shape)}")
         for name, v in (("uvmap", uvmap), ("mesh", mesh)):
-            if v.dtype != torch.float32:
-                raise ValueError(f"{fn}: `{name}` must be float32, got {v.dtype}")
+            L.float32(fn, name, v)
             if v.device != self.device:
                 raise ValueError(f"{fn}: `{name}` is on {v.device}, the mesh tables on {self.device}")
         H, W = (int(s) for s in render_shape)
@@ -294,8 +284,7 @@ class ShadedMeshRenderer(_CoverageTables):
                  blend_ratio: float = 1.0) -> torch.Tensor:
         fn = "ShadedMeshRenderer"
         for name, v in (("mesh", mesh), ("bkg", bkg)):
-            if not v.is_cuda:
-                raise RuntimeError(f"{fn}: `{name}` must be a CUDA tensor (got {v.device}); there is no CPU path")
+            L.cuda(fn, name, v)
         if mesh.dim() == 3 and mesh.shape[0] != 1:
             raise ValueError(f"{fn}: only a batch of 1 is supported (mesh {tuple(mesh.shape)})")
         if mesh.dim() not in (2, 3) or mesh.shape[-1] != 3 or mesh.shape[-2] != self.num_vertices:
@@ -307,8 +296,7 @@ class ShadedMeshRenderer(_CoverageTables):
         if H < 1 or W < 1 or H * W >= 2 ** 31:
             raise ValueError(f"{fn}: bad image size {(H, W)}")
         for name, v in (("mesh", mesh), ("bkg", bkg)):
-            if v.dtype != torch.float32:
-                raise ValueError(f"{fn}: `{name}` must be float32, got {v.dtype}")
+            L.float32(fn, name, v)
             if v.device != self.device:
                 raise ValueError(f"{fn}: `{name}` is on {v.device}, the mesh tables on {self.device}")
         if isinstance(blend_ratio, bool) or not isinstance(blend_ratio, numbers.Real) or \
@@ -320,19 +308,15 @@ class ShadedMeshRenderer(_CoverageTables):
 
     def _shade(self, x, normals, focal, princpt, bkg, blend_ratio: float) -> torch.Tensor:
         """b2r_mesh_shade_forward on checked, contiguous float32 tensors; `normals` (V,3) per vertex."""
-        lib = L.load()
         H, W = int(bkg.shape[0]), int(bkg.shape[1])
         m = self._struct(x, None, self.R, self.t, focal, princpt, H, W, self._keys_for(H * W))
-        nbytes = lib.b2r_mesh_render_scratch_bytes(self.num_faces)
+        nbytes = L.load().b2r_mesh_render_scratch_bytes(self.num_faces)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         out = torch.empty((H, W, 3), dtype=torch.float32, device=self.device)
         # vis.py's `render * blend_ratio + bkg / 255 * (1 - blend_ratio)`: numpy rounds the Python floats blend_ratio
         # and (1 - blend_ratio), the latter taken in double, to float32; ctypes' c_float rounds the same way
-        with torch.cuda.device(self.device):
-            L.check(lib.b2r_mesh_shade_forward(C.byref(m), _ptr(normals), _ptr(bkg), blend_ratio, 1.0 - blend_ratio,
-                                               _ptr(out), _ptr(scratch), nbytes,
-                                               torch.cuda.current_stream(self.device).cuda_stream),
-                    "b2r_mesh_shade_forward")
+        L.run("b2r_mesh_shade_forward", self.device, C.byref(m), L.ptr(normals), L.ptr(bkg), blend_ratio,
+              1.0 - blend_ratio, L.ptr(out), L.ptr(scratch), nbytes)
         return out
 
 

@@ -24,8 +24,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib as L
-from .perceptual import EPS, SCALE, SHIFT
-from .rasterizer import _ptr
+from .perceptual import EPS, SCALE, SHIFT, _lin_vectors, _lpips_modules
 
 # torchvision alexnet().features[0:12]: (child index, C_in, C_out, kernel, stride, padding) of the five convs
 ALEX_CONVS = ((0, 3, 64, 11, 4, 2), (3, 64, 192, 5, 1, 2), (6, 192, 384, 3, 1, 1), (8, 384, 256, 3, 1, 1),
@@ -60,17 +59,6 @@ def _alex_convs(features) -> List[torch.nn.Conv2d]:
                 or m.padding not in (0, (0, 0)) or m.ceil_mode:
             raise ValueError(f"neuman: module {i} must be a 3x3 stride-2 floor max pool, got {m}")
     return convs
-
-
-def _lin_vectors(lin_weights: Sequence[torch.Tensor]) -> List[torch.Tensor]:
-    if len(lin_weights) != 5:
-        raise ValueError(f"neuman: expected 5 lin weights, got {len(lin_weights)}")
-    out = []
-    for k, (w, c) in enumerate(zip(lin_weights, TAP_CHANNELS)):
-        if w.numel() != c:
-            raise ValueError(f"neuman: lin weight {k} must be (1,{c},1,1), got {tuple(w.shape)}")
-        out.append(w.detach().reshape(c))
-    return out
 
 
 def gaussian_window(device=None) -> torch.Tensor:
@@ -144,7 +132,7 @@ def neuman_scores_reference(render: torch.Tensor, target: torch.Tensor, mask: Op
         return [v / (torch.sqrt(torch.sum(v ** 2, dim=1, keepdim=True)) + EPS) for v in fs]
 
     lp = 0
-    for a, b, w in zip(taps(x), taps(y), _lin_vectors(lin_weights)):
+    for a, b, w in zip(taps(x), taps(y), _lin_vectors(lin_weights, TAP_CHANNELS, "neuman")):
         lp = lp + (w.to(device=dev, dtype=dtype).reshape(1, -1, 1, 1) * (a - b) ** 2).sum(1).mean((1, 2))
     return torch.stack((psnr, ssim, lp), 1)
 
@@ -163,7 +151,7 @@ class NeumanScores:
 
     def __init__(self, alex_features, lin_weights: Sequence[torch.Tensor], device):
         convs = _alex_convs(alex_features)
-        lins = _lin_vectors(lin_weights)
+        lins = _lin_vectors(lin_weights, TAP_CHANNELS, "neuman")
         dev = torch.device(device)
         if dev.type != "cuda":
             raise RuntimeError(f"neuman: device must be a CUDA device (got {dev}); there is no CPU fallback")
@@ -184,20 +172,14 @@ class NeumanScores:
         """From an `lpips.LPIPS(net='alex')` instance, or the `.net` of torchmetrics'
         LearnedPerceptualImagePatchSimilarity(net_type='alex'): the convs of `m.net.slice1..5` (which keep
         torchvision's child indices) and the weights `m.lin{k}.model[-1].weight`, on the device of those weights."""
-        mods = {}
-        for k in range(1, 6):
-            for name, mod in getattr(m.net, f"slice{k}").named_children():
-                mods[int(name)] = mod
-        if sorted(mods) != list(range(ALEX_SLICES[-1][1])):
-            raise ValueError(f"neuman: m.net.slice1..5 must hold alexnet().features[0:12], got indices {sorted(mods)}")
-        lins = [getattr(m, f"lin{k}").model[-1].weight for k in range(5)]
-        return cls(torch.nn.Sequential(*(mods[i] for i in range(ALEX_SLICES[-1][1]))), lins, lins[0].device)
+        features, lins = _lpips_modules(m, "alexnet().features", ALEX_SLICES[-1][1], "neuman")
+        return cls(features, lins, lins[0].device)
 
     def _args(self, W, H, N, x, y, m, mc) -> L.B2RNeumanScores:
-        p = L.B2RNeumanScores(width=W, height=H, n_images=N, mask_channels=mc, render=_ptr(x), target=_ptr(y),
-                              mask=_ptr(m))
+        p = L.B2RNeumanScores(width=W, height=H, n_images=N, mask_channels=mc, render=L.ptr(x), target=L.ptr(y),
+                              mask=L.ptr(m))
         for k in range(5):
-            p.w[k], p.bias[k], p.lin[k] = _ptr(self.w[k]), _ptr(self.bias[k]), _ptr(self.lin[k])
+            p.w[k], p.bias[k], p.lin[k] = L.ptr(self.w[k]), L.ptr(self.bias[k]), L.ptr(self.lin[k])
         return p
 
     def __call__(self, render: torch.Tensor, target: torch.Tensor,
@@ -216,10 +198,9 @@ class NeumanScores:
         bit-identical scores.  The caller averages the rows, as eval_neuman averages the frames.
         """
         for name, v in (("render", render), ("target", target), ("mask", mask)):
-            if v is not None and not v.is_cuda:
-                raise RuntimeError(f"neuman: `{name}` must be a CUDA tensor (got {v.device}); there is no CPU fallback")
-            if v is not None and v.dtype != torch.float32:
-                raise ValueError(f"neuman: `{name}` must be float32, got {v.dtype}")
+            if v is not None:
+                L.cuda("neuman", name, v)
+                L.float32("neuman", name, v)
         if render.dim() not in (3, 4) or render.shape[-3] != 3:
             raise ValueError(f"neuman: render must be (3,H,W) or (N,3,H,W), got {tuple(render.shape)}")
         if target.shape != render.shape:
@@ -234,17 +215,13 @@ class NeumanScores:
             if mc not in (1, 3) or mask.shape[:-3] != render.shape[:-3] or mask.shape[-2:] != render.shape[-2:]:
                 raise ValueError(f"neuman: mask must be {tuple(render.shape[:-3])} x (1 or 3,H,W) to match render "
                                  f"{tuple(render.shape)}, got {tuple(mask.shape)}")
-        if len({t.device for t in (render, target, mask) if t is not None} | {self.device}) != 1:
-            raise ValueError("neuman: all tensors must be on the op's device")
-        lib = L.load()
+        L.same_device("neuman", (render, target, mask), self.device)
         x = render.detach().contiguous()
         y = target.detach().contiguous()
         m = None if mask is None else mask.detach().contiguous()
-        n_scratch = lib.b2r_neuman_scratch_bytes(W, H, N)
+        n_scratch = L.load().b2r_neuman_scratch_bytes(W, H, N)
         scratch = torch.empty(n_scratch, dtype=torch.uint8, device=self.device)
         out = torch.empty((N, 3), dtype=torch.float32, device=self.device)
         p = self._args(W, H, N, x, y, m, mc)
-        with torch.cuda.device(self.device):
-            L.check(lib.b2r_neuman_scores(C.byref(p), _ptr(out), _ptr(scratch), n_scratch,
-                                          torch.cuda.current_stream(self.device).cuda_stream), "b2r_neuman_scores")
+        L.run("b2r_neuman_scores", self.device, C.byref(p), L.ptr(out), L.ptr(scratch), n_scratch)
         return out

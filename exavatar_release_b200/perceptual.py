@@ -23,7 +23,6 @@ import torch.nn.functional as F
 
 from . import _lib as L
 from .losses import crop_box
-from .rasterizer import _ptr
 
 SHIFT = (-.030, -.088, -.188)  # lpips ScalingLayer
 SCALE = (.458, .448, .450)
@@ -46,15 +45,28 @@ def _vgg_convs(vgg_features) -> List[torch.nn.Conv2d]:
     return convs
 
 
-def _lin_vectors(lin_weights: Sequence[torch.Tensor]) -> List[torch.Tensor]:
-    if len(lin_weights) != 5:
-        raise ValueError(f"lpips: expected 5 lin weights, got {len(lin_weights)}")
+def _lin_vectors(lin_weights: Sequence[torch.Tensor], channels: Sequence[int], prefix: str) -> List[torch.Tensor]:
+    """The (1,C,1,1) weights of lpips's lin layers as C-vectors, one per tap of `channels`."""
+    if len(lin_weights) != len(channels):
+        raise ValueError(f"{prefix}: expected {len(channels)} lin weights, got {len(lin_weights)}")
     out = []
-    for k, (w, c) in enumerate(zip(lin_weights, TAP_CHANNELS)):
+    for k, (w, c) in enumerate(zip(lin_weights, channels)):
         if w.numel() != c:
-            raise ValueError(f"lpips: lin weight {k} must be (1,{c},1,1), got {tuple(w.shape)}")
+            raise ValueError(f"{prefix}: lin weight {k} must be (1,{c},1,1), got {tuple(w.shape)}")
         out.append(w.detach().reshape(c))
     return out
+
+
+def _lpips_modules(m, features: str, n: int, prefix: str) -> Tuple[torch.nn.Sequential, List[torch.Tensor]]:
+    """The first `n` modules of the backbone's `features` held by an lpips.LPIPS instance's `m.net.slice1..5` (which
+    keep torchvision's child indices), and its lin weights `m.lin{k}.model[-1].weight`."""
+    mods = {}
+    for k in range(1, 6):
+        for name, mod in getattr(m.net, f"slice{k}").named_children():
+            mods[int(name)] = mod
+    if sorted(mods) != list(range(n)):
+        raise ValueError(f"{prefix}: m.net.slice1..5 must hold {features}[0:{n}], got indices {sorted(mods)}")
+    return torch.nn.Sequential(*(mods[i] for i in range(n))), [getattr(m, f"lin{k}").model[-1].weight for k in range(5)]
 
 
 def _image_shape(name: str, t: torch.Tensor, batch: bool) -> Tuple[int, int]:
@@ -80,9 +92,7 @@ class _Lpips(torch.autograd.Function):
         saved = torch.empty(n_saved, dtype=torch.uint8, device=dev)
         scratch = torch.empty(n_scratch, dtype=torch.uint8, device=dev)
         out = torch.empty(N, dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_lpips_forward(C.byref(p), _ptr(out), _ptr(saved), n_saved, _ptr(scratch), n_scratch,
-                                          torch.cuda.current_stream(dev).cuda_stream), "b2r_lpips_forward")
+        L.run("b2r_lpips_forward", dev, C.byref(p), L.ptr(out), L.ptr(saved), n_saved, L.ptr(scratch), n_scratch)
         ctx.save_for_backward(x, y, b, saved)
         ctx.op = op
         ctx.img_shape = img.shape
@@ -93,18 +103,15 @@ class _Lpips(torch.autograd.Function):
         if not ctx.needs_input_grad[0]:
             return None, None, None, None
         x, y, b, saved = ctx.saved_tensors
-        lib = L.load()
         dev = x.device
         N, _, H, W = x.shape
         g = dout.reshape(N).to(torch.float32).contiguous()
         dimg = torch.empty((N, 3, H, W), dtype=torch.float32, device=dev)
-        n_scratch = lib.b2r_lpips_scratch_bytes(W, H)
+        n_scratch = L.load().b2r_lpips_scratch_bytes(W, H)
         scratch = torch.empty(n_scratch, dtype=torch.uint8, device=dev)
         p = ctx.op._args(W, H, N, x, y, b)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_lpips_backward(C.byref(p), _ptr(saved), saved.numel(), _ptr(g), _ptr(dimg), _ptr(scratch),
-                                           n_scratch, torch.cuda.current_stream(dev).cuda_stream),
-                    "b2r_lpips_backward")
+        L.run("b2r_lpips_backward", dev, C.byref(p), L.ptr(saved), saved.numel(), L.ptr(g), L.ptr(dimg), L.ptr(scratch),
+              n_scratch)
         return dimg.reshape(ctx.img_shape), None, None, None
 
 
@@ -124,7 +131,7 @@ class LPIPS:
 
     def __init__(self, vgg_features, lin_weights: Sequence[torch.Tensor], device):
         convs = _vgg_convs(vgg_features)
-        lins = _lin_vectors(lin_weights)
+        lins = _lin_vectors(lin_weights, TAP_CHANNELS, "lpips")
         dev = torch.device(device)
         if dev.type != "cuda":
             raise RuntimeError(f"lpips: device must be a CUDA device (got {dev}); there is no CPU fallback")
@@ -140,25 +147,19 @@ class LPIPS:
     def from_lpips(cls, m) -> "LPIPS":
         """From an `lpips.LPIPS(net='vgg')` instance: the convs of `m.net.slice1..5` (which keep torchvision's child
         indices) and the weights `m.lin{k}.model[-1].weight`, on the device of those weights."""
-        mods = {}
-        for k in range(1, 6):
-            for name, mod in getattr(m.net, f"slice{k}").named_children():
-                mods[int(name)] = mod
-        if sorted(mods) != list(range(SLICES[-1][1])):
-            raise ValueError(f"lpips: m.net.slice1..5 must hold vgg16().features[0:30], got indices {sorted(mods)}")
-        lins = [getattr(m, f"lin{k}").model[-1].weight for k in range(5)]
-        return cls(torch.nn.Sequential(*(mods[i] for i in range(SLICES[-1][1]))), lins, lins[0].device)
+        features, lins = _lpips_modules(m, "vgg16().features", SLICES[-1][1], "lpips")
+        return cls(features, lins, lins[0].device)
 
     def _args(self, W, H, N, x, y, b) -> L.B2RLpips:
-        p = L.B2RLpips(width=W, height=H, n_images=N, img=_ptr(x), target=_ptr(y), bbox=_ptr(b))
-        p.w_fwd[0] = _ptr(self.w_fwd[0])
+        p = L.B2RLpips(width=W, height=H, n_images=N, img=L.ptr(x), target=L.ptr(y), bbox=L.ptr(b))
+        p.w_fwd[0] = L.ptr(self.w_fwd[0])
         for k in range(1, 13):
-            p.w_fwd[k] = _ptr(self.w_fwd[k])
-            p.w_bwd[k] = _ptr(self.w_bwd[k - 1])
+            p.w_fwd[k] = L.ptr(self.w_fwd[k])
+            p.w_bwd[k] = L.ptr(self.w_bwd[k - 1])
         for k in range(13):
-            p.bias[k] = _ptr(self.bias[k])
+            p.bias[k] = L.ptr(self.bias[k])
         for k in range(5):
-            p.lin[k] = _ptr(self.lin[k])
+            p.lin[k] = L.ptr(self.lin[k])
         return p
 
     def __call__(self, img_out: torch.Tensor, img_target: torch.Tensor,
@@ -179,8 +180,8 @@ class LPIPS:
         carry a box of another size), and every reduction runs in a fixed order: two runs give bit-identical results.
         """
         for name, v in (("img_out", img_out), ("img_target", img_target), ("bbox", bbox)):
-            if v is not None and not v.is_cuda:
-                raise RuntimeError(f"lpips: `{name}` must be a CUDA tensor (got {v.device}); there is no CPU fallback")
+            if v is not None:
+                L.cuda("lpips", name, v)
         H, W = _image_shape("img_out", img_out, True)
         if _image_shape("img_target", img_target, False) != (H, W):
             raise ValueError(f"lpips: img_target {tuple(img_target.shape)} does not match img_out "
@@ -188,15 +189,13 @@ class LPIPS:
         if H < MIN_CROP or W < MIN_CROP:
             raise ValueError(f"lpips: images must be at least {MIN_CROP}x{MIN_CROP}, got {H}x{W}")
         for name, v in (("img_out", img_out), ("img_target", img_target)):
-            if v.dtype != torch.float32:
-                raise ValueError(f"lpips: `{name}` must be float32, got {v.dtype}")
+            L.float32("lpips", name, v)
         if bbox is not None and (tuple(bbox.shape) not in ((4,), (1, 4)) or not bbox.is_floating_point()):
             raise ValueError(f"lpips: bbox must be a float tensor of shape (4,) or (1,4), got {bbox.dtype} "
                              f"{tuple(bbox.shape)}")
         if img_target.requires_grad:
             raise ValueError("lpips: `img_target` requires grad, but the op returns a gradient for `img_out` only")
-        if len({t.device for t in (img_out, img_target, bbox) if t is not None} | {self.device}) != 1:
-            raise ValueError("lpips: all tensors must be on the op's device")
+        L.same_device("lpips", (img_out, img_target, bbox), self.device)
         return _Lpips.apply(img_out, self, img_target, bbox)
 
 
@@ -236,7 +235,7 @@ def lpips_reference(img_out: torch.Tensor, img_target: torch.Tensor, bbox: Optio
 
     fa, fb = taps(img_out), taps(img_target)
     val = 0
-    for a, b, w in zip(fa, fb, _lin_vectors(lin_weights)):
+    for a, b, w in zip(fa, fb, _lin_vectors(lin_weights, TAP_CHANNELS, "lpips")):
         lin = F.conv2d((a - b) ** 2, w.to(device=dev, dtype=dtype).reshape(1, -1, 1, 1))
         val = val + lin.mean([2, 3], keepdim=True)
     return val

@@ -18,7 +18,7 @@ from typing import Dict, Optional
 import torch
 
 from . import _lib as L
-from .rasterizer import _f32c, _make_scene, _ptr
+from .rasterizer import _f32c, _make_scene
 
 # the per-Gaussian asset tensors of a render: asset key -> (name of its gradient, floats per Gaussian)
 ASSETS = {"mean_3d": ("means3D", 3), "opacity": ("opacities", 1), "scale": ("scales", 3), "rotation": ("rotations", 4),
@@ -32,7 +32,7 @@ def _backward_args(images, grads, accumulate: bool = False, first_row: int = 0, 
     outs = [grads.get(k) for k in ("means3D", "means2D", "shs", "colors", "opacities", "scales", "rotations", "cov3D")]
     dens = [(densify or {}).get(k) for k in ("grad_accum", "count", "radius_max")]
     flags = (L.B2R_BWD_ACCUMULATE if accumulate else 0) | L.B2R_BWD_SCRATCH_ZEROED
-    return L.B2RBackwardArgs(*map(_ptr, images), *map(_ptr, outs), flags, int(first_row), *map(_ptr, dens),
+    return L.B2RBackwardArgs(*map(L.ptr, images), *map(L.ptr, outs), flags, int(first_row), *map(L.ptr, dens),
                              int(densify_rows) if densify is not None else 0)
 
 
@@ -488,7 +488,7 @@ class MergedFivePlan(_FiveRenders):
         # human-only view shows the bare background there.  Both are pre-filled (`_forward_view`) and skipped by the
         # kernels.
         skip = self.Ps if name != "scene" else 0
-        return L.B2RView(lo, hi, _ptr(bg), fT.data_ptr(), nc.data_ptr(), ps.ck[v].data_ptr(), ps.ckpt_bytes, skip, 0)
+        return L.B2RView(lo, hi, L.ptr(bg), fT.data_ptr(), nc.data_ptr(), ps.ck[v].data_ptr(), ps.ckpt_bytes, skip, 0)
 
     # ---- the steps of a frame; each enqueues on the stream `s` it is given, which is also the current stream ----
     def _start_pass(self, s, pk, key, settings, src, bg_h, a_binned) -> None:

@@ -29,6 +29,7 @@ import torch
 from torch import nn
 
 from . import _lib as L
+from .skinning import skin_gaussians
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -54,10 +55,6 @@ CAPACITY_HEADROOM = 1.25
 # capturable in a CUDA graph (torch.cuda.graph) together with the caller's loss, backward and copies.  Overflow is
 # not repaired on the fly in this mode: check `overflowed()` after the step (outputs are truncated, never corrupt).
 FIXED_CAPACITY = None
-
-
-def _ptr(t: Optional[torch.Tensor]):
-    return None if t is None or t.numel() == 0 else t.data_ptr()
 
 
 def _f32c(t: torch.Tensor, name: str) -> torch.Tensor:
@@ -107,18 +104,18 @@ def _make_scene(settings: GaussianRasterizationSettings, means3D, shs, colors, o
     if tanfov is None:
         sc.tanfovx = float(settings.tanfovx)
         sc.tanfovy = float(settings.tanfovy)
-    sc.tanfov = _ptr(keep["tanfov"])
-    sc.bg = _ptr(keep["bg"])
-    sc.viewmatrix = _ptr(keep["view"])
-    sc.projmatrix = _ptr(keep["proj"])
-    sc.campos = _ptr(keep["campos"])
-    sc.means3D = _ptr(means3D)
-    sc.shs = _ptr(shs)
-    sc.colors_precomp = _ptr(colors)
-    sc.opacities = _ptr(opac)
-    sc.scales = _ptr(scales)
-    sc.rotations = _ptr(rots)
-    sc.cov3D_precomp = _ptr(cov)
+    sc.tanfov = L.ptr(keep["tanfov"])
+    sc.bg = L.ptr(keep["bg"])
+    sc.viewmatrix = L.ptr(keep["view"])
+    sc.projmatrix = L.ptr(keep["proj"])
+    sc.campos = L.ptr(keep["campos"])
+    sc.means3D = L.ptr(means3D)
+    sc.shs = L.ptr(shs)
+    sc.colors_precomp = L.ptr(colors)
+    sc.opacities = L.ptr(opac)
+    sc.scales = L.ptr(scales)
+    sc.rotations = L.ptr(rots)
+    sc.cov3D_precomp = L.ptr(cov)
     return sc, keep
 
 
@@ -194,14 +191,11 @@ class GaussianRasterizer(nn.Module):
 
     def markVisible(self, positions):
         """bool (P): Gaussians in front of the near plane (z_view > 0.2).  Unused by ExAvatar; kept for API parity."""
-        lib = L.load()
         with torch.no_grad():
             p = _f32c(positions, "positions")
             view = _f32c(self.raster_settings.viewmatrix.to(p.device), "viewmatrix")
             present = torch.empty(p.shape[0], dtype=torch.uint8, device=p.device)
-            with torch.cuda.device(p.device):
-                L.check(lib.b2r_mark_visible(p.shape[0], _ptr(p), _ptr(view), _ptr(present),
-                                             torch.cuda.current_stream(p.device).cuda_stream), "b2r_mark_visible")
+            L.run("b2r_mark_visible", p.device, p.shape[0], L.ptr(p), L.ptr(view), L.ptr(present))
             return present.bool()
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
@@ -247,19 +241,8 @@ class SkinnedGaussianRasterizer(nn.Module):
 
     def forward(self, xyz, skin_weights, joint_mats, trans, cam_R, cam_t, means2D, opacities, colors_precomp, scales,
                 rotations):
-        from .skinning import skin_gaussians  # skinning.py imports this module's tensor helpers
         posed = skin_gaussians(xyz, None, skin_weights, None, joint_mats, trans, cam_R, cam_t)[0]
         color, radii, depth, alpha = GaussianRasterizer(self.raster_settings)(
             means3D=posed, means2D=means2D, opacities=opacities, colors_precomp=colors_precomp, scales=scales,
             rotations=rotations)
         return color, radii, depth, alpha, posed
-
-
-def _inv3(R: torch.Tensor) -> torch.Tensor:
-    """3x3 inverse by cofactors: a handful of elementwise kernels, no cuSOLVER call -- capturable in a CUDA graph
-    (`torch.inverse`, which the reference uses at module.py:556, synchronises)."""
-    a, b, c, d, e, f, g, h, i = R.reshape(9).unbind()
-    adj = torch.stack((e * i - f * h, c * h - b * i, b * f - c * e,
-                       f * g - d * i, a * i - c * g, c * d - a * f,
-                       d * h - e * g, b * g - a * h, a * e - b * d)).reshape(3, 3)
-    return adj / (a * (e * i - f * h) - b * (d * i - f * g) + c * (d * h - e * g))

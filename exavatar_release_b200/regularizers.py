@@ -26,7 +26,6 @@ import torch.nn.functional as F
 
 from . import _lib as L
 from .geometry import VertexNormals, vertex_normals_reference
-from .rasterizer import _ptr
 
 KEYS = ("gaussian_mean_reg", "gaussian_mean_hand_reg", "gaussian_scale_reg", "lap_mean", "lap_scale", "lap_rgb",
         "hand_rgb_reg", "arm_rgb_reg", "joint_offset_reg", "joint_offset_sym_reg")
@@ -93,17 +92,14 @@ def _rows(name: str, t: torch.Tensor, P: int, k: int) -> torch.Tensor:
     ok = shape in ((P, k), (1, P, k)) or (k == 1 and shape in ((P,), (1, P)))
     if not ok:
         raise ValueError(f"HumanRegularizers: `{name}` must be ({P},{k}) or (1,{P},{k}), got {shape}")
-    if not t.is_cuda:
-        raise RuntimeError(f"HumanRegularizers: `{name}` must be a CUDA tensor (got {t.device}); there is no CPU path")
-    if t.dtype != torch.float32:
-        raise ValueError(f"HumanRegularizers: `{name}` must be float32, got {t.dtype}")
+    L.cuda("HumanRegularizers", name, t)
+    L.float32("HumanRegularizers", name, t)
     return t.detach().reshape(P * k).contiguous()
 
 
 class _Regs(torch.autograd.Function):
     @staticmethod
     def forward(ctx, regs, mesh, mo, moo, so, s, sr, rgb, rgbr, jo, sreg):
-        lib = L.load()
         P, dev = regs.num_vertices, regs.device
         ins = [_rows("mesh_neutral_pose", mesh, P, 3), _rows("mean_offset", mo, P, 3),
                _rows("mean_offset_offset", moo, P, 3), _rows("scale_offset", so, P, 1), _rows("scale", s, P, 3),
@@ -116,9 +112,7 @@ class _Regs(torch.autograd.Function):
         nbytes = regs.scratch_bytes
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         out = torch.empty(len(KEYS), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_regs_forward(C.byref(st), _ptr(out), _ptr(scratch), nbytes,
-                                         torch.cuda.current_stream(dev).cuda_stream), "b2r_regs_forward")
+        L.run("b2r_regs_forward", dev, C.byref(st), L.ptr(out), L.ptr(scratch), nbytes)
         ctx.regs = regs
         ctx.shapes = [t.shape for t in (mo, moo, so, s, sr, rgb, rgbr, jo)] + [None if sreg is None else sreg.shape]
         ctx.save_for_backward(*[t for t in ins if t is not None], scratch)
@@ -132,16 +126,13 @@ class _Regs(torch.autograd.Function):
         ins = saved + ([] if ctx.has_sreg else [None])
         regs = ctx.regs
         dev = regs.device
-        lib = L.load()
         g = dout.to(torch.float32).contiguous()
         grads = [torch.empty_like(t) for t in ins[1:9]] + [None if ins[9] is None else torch.empty_like(ins[9])]
-        gs = L.B2RRegsGrads(**{k: _ptr(t) for k, t in zip(("mean_offset", "mean_offset_offset", "scale_offset", "scale",
-                                                            "scale_refined", "rgb", "rgb_refined", "joint_offset",
-                                                            "scale_reg"), grads)})
+        gs = L.B2RRegsGrads(**{k: L.ptr(t) for k, t in zip(("mean_offset", "mean_offset_offset", "scale_offset",
+                                                             "scale", "scale_refined", "rgb", "rgb_refined",
+                                                             "joint_offset", "scale_reg"), grads)})
         st = regs._struct(ins)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_regs_backward(C.byref(st), _ptr(g), C.byref(gs), _ptr(scratch), scratch.numel(),
-                                          torch.cuda.current_stream(dev).cuda_stream), "b2r_regs_backward")
+        L.run("b2r_regs_backward", dev, C.byref(st), L.ptr(g), C.byref(gs), L.ptr(scratch), scratch.numel())
         out = [None if t is None else t.reshape(shape) for t, shape in zip(grads, ctx.shapes)]
         return (None, None, *out)
 
@@ -182,7 +173,7 @@ class HumanRegularizers:
                 torch.device("cuda", torch.cuda.current_device())
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError(f"HumanRegularizers: device must be CUDA (got {device}); there is no CPU path")
+            raise RuntimeError(f"HumanRegularizers: device must be CUDA (got {device}); there is no CPU fallback")
         if device.index is None:
             device = torch.device("cuda", torch.cuda.current_device())
         P = int(num_vertices)
@@ -220,17 +211,18 @@ class HumanRegularizers:
         self._template = L.B2RRegs(
             P=P, J=self.num_joints, n_arm=self.n_arm, n_pairs=int(self.sym_pairs.shape[0]),
             n_hand=int((tab["is_rhand"] | tab["is_lhand"]).sum()), n_rhand=int(tab["is_rhand"].sum()),
-            faces=_ptr(self.normals.faces), vf_offsets=_ptr(self.normals.offsets), vf_entries=_ptr(self.normals.entries),
-            nbr_idx=_ptr(self.nbr_idx), nbr_w=_ptr(self.nbr_w), lapT_offsets=_ptr(self.lapT_offsets),
-            lapT_src=_ptr(self.lapT_src), lapT_w=_ptr(self.lapT_w), weights=_ptr(self.weights), hand=_ptr(self.hand),
-            arm_idx=_ptr(self.arm_idx) if self.n_arm else None, arm_slot=_ptr(self.arm_slot),
-            joint_target=_ptr(self.joint_target), joint_weight=_ptr(self.joint_weight), sym_pairs=_ptr(self.sym_pairs))
+            faces=L.ptr(self.normals.faces), vf_offsets=L.ptr(self.normals.offsets),
+            vf_entries=L.ptr(self.normals.entries), nbr_idx=L.ptr(self.nbr_idx), nbr_w=L.ptr(self.nbr_w),
+            lapT_offsets=L.ptr(self.lapT_offsets), lapT_src=L.ptr(self.lapT_src), lapT_w=L.ptr(self.lapT_w),
+            weights=L.ptr(self.weights), hand=L.ptr(self.hand), arm_idx=L.ptr(self.arm_idx) if self.n_arm else None,
+            arm_slot=L.ptr(self.arm_slot), joint_target=L.ptr(self.joint_target),
+            joint_weight=L.ptr(self.joint_weight), sym_pairs=L.ptr(self.sym_pairs))
 
     def _struct(self, ins) -> "L.B2RRegs":
         st = L.B2RRegs.from_buffer_copy(self._template)
         for name, t in zip(("mesh", "mean_offset", "mean_offset_offset", "scale_offset", "scale", "scale_refined", "rgb",
                             "rgb_refined", "joint_offset", "scale_reg"), ins):
-            setattr(st, name, _ptr(t))
+            setattr(st, name, L.ptr(t))
         return st
 
     def __call__(self, mesh_neutral_pose, mean_offset, mean_offset_offset, scale_offset, scale, scale_refined, rgb,

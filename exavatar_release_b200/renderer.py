@@ -72,10 +72,7 @@ def device_render_settings(img_shape, cam_param, bg):
     R, t, focal = (x.to(dev, torch.float32).contiguous() for x in (R.reshape(9), t.reshape(3), focal.reshape(2)))
     H, W = int(img_shape[0]), int(img_shape[1])
     block = torch.empty(37, dtype=torch.float32, device=dev)
-    lib = L.load()
-    with torch.cuda.device(dev):
-        L.check(lib.b2r_camera_setup(R.data_ptr(), t.data_ptr(), focal.data_ptr(), W, H, block.data_ptr(),
-                                     torch.cuda.current_stream(dev).cuda_stream), "b2r_camera_setup")
+    L.run("b2r_camera_setup", dev, R.data_ptr(), t.data_ptr(), focal.data_ptr(), W, H, block.data_ptr())
     return GaussianRasterizationSettings(image_height=H, image_width=W, tanfovx=block[35], tanfovy=block[36], bg=bg,
                                          scale_modifier=1.0, viewmatrix=block[0:16].view(4, 4),
                                          projmatrix=block[16:32].view(4, 4), sh_degree=0, campos=block[32:35],

@@ -24,7 +24,7 @@ from typing import Optional
 import torch
 
 from . import _lib as L
-from .rasterizer import _inv3, _ptr
+from .camera import _inv3
 from .sh import sh_to_rgb
 from .smplx_rig import matrix_to_quaternion, rotation_6d_to_matrix
 
@@ -41,16 +41,15 @@ def _rows(t: torch.Tensor, row_len: int):
 
 def _struct(P, M, mean, logit, log_scale, rot6d, dc, dc_stride, rest, rest_stride, deg, R, t) -> "L.B2RSceneAssets":
     s = L.B2RSceneAssets(P=P, M=M, dc_stride=dc_stride, rest_stride=rest_stride)
-    s.mean, s.opacity_logit, s.log_scale, s.rotation6d = _ptr(mean), _ptr(logit), _ptr(log_scale), _ptr(rot6d)
-    s.feature_dc, s.feature_rest, s.active_sh_degree = _ptr(dc), _ptr(rest), _ptr(deg)
-    s.cam_R, s.cam_t = _ptr(R), _ptr(t)
+    s.mean, s.opacity_logit, s.log_scale, s.rotation6d = L.ptr(mean), L.ptr(logit), L.ptr(log_scale), L.ptr(rot6d)
+    s.feature_dc, s.feature_rest, s.active_sh_degree = L.ptr(dc), L.ptr(rest), L.ptr(deg)
+    s.cam_R, s.cam_t = L.ptr(R), L.ptr(t)
     return s
 
 
 class _SceneAssets(torch.autograd.Function):
     @staticmethod
     def forward(ctx, mean, logit, log_scale, rot6d, feature_dc, feature_rest, deg, R, t):
-        lib = L.load()
         dev = logit.device
         P, M = logit.shape[0], 1 + feature_rest.shape[1]
         rgb = R is not None
@@ -61,9 +60,7 @@ class _SceneAssets(torch.autograd.Function):
         opacity, scale, rotation = f(P, 1), f(P, 3), f(P, 4)
         color = f(P, 3) if rgb else f(P, M, 3)
         st = _struct(P, M, *ins, dc, dc_stride, rest, rest_stride, deg, R, t)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_scene_assets_forward(C.byref(st), _ptr(opacity), _ptr(scale), _ptr(rotation), _ptr(color),
-                                                 torch.cuda.current_stream(dev).cuda_stream), "b2r_scene_assets_forward")
+        L.run("b2r_scene_assets_forward", dev, C.byref(st), L.ptr(opacity), L.ptr(scale), L.ptr(rotation), L.ptr(color))
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(*ins, dc, rest, deg, R, t, opacity, scale)
         ctx.meta = (P, M, dc_stride, rest_stride, logit.shape, feature_dc.shape, feature_rest.shape)
@@ -74,26 +71,21 @@ class _SceneAssets(torch.autograd.Function):
         mean, logit, log_scale, rot6d, dc, rest, deg, R, t, opacity, scale = ctx.saved_tensors
         P, M, dc_stride, rest_stride, logit_shape, dc_shape, rest_shape = ctx.meta
         dev = logit.device
-        lib = L.load()
         up = [None if g is None else g.to(torch.float32).contiguous() for g in (g_opacity, g_scale, g_rotation, g_color)]
         f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)  # noqa: E731
         d_logit, d_log_scale, d_rot6d = f(*logit_shape), f(P, 3), f(P, 6)
         d_dc, d_rest = f(*dc_shape), f(*rest_shape)
         d_mean = f(P, 3) if R is not None else None
-        gs = L.B2RSceneAssetsGrads(*[_ptr(x) for x in (opacity, scale, *up, d_logit, d_log_scale, d_rot6d, d_dc, d_rest,
-                                                       d_mean)])
+        gs = L.B2RSceneAssetsGrads(*[L.ptr(x) for x in (opacity, scale, *up, d_logit, d_log_scale, d_rot6d, d_dc,
+                                                        d_rest, d_mean)])
         st = _struct(P, M, mean, logit, log_scale, rot6d, dc, dc_stride, rest, rest_stride, deg, R, t)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_scene_assets_backward(C.byref(st), C.byref(gs), torch.cuda.current_stream(dev).cuda_stream),
-                    "b2r_scene_assets_backward")
+        L.run("b2r_scene_assets_backward", dev, C.byref(st), C.byref(gs))
         return d_mean, d_logit, d_log_scale, d_rot6d, d_dc, d_rest, None, None, None
 
 
 def _check(name, t, shape, dev):
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or (dev is not None and t.device != dev):
-        raise RuntimeError(f"scene_assets: `{name}` must be a CUDA tensor on {dev}; there is no CPU path")
-    if t.dtype != torch.float32:
-        raise ValueError(f"scene_assets: `{name}` must be float32, got {t.dtype}")
+    L.cuda("scene_assets", name, t, dev)
+    L.float32("scene_assets", name, t)
     if shape is not None and tuple(t.shape) != shape:
         raise ValueError(f"scene_assets: `{name}` must be {shape}, got {tuple(t.shape)}")
 
@@ -136,8 +128,7 @@ def scene_assets(mean, opacity_logit, log_scale, rotation6d, feature_dc, feature
         raise ValueError("scene_assets: `active_sh_degree` must be a one-element float32 CUDA buffer")
     R, t = cam_param["R"], cam_param["t"]
     for name, x in (("cam_param['R']", R), ("cam_param['t']", t)):
-        if not isinstance(x, torch.Tensor) or not x.is_cuda or x.device != dev:
-            raise RuntimeError(f"scene_assets: `{name}` must be a CUDA tensor on {dev}; there is no CPU path")
+        L.cuda("scene_assets", name, x, dev)
     if tuple(R.shape) != (3, 3) or t.numel() != 3:
         raise ValueError(f"scene_assets: cam_param R must be (3,3) and t have 3 elements, got {tuple(R.shape)}, "
                          f"{tuple(t.shape)}")

@@ -13,7 +13,7 @@ those colours.  `skin_gaussians` replaces those lines: one kernel blends M_i = s
 (reading the (V,J) weight table through the row index, without the (P,55) gather) and applies it to both sets; the
 backward recomputes M and reduces the joint-transform gradient deterministically (include/b200raster.h B2RSkin).
 
-`rasterizer.SkinnedGaussianRasterizer` is this op followed by one render.  CUDA tensors only: there is no CPU path.
+`rasterizer.SkinnedGaussianRasterizer` is this op followed by one render.  CUDA tensors only: there is no CPU fallback.
 """
 from __future__ import annotations
 
@@ -24,46 +24,43 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib as L
-from .rasterizer import _f32c, _inv3, _ptr
+from .camera import _inv3
 
 
-def _rows_i32(rows: torch.Tensor) -> torch.Tensor:
-    if not rows.is_cuda:
-        raise RuntimeError(f"b200raster: `rows` must be a CUDA tensor (got {rows.device}); there is no CPU fallback")
-    return rows.reshape(-1).to(torch.int32).contiguous()
+def _f32(t: torch.Tensor) -> torch.Tensor:
+    """A contiguous float32 view or copy: the op converts other dtypes (`skin_gaussians` has checked the device)."""
+    return t.to(torch.float32).contiguous()
 
 
 def _skin_struct(P, weights, rows, joint_mats, trans, Rinv, t, xyz, xyz_r, posed, posed_r) -> L.B2RSkin:
     s = L.B2RSkin()
     s.P, s.J, s.V = P, int(weights.shape[1]), int(weights.shape[0])
-    s.weights, s.rows, s.joint_mats, s.trans = _ptr(weights), _ptr(rows), _ptr(joint_mats), _ptr(trans)
-    s.cam_Rinv, s.cam_t = _ptr(Rinv), _ptr(t)
-    s.xyz[0], s.xyz[1] = _ptr(xyz), _ptr(xyz_r)
-    s.posed[0], s.posed[1] = _ptr(posed), _ptr(posed_r)
+    s.weights, s.rows, s.joint_mats, s.trans = L.ptr(weights), L.ptr(rows), L.ptr(joint_mats), L.ptr(trans)
+    s.cam_Rinv, s.cam_t = L.ptr(Rinv), L.ptr(t)
+    s.xyz[0], s.xyz[1] = L.ptr(xyz), L.ptr(xyz_r)
+    s.posed[0], s.posed[1] = L.ptr(posed), L.ptr(posed_r)
     return s
 
 
 class _SkinGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, xyz_refined, weights, rows, joint_mats, trans, cam_R, cam_t):
-        lib = L.load()
         dev = xyz.device
         P = int(xyz.shape[0])
-        x0 = _f32c(xyz, "xyz")
-        x1 = None if xyz_refined is None else _f32c(xyz_refined, "xyz_refined")
-        W = _f32c(weights, "skinning_weight")
-        r = None if rows is None else _rows_i32(rows)
-        A = _f32c(joint_mats, "joint_mats").reshape(-1, 16)
-        tr = _f32c(trans, "trans").reshape(3)
+        x0 = _f32(xyz)
+        x1 = None if xyz_refined is None else _f32(xyz_refined)
+        W = _f32(weights)
+        r = None if rows is None else rows.reshape(-1).to(torch.int32).contiguous()
+        A = _f32(joint_mats).reshape(-1, 16)
+        tr = _f32(trans).reshape(3)
         Rinv = t = None
         if cam_R is not None:
-            Rinv = _f32c(_inv3(_f32c(cam_R, "cam_R")), "cam_R")  # cofactors: no torch.inverse, no sync
-            t = _f32c(cam_t, "cam_t").reshape(3)
+            Rinv = _f32(_inv3(_f32(cam_R)))  # cofactors: no torch.inverse, no sync
+            t = _f32(cam_t).reshape(3)
         posed = torch.empty((P, 3), dtype=torch.float32, device=dev)
         posed_r = None if x1 is None else torch.empty((P, 3), dtype=torch.float32, device=dev)
         s = _skin_struct(P, W, r, A, tr, Rinv, t, x0, x1, posed, posed_r)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_skin_forward(C.byref(s), torch.cuda.current_stream(dev).cuda_stream), "b2r_skin_forward")
+        L.run("b2r_skin_forward", dev, C.byref(s))
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(x0, x1, W, r, A, tr, Rinv, t)
         ctx.shapes = (joint_mats.shape, trans.shape, xyz.shape, None if xyz_refined is None else xyz_refined.shape)
@@ -81,19 +78,17 @@ class _SkinGaussians(torch.autograd.Function):
         dev = x0.device
         P, J = int(x0.shape[0]), int(W.shape[1])
         f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
-        gp = [None if g is None else _f32c(g, "grad_posed").reshape(P, 3) for g in (g0, g1)]
+        gp = [None if g is None else _f32(g).reshape(P, 3) for g in (g0, g1)]
         d_xyz = [f(P, 3) if need[0] else None, f(P, 3) if (need[1] and x1 is not None) else None]
         d12 = f(J, 12) if (need[4] or need[5]) else None
         d_trans = f(3) if (need[4] or need[5]) else None
         sbytes = lib.b2r_skin_scratch_bytes(P, J)
         scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev) if d12 is not None else None
         s = _skin_struct(P, W, r, A, tr, Rinv, t, x0, x1, None, None)
-        dposed = (C.c_void_p * 2)(_ptr(gp[0]), _ptr(gp[1]))
-        dxyz = (C.c_void_p * 2)(_ptr(d_xyz[0]), _ptr(d_xyz[1]))
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_skin_backward(C.byref(s), dposed, dxyz, _ptr(d12), _ptr(d_trans), _ptr(scratch),
-                                          sbytes if scratch is not None else 0,
-                                          torch.cuda.current_stream(dev).cuda_stream), "b2r_skin_backward")
+        dposed = (C.c_void_p * 2)(L.ptr(gp[0]), L.ptr(gp[1]))
+        dxyz = (C.c_void_p * 2)(L.ptr(d_xyz[0]), L.ptr(d_xyz[1]))
+        L.run("b2r_skin_backward", dev, C.byref(s), dposed, dxyz, L.ptr(d12), L.ptr(d_trans), L.ptr(scratch),
+              sbytes if scratch is not None else 0)
         js, ts, xs, xrs = ctx.shapes
         d_joint = None
         if need[4]:  # (J,4,4) with the last row zero, like the unfused ops' gradient
@@ -122,8 +117,8 @@ def skin_gaussians(xyz: torch.Tensor, xyz_refined: Optional[torch.Tensor], skinn
     """
     for name, v in (("xyz", xyz), ("xyz_refined", xyz_refined), ("skinning_weight", skinning_weight), ("rows", rows),
                     ("joint_mats", joint_mats), ("trans", trans), ("cam_R", cam_R), ("cam_t", cam_t)):
-        if v is not None and not v.is_cuda:
-            raise RuntimeError(f"skin_gaussians: `{name}` must be a CUDA tensor (got {v.device}); there is no CPU path")
+        if v is not None:
+            L.cuda("skin_gaussians", name, v)
     if xyz.dim() != 2 or xyz.shape[1] != 3:
         raise ValueError(f"skin_gaussians: xyz must be (P,3), got {tuple(xyz.shape)}")
     P = xyz.shape[0]

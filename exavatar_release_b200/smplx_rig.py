@@ -40,7 +40,6 @@ import numpy as np
 import torch
 
 from . import _lib as L
-from .rasterizer import _ptr
 from .synthetic import subdivide_edges
 
 JMAX = 64       # joints: one thread per joint in the op's single-CTA kernels
@@ -217,7 +216,6 @@ def _t(x, dtype=torch.float64) -> torch.Tensor:
 class _Rig(torch.autograd.Function):
     @staticmethod
     def forward(ctx, rig, shape_param, joint_offset, full_pose, expr):
-        lib = L.load()
         dev = rig.device
         ins = [rig._input(t, n, name) for t, n, name in ((shape_param, rig.NB, "shape_param"),
                                                           (joint_offset, 3 * rig.J, "joint_offset"),
@@ -227,9 +225,7 @@ class _Rig(torch.autograd.Function):
         outs = [f(rig.P, 3), f(rig.V, 3), f(rig.J, 4, 4), f(rig.P, 3), f(rig.P, 3), f(6 * rig.n_body)]
         scratch = torch.empty(rig.scratch_bytes, dtype=torch.uint8, device=dev)
         st = rig._struct(ins)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_rig_forward(C.byref(st), *[_ptr(o) for o in outs], _ptr(scratch), rig.scratch_bytes,
-                                        torch.cuda.current_stream(dev).cuda_stream), "b2r_rig_forward")
+        L.run("b2r_rig_forward", dev, C.byref(st), *[L.ptr(o) for o in outs], L.ptr(scratch), rig.scratch_bytes)
         ctx.rig = rig
         ctx.set_materialize_grads(False)
         ctx.mark_non_differentiable(outs[1], outs[3], outs[5])
@@ -242,22 +238,18 @@ class _Rig(torch.autograd.Function):
         *ins, scratch = ctx.saved_tensors
         rig = ctx.rig
         dev = rig.device
-        lib = L.load()
         grads = [torch.empty(n, dtype=torch.float32, device=dev) for n in (rig.NB, 3 * rig.J, 3 * rig.J, rig.NE)]
-        gs = L.B2RRigGrads(*[_ptr(g) for g in grads])
+        gs = L.B2RRigGrads(*[L.ptr(g) for g in grads])
         up = [None if g is None else g.to(torch.float32).contiguous() for g in (g_mesh, g_jm, g_eo)]
         st = rig._struct(ins)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_rig_backward(C.byref(st), *[_ptr(g) for g in up], C.byref(gs), _ptr(scratch),
-                                         scratch.numel(), torch.cuda.current_stream(dev).cuda_stream),
-                    "b2r_rig_backward")
+        L.run("b2r_rig_backward", dev, C.byref(st), *[L.ptr(g) for g in up], C.byref(gs), L.ptr(scratch),
+              scratch.numel())
         return (None, *[g.reshape(s) for g, s in zip(grads, ctx.shapes)])
 
 
 class _Body(torch.autograd.Function):
     @staticmethod
     def forward(ctx, rig, shape_param, joint_offset, full_pose, expr, trans, cam_R, cam_t):
-        lib = L.load()
         dev = rig.device
         ins = [rig._input(t, n, name) for t, n, name in ((shape_param, rig.NB, "shape_param"),
                                                           (joint_offset, 3 * rig.J, "joint_offset"),
@@ -269,9 +261,7 @@ class _Body(torch.autograd.Function):
         mesh = torch.empty((rig.V, 3), dtype=torch.float32, device=dev)
         scratch = torch.empty(rig.body_scratch_bytes, dtype=torch.uint8, device=dev)
         st = rig._body_struct(ins, cam)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_smplx_body_forward(C.byref(st), _ptr(mesh), _ptr(scratch), rig.body_scratch_bytes,
-                                               torch.cuda.current_stream(dev).cuda_stream), "b2r_smplx_body_forward")
+        L.run("b2r_smplx_body_forward", dev, C.byref(st), L.ptr(mesh), L.ptr(scratch), rig.body_scratch_bytes)
         ctx.rig = rig
         ctx.n_cam = len(cam)
         ctx.set_materialize_grads(False)
@@ -285,14 +275,11 @@ class _Body(torch.autograd.Function):
         ins, cam = ins[:5], ins[5:]
         rig = ctx.rig
         dev = rig.device
-        lib = L.load()
         grads = [torch.empty(n, dtype=torch.float32, device=dev) for n in (rig.NB, 3 * rig.J, 3 * rig.J, rig.NE, 3)]
-        gs = L.B2RSmplxBodyGrads(*[_ptr(g) for g in grads])
+        gs = L.B2RSmplxBodyGrads(*[L.ptr(g) for g in grads])
         up = None if g_mesh is None else g_mesh.to(torch.float32).contiguous()
         st = rig._body_struct(ins, cam)
-        with torch.cuda.device(dev):
-            L.check(lib.b2r_smplx_body_backward(C.byref(st), _ptr(up), C.byref(gs), _ptr(scratch), scratch.numel(),
-                                                torch.cuda.current_stream(dev).cuda_stream), "b2r_smplx_body_backward")
+        L.run("b2r_smplx_body_backward", dev, C.byref(st), L.ptr(up), C.byref(gs), L.ptr(scratch), scratch.numel())
         return (None, *[g.reshape(s) for g, s in zip(grads, ctx.shapes)], None, None)
 
 
@@ -321,7 +308,7 @@ class SmplxRig:
                  face_offset, faces, neutral_body_pose, is_rhand, is_lhand, is_face_expr, device=None):
         device = torch.device(device if device is not None else "cuda")
         if device.type != "cuda":
-            raise RuntimeError(f"SmplxRig: device must be CUDA (got {device}); there is no CPU path")
+            raise RuntimeError(f"SmplxRig: device must be CUDA (got {device}); there is no CPU fallback")
         if device.index is None:
             device = torch.device("cuda", torch.cuda.current_device())
         self.device = device
@@ -364,7 +351,7 @@ class SmplxRig:
         self.body_scratch_bytes = int(L.load().b2r_smplx_body_scratch_bytes(V, J))
         self._template = L.B2RRig(
             V=V, V1=self.V1, P=self.P, J=J, NB=self.NB, NE=self.NE, n_body=self.n_body,
-            **{k: _ptr(getattr(self, a)) for k, a in (
+            **{k: L.ptr(getattr(self, a)) for k, a in (
                 ("template_", "template"), ("shapedirs", "shapedirs"), ("expr_dirs", "expr_dirs"),
                 ("posedirs_t", "posedirs_t"), ("pose_offset0", "pose_offset0"), ("lbs_weights", "lbs_weights"),
                 ("jreg_offsets", "jreg_offsets"), ("jreg_cols", "jreg_cols"), ("jreg_vals", "jreg_vals"),
@@ -374,15 +361,15 @@ class SmplxRig:
                 ("upT_rows", "upT_rows"), ("upT_w", "upT_w"), ("mask", "mask"))})
 
     def _input(self, t: torch.Tensor, n: int, name: str) -> torch.Tensor:
-        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != self.device:
-            raise RuntimeError(f"SmplxRig: `{name}` must be a CUDA tensor on {self.device}; there is no CPU path")
-        if t.dtype != torch.float32 or t.numel() != n:
-            raise ValueError(f"SmplxRig: `{name}` must be float32 with {n} elements, got {t.dtype} {tuple(t.shape)}")
+        L.cuda("SmplxRig", name, t, self.device)
+        L.float32("SmplxRig", name, t)
+        if t.numel() != n:
+            raise ValueError(f"SmplxRig: `{name}` must have {n} elements, got {tuple(t.shape)}")
         return t.detach().reshape(n).contiguous()
 
     def _struct(self, ins) -> "L.B2RRig":
         st = L.B2RRig.from_buffer_copy(self._template)
-        st.shape_param, st.joint_offset, st.full_pose, st.expr = (_ptr(t) for t in ins)
+        st.shape_param, st.joint_offset, st.full_pose, st.expr = (L.ptr(t) for t in ins)
         return st
 
     def __call__(self, shape_param, joint_offset, full_pose, expr) -> RigOutputs:
@@ -393,10 +380,10 @@ class SmplxRig:
         return smplx_rig_reference(self.model, *args, **kw)
 
     def _body_struct(self, ins, cam) -> "L.B2RSmplxBody":
-        st = L.B2RSmplxBody(rig=self._template, pose_mean=_ptr(self.pose_mean))
-        st.shape_param, st.joint_offset, st.full_pose, st.expr, st.trans = (_ptr(t) for t in ins)
+        st = L.B2RSmplxBody(rig=self._template, pose_mean=L.ptr(self.pose_mean))
+        st.shape_param, st.joint_offset, st.full_pose, st.expr, st.trans = (L.ptr(t) for t in ins)
         if cam:
-            st.cam_R, st.cam_t = (_ptr(t) for t in cam)
+            st.cam_R, st.cam_t = (L.ptr(t) for t in cam)
         return st
 
     def body_mesh(self, shape_param, joint_offset, full_pose, expr, trans, cam_R=None, cam_t=None) -> torch.Tensor:

@@ -157,7 +157,7 @@ def test_posed_positions_of_the_fused_path_are_differentiable(only_posed):
 
 def test_host_helpers_of_the_skinning_backward():
     """`_inv3` (graph-capturable 3x3 inverse) against torch.inverse."""
-    from exavatar_release_b200.rasterizer import _inv3
+    from exavatar_release_b200.camera import _inv3
     g = torch.Generator().manual_seed(11)
     for _ in range(5):
         R = torch.randn(3, 3, generator=g, dtype=torch.float64) + 2 * torch.eye(3, dtype=torch.float64)

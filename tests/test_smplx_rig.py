@@ -347,7 +347,7 @@ def test_cuda_graph_replay_equals_eager(c4):
 @pytest.mark.gpu
 def test_non_topological_parents_give_nan_on_the_device(c4):
     """The C ABI cannot check `parents` on the host (a device pointer): the chain kernels find it and write NaN."""
-    from exavatar_release_b200.rasterizer import _ptr
+    from exavatar_release_b200._lib import ptr as _ptr
     rig, _ = c4
     lib = L.load()
     ins = [rig._input(t, n, k) for t, n, k in zip(_inputs(rig.J, rig.NB, rig.NE, seed=13, device="cuda"),

@@ -27,7 +27,7 @@ from benchkit import alternate, arg_parser, card, cuda_device, emit, graph_repla
 from exavatar_release_b200 import TrainingFrameRenderer  # noqa: E402
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
 from exavatar_release_b200.plan import RENDERS  # noqa: E402
-from exavatar_release_b200.rasterizer import _inv3  # noqa: E402
+from exavatar_release_b200.camera import _inv3  # noqa: E402
 from exavatar_release_b200.renderer import lbs_reference  # noqa: E402
 from exavatar_release_b200.skinning import skin_gaussians  # noqa: E402
 from exavatar_release_b200.synthetic import WORKLOADS, make_grad_image, make_population_assets  # noqa: E402
