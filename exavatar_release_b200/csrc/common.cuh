@@ -530,6 +530,57 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Fixed-order sums, behind every op's "bit-identical run to run" and "no float atomics".  A warp sums by an xor
+// butterfly (16, 8, 4, 2, 1); a block stores one value per warp in shared memory and thread 0 folds them in warp order,
+// starting from zero (so a zero sum keeps its sign).  They only add: --fmad=false does not change them.
+// ---------------------------------------------------------------------------------------------------------------
+template <typename T>
+__device__ __forceinline__ T warp_sum(T v) {  // every lane ends with the same bits
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+  return v;
+}
+
+// v[0..N) already the same across each warp of a THREADS-thread block -> thread 0's v holds the block's N sums (the
+// other threads' v is unchanged).  wsum: THREADS / 32 x N values in shared memory, warp-major.  Every thread of the
+// block calls it; the barrier in front lets the next call reuse wsum.
+template <int THREADS, typename T, int N>
+__device__ __forceinline__ void block_fold(T (&v)[N], T* wsum) {
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0)
+#pragma unroll
+    for (int i = 0; i < N; i++) wsum[(threadIdx.x >> 5) * N + i] = v[i];
+  __syncthreads();
+  if (threadIdx.x == 0)
+#pragma unroll
+    for (int i = 0; i < N; i++) {
+      T s = T(0);
+      for (int w = 0; w < THREADS / 32; w++) s += wsum[w * N + i];
+      v[i] = s;
+    }
+}
+
+// the block's N sums of v[0..N), in thread 0 (block_fold after warp_sum)
+template <int THREADS, typename T, int N>
+__device__ __forceinline__ void block_sum(T (&v)[N], T* wsum) {
+#pragma unroll
+  for (int i = 0; i < N; i++) v[i] = warp_sum(v[i]);
+  block_fold<THREADS>(v, wsum);
+}
+
+// the column sums of n rows of N partials at p (row-major) into v, in thread 0: thread t adds rows t, t + THREADS, ...
+// and then block_sum runs
+template <int THREADS, typename T, int N>
+__device__ __forceinline__ void block_sum_strided(const T* p, int n, T (&v)[N], T* wsum) {
+#pragma unroll
+  for (int i = 0; i < N; i++) v[i] = T(0);
+  for (int r = threadIdx.x; r < n; r += THREADS)
+#pragma unroll
+    for (int i = 0; i < N; i++) v[i] += p[r * N + i];
+  block_sum<THREADS>(v, wsum);
+}
+
 // launch wrappers (one per translation unit)
 int launch_project(const B2RScene& sc, const Ctx& cx, int32_t* radii, cudaStream_t st, int first_row = 0);
 int launch_binning(const B2RScene& sc, const Ctx& cx, bool rescan, cudaStream_t st);

@@ -39,28 +39,13 @@ __host__ __device__ inline int ls_tiles_x(int W) { return (W + LS_T - 1) / LS_T;
 __host__ __device__ inline int ls_tiles_y(int H) { return (H + LS_T - 1) / LS_T; }
 static size_t ls_map_bytes(int W, int H) { return align_up((size_t)9 * W * H * sizeof(float)); }
 
-// fixed-order block sum of two values (shuffle tree per warp, then the eight warp sums in warp order)
-__device__ __forceinline__ float2 block_sum2(float a, float b) {
-  __shared__ float2 wsum[LS_WARPS];
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) {
-    a += __shfl_xor_sync(0xffffffffu, a, d);
-    b += __shfl_xor_sync(0xffffffffu, b, d);
-  }
-  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = make_float2(a, b);
-  __syncthreads();
-  float2 t = make_float2(0.f, 0.f);
-  if (threadIdx.x == 0)
-    for (int w = 0; w < LS_WARPS; w++) { t.x += wsum[w].x; t.y += wsum[w].y; }
-  return t;  // valid in thread 0
-}
-
 // maps: 9 planes of H*W floats, plane 3*k + c = partial k (dm/dmu_x, dm/dS_xx, dm/dS_xy) of channel c
 template <bool SSIM>
 __global__ void __launch_bounds__(LS_THREADS) l1ssim_fwd_kernel(const L1SsimIn a, float* __restrict__ maps,
                                                                 float2* __restrict__ tile_sums) {
   __shared__ float sx[LS_S * LS_S], sy[LS_S * LS_S];
   __shared__ float hm[5][LS_S * LS_T];  // horizontal pass: mu_x, mu_y, S_xx, S_yy, S_xy
+  __shared__ float wsum[LS_WARPS * 2];
   const Crop cr = read_crop(a.bbox, a.W, a.H);
   const int tx0 = blockIdx.x * LS_T, ty0 = blockIdx.y * LS_T;
   const int tile = blockIdx.y * gridDim.x + blockIdx.x;
@@ -138,26 +123,23 @@ __global__ void __launch_bounds__(LS_THREADS) l1ssim_fwd_kernel(const L1SsimIn a
       maps[(6 + c) * HW + o] = 2.f * A * inv;                                          // dm/dS_xy
     }
   }
-  const float2 t = block_sum2(l1, ssum);
-  if (threadIdx.x == 0) tile_sums[tile] = t;
+  float t[2] = {l1, ssum};
+  block_sum<LS_THREADS>(t, wsum);
+  if (threadIdx.x == 0) tile_sums[tile] = make_float2(t[0], t[1]);
 }
 
-// the tile partials in a fixed order (thread i over tiles i, i + 256, ...; then the block sum); means over 3 h w
-__global__ void __launch_bounds__(LS_THREADS) l1ssim_reduce_kernel(const float2* __restrict__ tile_sums, const int ntiles,
+// the tile partials (ntiles x 2 floats) in a fixed order; means over 3 h w
+__global__ void __launch_bounds__(LS_THREADS) l1ssim_reduce_kernel(const float* __restrict__ tile_sums, const int ntiles,
                                                                    const float* __restrict__ bbox, const int W,
                                                                    const int H, const int with_ssim,
                                                                    float* __restrict__ out) {
-  float a = 0.f, b = 0.f;
-  for (int t = threadIdx.x; t < ntiles; t += LS_THREADS) {
-    const float2 v = tile_sums[t];
-    a += v.x;
-    b += v.y;
-  }
-  const float2 s = block_sum2(a, b);
+  __shared__ float wsum[LS_WARPS * 2];
+  float s[2];
+  block_sum_strided<LS_THREADS>(tile_sums, ntiles, s, wsum);
   if (threadIdx.x == 0) {
     const float n = read_crop(bbox, W, H).count3();  // 0 for an empty crop: 0 / 0 = NaN, like mean() of nothing
-    out[0] = s.x / n;
-    if (with_ssim) out[1] = s.y / n;
+    out[0] = s[0] / n;
+    if (with_ssim) out[1] = s[1] / n;
   }
 }
 
@@ -257,7 +239,7 @@ int launch_l1ssim_forward(int W, int H, const float* img, const float* target, c
   }
   {
     ProfScope p(K_MISC, st);
-    launch_k(l1ssim_reduce_kernel, 1, LS_THREADS, 0, st, true, (const float2*)tiles, (int)(grid.x * grid.y), bbox, W,
+    launch_k(l1ssim_reduce_kernel, 1, LS_THREADS, 0, st, true, (const float*)tiles, (int)(grid.x * grid.y), bbox, W,
              H, with_ssim ? 1 : 0, out);
   }
   return check_launch();

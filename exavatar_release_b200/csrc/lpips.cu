@@ -307,8 +307,8 @@ __global__ void __launch_bounds__(256) lp_pool_kernel(const float* __restrict__ 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Heads: a warp per pixel, lane l holds channels 4 (l + 32 i) .. + 3.  Sums over channels are xor-shuffle trees (every
-// lane ends with the same value, in a fixed order).
+// Heads: a warp per pixel, lane l holds channels 4 (l + 32 i) .. + 3.  Sums over channels are warp_sum (every lane ends
+// with the same value).
 // ---------------------------------------------------------------------------------------------------------------------
 template <int C>
 struct HeadVec {
@@ -329,11 +329,6 @@ struct HeadVec {
     }
   }
 };
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-  return v;
-}
 template <int C>
 __device__ __forceinline__ float sum_sq(const HeadVec<C>& f) {
   float s = 0.f;
@@ -374,7 +369,7 @@ __global__ void __launch_bounds__(HD_WARPS * 32) lp_head_fwd_kernel(const float*
   const int ld = W >> level, lane = threadIdx.x & 31;
   HeadVec<C> w;
   w.load(lw, lane);
-  double acc = 0.0;
+  double acc[1] = {0.0};
   for (int k = 0; k < HD_PPW; k++) {
     const int p = blockIdx.x * HD_PIX + (threadIdx.x >> 5) * HD_PPW + k;
     const int y = p / ld, x = p - y * ld;
@@ -390,15 +385,10 @@ __global__ void __launch_bounds__(HD_WARPS * 32) lp_head_fwd_kernel(const float*
       const float a2 = v.v[i].z / s - n.v[i].z, a3 = v.v[i].w / s - n.v[i].w;
       d += w.v[i].x * (a0 * a0) + w.v[i].y * (a1 * a1) + w.v[i].z * (a2 * a2) + w.v[i].w * (a3 * a3);
     }
-    acc += (double)warp_sum(d);
+    acc[0] += (double)warp_sum(d);
   }
-  if (lane == 0) wsum[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double s = 0.0;
-    for (int i = 0; i < HD_WARPS; i++) s += wsum[i];
-    part[blockIdx.x] = s;
-  }
+  block_fold<HD_WARPS * 32>(acc, wsum);
+  if (threadIdx.x == 0) part[blockIdx.x] = acc[0];
 }
 
 struct LpParts {
@@ -411,18 +401,11 @@ __global__ void __launch_bounds__(256) lp_reduce_kernel(const LpParts parts, con
   __shared__ double ws[8];
   double total = 0.0;
   for (int t = 0; t < 5; t++) {
-    double s = 0.0;
-    for (int i = threadIdx.x; i < parts.n[t]; i += 256) s += parts.p[t][i];
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) s += __shfl_xor_sync(0xffffffffu, s, d);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = s;
-    __syncthreads();
+    double s[1];
+    block_sum_strided<256>(parts.p[t], parts.n[t], s, ws);
     if (threadIdx.x == 0) {
-      double b = 0.0;
-      for (int i = 0; i < 8; i++) b += ws[i];
       const LpExt ex = lp_extent(bbox, W, H, t);
-      total += b / ((double)ex.h * (double)ex.w);
+      total += s[0] / ((double)ex.h * (double)ex.w);
     }
   }
   if (threadIdx.x == 0) out[0] = (float)total;

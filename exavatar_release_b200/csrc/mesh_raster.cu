@@ -366,7 +366,7 @@ __global__ void __launch_bounds__(MR_THREADS) mr_face_bwd_kernel(const B2RMeshRe
     }
 #pragma unroll
     for (int i = 0; i < 9; i++) {
-      for (int d = 16; d > 0; d >>= 1) h[i] += __shfl_xor_sync(0xffffffffu, h[i], d);
+      h[i] = warp_sum(h[i]);
       if (lane == l) g[i] = h[i];
     }
   }

@@ -144,18 +144,6 @@ __global__ void __launch_bounds__(256) nm_prep_kernel(const float* __restrict__ 
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int SS_HW = SS_TW + 10, SS_HH = SS_TH + 10;
 
-__device__ __forceinline__ double block_sum_512(double v, double* red) {
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-    for (int k = 0; k < SS_TW * SS_TH / 32; k++) s += red[k];
-  return s;
-}
-
 __global__ void __launch_bounds__(SS_TW * SS_TH) nm_ssim_kernel(const float* __restrict__ q, int W, int H, int N,
                                                                 double* __restrict__ sse, double* __restrict__ ssim) {
   __shared__ float sx[SS_HH * SS_HW], sy[SS_HH * SS_HW];
@@ -211,10 +199,11 @@ __global__ void __launch_bounds__(SS_TW * SS_TH) nm_ssim_kernel(const float* __r
     }
   }
   const size_t slot = ((size_t)n * 3 + c) * (gridDim.x * gridDim.y) + blockIdx.y * gridDim.x + blockIdx.x;
-  const double ts = block_sum_512(s, red);
-  if (threadIdx.x == 0) ssim[slot] = ts;
-  const double td = block_sum_512(d2, red);
-  if (threadIdx.x == 0) sse[slot] = td;
+  double ts[1] = {s}, td[1] = {d2};
+  block_sum<SS_TW * SS_TH>(ts, red);
+  if (threadIdx.x == 0) ssim[slot] = ts[0];
+  block_sum<SS_TW * SS_TH>(td, red);
+  if (threadIdx.x == 0) sse[slot] = td[0];
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -351,15 +340,9 @@ __global__ void __launch_bounds__(256) nm_pool_kernel(const float* __restrict__ 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Heads: a warp per pixel, lane l holds channels 4 (l + 32 i) .. + 3 of both images' taps.  Channel sums are xor-shuffle
-// trees; the CTA's fp64 sum of sum_c w_c (n_c(f_x) - n_c(f_y))^2 goes to part[n][blockIdx.x].
+// Heads: a warp per pixel, lane l holds channels 4 (l + 32 i) .. + 3 of both images' taps.  Channel sums are warp_sum;
+// the CTA's fp64 sum of sum_c w_c (n_c(f_x) - n_c(f_y))^2 goes to part[n][blockIdx.x].
 // ---------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float nm_warp_sum(float v) {
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-  return v;
-}
-
 template <int C>
 __global__ void __launch_bounds__(HD_WARPS * 32) nm_head_kernel(const float* __restrict__ act,
                                                                 const float* __restrict__ lw, int npix, int N,
@@ -375,7 +358,7 @@ __global__ void __launch_bounds__(HD_WARPS * 32) nm_head_kernel(const float* __r
     const int c4 = lane + 32 * i;
     w[i] = c4 < C / 4 ? __ldg(reinterpret_cast<const float4*>(lw) + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
-  double acc = 0.0;
+  double acc[1] = {0.0};
   for (int k = 0; k < HD_PPW; k++) {
     const int p = blockIdx.x * HD_PIX + (threadIdx.x >> 5) * HD_PPW + k;
     if (p >= npix) continue;  // warp-uniform
@@ -390,7 +373,7 @@ __global__ void __launch_bounds__(HD_WARPS * 32) nm_head_kernel(const float* __r
       sa += a[i].x * a[i].x + a[i].y * a[i].y + a[i].z * a[i].z + a[i].w * a[i].w;
       sb += b[i].x * b[i].x + b[i].y * b[i].y + b[i].z * b[i].z + b[i].w * b[i].w;
     }
-    const float na = sqrtf(nm_warp_sum(sa)) + NM_EPS, nb = sqrtf(nm_warp_sum(sb)) + NM_EPS;
+    const float na = sqrtf(warp_sum(sa)) + NM_EPS, nb = sqrtf(warp_sum(sb)) + NM_EPS;
     float d = 0.f;
 #pragma unroll
     for (int i = 0; i < NV; i++) {
@@ -398,15 +381,10 @@ __global__ void __launch_bounds__(HD_WARPS * 32) nm_head_kernel(const float* __r
       const float d2 = a[i].z / na - b[i].z / nb, d3 = a[i].w / na - b[i].w / nb;
       d += w[i].x * (d0 * d0) + w[i].y * (d1 * d1) + w[i].z * (d2 * d2) + w[i].w * (d3 * d3);
     }
-    acc += (double)nm_warp_sum(d);
+    acc[0] += (double)warp_sum(d);
   }
-  if (lane == 0) wsum[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double s = 0.0;
-    for (int i = 0; i < HD_WARPS; i++) s += wsum[i];
-    part[(size_t)n * gridDim.x + blockIdx.x] = s;
-  }
+  block_fold<HD_WARPS * 32>(acc, wsum);
+  if (threadIdx.x == 0) part[(size_t)n * gridDim.x + blockIdx.x] = acc[0];
 }
 
 struct NmParts {
@@ -416,33 +394,22 @@ struct NmParts {
   int ssim_ctas, tap_ctas[5], tap_pix[5];
 };
 
-// one CTA per frame: sum of `n` partials at p, strided by thread then a fixed tree
-__device__ double nm_block_sum(const double* p, int n, double* ws) {
-  double s = 0.0;
-  for (int i = threadIdx.x; i < n; i += 256) s += p[i];
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) s += __shfl_xor_sync(0xffffffffu, s, d);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = s;
-  __syncthreads();
-  double b = 0.0;
-  for (int i = 0; i < 8; i++) b += ws[i];
-  return b;
-}
-
+// one CTA per frame: each run of partials in a fixed order
 __global__ void __launch_bounds__(256) nm_reduce_kernel(const NmParts P, int W, int H, float* __restrict__ out) {
   __shared__ double ws[8];
   const int n = blockIdx.x;
   const int per = 3 * P.ssim_ctas;
-  const double sse = nm_block_sum(P.sse + (size_t)n * per, per, ws);
-  const double ss = nm_block_sum(P.ssim + (size_t)n * per, per, ws);
-  double lp = 0.0;
-  for (int t = 0; t < 5; t++)
-    lp += nm_block_sum(P.tap[t] + (size_t)n * P.tap_ctas[t], P.tap_ctas[t], ws) / (double)P.tap_pix[t];
+  double sse[1], ss[1], tap[1], lp = 0.0;
+  block_sum_strided<256>(P.sse + (size_t)n * per, per, sse, ws);
+  block_sum_strided<256>(P.ssim + (size_t)n * per, per, ss, ws);
+  for (int t = 0; t < 5; t++) {
+    block_sum_strided<256>(P.tap[t] + (size_t)n * P.tap_ctas[t], P.tap_ctas[t], tap, ws);
+    lp += tap[0] / (double)P.tap_pix[t];
+  }
   if (threadIdx.x == 0) {
-    const double mse = sse / (3.0 * (double)W * (double)H);
+    const double mse = sse[0] / (3.0 * (double)W * (double)H);
     out[3 * n + 0] = (float)(10.0 * log10(1.0 / mse));
-    out[3 * n + 1] = (float)(ss / (3.0 * (double)(W - 10) * (double)(H - 10)));
+    out[3 * n + 1] = (float)(ss[0] / (3.0 * (double)(W - 10) * (double)(H - 10)));
     out[3 * n + 2] = (float)lp;
   }
 }

@@ -5,7 +5,7 @@
 // Forward (all launches on the caller's stream, counted under kernel id 8 misc):
 //   vertex_normals_kernel (geometry.cu) on mesh_neutral_pose: HandMeanReg and the arm split share it.
 //   regs_hand_partial_kernel  fp64 partial sums of rgb / rgb_refined over the right- and left-hand rows (grid-stride,
-//                             fixed row -> thread map, fixed-order block sums).
+//                             fixed row -> thread map, block_sum of common.cuh).
 //   regs_split_kernel         ONE CTA: the hand means from those partials; the arm rows classified upper (n_y > 0.5f)
 //                             or lower and compacted in vertex order with device-side counts; k reset to 50.
 //   regs_rank_kernel          rank of every upper row by (x, vertex index): integer counts, integer atomics.
@@ -100,23 +100,6 @@ inline RegsPtrs regs_ptrs(const B2RRegs& r, void* scratch) {
                   (double*)(s + L.term_part)};
 }
 
-// fixed-order block sum of N doubles per thread: shuffle tree per warp, then the warp sums in warp order (thread 0)
-template <int N, int THREADS>
-__device__ __forceinline__ void block_sum_d(double (&v)[N], double (*wsum)[N]) {
-#pragma unroll
-  for (int t = 0; t < N; t++)
-    for (int d = 16; d > 0; d >>= 1) v[t] += __shfl_xor_sync(0xffffffffu, v[t], d);
-  if ((threadIdx.x & 31) == 0)
-    for (int t = 0; t < N; t++) wsum[threadIdx.x >> 5][t] = v[t];
-  __syncthreads();
-  if (threadIdx.x == 0)
-    for (int t = 0; t < N; t++) {
-      double s = 0.0;
-      for (int w = 0; w < THREADS / 32; w++) s += wsum[w][t];
-      v[t] = s;
-    }
-}
-
 // x -> an unsigned key with the float order (negative values reversed), for the (x, index) sort of the upper rows
 __device__ __forceinline__ unsigned ordered_bits(float x) {
   const unsigned u = __float_as_uint(x);
@@ -124,7 +107,7 @@ __device__ __forceinline__ unsigned ordered_bits(float x) {
 }
 
 __global__ void __launch_bounds__(RG_THREADS) regs_hand_partial_kernel(const B2RRegs r, double* __restrict__ part) {
-  __shared__ double wsum[RG_THREADS / 32][12];
+  __shared__ double wsum[RG_THREADS / 32 * 12];
   double v[12];
 #pragma unroll
   for (int t = 0; t < 12; t++) v[t] = 0.0;
@@ -141,7 +124,7 @@ __global__ void __launch_bounds__(RG_THREADS) regs_hand_partial_kernel(const B2R
       }
     }
   }
-  block_sum_d<12, RG_THREADS>(v, wsum);
+  block_sum<RG_THREADS>(v, wsum);
   if (threadIdx.x == 0)
     for (int t = 0; t < 12; t++) part[blockIdx.x * 12 + t] = v[t];
 }
@@ -312,8 +295,7 @@ __global__ void __launch_bounds__(RG_THREADS) regs_select_kernel(const B2RRegs r
         }
     }
 #pragma unroll
-  for (int c = 0; c < 6; c++)
-    for (int d = 16; d > 0; d >>= 1) a[c] += __shfl_xor_sync(0xffffffffu, a[c], d);
+  for (int c = 0; c < 6; c++) a[c] = warp_sum(a[c]);
   if (lane == 0) {
     double term = 0.0;
     for (int c = 0; c < 6; c++) {
@@ -354,7 +336,7 @@ __device__ __forceinline__ float hand_dot(const float* n, const float* o) {
 }
 
 __global__ void __launch_bounds__(RG_THREADS) regs_terms_kernel(const B2RRegs r, const RegsPtrs s) {
-  __shared__ double wsum[RG_THREADS / 32][RG_NTERMS];
+  __shared__ double wsum[RG_THREADS / 32 * RG_NTERMS];
   const int v = blockIdx.x * RG_THREADS + threadIdx.x;
   double t[RG_NTERMS];
 #pragma unroll
@@ -421,14 +403,14 @@ __global__ void __launch_bounds__(RG_THREADS) regs_terms_kernel(const B2RRegs r,
       o[0] = ls[q].x; o[1] = ls[q].y; o[2] = ls[q].z;
     }
   }
-  block_sum_d<RG_NTERMS, RG_THREADS>(t, wsum);
+  block_sum<RG_THREADS>(t, wsum);
   if (threadIdx.x == 0)
     for (int q = 0; q < RG_NTERMS; q++) s.term_part[(size_t)blockIdx.x * RG_NTERMS + q] = t[q];
 }
 
 __global__ void __launch_bounds__(RG_THREADS) regs_reduce_kernel(const B2RRegs r, const RegsPtrs s, const int nb,
                                                                  float* __restrict__ out) {
-  __shared__ double wsum[RG_THREADS / 32][RG_NTERMS + 1];
+  __shared__ double wsum[RG_THREADS / 32 * (RG_NTERMS + 1)];
   double t[RG_NTERMS + 1];
 #pragma unroll
   for (int q = 0; q <= RG_NTERMS; q++) t[q] = 0.0;
@@ -436,7 +418,7 @@ __global__ void __launch_bounds__(RG_THREADS) regs_reduce_kernel(const B2RRegs r
     for (int q = 0; q < RG_NTERMS; q++) t[q] += s.term_part[(size_t)b * RG_NTERMS + q];
   const int n_lo = s.counters[1];
   for (int p = threadIdx.x; p < n_lo; p += RG_THREADS) t[RG_NTERMS] += s.arm_term[p];
-  block_sum_d<RG_NTERMS + 1, RG_THREADS>(t, wsum);
+  block_sum<RG_THREADS>(t, wsum);
   if (threadIdx.x != 0) return;
   const double n3 = 3.0 * r.P;
   double jreg = 0.0, jsym = 0.0;

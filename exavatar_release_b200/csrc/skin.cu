@@ -206,12 +206,10 @@ __global__ void __launch_bounds__(SKIN_THREADS) skin_pose_bwd_kernel(const B2RSk
       if (lane < 12) acc[j * 12 + lane] = fmaf(w[j], gk, acc[j * 12 + lane]);
     }
   }
-  // dL/dtrans: the block's sum of g_cam = G[:, 3], a fixed shuffle tree per warp
+  // dL/dtrans: the block's sum of g_cam = G[:, 3], a warp_sum per warp
   float t3[3] = {G[3], G[7], G[11]};
 #pragma unroll
-  for (int c = 0; c < 3; c++)
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) t3[c] += __shfl_xor_sync(0xffffffffu, t3[c], d);
+  for (int c = 0; c < 3; c++) t3[c] = warp_sum(t3[c]);
   __shared__ float wtrans[SKIN_WARPS][3];
   if (lane == 0) { wtrans[warp][0] = t3[0]; wtrans[warp][1] = t3[1]; wtrans[warp][2] = t3[2]; }
   __syncthreads();

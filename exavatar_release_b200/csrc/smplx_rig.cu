@@ -96,11 +96,6 @@ inline RigPtrs rig_ptrs(const B2RRig& r, void* scratch) {
   return p;
 }
 
-__device__ __forceinline__ float rig_warp_sum(float v) {
-  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);  // every lane ends with the same bits
-  return v;
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
 // pytorch3d 0.7.5 axis_angle_to_matrix = quaternion_to_matrix(axis_angle_to_quaternion(a)), in fp64, and its adjoint.
 
@@ -335,8 +330,8 @@ __global__ void __launch_bounds__(RIG_THREADS) rig_shape_kernel(const B2RRig r, 
       if (n < r.NB) as += S[n] * b[k];
       if (n < r.NE) ae += E[n] * e[k];
     }
-    as = rig_warp_sum(as);
-    ae = rig_warp_sum(ae);
+    as = warp_sum(as);
+    ae = warp_sum(ae);
     if (lane == 0) {
       s.vs[3 * v + c] = r.template_[3 * v + c] + as;
       s.ev[3 * v + c] = ae;
@@ -389,7 +384,7 @@ __global__ void __launch_bounds__(RIG_THREADS) rig_lbs_kernel(const B2RRig r, co
     const float* D = r.posedirs_t + ((size_t)v * 3 + c) * K;
     float a = 0.f;
     for (int k = lane; k < K; k += 32) a += feat[k] * D[k];
-    po[c] = rig_warp_sum(a);
+    po[c] = warp_sum(a);
   }
   float T[12];
   for (int t = 0; t < 12; t++) T[t] = 0.f;
@@ -397,7 +392,7 @@ __global__ void __launch_bounds__(RIG_THREADS) rig_lbs_kernel(const B2RRig r, co
     const float w = r.lbs_weights[(size_t)v * r.J + j];
     for (int t = 0; t < 12; t++) T[t] += w * an[12 * j + t];
   }
-  for (int t = 0; t < 12; t++) T[t] = rig_warp_sum(T[t]);
+  for (int t = 0; t < 12; t++) T[t] = warp_sum(T[t]);
   if (lane == 0) {
     float x[3];
     for (int c = 0; c < 3; c++) x[c] = s.vs[3 * v + c] + r.pose_offset0[3 * v + c];
@@ -469,8 +464,8 @@ __global__ void __launch_bounds__(RIG_THREADS) rig_bwd_vertex_kernel(const B2RRi
       }
     }
     for (int c = 0; c < 3; c++) {
-      g[c] = rig_warp_sum(g[c]);
-      ge[c] = rig_warp_sum(ge[c]);
+      g[c] = warp_sum(g[c]);
+      ge[c] = warp_sum(ge[c]);
     }
     float T[9];
     for (int t = 0; t < 9; t++) T[t] = 0.f;
@@ -482,7 +477,7 @@ __global__ void __launch_bounds__(RIG_THREADS) rig_bwd_vertex_kernel(const B2RRi
       for (int a = 0; a < 3; a++)
         for (int c = 0; c < 3; c++) T[3 * a + c] += w * an[12 * j + 4 * a + c];
     }
-    for (int t = 0; t < 9; t++) T[t] = rig_warp_sum(T[t]);
+    for (int t = 0; t < 9; t++) T[t] = warp_sum(T[t]);
     if (lane == 0)
       for (int c = 0; c < 3; c++) s.dvs[3 * v + c] = T[c] * g[0] + T[3 + c] * g[1] + T[6 + c] * g[2];
     for (int k = 0; k < 4; k++) {
@@ -889,7 +884,7 @@ __global__ void __launch_bounds__(RIG_THREADS) body_lbs_kernel(const B2RSmplxBod
     const float* D = r.posedirs_t + ((size_t)v * 3 + c) * K;
     float a = 0.f;
     for (int k = lane; k < K; k += 32) a += feat[k] * D[k];
-    po[c] = rig_warp_sum(a);
+    po[c] = warp_sum(a);
   }
   float T[12];
   for (int t = 0; t < 12; t++) T[t] = 0.f;
@@ -897,7 +892,7 @@ __global__ void __launch_bounds__(RIG_THREADS) body_lbs_kernel(const B2RSmplxBod
     const float w = r.lbs_weights[(size_t)v * r.J + j];
     for (int t = 0; t < 12; t++) T[t] += w * an[12 * j + t];
   }
-  for (int t = 0; t < 12; t++) T[t] = rig_warp_sum(T[t]);
+  for (int t = 0; t < 12; t++) T[t] = warp_sum(T[t]);
   if (lane == 0) {
     float x[3], m[3];
     for (int c = 0; c < 3; c++) {
@@ -959,7 +954,7 @@ __global__ void __launch_bounds__(BODY_THREADS) body_bwd_vertex_kernel(const B2R
       for (int a = 0; a < 3; a++)
         for (int c = 0; c < 3; c++) T[3 * a + c] += w * an[12 * j + 4 * a + c];
     }
-    for (int t = 0; t < 9; t++) T[t] = rig_warp_sum(T[t]);
+    for (int t = 0; t < 9; t++) T[t] = warp_sum(T[t]);
     float dvp[3];
     for (int c = 0; c < 3; c++) dvp[c] = T[c] * g[0] + T[3 + c] * g[1] + T[6 + c] * g[2];
     if (lane == 0)
@@ -993,7 +988,7 @@ __global__ void __launch_bounds__(RIG_THREADS) body_bwd_reduce_kernel(const Body
   if (t >= BODY_PART_W) return;
   double a = 0.0;
   for (int blk = lane; blk < BODY_PART_BLOCKS; blk += 32) a += s.part_v[(size_t)blk * BODY_PART_W + t];
-  for (int o = 16; o; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);  // a fixed butterfly: the same bits each run
+  a = warp_sum(a);
   if (lane == 0) s.red[t] = a;
 }
 
