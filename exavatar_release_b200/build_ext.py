@@ -51,7 +51,9 @@ NVCC_FLAGS = [
 # operation by operation.
 # metrics.cu: the PNG round trip, the mask composite and the ScalingLayer are torch's fp32 expressions rounded operation
 # by operation, and SSIM's numerator and denominator are the same bits for identical images (exactly 1).
-PER_FILE_FLAGS = {"metrics.cu": ["--fmad=false"],"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
+# compose.cu: the face and test composites are torch's fp32 expressions a * (1 - m) + b * m rounded operation by
+# operation, signed zeros included; a contracted fma would round once.
+PER_FILE_FLAGS = {"metrics.cu": ["--fmad=false"], "compose.cu": ["--fmad=false"],"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
                   "geometry.cu": ["--fmad=false"], "mesh_raster.cu": ["--fmad=false"],
                   "regularizers.cu": ["--fmad=false"], "smplx_rig.cu": ["--fmad=false"], "adam.cu": ["--fmad=false"],
                   "scene_assets.cu": ["--fmad=false"], "human_assets.cu": ["--fmad=false"],

@@ -134,6 +134,23 @@ int validate_neuman(const B2RNeumanScores* p) {
   return B2R_OK;
 }
 
+// compose.cu: sizes (a grid of N H W / 1024 CTAs stays far inside grid.x) and every image the calls read
+int validate_compose_size(int32_t W, int32_t H, int32_t N) {
+  if (W <= 0 || H <= 0 || N <= 0 || (int64_t)W * H * N >= (int64_t)1 << 36) return B2R_E_INVALID;
+  return B2R_OK;
+}
+
+int validate_test_outputs(const B2RTestOutputs* p) {
+  if (!p) return B2R_E_INVALID;
+  const int rc = validate_compose_size(p->width, p->height, p->n_images);
+  if (rc) return rc;
+  for (int i = 0; i < 5; i++)
+    if (!p->render[i]) return B2R_E_INVALID;
+  for (int k = 0; k < 2; k++)
+    if (!p->mask[k] || !p->face[k]) return B2R_E_INVALID;
+  return B2R_OK;
+}
+
 // sizes and the pointers both directions read; the index tables' contents are the caller's (see b200raster.h)
 int validate_mesh_render(const B2RMeshRender* m) {
   if (!m) return B2R_E_INVALID;
@@ -259,6 +276,8 @@ size_t b2r_sizeof(int which) {
     case 23: return sizeof(B2RSmplxBody);
     case 24: return sizeof(B2RSmplxBodyGrads);
     case 25: return sizeof(B2RNeumanScores);
+    case 26: return sizeof(B2RFaceComposite);
+    case 27: return sizeof(B2RTestOutputs);
     default: return 0;
   }
 }
@@ -688,6 +707,29 @@ int b2r_neuman_scores(const B2RNeumanScores* p, float* out, void* scratch, size_
   if (!out || !scratch) return B2R_E_INVALID;
   if (scratch_bytes < neuman_scratch_bytes(p->width, p->height, p->n_images)) return B2R_E_WORKSPACE;
   return launch_neuman_scores(*p, out, scratch, (cudaStream_t)stream);
+}
+
+int b2r_face_composite_forward(const B2RFaceComposite* p, float* out, void* stream) {
+  if (!p || !p->img || !p->face || !out) return B2R_E_INVALID;
+  const int rc = validate_compose_size(p->width, p->height, p->n_images);
+  if (rc) return rc;
+  return launch_face_composite_forward(*p, out, (cudaStream_t)stream);
+}
+
+int b2r_face_composite_backward(const B2RFaceComposite* p, const float* dout, float* dimg, float* dface, void* stream) {
+  if (!p || !p->face || !dout || (!dimg && !dface)) return B2R_E_INVALID;
+  const int rc = validate_compose_size(p->width, p->height, p->n_images);
+  if (rc) return rc;
+  return launch_face_composite_backward(*p, dout, dimg, dface, (cudaStream_t)stream);
+}
+
+int b2r_test_outputs(const B2RTestOutputs* p, float* const composite[4], uint8_t* png, void* stream) {
+  const int rc = validate_test_outputs(p);
+  if (rc) return rc;
+  if (!composite) return B2R_E_INVALID;
+  for (int k = 0; k < 4; k++)
+    if (!composite[k]) return B2R_E_INVALID;
+  return launch_test_outputs(*p, composite, png, (cudaStream_t)stream);
 }
 
 int b2r_scene_assets_forward(const B2RSceneAssets* s, float* opacity, float* scale, float* rotation, float* color,

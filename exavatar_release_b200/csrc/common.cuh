@@ -581,6 +581,16 @@ __device__ __forceinline__ void block_sum_strided(const T* p, int n, T (&v)[N], 
   block_sum<THREADS>(v, wsum);
 }
 
+// The byte ExAvatar's test.py stores for an fp32 value p: cv2.imwrite(path, img * 255) of a float32 array converts with
+// saturate_cast<uchar>, i.e. v = fl(p * 255), then 0 if v is NaN or |v| >= 2^31 (cvRound's out-of-range result
+// saturates to 0), else clamp(rint(v), 0, 255) with ties to even.  The PNG stores that byte losslessly.  Callers are
+// compiled with --fmad=false (metrics.cu, compose.cu), though the product is rounded on its own either way.
+__device__ __forceinline__ int png_u8(float p) {
+  const float v = p * 255.f;
+  if (isnan(v) || fabsf(v) >= 2147483648.f) return 0;  // cvRound's out-of-range result saturates to 0
+  return min(max(__float2int_rn(v), 0), 255);          // an integer: rint(-0.4) = -0 reads back as +0
+}
+
 // launch wrappers (one per translation unit)
 int launch_project(const B2RScene& sc, const Ctx& cx, int32_t* radii, cudaStream_t st, int first_row = 0);
 int launch_binning(const B2RScene& sc, const Ctx& cx, bool rescan, cudaStream_t st);
@@ -653,6 +663,10 @@ int launch_lpips_backward(const B2RLpips& p, const float* saved, const float* do
                           cudaStream_t st);
 size_t neuman_scratch_bytes(int W, int H, int N);
 int launch_neuman_scores(const B2RNeumanScores& p, float* out, void* scratch, cudaStream_t st);
+int launch_face_composite_forward(const B2RFaceComposite& p, float* out, cudaStream_t st);
+int launch_face_composite_backward(const B2RFaceComposite& p, const float* dout, float* dimg, float* dface,
+                                   cudaStream_t st);
+int launch_test_outputs(const B2RTestOutputs& p, float* const composite[4], uint8_t* png, cudaStream_t st);
 int launch_scene_assets_forward(const B2RSceneAssets& s, float* opacity, float* scale, float* rotation, float* color,
                                 cudaStream_t st);
 int launch_scene_assets_backward(const B2RSceneAssets& s, const B2RSceneAssetsGrads& g, cudaStream_t st);

@@ -107,12 +107,6 @@ static NmLayout nm_layout(int W, int H, int N) {
 // ---------------------------------------------------------------------------------------------------------------------
 // The round trip, the composite and the trunk's input: one thread per pixel of one of the 2N images.
 // ---------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int nm_png_u8(float p) {
-  const float v = p * 255.f;
-  if (isnan(v) || fabsf(v) >= 2147483648.f) return 0;  // cvRound's out-of-range result saturates to 0
-  return min(max(__float2int_rn(v), 0), 255);          // an integer: rint(-0.4) = -0 reads back as +0
-}
-
 __global__ void __launch_bounds__(256) nm_prep_kernel(const float* __restrict__ render, const float* __restrict__ target,
                                                       const float* __restrict__ mask, int mc, int W, int H, int N,
                                                       float* __restrict__ q, float4* __restrict__ in0) {
@@ -125,7 +119,7 @@ __global__ void __launch_bounds__(256) nm_prep_kernel(const float* __restrict__ 
   float r[4];
 #pragma unroll
   for (int c = 0; c < 3; c++) {
-    float v = (float)((double)nm_png_u8(__ldg(src + c * HW)) / 255.0);
+    float v = (float)((double)png_u8(__ldg(src + c * HW)) / 255.0);
     if (mask) {
       const float m = __ldg(mask + (n * mc + (mc == 3 ? c : 0)) * HW + p);
       v = v * m + (1.f - m);

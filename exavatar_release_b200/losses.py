@@ -8,7 +8,8 @@ on the device, so the block can run behind the renderer without draining the str
 
     l1, s = l1_ssim(scene_human_img, gt, bbox)             # rgb_human 0.8 * l1, ssim_human 0.2 * (1 - s)
     l1, s = l1_ssim(scene_img, gt, mask=1 - data['mask'])  # rgb_scene, ssim_scene
-    l1, _ = l1_ssim(face_composite, gt, bbox, ssim=False)  # rgb_face; rgb_human_rand_bg with the composite target
+    l1, _ = l1_ssim(face_composite(scene_human_img, face), gt, bbox, ssim=False)  # rgb_face (compose.face_composite)
+    l1, _ = l1_ssim(human_img, composite_target, bbox, ssim=False)  # rgb_human_rand_bg
 
 `l1_ssim_reference` restates the same semantics in plain torch (float64 by default) for tests and measurements.
 """

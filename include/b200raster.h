@@ -211,7 +211,8 @@ int b2r_last_cuda_error(void);
  * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin, 8 B2RMeshRender, 10 B2RGnMlp, 11 B2RRegs,
  * 12 B2RRegsGrads, 13 B2RRig, 14 B2RRigGrads, 15 B2RAdamSegment, 16 B2RLpips, 17 B2RSceneAssets,
  * 18 B2RSceneAssetsGrads, 19 B2RSmplxPose, 20 B2RSmplxPoseGrads, 21 B2RHumanAssets, 22 B2RHumanAssetsGrads,
- * 23 B2RSmplxBody, 24 B2RSmplxBodyGrads, 25 B2RNeumanScores; 0 for anything else
+ * 23 B2RSmplxBody, 24 B2RSmplxBodyGrads, 25 B2RNeumanScores, 26 B2RFaceComposite, 27 B2RTestOutputs; 0 for
+ * anything else
  * (7 and 9 are unused and report 0). */
 size_t b2r_sizeof(int which);
 
@@ -704,6 +705,45 @@ typedef struct B2RNeumanScores {
 size_t b2r_neuman_scratch_bytes(int32_t width, int32_t height, int32_t n_images);
 int b2r_neuman_scores(const B2RNeumanScores* p, float* out, void* scratch, size_t scratch_bytes, void* stream);
 
+/* ExAvatar's face composite of the rgb_face terms (avatar/main/model.py:200-201, 207-208) of n_images frames: `img`
+ * (N,3,H,W) and the face render `face` (N,4,H,W, -1 where no face), fp32, device, contiguous.  Per channel c < 3
+ *   m = (face[c] != -1 && face[3] == 1) ? 1 : 0,   out[c] = fl(fl(img[c] (1 - m)) + fl(face[c] m)).
+ * Backward (img is not read and may be NULL): dimg[c] = fl(dout[c] (1 - m)), dface[c] = fl(dout[c] m), dface[3] = 0 --
+ * torch autograd's gradients of the expression; either output may be NULL, not both.  One thread per 4 pixels, no
+ * atomics: bit-identical runs.  No allocation, no sync. */
+typedef struct B2RFaceComposite {
+  int32_t width, height, n_images, reserved;
+  const float* img;
+  const float* face;
+} B2RFaceComposite;
+
+int b2r_face_composite_forward(const B2RFaceComposite* p, float* out, void* stream);
+int b2r_face_composite_backward(const B2RFaceComposite* p, const float* dout, float* dimg, float* dface, void* stream);
+
+/* The test-time outputs of ExAvatar (Model.forward(mode='test'), avatar/main/model.py:268-276, and test.py's cv2.imwrite
+ * of every image) of n_images frames in one launch.  Inputs, fp32, device, contiguous: render[5] (N,3,H,W) in the order
+ * scene, human, scene_human, human_refined, scene_human_refined; mask[2] (N,1,H,W) of human and human_refined; face[2]
+ * (N,4,H,W) face renders for the unrefined and the refined human (-1 where no face); gt (N,3,H,W) or NULL.
+ * composite[4] (N,3,H,W), each torch's fp32 expression rounded operation by operation:
+ *   0 human_face_img                    m = fl((face0[c] != -1) face0[3]),  fl(fl(human (1 - m)) + fl(face0[c] m))
+ *   1 human_face_img_refined            the same with face1 and human_refined
+ *   2 scene_human_img_composed          f = (mask0 > 0.9f),  fl(fl(f human) + fl((1 - f) scene_human))
+ *   3 scene_human_img_refined_composed  the same with mask1, human_refined and scene_human_refined
+ * png (NULL: not written) is (K,N,H,W,3) uint8, K = 10 with gt and 9 without: the bytes test.py's
+ * cv2.imwrite(x.transpose(1,2,0)[:,:,::-1] * 255) stores (BGR, png_u8 of csrc/common.cuh) of scene, human,
+ * scene_human, human_refined, scene_human_refined, the four composites in the order above, and gt.  A thread owns 4
+ * pixels; with H W a multiple of 4 and 16-byte aligned pointers it reads and writes float4 and stores its 12 bytes of
+ * each image as three 4-byte words.  No allocation, no sync, no atomics; forward only. */
+typedef struct B2RTestOutputs {
+  int32_t width, height, n_images, reserved;
+  const float* render[5];
+  const float* mask[2];
+  const float* face[2];
+  const float* gt;
+} B2RTestOutputs;
+
+int b2r_test_outputs(const B2RTestOutputs* p, float* const composite[4], uint8_t* png, void* stream);
+
 /* ExAvatar's scene Gaussian assets (avatar/common/nets/module.py:253-272, SceneGaussian.forward) from the stored
  * parameters of P Gaussians with M SH coefficients (1 <= M <= B2R_SCENE_MAX_COEFFS): opacity = sigmoid(logit) (P,1),
  * scale = exp(log_scale) (P,3), rotation = pytorch3d 0.7.5's matrix_to_quaternion(rotation_6d_to_matrix(rotation6d))
@@ -848,7 +888,7 @@ int b2r_camera_setup(const float* R, const float* t, const float* focal, int32_t
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_neuman_scores, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_neuman_scores, b2r_face_composite_*, b2r_test_outputs, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
