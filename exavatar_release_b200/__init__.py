@@ -14,7 +14,8 @@ model.py:217-257), `SmplxRig` (the SMPL-X rig of HumanGaussian.forward, module.p
 step in one launch, base.py:83-85), `LPIPS` (the LPIPS-VGG terms, model.py:199,206), `NeumanScores` (the test-set
 PSNR / SSIM / LPIPS-AlexNet of tools/eval_neuman.py), `face_composite` and `test_outputs` (the face composite of the
 rgb_face terms, model.py:200-201,207-208, and the test-time composites and image bytes, model.py:268-276 and
-main/test.py), `scene_assets` (the scene
+main/test.py), `OrbitCamera`, `orbit_points` and `animation_panel` (the orbit camera, the recentred avatar and the
+three-panel video frame of the animation scripts, animate.py and animate_view_rot.py), `scene_assets` (the scene
 Gaussians' asset dict of SceneGaussian.forward, module.py:253-272), `decode_smplx_pose` (SMPLXParamDict.forward,
 module.py:673-684), `HumanAssets` (HumanGaussian's geometry and colour code around its networks, module.py:524-539,561-565
 and model.py:92-96), synthetic workloads and the frame-sharding helper used by bench.py.
@@ -32,6 +33,7 @@ from .scene_assets import scene_assets  # noqa: F401
 from .perceptual import LPIPS  # noqa: F401
 from .metrics import NeumanScores  # noqa: F401
 from .compose import face_composite, test_outputs  # noqa: F401
+from .animation import OrbitCamera, animation_panel, orbit_points  # noqa: F401
 from .human_assets import HumanAssets, decode_smplx_pose  # noqa: F401
 
 
@@ -45,4 +47,5 @@ def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loa
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "GaussianRenderer",
            "render_settings", "device_render_settings", "TrainingFrameRenderer", "skin_gaussians", "l1_ssim", "nearest_rows", "VertexNormals",
            "FaceMeshRenderer", "ShadedMeshRenderer", "HumanRegularizers", "SmplxRig", "cat_full_pose", "Adam",
-           "scene_assets", "LPIPS", "NeumanScores", "face_composite", "test_outputs", "decode_smplx_pose", "HumanAssets"]
+           "scene_assets", "LPIPS", "NeumanScores", "face_composite", "test_outputs", "OrbitCamera", "orbit_points", "animation_panel",
+           "decode_smplx_pose", "HumanAssets"]

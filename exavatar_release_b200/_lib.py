@@ -180,6 +180,22 @@ class B2RTestOutputs(C.Structure):
                 ("render", _fp * 5), ("mask", _fp * 2), ("face", _fp * 2), ("gt", _fp)]
 
 
+ORBIT_STATE = 20  # B2R_ORBIT_STATE
+
+
+class B2ROrbitCamera(C.Structure):
+    """The animation scripts' orbit camera (b2r_orbit_camera): k, the frame count, the anchor mode, the frame's camera
+    and root joint, the device frame index and the state block."""
+    _fields_ = [("k", C.c_int32), ("n_frames", C.c_int32), ("anchor", C.c_int32), ("reserved", C.c_int32),
+                ("cam_R", _fp), ("cam_t", _fp), ("root_cam", _fp), ("index", _fp), ("state", _fp)]
+
+
+class B2RAnimationPanel(C.Structure):
+    """The animation scripts' three-panel video frame (b2r_animation_panel)."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("reserved", C.c_int32 * 2),
+                ("frame", _fp), ("mesh_panel", _fp), ("render", _fp)]
+
+
 class B2RSceneAssets(C.Structure):
     """ExAvatar's scene Gaussian assets (b2r_scene_assets_forward / b2r_scene_assets_backward): the parameters, their
     row strides, the device degree buffer and the camera (NULL: shs mode)."""
@@ -323,6 +339,10 @@ SYMBOLS = [
     ("b2r_face_composite_forward", C.c_int, [C.POINTER(B2RFaceComposite), _fp, _fp]),
     ("b2r_face_composite_backward", C.c_int, [C.POINTER(B2RFaceComposite), _fp, _fp, _fp, _fp]),
     ("b2r_test_outputs", C.c_int, [C.POINTER(B2RTestOutputs), C.POINTER(_fp), _fp, _fp]),
+    ("b2r_orbit_camera", C.c_int, [C.POINTER(B2ROrbitCamera), _fp]),
+    ("b2r_orbit_points", C.c_int, [C.c_int32, _fp, _fp, C.c_int32, _fp, _fp]),
+    ("b2r_animation_panel", C.c_int, [C.POINTER(B2RAnimationPanel), _fp, _fp]),
+    ("b2r_smplx_body_joints", C.c_int, [C.POINTER(B2RSmplxBody), _fp, C.c_size_t, _fp, _fp]),
     ("b2r_scene_assets_forward", C.c_int, [C.POINTER(B2RSceneAssets), _fp, _fp, _fp, _fp, _fp]),
     ("b2r_scene_assets_backward", C.c_int, [C.POINTER(B2RSceneAssets), C.POINTER(B2RSceneAssetsGrads), _fp]),
     ("b2r_decode_pose_forward", C.c_int, [C.POINTER(B2RSmplxPose), _fp, _fp]),
@@ -364,14 +384,15 @@ def load():
     # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8, B2RGnMlp 10 (9 unused too), B2RRegs 11,
     # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14, B2RAdamSegment 15, B2RLpips 16, B2RSceneAssets 17,
     # B2RSceneAssetsGrads 18, B2RSmplxPose 19, B2RSmplxPoseGrads 20, B2RHumanAssets 21, B2RHumanAssetsGrads 22,
-    # B2RSmplxBody 23, B2RSmplxBodyGrads 24, B2RNeumanScores 25, B2RFaceComposite 26, B2RTestOutputs 27
+    # B2RSmplxBody 23, B2RSmplxBodyGrads 24, B2RNeumanScores 25, B2RFaceComposite 26, B2RTestOutputs 27,
+    # B2ROrbitCamera 28, B2RAnimationPanel 29
     for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
                      (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp), (11, B2RRegs),
                      (12, B2RRegsGrads), (13, B2RRig), (14, B2RRigGrads), (15, B2RAdamSegment),
                      (16, B2RLpips), (17, B2RSceneAssets), (18, B2RSceneAssetsGrads), (19, B2RSmplxPose),
                      (20, B2RSmplxPoseGrads), (21, B2RHumanAssets), (22, B2RHumanAssetsGrads), (23, B2RSmplxBody),
                      (24, B2RSmplxBodyGrads), (25, B2RNeumanScores), (26, B2RFaceComposite),
-                     (27, B2RTestOutputs)):
+                     (27, B2RTestOutputs), (28, B2ROrbitCamera), (29, B2RAnimationPanel)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

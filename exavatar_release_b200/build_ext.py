@@ -53,7 +53,9 @@ NVCC_FLAGS = [
 # by operation, and SSIM's numerator and denominator are the same bits for identical images (exactly 1).
 # compose.cu: the face and test composites are torch's fp32 expressions a * (1 - m) + b * m rounded operation by
 # operation, signed zeros included; a contracted fma would round once.
-PER_FILE_FLAGS = {"metrics.cu": ["--fmad=false"], "compose.cu": ["--fmad=false"],"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
+# animate.cu: the orbit camera is pytorch3d's look_at_view_transform in fp32 and the recentring is
+# fl(fl(p - root) + at), both rounded operation by operation like the scripts' torch expressions.
+PER_FILE_FLAGS = {"metrics.cu": ["--fmad=false"], "compose.cu": ["--fmad=false"], "animate.cu": ["--fmad=false"],"project.cu": ["--fmad=false"], "binning.cu": ["--fmad=false"], "skin.cu": ["--fmad=false"],
                   "geometry.cu": ["--fmad=false"], "mesh_raster.cu": ["--fmad=false"],
                   "regularizers.cu": ["--fmad=false"], "smplx_rig.cu": ["--fmad=false"], "adam.cu": ["--fmad=false"],
                   "scene_assets.cu": ["--fmad=false"], "human_assets.cu": ["--fmad=false"],

@@ -278,6 +278,8 @@ size_t b2r_sizeof(int which) {
     case 25: return sizeof(B2RNeumanScores);
     case 26: return sizeof(B2RFaceComposite);
     case 27: return sizeof(B2RTestOutputs);
+    case 28: return sizeof(B2ROrbitCamera);
+    case 29: return sizeof(B2RAnimationPanel);
     default: return 0;
   }
 }
@@ -730,6 +732,34 @@ int b2r_test_outputs(const B2RTestOutputs* p, float* const composite[4], uint8_t
   for (int k = 0; k < 4; k++)
     if (!composite[k]) return B2R_E_INVALID;
   return launch_test_outputs(*p, composite, png, (cudaStream_t)stream);
+}
+
+int b2r_orbit_camera(const B2ROrbitCamera* p, void* stream) {
+  if (!p || !p->index || !p->state || p->k <= 0 || p->n_frames <= 0 || p->anchor < 0 || p->anchor > 2)
+    return B2R_E_INVALID;
+  const bool any_cam = p->cam_R || p->cam_t || p->root_cam, all_cam = p->cam_R && p->cam_t && p->root_cam;
+  if (any_cam != all_cam || (p->anchor != 0 && !all_cam)) return B2R_E_INVALID;
+  return launch_orbit_camera(*p, (cudaStream_t)stream);
+}
+
+int b2r_orbit_points(int32_t n, const float* points, const float* state, int32_t view, float* out, void* stream) {
+  if (n <= 0 || !points || !state || !out) return B2R_E_INVALID;
+  return launch_orbit_points(n, points, state, view != 0, out, (cudaStream_t)stream);
+}
+
+int b2r_animation_panel(const B2RAnimationPanel* p, uint8_t* out, void* stream) {
+  if (!p || !p->frame || !p->mesh_panel || !p->render || !out) return B2R_E_INVALID;
+  if (p->width <= 0 || p->height <= 0 || (int64_t)p->width * p->height >= (int64_t)1 << 31) return B2R_E_INVALID;
+  return launch_animation_panel(*p, out, (cudaStream_t)stream);
+}
+
+int b2r_smplx_body_joints(const B2RSmplxBody* b, const void* scratch, size_t scratch_bytes, float* joints,
+                          void* stream) {
+  const int rc = validate_body(b);
+  if (rc) return rc;
+  if (!joints || !scratch) return B2R_E_INVALID;
+  if (scratch_bytes < smplx_body_scratch_bytes(b->rig.V)) return B2R_E_WORKSPACE;
+  return launch_smplx_body_joints(*b, scratch, joints, (cudaStream_t)stream);
 }
 
 int b2r_scene_assets_forward(const B2RSceneAssets* s, float* opacity, float* scale, float* rotation, float* color,

@@ -655,6 +655,10 @@ size_t smplx_body_scratch_bytes(int V);
 int launch_smplx_body_forward(const B2RSmplxBody& b, float* mesh, void* scratch, cudaStream_t st);
 int launch_smplx_body_backward(const B2RSmplxBody& b, const float* dmesh, const B2RSmplxBodyGrads& g, void* scratch,
                                cudaStream_t st);
+int launch_smplx_body_joints(const B2RSmplxBody& b, const void* scratch, float* joints, cudaStream_t st);
+int launch_orbit_camera(const B2ROrbitCamera& p, cudaStream_t st);
+int launch_orbit_points(int n, const float* points, const float* state, int view, float* out, cudaStream_t st);
+int launch_animation_panel(const B2RAnimationPanel& p, uint8_t* out, cudaStream_t st);
 int launch_adam_step(const B2RAdamSegment* table, int n_segments, int64_t n_chunks, cudaStream_t st);
 size_t lpips_saved_bytes(int W, int H, int N);
 size_t lpips_scratch_bytes(int W, int H);

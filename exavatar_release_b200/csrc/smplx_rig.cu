@@ -1080,7 +1080,26 @@ __global__ void __launch_bounds__(2 * RIG_CMAX) body_bwd_coeff_kernel(const B2RS
   (shape ? gr.shape_param : gr.expr)[n] = (float)a;
 }
 
+// smplx's output.joints[:J]: batch_rigid_transform's posed joints (the chain's translations) + transl, from the
+// forward's saved rest joints -- the same chain the backward reruns
+__global__ void __launch_bounds__(RIG_JMAX) body_joints_kernel(const B2RSmplxBody b, const BodyPtrs s,
+                                                               float* __restrict__ joints) {
+  __shared__ BodyChainSm sm;
+  body_chain(b, s, sm, false);
+  const int tid = threadIdx.x;
+  if (tid >= b.rig.J) return;
+  for (int c = 0; c < 3; c++) joints[3 * tid + c] = sm.bad ? nanf("") : (float)sm.G[12 * tid + 4 * c + 3] + b.trans[c];
+}
+
 size_t smplx_body_scratch_bytes(int V) { return body_layout(V).total; }
+
+int launch_smplx_body_joints(const B2RSmplxBody& body, const void* scratch, float* joints, cudaStream_t st) {
+  const B2RSmplxBody b = with_body_inputs(body);
+  const BodyPtrs s = body_ptrs(b, const_cast<void*>(scratch));  // the kernel only reads the saved joints
+  ProfScope p(K_MISC, st);
+  launch_k(body_joints_kernel, 1, RIG_JMAX, 0, st, true, b, s, joints);
+  return check_launch();
+}
 
 int launch_smplx_body_forward(const B2RSmplxBody& body, float* mesh, void* scratch, cudaStream_t st) {
   const B2RSmplxBody b = with_body_inputs(body);

@@ -249,7 +249,7 @@ class _Rig(torch.autograd.Function):
 
 class _Body(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, rig, shape_param, joint_offset, full_pose, expr, trans, cam_R, cam_t):
+    def forward(ctx, rig, shape_param, joint_offset, full_pose, expr, trans, cam_R, cam_t, joints=None):
         dev = rig.device
         ins = [rig._input(t, n, name) for t, n, name in ((shape_param, rig.NB, "shape_param"),
                                                           (joint_offset, 3 * rig.J, "joint_offset"),
@@ -262,6 +262,8 @@ class _Body(torch.autograd.Function):
         scratch = torch.empty(rig.body_scratch_bytes, dtype=torch.uint8, device=dev)
         st = rig._body_struct(ins, cam)
         L.run("b2r_smplx_body_forward", dev, C.byref(st), L.ptr(mesh), L.ptr(scratch), rig.body_scratch_bytes)
+        if joints is not None:
+            L.run("b2r_smplx_body_joints", dev, C.byref(st), L.ptr(scratch), rig.body_scratch_bytes, L.ptr(joints))
         ctx.rig = rig
         ctx.n_cam = len(cam)
         ctx.set_materialize_grads(False)
@@ -280,7 +282,7 @@ class _Body(torch.autograd.Function):
         up = None if g_mesh is None else g_mesh.to(torch.float32).contiguous()
         st = rig._body_struct(ins, cam)
         L.run("b2r_smplx_body_backward", dev, C.byref(st), L.ptr(up), C.byref(gs), L.ptr(scratch), scratch.numel())
-        return (None, *[g.reshape(s) for g, s in zip(grads, ctx.shapes)], None, None)
+        return (None, *[g.reshape(s) for g, s in zip(grads, ctx.shapes)], None, None, None)
 
 
 class SmplxRig:
@@ -386,7 +388,7 @@ class SmplxRig:
             st.cam_R, st.cam_t = (L.ptr(t) for t in cam)
         return st
 
-    def body_mesh(self, shape_param, joint_offset, full_pose, expr, trans, cam_R=None, cam_t=None) -> torch.Tensor:
+    def body_mesh(self, shape_param, joint_offset, full_pose, expr, trans, cam_R=None, cam_t=None, joints=False):
         """The frame's SMPL-X body mesh (V,3) float32: ExAvatar's get_smplx_outputs (model.py:37-58), i.e. smplx's
         SMPLX.forward + lbs (body_models.py:1122-1300, lbs.py:155-250) with face_offset, the raw joint_offset and transl,
         then R^-1 (mesh - t) in world coordinates.  Without a camera the mesh stays in camera coordinates (animate.py).
@@ -398,8 +400,16 @@ class SmplxRig:
         the camera gets none.  The layer's landmarks, extra joints and `joints` output, which both callers discard, are
         not computed.  Divergence from the reference: v_shaped is (template + shapedirs . beta) + expr_dirs . expr in
         fp32 (smplx contracts the 150 coefficients in one einsum), the joints, rotations and chain run in fp64, and
-        R^-1 is taken by cofactors instead of torch.inverse, so nothing synchronises the host."""
-        return _Body.apply(self, shape_param, joint_offset, full_pose, expr, trans, cam_R, cam_t)
+        R^-1 is taken by cofactors instead of torch.inverse, so nothing synchronises the host.
+
+        With joints=True it returns (mesh, joints): joints (J,3) float32 with no gradient, the first J rows of smplx's
+        `output.joints` (the posed joints plus transl, in the layer's camera coordinates whether or not a camera is
+        given), from the same chain in one more launch -- animate_view_rot.py's root joint is joints[0]."""
+        out = None
+        if joints:
+            out = torch.empty((self.J, 3), dtype=torch.float32, device=self.device)
+        mesh = _Body.apply(self, shape_param, joint_offset, full_pose, expr, trans, cam_R, cam_t, out)
+        return mesh if out is None else (mesh, out)
 
 
 def validate_model(*, v_template, shapedirs, expr_dirs, posedirs, J_regressor, parents, lbs_weights, pose_mean,
@@ -517,12 +527,13 @@ def smplx_rig_reference(model: dict, shape_param, joint_offset, full_pose, expr,
 
 
 def smplx_body_reference(model: dict, shape_param, joint_offset, full_pose, expr, trans, cam_R=None, cam_t=None, *,
-                         dtype=torch.float64, device=None) -> torch.Tensor:
+                         dtype=torch.float64, device=None, joints: bool = False):
     """get_smplx_outputs (avatar/main/model.py:37-58) restated in torch, differentiable in the five inputs: smplx's
     SMPLX.forward + lbs for one frame with face_offset, the raw joint_offset and transl (body_models.py:1233 adds
     pose_mean; lbs.py:155-250 with smplx's batch_rodrigues and batch_rigid_transform), then torch.inverse(R) (mesh - t)
     when a camera is given.  `model` is validate_model's dict (SmplxRig.model); the tables are cast to `dtype`, so
-    dtype=torch.float32 is ExAvatar's own fp32 route.  The product never calls this."""
+    dtype=torch.float32 is ExAvatar's own fp32 route.  With joints=True it returns (mesh, joints), joints (J,3) being
+    smplx's output.joints[:J]: the posed joints + transl, never moved by the camera.  The product never calls this."""
     dev = torch.device(device) if device is not None else shape_param.device
     cv = lambda t: t.to(device=dev, dtype=dtype)  # noqa: E731
     V, J = model["V"], model["J"]
@@ -535,9 +546,9 @@ def smplx_body_reference(model: dict, shape_param, joint_offset, full_pose, expr
     rot = batch_rodrigues(pose + cv(model["pose_mean"]).view(J, 3))
     eye = torch.eye(3, dtype=dtype, device=dev)
     v_posed = v_shaped + ((rot[1:] - eye).reshape(1, -1) @ cv(model["posedirs"])).view(V, 3)
-    _, A = rigid_transform(rot, Jr, model["parents"].tolist())
+    posed, A = rigid_transform(rot, Jr, model["parents"].tolist())
     T = (cv(model["lbs_weights"]) @ A.reshape(J, 16)).view(V, 4, 4)
     mesh = (T @ torch.cat([v_posed, torch.ones_like(v_posed[:, :1])], 1)[:, :, None])[:, :3, 0] + tr
     if cam_R is not None:
         mesh = torch.matmul(torch.inverse(cv(cam_R)), (mesh - cv(cam_t).view(1, 3)).permute(1, 0)).permute(1, 0)
-    return mesh
+    return (mesh, posed + tr) if joints else mesh

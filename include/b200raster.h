@@ -211,8 +211,8 @@ int b2r_last_cuda_error(void);
  * 3 B2RForwardOutputs, 4 B2RBackwardArgs, 5 B2RView, 6 B2RSkin, 8 B2RMeshRender, 10 B2RGnMlp, 11 B2RRegs,
  * 12 B2RRegsGrads, 13 B2RRig, 14 B2RRigGrads, 15 B2RAdamSegment, 16 B2RLpips, 17 B2RSceneAssets,
  * 18 B2RSceneAssetsGrads, 19 B2RSmplxPose, 20 B2RSmplxPoseGrads, 21 B2RHumanAssets, 22 B2RHumanAssetsGrads,
- * 23 B2RSmplxBody, 24 B2RSmplxBodyGrads, 25 B2RNeumanScores, 26 B2RFaceComposite, 27 B2RTestOutputs; 0 for
- * anything else
+ * 23 B2RSmplxBody, 24 B2RSmplxBodyGrads, 25 B2RNeumanScores, 26 B2RFaceComposite, 27 B2RTestOutputs,
+ * 28 B2ROrbitCamera, 29 B2RAnimationPanel; 0 for anything else
  * (7 and 9 are unused and report 0). */
 size_t b2r_sizeof(int which);
 
@@ -744,6 +744,64 @@ typedef struct B2RTestOutputs {
 
 int b2r_test_outputs(const B2RTestOutputs* p, float* const composite[4], uint8_t* png, void* stream);
 
+/* The orbit camera of ExAvatar's animation scripts (avatar/main/animate_view_rot.py:79-95, get_neutral_pose.py:76-82):
+ * pytorch3d's look_at_view_transform(dist, elev, azim, degrees=False, at, up=((0,1,0),)) and the script's
+ * torch.inverse of its R, one thread on the device.  `state` is a B2R_ORBIT_STATE-float block the caller owns:
+ *   [0,3) at   [3] elev   [4] dist   (the anchors)   [5,14) R (3,3) row-major   [14,17) t   [17,20) root_world
+ * Anchors: with anchor = 2, or anchor = 1 and *index == 0, they are set from this call's camera first (the script's
+ * `if i == 0`): root_world = R^-1 (root_cam - t) with R^-1 by cofactors (camera._inv3's fp32 expressions),
+ * at = root_world, cam_pos = R^-1 (-t), elev = atanf(|root_cam.y| / |root_cam.z|), dist = sqrtf(sum (cam_pos - at)^2).
+ * With anchor = 0 they are the caller's (written once, e.g. get_neutral_pose's fixed at / elev / dist).
+ * Every call then writes frame i = *index (int32, device; one captured graph serves every frame) in fp32, each
+ * operation rounded on its own:
+ *   azim = float(pi + ((pi k) i) / n_frames) evaluated in double;
+ *   C = (dist cos(elev) sin(azim), dist sin(elev), dist cos(elev) cos(azim)) + at;
+ *   z = n(at - C), x = n(up x z), y = n(z x x) with up = (0,1,0), n(v) = v / max(|v|, 1e-5);
+ *   if every |x_c| <= 5e-3: x = n(y x z) (look_at_rotation's is_close branch);
+ *   R_p3d = [x y z] (columns), T = -R_p3d^T C;  the state's R = R_p3d^-1 by cofactors, t = T;
+ *   root_world = R^-1 (root_cam - t) of this call's camera (= at when cam_R, cam_t and root_cam are all NULL, which
+ *   only anchor = 0 allows).
+ * 1 <= k, 1 <= n_frames, anchor in {0, 1, 2}.  One launch of one thread; no allocation, no sync. */
+#define B2R_ORBIT_STATE 20
+typedef struct B2ROrbitCamera {
+  int32_t k, n_frames, anchor, reserved;
+  const float* cam_R;     /* (3,3) the frame's camera */
+  const float* cam_t;     /* (3) */
+  const float* root_cam;  /* (3) the root joint in that camera's coordinates */
+  const int32_t* index;   /* (1) the frame index i */
+  float* state;           /* (B2R_ORBIT_STATE) */
+} B2ROrbitCamera;
+
+int b2r_orbit_camera(const B2ROrbitCamera* p, void* stream);
+
+/* The recentring of animate_view_rot.py:92 and :103, and optionally the view transform of :97, on n (n,3) fp32 rows,
+ * one thread per row, with the state block b2r_orbit_camera wrote: out[r] = (fl(fl(p0 - root_world0) + at0), p1,
+ * fl(fl(p2 - root_world2) + at2)); with view != 0 then out[r] = R q + t, ((R_c0 q0 + R_c1 q1) + R_c2 q2) + t_c.
+ * points and out must not overlap.  No allocation, no sync. */
+int b2r_orbit_points(int32_t n, const float* points, const float* state, int32_t view, float* out, void* stream);
+
+/* The uint8 (H, 3W, 3) BGR video frame of animate.py:86,94 and animate_view_rot.py:107,115 before the text, in one
+ * launch: left the source frame (H,W,3) uint8 BGR copied as is; middle trunc(mesh_panel) of the (H,W,3) fp32
+ * ShadedMeshRenderer output; right trunc(fl(render[2-c] * 255)) of the (3,H,W) fp32 render, channels reversed.
+ * trunc rounds toward zero (numpy's astype(np.uint8) on [0, 256)); values outside saturate to 0 / 255, NaN gives 0.
+ * A thread owns 8 pixels of a row in all three panels; with W a multiple of 8, 16-byte aligned float inputs and 8-byte
+ * aligned frame / out it reads float4 / 8-byte words and stores 8-byte words.  No allocation, no sync. */
+typedef struct B2RAnimationPanel {
+  int32_t width, height, reserved[2];
+  const uint8_t* frame;
+  const float* mesh_panel;
+  const float* render;
+} B2RAnimationPanel;
+
+int b2r_animation_panel(const B2RAnimationPanel* p, uint8_t* out, void* stream);
+
+/* The first J rows of smplx's `output.joints` for the body b2r_smplx_body_forward last posed with `scratch` (the same
+ * B2RSmplxBody and inputs, still unchanged): the posed joints of the chain, rerun in fp64 from the forward's saved rest
+ * joints, plus trans in fp32 -- in the layer's camera coordinates whether or not b->cam_R is set.  joints (J,3) fp32.
+ * One CTA; no allocation, no sync. */
+int b2r_smplx_body_joints(const B2RSmplxBody* b, const void* scratch, size_t scratch_bytes, float* joints,
+                          void* stream);
+
 /* ExAvatar's scene Gaussian assets (avatar/common/nets/module.py:253-272, SceneGaussian.forward) from the stored
  * parameters of P Gaussians with M SH coefficients (1 <= M <= B2R_SCENE_MAX_COEFFS): opacity = sigmoid(logit) (P,1),
  * scale = exp(log_scale) (P,3), rotation = pytorch3d 0.7.5's matrix_to_quaternion(rotation_6d_to_matrix(rotation6d))
@@ -888,7 +946,7 @@ int b2r_camera_setup(const float* R, const float* t, const float* focal, int32_t
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_neuman_scores, b2r_face_composite_*, b2r_test_outputs, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_neuman_scores, b2r_face_composite_*, b2r_test_outputs, b2r_orbit_*, b2r_animation_panel, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
