@@ -99,6 +99,14 @@ int validate_pose(const B2RSmplxPose* p) {
   return J >= 1 && J <= B2R_POSE_MAX_JOINTS ? B2R_OK : B2R_E_INVALID;
 }
 
+// a parameter table's sizes (one thread per joint, at least one frame) and its tables
+int validate_param_table(const B2RSmplxParamTable* t) {
+  if (!t || !t->pose || !t->trans) return B2R_E_INVALID;
+  if (t->n_frames < 1 || t->n_joints < 1 || t->n_joints > B2R_POSE_MAX_JOINTS || t->n_expr < 0) return B2R_E_INVALID;
+  if (t->n_expr > 0 && !t->expr) return B2R_E_INVALID;
+  return B2R_OK;
+}
+
 // sizes, row strides and every input pointer (an empty set reads nothing)
 int validate_human_assets(const B2RHumanAssets* h) {
   if (!h || h->P < 0 || (h->warmup != 0 && h->warmup != 1)) return B2R_E_INVALID;
@@ -280,6 +288,8 @@ size_t b2r_sizeof(int which) {
     case 27: return sizeof(B2RTestOutputs);
     case 28: return sizeof(B2ROrbitCamera);
     case 29: return sizeof(B2RAnimationPanel);
+    case 31: return sizeof(B2RSmplxParamTable);  // 30 stays unused
+    case 32: return sizeof(B2RSmplxParamTableGrads);
     default: return 0;
   }
 }
@@ -798,6 +808,20 @@ int b2r_decode_pose_backward(const B2RSmplxPose* p, const float* dL_dfull_pose, 
   for (int k = 0; k < B2R_POSE_PARAMS; ++k)
     if (p->rows[k] > 0 && !grads->param[k]) return B2R_E_INVALID;
   return launch_decode_pose_backward(*p, dL_dfull_pose, *grads, (cudaStream_t)stream);
+}
+
+int b2r_param_table_forward(const B2RSmplxParamTable* t, float* full_pose, float* expr, float* trans, void* stream) {
+  const int rc = validate_param_table(t);
+  if (rc) return rc;
+  if (!full_pose || !trans || (t->n_expr > 0 && !expr)) return B2R_E_INVALID;
+  return launch_param_table_forward(*t, full_pose, expr, trans, (cudaStream_t)stream);
+}
+
+int b2r_param_table_backward(const B2RSmplxParamTable* t, const B2RSmplxParamTableGrads* g, void* stream) {
+  const int rc = validate_param_table(t);
+  if (rc) return rc;
+  if (!g || !g->pose || !g->trans || (t->n_expr > 0 && !g->expr)) return B2R_E_INVALID;
+  return launch_param_table_backward(*t, *g, (cudaStream_t)stream);
 }
 
 int b2r_human_geometry_forward(const B2RHumanAssets* h, float* mean_3d, float* mean_3d_refined, float* scale,

@@ -676,6 +676,9 @@ int launch_scene_assets_forward(const B2RSceneAssets& s, float* opacity, float* 
 int launch_scene_assets_backward(const B2RSceneAssets& s, const B2RSceneAssetsGrads& g, cudaStream_t st);
 int launch_decode_pose_forward(const B2RSmplxPose& p, float* full_pose, cudaStream_t st);
 int launch_decode_pose_backward(const B2RSmplxPose& p, const float* dfull, const B2RSmplxPoseGrads& g, cudaStream_t st);
+int launch_param_table_forward(const B2RSmplxParamTable& t, float* full_pose, float* expr, float* trans,
+                               cudaStream_t st);
+int launch_param_table_backward(const B2RSmplxParamTable& t, const B2RSmplxParamTableGrads& g, cudaStream_t st);
 int launch_human_geometry_forward(const B2RHumanAssets& h, float* mean, float* mean_r, float* scale, float* scale_r,
                                   float* mmo, float* scale_wo, float* scale_r_wo, cudaStream_t st);
 int launch_human_geometry_backward(const B2RHumanAssets& h, const B2RHumanAssetsGrads& g, cudaStream_t st);

@@ -9,7 +9,7 @@
 //
 // Scope: every rasteriser call -- adaptive capacity, fixed capacity (no polling, capturable in a CUDA graph) and
 // debug=True (synchronises after each call).  rasterizer.py only maps the public arguments onto `rasterize` and dumps
-// the inputs of a failed debug call.  Also here: the host side of optim.Adam's step (`adam_step`), whose walk over
+// the inputs of a failed debug call.  Also here: the host side of optim.Adam's step (`adam_stage`, `adam_launch`), whose walk over
 // thousands of SMPL-X param groups per step costs milliseconds in Python.
 #include <torch/extension.h>
 
@@ -388,13 +388,33 @@ bool row_layout(const at::Tensor& p, int64_t& row_len, int64_t& row_stride) {
 
 [[noreturn]] void value_error(const std::string& what) { throw py::value_error("Adam: " + what); }
 
-// One Adam step over every param with a gradient in `groups` (the optimizer's param_groups), with torch.optim.Adam's
-// lazy state in `state`: one pinned segment table, one async H2D copy, one launch on the current stream of `device`.
-void adam_step(const py::list& groups, const py::object& state, int64_t device, int64_t chunk) {
+// The host half of an Adam step over every param with a gradient in `groups` (the optimizer's param_groups), with
+// torch.optim.Adam's lazy state in `state`: the walk, the lazy state, the step counts, the scalars and the segment
+// table, written into the resident device table `table` (reallocated when undefined or too small) with one async H2D
+// copy from pinned memory on the current stream of `device`.  A group with a true "frame_rows" key has dim 0 = frame:
+// only row `rows` of each of its params is stepped, with that row's own count in state["step"], a (rows,) CPU float32
+// tensor.  Returns (table, n_segments, n_chunks, layout): `layout` names what a launch captured in a graph depends on
+// (the tensors and their sizes, the chunk count; not the rows, the scalars or the counts).  Every check runs before
+// anything is created or counted.  When `expect` is not None and the layout differs from it, no state is created,
+// nothing is counted, copied or written, and the table comes back as it was.  With no gradient at all the table also
+// comes back as it was (undefined if it never existed) and n_chunks is 0: nothing to launch.
+py::tuple adam_stage(const py::list& groups, const py::object& state, int64_t device, int64_t chunk,
+                     const py::object& rows, const c10::optional<at::Tensor>& table_in, const py::object& expect) {
+  at::Tensor table = table_in.has_value() ? *table_in : at::Tensor();
   const at::Device dev(at::kCUDA, (c10::DeviceIndex)device);
-  std::vector<B2RAdamSegment> segs;
+  struct Entry {
+    py::handle ph;
+    at::Tensor p, g;
+    bool frame_rows;
+    int64_t row;  // -1: the whole tensor
+    int64_t numel, row_len, row_stride;
+    double lr, beta1, beta2, eps;
+  };
+  // pass 1: every check, nothing created or counted
+  std::vector<Entry> entries;
   for (const py::handle gh : groups) {
     const py::dict group = py::reinterpret_borrow<py::dict>(gh);
+    const bool frame_rows = group.contains("frame_rows") && py::bool_(group["frame_rows"]);
     bool scalars = false;
     double lr = 0, beta1 = 0, beta2 = 0, eps = 0;
     for (const py::handle ph : py::reinterpret_borrow<py::list>(group["params"])) {
@@ -402,6 +422,15 @@ void adam_step(const py::list& groups, const py::object& state, int64_t device, 
       const at::Tensor& g = p.grad();
       if (!g.defined()) continue;
       if (g.is_sparse()) value_error("sparse gradients are not supported");
+      int64_t row = -1;
+      if (frame_rows) {
+        if (rows.is_none()) value_error("a frame-row group is stepped only with `rows` (the frame's slot)");
+        if (p.dim() < 1 || !p.is_contiguous()) value_error("a frame-row parameter must be contiguous with dim 0 = frame");
+        row = rows.cast<int64_t>();
+        if (row < 0 || row >= p.size(0))
+          value_error("rows=" + std::to_string(row) + " lies outside a frame-row parameter's " +
+                      std::to_string(p.size(0)) + " rows");
+      }
       if (p.device() != dev || p.scalar_type() != at::kFloat)
         value_error("parameters must be float32 tensors on the optimizer's CUDA device");
       if (g.scalar_type() != at::kFloat || g.device() != dev || g.sizes() != p.sizes() || !g.is_contiguous())
@@ -414,50 +443,108 @@ void adam_step(const py::list& groups, const py::object& state, int64_t device, 
         eps = group["eps"].cast<double>();
         scalars = true;
       }
-      py::object st = state[ph];  // a defaultdict: the first access creates the empty state
-      if (py::len(st) == 0) {     // torch.optim.Adam._init_group's lazy state (capturable=False, fused=False)
-        st["step"] = at::zeros({}, at::TensorOptions().dtype(at::kFloat));
-        st["exp_avg"] = at::zeros_like(p, at::MemoryFormat::Preserve);
-        st["exp_avg_sq"] = at::zeros_like(p, at::MemoryFormat::Preserve);
+      if (state.contains(ph)) {
+        const py::object st = state[ph];
+        if (py::len(st) != 0) {
+          const at::Tensor step = st["step"].cast<at::Tensor>();
+          const at::Tensor m = st["exp_avg"].cast<at::Tensor>(), v = st["exp_avg_sq"].cast<at::Tensor>();
+          if (!step.device().is_cpu() || step.scalar_type() != at::kFloat || !step.is_contiguous() ||
+              (frame_rows ? step.dim() != 1 || step.size(0) != p.size(0) : step.numel() != 1))
+            value_error(frame_rows ? "state 'step' of a frame-row parameter must be a (rows,) CPU float32 tensor"
+                                   : "state 'step' must be a CPU float32 scalar tensor");
+          for (const at::Tensor* t : {&m, &v})
+            if (t->device() != dev || t->scalar_type() != at::kFloat || t->sizes() != p.sizes() || !t->is_contiguous())
+              value_error("exp_avg / exp_avg_sq must be contiguous float32 tensors shaped and placed as their parameter");
+        }
       }
-      const at::Tensor step = st["step"].cast<at::Tensor>();
-      const at::Tensor m = st["exp_avg"].cast<at::Tensor>(), v = st["exp_avg_sq"].cast<at::Tensor>();
-      if (!step.device().is_cpu() || step.scalar_type() != at::kFloat || step.numel() != 1)
-        value_error("state 'step' must be a CPU float32 scalar tensor");
-      for (const at::Tensor* t : {&m, &v})
-        if (t->device() != dev || t->scalar_type() != at::kFloat || t->sizes() != p.sizes() || !t->is_contiguous())
-          value_error("exp_avg / exp_avg_sq must be contiguous float32 tensors shaped and placed as their parameter");
-      // as torch's _foreach_add_(steps, tensor(1.), alpha=1.): every step count of a param with a gradient advances
-      float* sp = step.data_ptr<float>();
-      *sp = *sp + 1.0f;
-      if (p.numel() == 0) continue;
-      B2RAdamSegment s{};
-      if (!row_layout(p, s.row_len, s.row_stride))
+      const int64_t numel = row < 0 ? p.numel() : p.numel() / p.size(0);
+      int64_t row_len = numel, row_stride = numel;
+      if (numel > 0 && row < 0 && !row_layout(p, row_len, row_stride))
         value_error("a parameter must be contiguous or rows of contiguous floats at one stride");
-      s.param = p.data_ptr<float>();
-      s.grad = g.data_ptr<float>();
-      s.exp_avg = m.data_ptr<float>();
-      s.exp_avg_sq = v.data_ptr<float>();
-      s.numel = p.numel();
-      adam_scalars(lr, beta1, beta2, eps, (double)*sp, s);
-      segs.push_back(s);
+      entries.push_back({ph, p, g, frame_rows, row, numel, row_len, row_stride, lr, beta1, beta2, eps});
     }
   }
-  if (segs.empty()) return;
   int64_t n_chunks = 0;
-  for (auto& s : segs) {
-    s.first_chunk = n_chunks;
-    n_chunks += (s.numel + chunk - 1) / chunk;
+  for (const Entry& e : entries)
+    if (e.numel > 0) n_chunks += (e.numel + chunk - 1) / chunk;
+  // the layout a captured launch depends on; moments not created yet count as address 0
+  auto layout_of = [&](const std::vector<std::pair<const void*, const void*>>& moments) {
+    std::vector<int64_t> layout;
+    for (size_t i = 0; i < entries.size(); ++i) {
+      const Entry& e = entries[i];
+      for (const int64_t x : {(int64_t)(uintptr_t)e.p.data_ptr(), (int64_t)(uintptr_t)e.g.data_ptr(),
+                              (int64_t)(uintptr_t)moments[i].first, (int64_t)(uintptr_t)moments[i].second, e.numel,
+                              e.row_len, e.row_stride, (int64_t)(e.row >= 0)})
+        layout.push_back(x);
+    }
+    layout.push_back(n_chunks);
+    return py::bytes(reinterpret_cast<const char*>(layout.data()), layout.size() * sizeof(int64_t));
+  };
+  std::vector<std::pair<const void*, const void*>> moments;
+  for (const Entry& e : entries) {
+    const void *m = nullptr, *v = nullptr;
+    if (state.contains(e.ph) && py::len(state[e.ph]) != 0) {
+      m = state[e.ph]["exp_avg"].cast<at::Tensor>().data_ptr();
+      v = state[e.ph]["exp_avg_sq"].cast<at::Tensor>().data_ptr();
+    }
+    moments.emplace_back(m, v);
   }
+  if (!expect.is_none() && !layout_of(moments).equal(expect))
+    return py::make_tuple(table, 0, 0, layout_of(moments));
+  // pass 2: lazy state, counts, scalars, segments
+  std::vector<B2RAdamSegment> segs;
+  moments.clear();
+  n_chunks = 0;
+  for (const Entry& e : entries) {
+    py::object st = state[e.ph];  // a defaultdict: the first access creates the empty state
+    if (py::len(st) == 0) {       // torch.optim.Adam._init_group's lazy state (capturable=False, fused=False)
+      st["step"] = e.frame_rows ? at::zeros({e.p.size(0)}, at::TensorOptions().dtype(at::kFloat))
+                                : at::zeros({}, at::TensorOptions().dtype(at::kFloat));
+      st["exp_avg"] = at::zeros_like(e.p, at::MemoryFormat::Preserve);
+      st["exp_avg_sq"] = at::zeros_like(e.p, at::MemoryFormat::Preserve);
+    }
+    const at::Tensor step = st["step"].cast<at::Tensor>();
+    const at::Tensor m = st["exp_avg"].cast<at::Tensor>(), v = st["exp_avg_sq"].cast<at::Tensor>();
+    moments.emplace_back(m.data_ptr(), v.data_ptr());
+    // as torch's _foreach_add_(steps, tensor(1.), alpha=1.): every step count of a param with a gradient advances
+    float* sp = step.data_ptr<float>() + (e.row < 0 ? 0 : e.row);
+    *sp = *sp + 1.0f;
+    if (e.numel == 0) continue;
+    const int64_t off = e.row < 0 ? 0 : e.row * e.numel;
+    B2RAdamSegment s{};
+    s.row_len = e.row_len;
+    s.row_stride = e.row_stride;
+    s.param = e.p.data_ptr<float>() + off;
+    s.grad = e.g.data_ptr<float>() + off;
+    s.exp_avg = m.data_ptr<float>() + off;
+    s.exp_avg_sq = v.data_ptr<float>() + off;
+    s.numel = e.numel;
+    s.first_chunk = n_chunks;
+    n_chunks += (e.numel + chunk - 1) / chunk;
+    adam_scalars(e.lr, e.beta1, e.beta2, e.eps, (double)*sp, s);
+    segs.push_back(s);
+  }
+  const py::bytes layout = layout_of(moments);
+  if (entries.empty()) return py::make_tuple(table, 0, 0, layout);
   const int64_t bytes = (int64_t)(segs.size() * sizeof(B2RAdamSegment));
-  // the caching host allocator records the copy on the stream and keeps `host` from reuse until the copy has run
-  at::Tensor host = at::empty({bytes}, at::TensorOptions().dtype(at::kByte).pinned_memory(true));
-  std::memcpy(host.data_ptr(), segs.data(), (size_t)bytes);
   c10::cuda::CUDAGuard guard(dev);
-  at::Tensor table = at::empty({bytes}, at::TensorOptions().dtype(at::kByte).device(dev));
-  table.copy_(host, /*non_blocking=*/true);
-  const cudaStream_t stream = c10::cuda::getCurrentCUDAStream(dev.index()).stream();
-  const int rc = b2r_adam_step((const B2RAdamSegment*)table.data_ptr(), (int32_t)segs.size(), n_chunks, stream);
+  if (!table.defined() || table.device() != dev || table.numel() < std::max<int64_t>(bytes, 1))
+    table = at::empty({std::max<int64_t>(bytes, 1)}, at::TensorOptions().dtype(at::kByte).device(dev));
+  if (bytes > 0) {
+    // the caching host allocator records the copy on the stream and keeps `host` from reuse until the copy has run
+    at::Tensor host = at::empty({bytes}, at::TensorOptions().dtype(at::kByte).pinned_memory(true));
+    std::memcpy(host.data_ptr(), segs.data(), (size_t)bytes);
+    table.narrow(0, 0, bytes).copy_(host, /*non_blocking=*/true);
+  }
+  return py::make_tuple(table, (int64_t)segs.size(), n_chunks, layout);
+}
+
+// The device half: one launch of csrc/adam.cu over a staged table on the current stream of `device` (capturable)
+void adam_launch(const at::Tensor& table, int64_t n_segments, int64_t n_chunks, int64_t device) {
+  if (n_chunks == 0) return;
+  c10::cuda::CUDAGuard guard((c10::DeviceIndex)device);
+  const cudaStream_t stream = c10::cuda::getCurrentCUDAStream((c10::DeviceIndex)device).stream();
+  const int rc = b2r_adam_step((const B2RAdamSegment*)table.data_ptr(), (int32_t)n_segments, n_chunks, stream);
   if (rc != B2R_OK)
     throw std::runtime_error(std::string("b200raster: b2r_adam_step failed: ") + b2r_strerror(rc) + " (cudaError " +
                              std::to_string(b2r_last_cuda_error()) + ")");
@@ -466,7 +553,8 @@ void adam_step(const py::list& groups, const py::object& state, int64_t device, 
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.def("adam_step", &adam_step, "optim.Adam.step: one launch over every param with a gradient (csrc/adam.cu)");
+  m.def("adam_stage", &adam_stage, "optim.Adam.stage: the host half of a step, staged into a resident device table");
+  m.def("adam_launch", &adam_launch, "optim.Adam.launch: one launch of csrc/adam.cu over a staged table");
   m.def("adam_scalars", [](double lr, double beta1, double beta2, double eps, double step) {
     B2RAdamSegment s{};
     adam_scalars(lr, beta1, beta2, eps, step, s);

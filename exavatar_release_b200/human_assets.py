@@ -24,6 +24,7 @@ device-agnostic torch (float64 or float32) for tests and measurements; the produ
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 
 import torch
 
@@ -92,6 +93,170 @@ def decode_smplx_pose(smplx_param) -> dict:
             out[k] = smplx_param[k]
     out["full_pose"] = full
     return out
+
+
+class _TableDecode(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, table, slot_t, host_slot, pose, expr, trans):
+        st = table._struct(slot_t, host_slot)
+        dev = table.device
+        full = torch.empty((table.n_joints, 3), dtype=torch.float32, device=dev)
+        e = torch.empty((table.n_expr,), dtype=torch.float32, device=dev)
+        t = torch.empty((3,), dtype=torch.float32, device=dev)
+        L.run("b2r_param_table_forward", dev, C.byref(st), L.ptr(full), L.ptr(e), L.ptr(t))
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(*(x for x in (slot_t,) if x is not None))
+        ctx.meta = (table, slot_t is not None, host_slot)
+        return full, e, t
+
+    @staticmethod
+    def backward(ctx, g_full, g_expr, g_trans):
+        table, on_device, host_slot = ctx.meta
+        slot_t = ctx.saved_tensors[0] if on_device else None
+        st = table._struct(slot_t, host_slot)
+        up = [None if g is None else g.to(torch.float32).contiguous() for g in (g_full, g_expr, g_trans)]
+        outs = [torch.empty_like(x) for x in (table.pose, table.expr, table.trans)]
+        gs = L.B2RSmplxParamTableGrads(*[L.ptr(x) for x in (*up, *outs)])
+        L.run("b2r_param_table_backward", table.device, C.byref(st), C.byref(gs))
+        return (None, None, None, *outs)
+
+
+class SmplxParamTable:
+    """Every frame's SMPL-X parameters of SMPLXParamDict (module.py:654-684) in three fp32 CUDA leaves, one frame read
+    by a slot on the device, so that one captured graph serves every frame:
+
+        pose  (F, 55, 6)  ExAvatar's stored 6D values as they are, in POSE_KEYS / POSE_ROWS (cat_full_pose) order
+        expr  (F, NE)
+        trans (F, 3)
+
+        table = SmplxParamTable.from_param_dict(smplx_params)   # SMPLXParamDict.smplx_params, frame key -> nine keys
+        smplx_param = table(table.slot_of(frame_idx))           # decode_smplx_pose's dict for that frame
+        table.write_to(smplx_params)                            # the rows back, e.g. before a checkpoint
+
+    `table(slot)` is one launch each way and bit-identical to `decode_smplx_pose` on that frame's ParameterDict,
+    forward and gradients.  The backward writes the whole (F, ...) gradients: the slot's rows, zeros elsewhere.  The
+    slot is a host int (checked on the host) or a one-element int32 CUDA tensor read on the device; a device slot
+    outside [0, F) reads and writes no frame's row: the outputs are NaN and the gradients zero."""
+
+    def __init__(self, pose, expr, trans, frames=None, pose_shapes=None):
+        """pose (F, 55, 6), expr (F, NE) and trans (F, 3) contiguous float32 tensors on one CUDA device, used as they
+        are (leaves with requires_grad); `frames` the frame keys of the F slots in order (default "0" ... "F-1");
+        `pose_shapes` the stored shape of each pose key, (6,) or (n,6) (default (6,) for the one-row keys, as
+        SMPLXParamDict.init stores them)."""
+        fn = "SmplxParamTable"
+        for name, t in (("pose", pose), ("expr", expr), ("trans", trans)):
+            L.cuda(fn, name, t, pose.device if isinstance(pose, torch.Tensor) else None)
+            L.float32(fn, name, t)
+            if not t.is_contiguous():
+                raise ValueError(f"{fn}: `{name}` must be contiguous")
+        J = sum(POSE_ROWS)
+        F = pose.shape[0] if pose.dim() == 3 else -1
+        if F < 1 or tuple(pose.shape[1:]) != (J, 6):
+            raise ValueError(f"{fn}: `pose` must be (F, {J}, 6) with F >= 1, got {tuple(pose.shape)}")
+        if expr.dim() != 2 or expr.shape[0] != F:
+            raise ValueError(f"{fn}: `expr` must be ({F}, NE), got {tuple(expr.shape)}")
+        if tuple(trans.shape) != (F, 3):
+            raise ValueError(f"{fn}: `trans` must be ({F}, 3), got {tuple(trans.shape)}")
+        if F >= 2 ** 31:
+            raise ValueError(f"{fn}: at most 2^31 - 1 frames")
+        frames = [str(f) for f in (range(F) if frames is None else frames)]
+        if len(frames) != F or len(set(frames)) != F:
+            raise ValueError(f"{fn}: `frames` must name the {F} slots once each")
+        self.pose, self.expr, self.trans = pose, expr, trans
+        self.device = pose.device
+        self.n_frames, self.n_joints, self.n_expr = F, int(pose.shape[1]), int(expr.shape[1])
+        self.frames = frames
+        self._slot = {f: i for i, f in enumerate(frames)}
+        self.pose_shapes = tuple((6,) if n == 1 else (n, 6) for n in POSE_ROWS) if pose_shapes is None else \
+            tuple(tuple(s) for s in pose_shapes)
+        for n, shp in zip(POSE_ROWS, self.pose_shapes):
+            if not (shp == (n, 6) or (n == 1 and shp == (6,))):
+                raise ValueError(f"{fn}: `pose_shapes` must be (n,6) or, for one row, (6,), got {shp}")
+
+    @classmethod
+    def from_param_dict(cls, smplx_params, device=None) -> "SmplxParamTable":
+        """The table of `SMPLXParamDict.smplx_params` (frame key -> the seven 6D pose keys, (6,) or (n,6), plus expr
+        and trans), slots in the dict's order, values copied bit for bit into new leaves (requires_grad=True)."""
+        fn = "SmplxParamTable.from_param_dict"
+        frames = list(smplx_params.keys())
+        if not frames:
+            raise ValueError(f"{fn}: no frames")
+        poses, exprs, transs = [], [], []
+        for f in frames:
+            d = smplx_params[f]
+            missing = [k for k in (*POSE_KEYS, "expr", "trans") if k not in d]
+            if missing:
+                raise ValueError(f"{fn}: frame {f!r} lacks {missing}")
+            for k, n in zip(POSE_KEYS, POSE_ROWS):
+                v, v0 = d[k], smplx_params[frames[0]][k]
+                if not (tuple(v.shape) == (n, 6) or (n == 1 and tuple(v.shape) == (6,))):
+                    want = f"({n},6)" + (" or (6,)" if n == 1 else "")
+                    raise ValueError(f"{fn}: frame {f!r} `{k}` must be {want}, got {tuple(v.shape)}")
+                if v.shape != v0.shape:
+                    raise ValueError(f"{fn}: frame {f!r} stores `{k}` as {tuple(v.shape)}, the first frame as "
+                                     f"{tuple(v0.shape)}")
+            if d["expr"].dim() != 1 or tuple(d["trans"].shape) != (3,):
+                raise ValueError(f"{fn}: frame {f!r} needs expr (NE,) and trans (3,), got "
+                                 f"{tuple(d['expr'].shape)} and {tuple(d['trans'].shape)}")
+            poses.append(torch.cat([d[k].detach().reshape(-1, 6) for k in POSE_KEYS]))
+            exprs.append(d["expr"].detach())
+            transs.append(d["trans"].detach())
+        if len({e.shape[0] for e in exprs}) != 1:
+            raise ValueError(f"{fn}: the frames' expr lengths differ")
+        dev = torch.device(device) if device is not None else poses[0].device
+        leaf = lambda xs: torch.stack(xs).to(device=dev, dtype=torch.float32).contiguous().requires_grad_()  # noqa: E731
+        first = smplx_params[frames[0]]
+        return cls(leaf(poses), leaf(exprs), leaf(transs), frames, [tuple(first[k].shape) for k in POSE_KEYS])
+
+    @torch.no_grad()
+    def write_to(self, smplx_params) -> None:
+        """Copies every slot's rows back into `smplx_params` (the dict from_param_dict read), in place and bit for
+        bit, each key keeping its stored shape."""
+        for f, i in self._slot.items():
+            d, r0 = smplx_params[f], 0
+            for k, n in zip(POSE_KEYS, POSE_ROWS):
+                d[k].copy_(self.pose[i, r0:r0 + n].reshape(d[k].shape))
+                r0 += n
+            d["expr"].copy_(self.expr[i])
+            d["trans"].copy_(self.trans[i])
+
+    def slot_of(self, frame_idx) -> int:
+        """The slot of a frame: its key, or ExAvatar's int frame index (looked up as str(int(frame_idx)))."""
+        key = frame_idx if isinstance(frame_idx, str) else str(int(frame_idx))
+        if key not in self._slot:
+            raise KeyError(f"SmplxParamTable: no frame {key!r}")
+        return self._slot[key]
+
+    def parameters(self):
+        return [self.pose, self.expr, self.trans]
+
+    def _struct(self, slot_t, host_slot: int = 0):
+        return L.B2RSmplxParamTable(n_frames=self.n_frames, n_joints=self.n_joints, n_expr=self.n_expr,
+                                    host_slot=host_slot, pose=L.ptr(self.pose), expr=L.ptr(self.expr),
+                                    trans=L.ptr(self.trans), slot=L.ptr(slot_t))
+
+    def __call__(self, slot) -> dict:
+        """decode_smplx_pose's dict for the frame in `slot`: the seven pose keys in axis-angle as views of
+        `full_pose` (J,3), plus `full_pose`, `expr` (NE) and `trans` (3), all fresh tensors."""
+        fn = "SmplxParamTable"
+        if isinstance(slot, torch.Tensor):
+            L.cuda(fn, "slot", slot, self.device)
+            if slot.dtype != torch.int32 or slot.numel() != 1 or not slot.is_contiguous():
+                raise ValueError(f"{fn}: a tensor `slot` must be one contiguous int32 value, got {slot.dtype} "
+                                 f"{tuple(slot.shape)}")
+            full, expr, trans = _TableDecode.apply(self, slot, 0, self.pose, self.expr, self.trans)
+        elif isinstance(slot, numbers.Integral) and not isinstance(slot, bool):
+            if not 0 <= int(slot) < self.n_frames:
+                raise IndexError(f"{fn}: slot {int(slot)} outside [0, {self.n_frames})")
+            full, expr, trans = _TableDecode.apply(self, None, int(slot), self.pose, self.expr, self.trans)
+        else:
+            raise ValueError(f"{fn}: `slot` must be an int or a (1,) int32 CUDA tensor, got {type(slot).__name__}")
+        out, r0 = {}, 0
+        for k, n, shp in zip(POSE_KEYS, POSE_ROWS, self.pose_shapes):
+            out[k] = full[r0:r0 + n] if len(shp) == 2 else full[r0]
+            r0 += n
+        out.update(expr=expr, trans=trans, full_pose=full)
+        return out
 
 
 def decode_smplx_pose_reference(smplx_param) -> dict:

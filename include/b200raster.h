@@ -212,7 +212,8 @@ int b2r_last_cuda_error(void);
  * 12 B2RRegsGrads, 13 B2RRig, 14 B2RRigGrads, 15 B2RAdamSegment, 16 B2RLpips, 17 B2RSceneAssets,
  * 18 B2RSceneAssetsGrads, 19 B2RSmplxPose, 20 B2RSmplxPoseGrads, 21 B2RHumanAssets, 22 B2RHumanAssetsGrads,
  * 23 B2RSmplxBody, 24 B2RSmplxBodyGrads, 25 B2RNeumanScores, 26 B2RFaceComposite, 27 B2RTestOutputs,
- * 28 B2ROrbitCamera, 29 B2RAnimationPanel; 0 for anything else
+ * 28 B2ROrbitCamera, 29 B2RAnimationPanel, 31 B2RSmplxParamTable, 32 B2RSmplxParamTableGrads (30 unused); 0 for
+ * anything else
  * (7 and 9 are unused and report 0). */
 size_t b2r_sizeof(int which);
 
@@ -877,6 +878,37 @@ int b2r_decode_pose_forward(const B2RSmplxPose* p, float* full_pose, void* strea
 int b2r_decode_pose_backward(const B2RSmplxPose* p, const float* dL_dfull_pose, const B2RSmplxPoseGrads* grads,
                              void* stream);
 
+/* Every frame's SMPL-X parameters in one table, the frame chosen on the device (exavatar_release_b200/human_assets.py
+ * SmplxParamTable): pose (n_frames, n_joints, 6) holds each frame's 6D pose rows in cat_full_pose order, expr
+ * (n_frames, n_expr) and trans (n_frames, 3); fp32, device, contiguous.  The frame is *slot (int32, device: one captured
+ * graph serves every frame) or, with slot NULL, host_slot.  Forward: full_pose (n_joints,3) is b2r_decode_pose_forward
+ * of the frame's pose rows, the same per-joint arithmetic bit for bit; expr (n_expr) and trans (3) are copies of its
+ * rows.  Backward: from dL_dfull_pose (n_joints,3), dL_dexpr (n_expr) and dL_dtrans (3), each of them NULL for zero, it
+ * writes every element of the table-shaped gradients pose, expr and trans: b2r_decode_pose_backward's rows and the two
+ * upstream gradients in the frame's rows, zeros in every other row.  A slot outside [0, n_frames) reads and writes no
+ * frame's row: the forward writes NaN and the backward zeros.  n_frames >= 1, 1 <= n_joints <= B2R_POSE_MAX_JOINTS,
+ * n_expr >= 0 (expr may be NULL when 0).  Forward one CTA, backward one CTA per frame; no atomics, no allocation, no
+ * sync. */
+typedef struct B2RSmplxParamTable {
+  int32_t n_frames, n_joints, n_expr, host_slot;
+  const float* pose;
+  const float* expr;
+  const float* trans;
+  const int32_t* slot;
+} B2RSmplxParamTable;
+
+typedef struct B2RSmplxParamTableGrads {
+  const float* dL_dfull_pose;
+  const float* dL_dexpr;
+  const float* dL_dtrans;
+  float* pose;
+  float* expr;
+  float* trans;
+} B2RSmplxParamTableGrads;
+
+int b2r_param_table_forward(const B2RSmplxParamTable* t, float* full_pose, float* expr, float* trans, void* stream);
+int b2r_param_table_backward(const B2RSmplxParamTable* t, const B2RSmplxParamTableGrads* g, void* stream);
+
 /* HumanGaussian's geometry around its networks (avatar/common/nets/module.py:524-539 with get_mean_offset_offset's
  * mask, :489-493, and model.py:92-96's warm-up clamp), per Gaussian p of P, in ExAvatar's fp32 operations and order:
  *   m = mesh + geo[0:3];  mmo = geo_offset[0:3] * (1 - mask);  mean_3d = m + expr_offset;
@@ -946,7 +978,7 @@ int b2r_camera_setup(const float* R, const float* t, const float* focal, int32_t
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_neuman_scores, b2r_face_composite_*, b2r_test_outputs, b2r_orbit_*, b2r_animation_panel, b2r_scene_assets_*, b2r_decode_pose_* and b2r_human_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_neuman_scores, b2r_face_composite_*, b2r_test_outputs, b2r_orbit_*, b2r_animation_panel, b2r_scene_assets_*, b2r_decode_pose_*, b2r_param_table_* and b2r_human_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
