@@ -19,6 +19,7 @@ three-panel video frame of the animation scripts, animate.py and animate_view_ro
 Gaussians' asset dict of SceneGaussian.forward, module.py:253-272), `decode_smplx_pose` (SMPLXParamDict.forward,
 module.py:673-684), `SmplxParamTable` (every frame's SMPL-X parameters in one table, the frame picked on the device),
 `IterationGraph` (a whole training iteration, forward, backward and Adam, as one CUDA graph per key for every frame),
+`FrameTable` (every training frame's image, mask, box and camera on the device, the frame picked by the same slot),
 `HumanAssets` (HumanGaussian's geometry and colour code around its networks, module.py:524-539,561-565
 and model.py:92-96), synthetic workloads and the frame-sharding helper used by bench.py.
 """
@@ -38,6 +39,7 @@ from .compose import face_composite, test_outputs  # noqa: F401
 from .animation import OrbitCamera, animation_panel, orbit_points  # noqa: F401
 from .human_assets import HumanAssets, SmplxParamTable, decode_smplx_pose  # noqa: F401
 from .iteration import IterationGraph  # noqa: F401
+from .frames import FrameTable  # noqa: F401
 
 
 def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loaded on first use
@@ -51,4 +53,4 @@ __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gau
            "render_settings", "device_render_settings", "TrainingFrameRenderer", "skin_gaussians", "l1_ssim", "nearest_rows", "VertexNormals",
            "FaceMeshRenderer", "ShadedMeshRenderer", "HumanRegularizers", "SmplxRig", "cat_full_pose", "Adam",
            "scene_assets", "LPIPS", "NeumanScores", "face_composite", "test_outputs", "OrbitCamera", "orbit_points", "animation_panel",
-           "decode_smplx_pose", "SmplxParamTable", "HumanAssets", "IterationGraph"]
+           "decode_smplx_pose", "SmplxParamTable", "HumanAssets", "IterationGraph", "FrameTable"]

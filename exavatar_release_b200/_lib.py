@@ -231,6 +231,13 @@ class B2RSmplxParamTableGrads(C.Structure):
     _fields_ = [(n, _fp) for n in ("dL_dfull_pose", "dL_dexpr", "dL_dtrans", "pose", "expr", "trans")]
 
 
+class B2RFrameTable(C.Structure):
+    """Every frame of a split and the frame's slot (b2r_frame_unpack)."""
+    _fields_ = [("n_rows", C.c_int32), ("n_slots", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
+                ("host_slot", C.c_int32), ("reserved", C.c_int32),
+                *[(n, _fp) for n in ("pixels", "bbox", "R", "t", "focal", "princpt", "frame_idx", "slot_row", "slot")]]
+
+
 class B2RHumanAssets(C.Structure):
     """HumanGaussian's geometry around its networks (b2r_human_geometry_forward / b2r_human_geometry_backward)."""
     _fields_ = [
@@ -359,6 +366,7 @@ SYMBOLS = [
     ("b2r_decode_pose_backward", C.c_int, [C.POINTER(B2RSmplxPose), _fp, C.POINTER(B2RSmplxPoseGrads), _fp]),
     ("b2r_param_table_forward", C.c_int, [C.POINTER(B2RSmplxParamTable), _fp, _fp, _fp, _fp]),
     ("b2r_param_table_backward", C.c_int, [C.POINTER(B2RSmplxParamTable), C.POINTER(B2RSmplxParamTableGrads), _fp]),
+    ("b2r_frame_unpack", C.c_int, [C.POINTER(B2RFrameTable), _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     ("b2r_human_geometry_forward", C.c_int, [C.POINTER(B2RHumanAssets), _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     ("b2r_human_geometry_backward", C.c_int, [C.POINTER(B2RHumanAssets), C.POINTER(B2RHumanAssetsGrads), _fp]),
     ("b2r_human_colors_forward", C.c_int, [C.c_int32, _fp, _fp, _fp, _fp, _fp]),
@@ -397,7 +405,8 @@ def load():
     # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14, B2RAdamSegment 15, B2RLpips 16, B2RSceneAssets 17,
     # B2RSceneAssetsGrads 18, B2RSmplxPose 19, B2RSmplxPoseGrads 20, B2RHumanAssets 21, B2RHumanAssetsGrads 22,
     # B2RSmplxBody 23, B2RSmplxBodyGrads 24, B2RNeumanScores 25, B2RFaceComposite 26, B2RTestOutputs 27,
-    # B2ROrbitCamera 28, B2RAnimationPanel 29, B2RSmplxParamTable 31, B2RSmplxParamTableGrads 32 (30 unused)
+    # B2ROrbitCamera 28, B2RAnimationPanel 29, B2RSmplxParamTable 31, B2RSmplxParamTableGrads 32, B2RFrameTable 33
+    # (30 unused)
     for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
                      (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp), (11, B2RRegs),
                      (12, B2RRegsGrads), (13, B2RRig), (14, B2RRigGrads), (15, B2RAdamSegment),
@@ -405,7 +414,7 @@ def load():
                      (20, B2RSmplxPoseGrads), (21, B2RHumanAssets), (22, B2RHumanAssetsGrads), (23, B2RSmplxBody),
                      (24, B2RSmplxBodyGrads), (25, B2RNeumanScores), (26, B2RFaceComposite),
                      (27, B2RTestOutputs), (28, B2ROrbitCamera), (29, B2RAnimationPanel),
-                     (31, B2RSmplxParamTable), (32, B2RSmplxParamTableGrads)):
+                     (31, B2RSmplxParamTable), (32, B2RSmplxParamTableGrads), (33, B2RFrameTable)):
         if lib.b2r_sizeof(idx) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
                                f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")

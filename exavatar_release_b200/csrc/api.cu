@@ -107,6 +107,15 @@ int validate_param_table(const B2RSmplxParamTable* t) {
   return B2R_OK;
 }
 
+// a frame table's sizes and arrays, and the host slot when no device slot is given
+int validate_frame_table(const B2RFrameTable* t) {
+  if (!t || !t->pixels || !t->bbox || !t->R || !t->t || !t->focal || !t->princpt || !t->frame_idx || !t->slot_row)
+    return B2R_E_INVALID;
+  if (t->n_rows < 1 || t->n_slots < 1 || t->height < 1 || t->width < 1) return B2R_E_INVALID;
+  if (!t->slot && (t->host_slot < 0 || t->host_slot >= t->n_slots)) return B2R_E_INVALID;
+  return B2R_OK;
+}
+
 // sizes, row strides and every input pointer (an empty set reads nothing)
 int validate_human_assets(const B2RHumanAssets* h) {
   if (!h || h->P < 0 || (h->warmup != 0 && h->warmup != 1)) return B2R_E_INVALID;
@@ -290,6 +299,7 @@ size_t b2r_sizeof(int which) {
     case 29: return sizeof(B2RAnimationPanel);
     case 31: return sizeof(B2RSmplxParamTable);  // 30 stays unused
     case 32: return sizeof(B2RSmplxParamTableGrads);
+    case 33: return sizeof(B2RFrameTable);
     default: return 0;
   }
 }
@@ -822,6 +832,14 @@ int b2r_param_table_backward(const B2RSmplxParamTable* t, const B2RSmplxParamTab
   if (rc) return rc;
   if (!g || !g->pose || !g->trans || (t->n_expr > 0 && !g->expr)) return B2R_E_INVALID;
   return launch_param_table_backward(*t, *g, (cudaStream_t)stream);
+}
+
+int b2r_frame_unpack(const B2RFrameTable* table, float* img, float* mask, float* bbox, float* R, float* t,
+                     float* focal, float* princpt, int64_t* frame_idx, void* stream) {
+  const int rc = validate_frame_table(table);
+  if (rc) return rc;
+  if (!img || !mask || !bbox || !R || !t || !focal || !princpt || !frame_idx) return B2R_E_INVALID;
+  return launch_frame_unpack(*table, img, mask, bbox, R, t, focal, princpt, frame_idx, (cudaStream_t)stream);
 }
 
 int b2r_human_geometry_forward(const B2RHumanAssets* h, float* mean_3d, float* mean_3d_refined, float* scale,

@@ -679,6 +679,8 @@ int launch_decode_pose_backward(const B2RSmplxPose& p, const float* dfull, const
 int launch_param_table_forward(const B2RSmplxParamTable& t, float* full_pose, float* expr, float* trans,
                                cudaStream_t st);
 int launch_param_table_backward(const B2RSmplxParamTable& t, const B2RSmplxParamTableGrads& g, cudaStream_t st);
+int launch_frame_unpack(const B2RFrameTable& t, float* img, float* mask, float* bbox, float* R, float* tr, float* focal,
+                        float* princpt, int64_t* frame_idx, cudaStream_t st);
 int launch_human_geometry_forward(const B2RHumanAssets& h, float* mean, float* mean_r, float* scale, float* scale_r,
                                   float* mmo, float* scale_wo, float* scale_r_wo, cudaStream_t st);
 int launch_human_geometry_backward(const B2RHumanAssets& h, const B2RHumanAssetsGrads& g, cudaStream_t st);

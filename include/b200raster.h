@@ -212,8 +212,8 @@ int b2r_last_cuda_error(void);
  * 12 B2RRegsGrads, 13 B2RRig, 14 B2RRigGrads, 15 B2RAdamSegment, 16 B2RLpips, 17 B2RSceneAssets,
  * 18 B2RSceneAssetsGrads, 19 B2RSmplxPose, 20 B2RSmplxPoseGrads, 21 B2RHumanAssets, 22 B2RHumanAssetsGrads,
  * 23 B2RSmplxBody, 24 B2RSmplxBodyGrads, 25 B2RNeumanScores, 26 B2RFaceComposite, 27 B2RTestOutputs,
- * 28 B2ROrbitCamera, 29 B2RAnimationPanel, 31 B2RSmplxParamTable, 32 B2RSmplxParamTableGrads (30 unused); 0 for
- * anything else
+ * 28 B2ROrbitCamera, 29 B2RAnimationPanel, 31 B2RSmplxParamTable, 32 B2RSmplxParamTableGrads, 33 B2RFrameTable
+ * (30 unused); 0 for anything else
  * (7 and 9 are unused and report 0). */
 size_t b2r_sizeof(int which);
 
@@ -909,6 +909,33 @@ typedef struct B2RSmplxParamTableGrads {
 int b2r_param_table_forward(const B2RSmplxParamTable* t, float* full_pose, float* expr, float* trans, void* stream);
 int b2r_param_table_backward(const B2RSmplxParamTable* t, const B2RSmplxParamTableGrads* g, void* stream);
 
+/* Every training frame of a split in one table, the frame chosen on the device (exavatar_release_b200/frames.py
+ * FrameTable): row r holds pixels (height, width, 4) uint8 -- R, G, B and the training mask as 0 / 1 -- and bbox (4),
+ * R (3,3), t (3), focal (2), princpt (2) fp32 and frame_idx int64; the arrays are (n_rows, ...), device, contiguous.
+ * slot_row (n_slots) int32 maps a slot to its row, -1 for a slot without a frame.  The slot is *slot (int32, device:
+ * one captured graph serves every frame) or, with slot NULL, host_slot, which must lie in [0, n_slots).
+ * b2r_frame_unpack writes the row's image planar, img (3, height, width) = fl(k / 255) per byte k (IEEE-rounded
+ * division, the fp32 value of ExAvatar's ToTensor(img) / 255.), mask (height, width) = the mask byte as 0.f / 1.f, and
+ * copies bbox, R, t, focal, princpt and frame_idx.  A slot outside [0, n_slots) or without a row reads no row: every
+ * float output is NaN and frame_idx -1.  One launch; a thread owns 4 pixels, and with height * width a multiple of 4
+ * and 16-byte aligned pixels, img and mask it loads 16 bytes and stores one float4 per plane.  No allocation, no
+ * sync. */
+typedef struct B2RFrameTable {
+  int32_t n_rows, n_slots, height, width, host_slot, reserved;
+  const uint8_t* pixels;
+  const float* bbox;
+  const float* R;
+  const float* t;
+  const float* focal;
+  const float* princpt;
+  const int64_t* frame_idx;
+  const int32_t* slot_row;
+  const int32_t* slot;
+} B2RFrameTable;
+
+int b2r_frame_unpack(const B2RFrameTable* table, float* img, float* mask, float* bbox, float* R, float* t,
+                     float* focal, float* princpt, int64_t* frame_idx, void* stream);
+
 /* HumanGaussian's geometry around its networks (avatar/common/nets/module.py:524-539 with get_mean_offset_offset's
  * mask, :489-493, and model.py:92-96's warm-up clamp), per Gaussian p of P, in ExAvatar's fp32 operations and order:
  *   m = mesh + geo[0:3];  mmo = geo_offset[0:3] * (1 - mask);  mean_3d = m + expr_offset;
@@ -978,7 +1005,7 @@ int b2r_camera_setup(const float* R, const float* t, const float* focal, int32_t
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_neuman_scores, b2r_face_composite_*, b2r_test_outputs, b2r_orbit_*, b2r_animation_panel, b2r_scene_assets_*, b2r_decode_pose_*, b2r_param_table_* and b2r_human_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_neuman_scores, b2r_face_composite_*, b2r_test_outputs, b2r_orbit_*, b2r_animation_panel, b2r_scene_assets_*, b2r_decode_pose_*, b2r_param_table_*, b2r_frame_unpack and b2r_human_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */
