@@ -28,6 +28,7 @@ _fp = C.c_void_p  # device pointers travel as plain addresses
 
 
 class B2RScene(C.Structure):
+    ID = 0
     _fields_ = [
         ("P", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("sh_degree", C.c_int32),
         ("sh_coeffs", C.c_int32), ("flags", C.c_uint32),
@@ -43,6 +44,7 @@ class B2RScene(C.Structure):
 
 
 class B2RStatus(C.Structure):
+    ID = 1
     _fields_ = [
         ("num_dups", C.c_uint64), ("dup_capacity", C.c_uint64), ("overflow", C.c_uint32), ("num_visible", C.c_uint32),
         ("consumed_fwd", C.c_uint64), ("consumed_bwd", C.c_uint64), ("token", C.c_uint64), ("reserved", C.c_uint64 * 2),
@@ -50,6 +52,7 @@ class B2RStatus(C.Structure):
 
 
 class B2RWorkspace(C.Structure):
+    ID = 2
     _fields_ = [
         ("ctx", _fp), ("ctx_bytes", C.c_size_t), ("dup_ids", _fp), ("dup_capacity", C.c_uint64),
         ("scratch", _fp), ("scratch_bytes", C.c_size_t), ("status_mirror", _fp), ("status_token", C.c_uint64),
@@ -58,6 +61,7 @@ class B2RWorkspace(C.Structure):
 
 
 class B2RView(C.Structure):
+    ID = 5
     _fields_ = [
         ("id_begin", C.c_uint32), ("id_end", C.c_uint32), ("bg", _fp), ("final_T", _fp), ("n_contrib", _fp),
         ("checkpoints", _fp), ("checkpoint_bytes", C.c_size_t), ("skip_below", C.c_uint32), ("reserved", C.c_uint32),
@@ -66,6 +70,7 @@ class B2RView(C.Structure):
 
 class B2RSkin(C.Structure):
     """Standalone skinning of one or two Gaussian sets sharing a rig (b2r_skin_forward / b2r_skin_backward)."""
+    ID = 6
     _fields_ = [
         ("P", C.c_int32), ("J", C.c_int32), ("V", C.c_int32), ("reserved", C.c_int32),
         ("weights", _fp), ("rows", _fp), ("joint_mats", _fp), ("trans", _fp), ("cam_Rinv", _fp), ("cam_t", _fp),
@@ -75,6 +80,7 @@ class B2RSkin(C.Structure):
 
 class B2RMeshRender(C.Structure):
     """Textured mesh render (b2r_mesh_render_forward / b2r_mesh_render_backward): ExAvatar's face render."""
+    ID = 8
     _fields_ = [
         ("V", C.c_int32), ("F", C.c_int32), ("Vt", C.c_int32), ("C", C.c_int32),
         ("tex_height", C.c_int32), ("tex_width", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
@@ -86,6 +92,7 @@ class B2RMeshRender(C.Structure):
 
 class B2RGnMlp(C.Structure):
     """One GroupNorm MLP stack (b2r_gn_mlp_forward / b2r_gn_mlp_backward): HumanGaussian's networks."""
+    ID = 10
     _fields_ = [
         ("P", C.c_int32), ("K", C.c_int32), ("H", C.c_int32), ("reserved", C.c_int32),
         ("x", _fp), ("w", _fp * 3), ("b", _fp * 3), ("gamma", _fp * 3), ("beta", _fp * 3),
@@ -95,6 +102,7 @@ class B2RGnMlp(C.Structure):
 
 class B2RRegs(C.Structure):
     """ExAvatar's human regularisers (b2r_regs_forward / b2r_regs_backward): the inputs and the model's tables."""
+    ID = 11
     _fields_ = [
         ("P", C.c_int32), ("J", C.c_int32), ("n_arm", C.c_int32), ("n_pairs", C.c_int32), ("n_hand", C.c_int32),
         ("n_rhand", C.c_int32), ("reserved", C.c_int32 * 2),
@@ -107,12 +115,14 @@ class B2RRegs(C.Structure):
 
 
 class B2RRegsGrads(C.Structure):
+    ID = 12
     _fields_ = [(n, _fp) for n in ("mean_offset", "mean_offset_offset", "scale_offset", "scale", "scale_refined", "rgb",
                                    "rgb_refined", "scale_reg", "joint_offset")]
 
 
 class B2RRig(C.Structure):
     """ExAvatar's SMPL-X rig (b2r_rig_forward / b2r_rig_backward): the per-call inputs and the model's tables."""
+    ID = 13
     _fields_ = [
         ("V", C.c_int32), ("V1", C.c_int32), ("P", C.c_int32), ("J", C.c_int32), ("NB", C.c_int32), ("NE", C.c_int32),
         ("n_body", C.c_int32), ("reserved", C.c_int32),
@@ -124,23 +134,27 @@ class B2RRig(C.Structure):
 
 
 class B2RRigGrads(C.Structure):
+    ID = 14
     _fields_ = [(n, _fp) for n in ("shape_param", "joint_offset", "full_pose", "expr")]
 
 
 class B2RSmplxBody(C.Structure):
     """The frame's SMPL-X body mesh (b2r_smplx_body_forward / b2r_smplx_body_backward): the rig's tables, pose_mean,
     the five per-call inputs and the optional camera."""
+    ID = 23
     _fields_ = [("rig", B2RRig), *[(n, _fp) for n in ("pose_mean", "shape_param", "joint_offset", "full_pose", "expr",
                                                       "trans", "cam_R", "cam_t")]]
 
 
 class B2RSmplxBodyGrads(C.Structure):
+    ID = 24
     _fields_ = [(n, _fp) for n in ("shape_param", "joint_offset", "full_pose", "expr", "trans")]
 
 
 class B2RAdamSegment(C.Structure):
     """One tensor of an Adam step (b2r_adam_step): its four device pointers, numel, first chunk, the param's row layout
     and the fp32 scalars."""
+    ID = 15
     _fields_ = [
         ("param", _fp), ("grad", _fp), ("exp_avg", _fp), ("exp_avg_sq", _fp), ("numel", C.c_int64),
         ("first_chunk", C.c_int64), ("row_len", C.c_int64), ("row_stride", C.c_int64), ("lerp_weight", C.c_float), ("beta2", C.c_float), ("one_minus_beta2", C.c_float),
@@ -151,6 +165,7 @@ class B2RAdamSegment(C.Structure):
 class B2RLpips(C.Structure):
     """ExAvatar's LPIPS-VGG terms (b2r_lpips_forward / b2r_lpips_backward): the images, the box and the weights in the
     kernels' layouts."""
+    ID = 16
     _fields_ = [
         ("width", C.c_int32), ("height", C.c_int32), ("n_images", C.c_int32), ("reserved", C.c_int32),
         ("img", _fp), ("target", _fp), ("bbox", _fp), ("w_fwd", _fp * 13), ("w_bwd", _fp * 13), ("bias", _fp * 13),
@@ -161,6 +176,7 @@ class B2RLpips(C.Structure):
 class B2RNeumanScores(C.Structure):
     """The NeuMan test-set scores (b2r_neuman_scores): the frames, the optional mask and the AlexNet weights in the
     kernels' layouts."""
+    ID = 25
     _fields_ = [
         ("width", C.c_int32), ("height", C.c_int32), ("n_images", C.c_int32), ("mask_channels", C.c_int32),
         ("render", _fp), ("target", _fp), ("mask", _fp), ("w", _fp * 5), ("bias", _fp * 5), ("lin", _fp * 5),
@@ -169,6 +185,7 @@ class B2RNeumanScores(C.Structure):
 
 class B2RFaceComposite(C.Structure):
     """ExAvatar's training face composite (b2r_face_composite_forward / b2r_face_composite_backward)."""
+    ID = 26
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("n_images", C.c_int32), ("reserved", C.c_int32),
                 ("img", _fp), ("face", _fp)]
 
@@ -176,6 +193,7 @@ class B2RFaceComposite(C.Structure):
 class B2RTestOutputs(C.Structure):
     """ExAvatar's test-time composites and test.py's image bytes (b2r_test_outputs): the renders in plan.RENDERS
     order, the two human masks, the two face renders and the optional ground truth."""
+    ID = 27
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("n_images", C.c_int32), ("reserved", C.c_int32),
                 ("render", _fp * 5), ("mask", _fp * 2), ("face", _fp * 2), ("gt", _fp)]
 
@@ -186,12 +204,14 @@ ORBIT_STATE = 20  # B2R_ORBIT_STATE
 class B2ROrbitCamera(C.Structure):
     """The animation scripts' orbit camera (b2r_orbit_camera): k, the frame count, the anchor mode, the frame's camera
     and root joint, the device frame index and the state block."""
+    ID = 28
     _fields_ = [("k", C.c_int32), ("n_frames", C.c_int32), ("anchor", C.c_int32), ("reserved", C.c_int32),
                 ("cam_R", _fp), ("cam_t", _fp), ("root_cam", _fp), ("index", _fp), ("state", _fp)]
 
 
 class B2RAnimationPanel(C.Structure):
     """The animation scripts' three-panel video frame (b2r_animation_panel)."""
+    ID = 29
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("reserved", C.c_int32 * 2),
                 ("frame", _fp), ("mesh_panel", _fp), ("render", _fp)]
 
@@ -199,6 +219,7 @@ class B2RAnimationPanel(C.Structure):
 class B2RSceneAssets(C.Structure):
     """ExAvatar's scene Gaussian assets (b2r_scene_assets_forward / b2r_scene_assets_backward): the parameters, their
     row strides, the device degree buffer and the camera (NULL: shs mode)."""
+    ID = 17
     _fields_ = [
         ("P", C.c_int32), ("M", C.c_int32), ("dc_stride", C.c_int64), ("rest_stride", C.c_int64),
         *[(n, _fp) for n in ("mean", "opacity_logit", "log_scale", "rotation6d", "feature_dc", "feature_rest",
@@ -207,6 +228,7 @@ class B2RSceneAssets(C.Structure):
 
 
 class B2RSceneAssetsGrads(C.Structure):
+    ID = 18
     _fields_ = [(n, _fp) for n in ("opacity", "scale", "dL_dopacity", "dL_dscale", "dL_drotation", "dL_dcolor",
                                    "dL_dlogit", "dL_dlog_scale", "dL_drotation6d", "dL_dfeature_dc",
                                    "dL_dfeature_rest", "dL_dmean")]
@@ -214,25 +236,30 @@ class B2RSceneAssetsGrads(C.Structure):
 
 class B2RSmplxPose(C.Structure):
     """One frame's seven 6D pose parameters (b2r_decode_pose_forward / b2r_decode_pose_backward): pointers and rows."""
+    ID = 19
     _fields_ = [("param", _fp * 7), ("rows", C.c_int32 * 7), ("reserved", C.c_int32)]
 
 
 class B2RSmplxPoseGrads(C.Structure):
+    ID = 20
     _fields_ = [("param", _fp * 7)]
 
 
 class B2RSmplxParamTable(C.Structure):
     """Every frame's SMPL-X parameters in one table and the frame's slot (b2r_param_table_forward / _backward)."""
+    ID = 31
     _fields_ = [("n_frames", C.c_int32), ("n_joints", C.c_int32), ("n_expr", C.c_int32), ("host_slot", C.c_int32),
                 ("pose", _fp), ("expr", _fp), ("trans", _fp), ("slot", _fp)]
 
 
 class B2RSmplxParamTableGrads(C.Structure):
+    ID = 32
     _fields_ = [(n, _fp) for n in ("dL_dfull_pose", "dL_dexpr", "dL_dtrans", "pose", "expr", "trans")]
 
 
 class B2RFrameTable(C.Structure):
     """Every frame of a split and the frame's slot (b2r_frame_unpack)."""
+    ID = 33
     _fields_ = [("n_rows", C.c_int32), ("n_slots", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
                 ("host_slot", C.c_int32), ("reserved", C.c_int32),
                 *[(n, _fp) for n in ("pixels", "bbox", "R", "t", "focal", "princpt", "frame_idx", "slot_row", "slot")]]
@@ -240,6 +267,7 @@ class B2RFrameTable(C.Structure):
 
 class B2RHumanAssets(C.Structure):
     """HumanGaussian's geometry around its networks (b2r_human_geometry_forward / b2r_human_geometry_backward)."""
+    ID = 21
     _fields_ = [
         ("P", C.c_int32), ("warmup", C.c_int32), ("geo_stride", C.c_int64), ("geo_offset_stride", C.c_int64),
         *[(n, _fp) for n in ("mesh", "pose_offset", "expr_offset", "geo", "geo_offset", "mask")],
@@ -247,16 +275,19 @@ class B2RHumanAssets(C.Structure):
 
 
 class B2RHumanAssetsGrads(C.Structure):
+    ID = 22
     _fields_ = [(n, _fp) for n in ("dL_dmean_3d", "dL_dmean_3d_refined", "dL_dscale", "dL_dscale_refined",
                                    "dL_dmean_offset_offset", "dL_dscale_wo_clamp", "dL_dscale_refined_wo_clamp",
                                    "dL_dmesh", "dL_dexpr_offset", "dL_dgeo", "dL_dgeo_offset")]
 
 
 class B2RForwardOutputs(C.Structure):
+    ID = 3
     _fields_ = [("color", _fp), ("depth", _fp), ("alpha", _fp), ("radii", _fp)]
 
 
 class B2RBackwardArgs(C.Structure):
+    ID = 4
     _fields_ = [
         ("dL_dcolor", _fp), ("dL_ddepth", _fp), ("dL_dalpha", _fp),
         ("dL_dmeans3D", _fp), ("dL_dmeans2D", _fp), ("dL_dshs", _fp), ("dL_dcolors", _fp), ("dL_dopacities", _fp),
@@ -401,23 +432,12 @@ def load():
         fn.argtypes = argtypes
     if lib.b2r_abi_version() != ABI_VERSION:
         raise RuntimeError("b200raster: ABI version mismatch between the Python binding and libb200raster.so")
-    # index 7 is unused (b2r_sizeof reports 0 there); B2RMeshRender is 8, B2RGnMlp 10 (9 unused too), B2RRegs 11,
-    # B2RRegsGrads 12, B2RRig 13, B2RRigGrads 14, B2RAdamSegment 15, B2RLpips 16, B2RSceneAssets 17,
-    # B2RSceneAssetsGrads 18, B2RSmplxPose 19, B2RSmplxPoseGrads 20, B2RHumanAssets 21, B2RHumanAssetsGrads 22,
-    # B2RSmplxBody 23, B2RSmplxBodyGrads 24, B2RNeumanScores 25, B2RFaceComposite 26, B2RTestOutputs 27,
-    # B2ROrbitCamera 28, B2RAnimationPanel 29, B2RSmplxParamTable 31, B2RSmplxParamTableGrads 32, B2RFrameTable 33
-    # (30 unused)
-    for idx, cls in ((0, B2RScene), (1, B2RStatus), (2, B2RWorkspace), (3, B2RForwardOutputs), (4, B2RBackwardArgs),
-                     (5, B2RView), (6, B2RSkin), (8, B2RMeshRender), (10, B2RGnMlp), (11, B2RRegs),
-                     (12, B2RRegsGrads), (13, B2RRig), (14, B2RRigGrads), (15, B2RAdamSegment),
-                     (16, B2RLpips), (17, B2RSceneAssets), (18, B2RSceneAssetsGrads), (19, B2RSmplxPose),
-                     (20, B2RSmplxPoseGrads), (21, B2RHumanAssets), (22, B2RHumanAssetsGrads), (23, B2RSmplxBody),
-                     (24, B2RSmplxBodyGrads), (25, B2RNeumanScores), (26, B2RFaceComposite),
-                     (27, B2RTestOutputs), (28, B2ROrbitCamera), (29, B2RAnimationPanel),
-                     (31, B2RSmplxParamTable), (32, B2RSmplxParamTableGrads), (33, B2RFrameTable)):
-        if lib.b2r_sizeof(idx) != C.sizeof(cls):
+    # every struct mirror carries its b2r_sizeof index as `ID`
+    for cls in globals().values():
+        if isinstance(cls, type) and issubclass(cls, C.Structure) and hasattr(cls, "ID") \
+                and lib.b2r_sizeof(cls.ID) != C.sizeof(cls):
             raise RuntimeError(f"b200raster: struct layout drift for {cls.__name__}: "
-                               f"{lib.b2r_sizeof(idx)} (C) vs {C.sizeof(cls)} (ctypes)")
+                               f"{lib.b2r_sizeof(cls.ID)} (C) vs {C.sizeof(cls)} (ctypes)")
     _lib = lib
     return lib
 

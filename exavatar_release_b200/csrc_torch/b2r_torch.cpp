@@ -544,10 +544,7 @@ void adam_launch(const at::Tensor& table, int64_t n_segments, int64_t n_chunks, 
   if (n_chunks == 0) return;
   c10::cuda::CUDAGuard guard((c10::DeviceIndex)device);
   const cudaStream_t stream = c10::cuda::getCurrentCUDAStream((c10::DeviceIndex)device).stream();
-  const int rc = b2r_adam_step((const B2RAdamSegment*)table.data_ptr(), (int32_t)n_segments, n_chunks, stream);
-  if (rc != B2R_OK)
-    throw std::runtime_error(std::string("b200raster: b2r_adam_step failed: ") + b2r_strerror(rc) + " (cudaError " +
-                             std::to_string(b2r_last_cuda_error()) + ")");
+  check(b2r_adam_step((const B2RAdamSegment*)table.data_ptr(), (int32_t)n_segments, n_chunks, stream), "b2r_adam_step");
 }
 
 }  // namespace

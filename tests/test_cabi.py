@@ -2,25 +2,16 @@
 agree with the ctypes mirror, argument validation returns the documented codes before any CUDA call."""
 import ctypes as C
 import os
-import re
 
 import pytest
 
+from util import header_structs, header_symbols
 from exavatar_release_b200 import _lib as L
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "b200raster.h")
-
-
-def declared_symbols():
-    src = open(HEADER).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(b2r_[a-z_0-9A-Z]+)\s*\(", src)))
 
 
 def test_library_exports_every_declared_symbol():
     lib = C.CDLL(L.LIB_PATH)
-    names = declared_symbols()
+    names = header_symbols()
     assert len(names) >= 20
     for n in names:
         assert hasattr(lib, n), f"{n} declared in b200raster.h but not exported"
@@ -30,11 +21,20 @@ def test_library_exports_every_declared_symbol():
 
 
 def test_struct_layouts_and_version():
+    """Every ctypes mirror against the header's typedef and the library's b2r_sizeof: size, field names in order, and
+    one mirror per index the library reports, without a device."""
     lib = L.load()
     assert lib.b2r_abi_version() == 4 == L.ABI_VERSION
-    for idx, cls in enumerate((L.B2RScene, L.B2RStatus, L.B2RWorkspace, L.B2RForwardOutputs, L.B2RBackwardArgs, L.B2RView)):
-        assert lib.b2r_sizeof(idx) == C.sizeof(cls)
-    assert lib.b2r_sizeof(99) == 0
+    mirrors = [c for c in vars(L).values() if isinstance(c, type) and issubclass(c, C.Structure) and hasattr(c, "ID")]
+    structs = header_structs()
+    for cls in mirrors:
+        assert lib.b2r_sizeof(cls.ID) == C.sizeof(cls), cls.__name__
+        assert [n for n, _ in cls._fields_] == structs[cls.__name__], cls.__name__
+    ids = sorted(c.ID for c in mirrors)
+    assert len(set(ids)) == len(ids), ids
+    assert ids == [i for i in range(64) if lib.b2r_sizeof(i)]
+    assert lib.b2r_sizeof(7) == lib.b2r_sizeof(9) == lib.b2r_sizeof(30) == lib.b2r_sizeof(99) == 0
+    assert sorted(c.__name__ for c in mirrors) == sorted(structs)  # and every struct of the header has a mirror
     assert C.sizeof(L.B2RStatus) == 64
 
 

@@ -59,8 +59,6 @@ def test_symbols_and_struct_mirror():
     for name in ("b2r_mesh_render_scratch_bytes", "b2r_mesh_render_forward", "b2r_mesh_render_backward"):
         assert hasattr(raw, name), name
         assert name in {s[0] for s in L.SYMBOLS}, name
-    assert lib.b2r_sizeof(8) == C.sizeof(L.B2RMeshRender)
-    assert lib.b2r_sizeof(7) == 0 and lib.b2r_sizeof(9) == 0  # 7 stays unused
     assert lib.b2r_mesh_render_scratch_bytes(9558) >= 9558 * (64 + 36)
     assert lib.b2r_mesh_render_scratch_bytes(0) > 0
 

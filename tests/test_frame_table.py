@@ -1,6 +1,5 @@
 """`FrameTable` (exavatar_release_b200/frames.py, csrc/frames.cu b2r_frame_unpack): every frame of a split on the
-device, the frame of a slot expanded into the DataLoader's collated batch.  CPU: the struct against its ctypes mirror,
-the C ABI's refusals and the builder's checks, which raise before anything is uploaded for the frame they name.  GPU:
+device, the frame of a slot expanded into the DataLoader's collated batch.  CPU: the C ABI's refusals and the builder's checks, which raise before anything is uploaded for the frame they name.  GPU:
 the unpack bit-identical to torch's default collate of NeuMan's __getitem__ at 37x53, 512x512 and 1080x1920 through
 host and device slots; slots shared with a SmplxParamTable; out-of-range slots inside guarded allocations; one graph
 replayed for every slot without a host sync; eval_neuman's ground-truth read; and a training iteration under
@@ -21,26 +20,11 @@ from exavatar_release_b200 import frames as FR
 from exavatar_release_b200.frames import FrameTable
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "b200raster.h")
 if os.path.join(ROOT, "tools") not in sys.path:
     sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 
 # ---------------------------------------------------------------------------------------------------------- CPU tests
-
-def test_struct_layout_matches_header():
-    lib = L.load()
-    assert lib.b2r_sizeof(33) == C.sizeof(L.B2RFrameTable)
-    src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
-    body = re.search(r"typedef struct B2RFrameTable \{(.*?)\} B2RFrameTable;", src, re.S).group(1)
-    names = []
-    for decl in body.split(";"):
-        decl = decl.strip()
-        if decl:
-            names += [n.strip().lstrip("*") for n in re.sub(r"^(const\s+)?\w+\*?\s+", "", decl).split(",")]
-    assert names == [n for n, _ in L.B2RFrameTable._fields_]
-    assert lib.b2r_sizeof(7) == lib.b2r_sizeof(9) == lib.b2r_sizeof(30) == lib.b2r_sizeof(99) == 0
-
 
 def test_abi_refusals_without_touching_cuda():
     lib = L.load()

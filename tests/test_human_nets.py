@@ -61,8 +61,7 @@ def test_abi_symbols_and_struct():
                  "b2r_gn_mlp_forward", "b2r_gn_mlp_backward"):
         assert hasattr(raw, name), name
         assert name in {s[0] for s in L.SYMBOLS}, name
-    assert lib.b2r_sizeof(10) == C.sizeof(L.B2RGnMlp) == 16 + 8 * 15
-    assert lib.b2r_sizeof(9) == 0
+    assert C.sizeof(L.B2RGnMlp) == 16 + 8 * 15
     assert lib.b2r_gn_mlp_grads_count(222, 4) == 128 * 222 + 2 * 128 * 128 + 9 * 128 + 4 * 128 + 4
     # the backward keeps dz_0..2 and a_0, a_1 (5 x P x 128 fp32) plus its partials
     assert lib.b2r_gn_mlp_scratch_bytes(P_C4) >= 5 * P_C4 * 128 * 4

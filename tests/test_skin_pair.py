@@ -32,8 +32,6 @@ J = 55
 def test_skin_struct_layout_and_symbols():
     lib = L.load()
     assert lib.b2r_abi_version() == 4
-    assert C.sizeof(L.B2RSkin) == lib.b2r_sizeof(6)
-    assert lib.b2r_sizeof(7) == 0
     raw = C.CDLL(L.LIB_PATH)
     for name in ("b2r_skin_forward", "b2r_skin_backward", "b2r_skin_scratch_bytes"):
         assert hasattr(raw, name), name

@@ -153,8 +153,8 @@ def test_cabi_symbols_and_argument_checks():
     raw = C.CDLL(L.LIB_PATH)
     for name in ("b2r_smplx_body_scratch_bytes", "b2r_smplx_body_forward", "b2r_smplx_body_backward"):
         assert hasattr(raw, name) and name in {s[0] for s in L.SYMBOLS}, name
-    assert lib.b2r_sizeof(23) == C.sizeof(L.B2RSmplxBody) == C.sizeof(L.B2RRig) + 8 * 8
-    assert lib.b2r_sizeof(24) == C.sizeof(L.B2RSmplxBodyGrads) == 8 * 5
+    assert C.sizeof(L.B2RSmplxBody) == C.sizeof(L.B2RRig) + 8 * 8
+    assert C.sizeof(L.B2RSmplxBodyGrads) == 8 * 5
     nb = lib.b2r_smplx_body_scratch_bytes(100, 55)
     assert nb > lib.b2r_smplx_body_scratch_bytes(10, 55) > 0
     grads = L.B2RSmplxBodyGrads(FAKE, FAKE, FAKE, FAKE, FAKE)

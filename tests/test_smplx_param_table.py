@@ -1,11 +1,9 @@
 """`SmplxParamTable` (csrc/smplx_pose.cu b2r_param_table_*): every frame's SMPL-X parameters in one table, the frame
-chosen by a slot read on the device.  CPU: the structs against their ctypes mirrors, the C ABI's refusals and the
-host checks of the class.  GPU: forward and gradients bit-identical to `decode_smplx_pose` on the frame's
+chosen by a slot read on the device.  CPU: the C ABI's refusals and the host checks of the
+class.  GPU: forward and gradients bit-identical to `decode_smplx_pose` on the frame's
 ParameterDict for every slot, as an int and as a CUDA tensor; zeros in every other row; NaN outputs and zero gradients
 for an out-of-range device slot with the guards around the tables intact; the dict round trip bit for bit."""
 import ctypes as C
-import os
-import re
 
 import pytest
 import torch
@@ -14,28 +12,10 @@ import torch.nn as nn
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.human_assets import POSE_KEYS, POSE_ROWS, SmplxParamTable, decode_smplx_pose
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "b200raster.h")
 NE = 50
 
 
 # ---------------------------------------------------------------------------------------------------------- CPU tests
-
-@pytest.mark.parametrize("idx,cls,name", [(31, L.B2RSmplxParamTable, "B2RSmplxParamTable"),
-                                          (32, L.B2RSmplxParamTableGrads, "B2RSmplxParamTableGrads")])
-def test_struct_layouts_match_header(idx, cls, name):
-    lib = L.load()
-    assert lib.b2r_sizeof(idx) == C.sizeof(cls)
-    src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
-    body = re.search(r"typedef struct %s \{(.*?)\} %s;" % (name, name), src, re.S).group(1)
-    names = []
-    for decl in body.split(";"):
-        decl = decl.strip()
-        if decl:
-            names += [n.strip().lstrip("*") for n in re.sub(r"^(const\s+)?\w+\*?\s+", "", decl).split(",")]
-    assert names == [n for n, _ in cls._fields_]
-    assert lib.b2r_sizeof(7) == lib.b2r_sizeof(9) == lib.b2r_sizeof(30) == lib.b2r_sizeof(99) == 0
-
 
 def test_abi_refusals_without_touching_cuda():
     lib = L.load()

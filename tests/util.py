@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import os
+import re
 import sys
 
 import numpy as np
@@ -10,6 +11,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+HEADER = os.path.join(ROOT, "include", "b200raster.h")
 
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
 from exavatar_release_b200.renderer import render_settings  # noqa: E402
@@ -64,3 +66,27 @@ def settings_on(st, device, settings_cls):
         if isinstance(v, torch.Tensor):
             d[k] = v.to(device)
     return settings_cls(**d)
+
+
+def _header_source():
+    """include/b200raster.h without its comments."""
+    with open(HEADER) as f:
+        return re.sub(r"/\*.*?\*/", "", f.read(), flags=re.S)
+
+
+def header_structs():
+    """{name: field names in declaration order} of every typedef'd struct of the header.  A declaration may name several
+    fields (`int32_t P, J, reserved[2]`); the type, a nested struct's included, and array sizes are dropped."""
+    return {name: [re.findall(r"\w+", re.sub(r"\[.*?\]", "", d))[-1]
+                   for decl in body.split(";") if decl.strip() for d in decl.split(",")]
+            for name, body in re.findall(r"typedef struct (\w+) \{(.*?)\} \1;", _header_source(), re.S)}
+
+
+def header_symbols():
+    """The b2r_* functions the header declares, sorted."""
+    return sorted(set(re.findall(r"\b(b2r_\w+)\s*\(", _header_source())))
+
+
+def header_defines():
+    """{name: value as written} of the header's #defines."""
+    return dict(re.findall(r"^#define[ \t]+(\w+)[ \t]*(.*?)[ \t]*$", _header_source(), re.M))
