@@ -15,6 +15,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict, Optional
 
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -67,6 +68,25 @@ class _Workspace:
 
     def status(self) -> dict:
         return L.read_status(self.ctx_buf)
+
+    def read_ctx(self) -> Dict[str, np.ndarray]:
+        """The last forward's lists and records as host arrays: `ranges` (tiles, 2) uint32 per 16x16 tile, `ids` the
+        duplicate ids uint32, `n_contrib` (H, W) uint32, `final_T` (H, W) float32, `geom` (P, 12) float32 and `aux`
+        (P, 4) int32 per Gaussian.  Like `status()`, it copies the buffers to the host and so synchronises."""
+        buf = self.ctx_buf.cpu().numpy()
+        P, W, H = self.P, self.W, self.H
+        tiles = ((W + 15) // 16) * ((H + 15) // 16)
+
+        def take(fn, dtype, *shape):
+            o = fn(C.byref(self.ws), P, W, H) - self.ctx_buf.data_ptr()
+            return buf[o:o + int(np.prod(shape)) * np.dtype(dtype).itemsize].view(dtype).reshape(shape)
+
+        return {"ranges": take(self.lib.b2r_ctx_ranges, np.uint32, tiles, 2),
+                "ids": self.ids.cpu().numpy().view(np.uint32),
+                "n_contrib": take(self.lib.b2r_ctx_n_contrib, np.uint32, H, W),
+                "final_T": take(self.lib.b2r_ctx_final_T, np.float32, H, W),
+                "geom": take(self.lib.b2r_ctx_geom, np.float32, P, 12),
+                "aux": take(self.lib.b2r_ctx_aux, np.int32, P, 4)}
 
 
 class FramePlan(_Workspace):

@@ -12,7 +12,7 @@ import pytest
 import torch
 import torch.nn as nn
 
-from util import header_defines
+from util import header_defines, no_host_sync
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.optim import Adam
 from exavatar_release_b200.rasterizer import _compiled_binding
@@ -413,11 +413,8 @@ def test_no_sync_and_one_launch_per_step_with_1000_frames():
                 p.grad = torch.randn(p.shape, device=dev, generator=gen) if on else None
         torch.cuda.synchronize()
         n0 = lib.b2r_launch_count()
-        torch.cuda.set_sync_debug_mode("error")
-        try:
+        with no_host_sync():
             mine.step()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
         assert lib.b2r_launch_count() == n0 + 1
     for gr in mine.param_groups:
         for p in gr["params"]:

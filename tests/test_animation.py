@@ -12,18 +12,13 @@ import pytest
 import torch
 
 from util import ROOT  # noqa: F401  (path setup)
+from util import capture, no_host_sync
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.animation import (OrbitCamera, animation_panel, animation_panel_reference,
                                              look_at_view_transform_reference, orbit_points, orbit_reference)
 
 EPS = 2.0 ** -23
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
 
 
 def _camera(seed, dev, shape=None):
@@ -313,12 +308,8 @@ def test_no_host_sync(dev):
     set_fixed_capacity(1 << 21)
     try:
         _op_frame(rig, mesh_r, orbit, assets, ins, cam, frame_u8, index, bkg, bg)
-        torch.cuda.synchronize()
-        torch.cuda.set_sync_debug_mode("error")
-        try:
+        with no_host_sync():
             _op_frame(rig, mesh_r, orbit, assets, ins, cam, frame_u8, index, bkg, bg)
-        finally:
-            torch.cuda.set_sync_debug_mode("default")
     finally:
         set_fixed_capacity(None)
     torch.cuda.synchronize()
@@ -341,15 +332,7 @@ def test_one_graph_holds_the_video_frame(dev):
     try:
         run = lambda: _op_frame(rig, mesh_r, orbit, assets, ins, cam, frame_u8, index, bkg, bg)  # noqa: E731
         first = run()  # frame 0: anchors
-        side = torch.cuda.Stream(dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            run()
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            static = run()
+        graph, static = capture(run, 1)
         eager_orbit = OrbitCamera(16, 8, dev)
         graph.replay()  # frame 0 again: the same bytes
         torch.cuda.synchronize()

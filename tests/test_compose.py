@@ -11,15 +11,10 @@ from test_poisoned_buffers import poisoned
 from exavatar_release_b200 import compose as CP
 from exavatar_release_b200.compose import COMPOSITE_KEYS, RENDER_KEYS, face_composite, face_composite_reference
 from exavatar_release_b200.plan import RENDERS
+from util import capture, no_host_sync
+from util import dev  # noqa: F401
 
 SIZES = [(1, 31, 37), (3, 31, 37), (2, 512, 512), (1, 1080, 1920), (3, 1080, 1920)]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
 
 
 def on(dev, renders, *ts):
@@ -123,15 +118,10 @@ def test_no_host_sync(dev):
     renders, face, face_r, gt = on(dev, *inputs(1, 512, 512, seed=4))
     x, f = renders["scene_human"]["img"].clone().requires_grad_(), face.clone().requires_grad_()
     g = torch.randn(1, 3, 512, 512, device=dev)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         with torch.no_grad():
             CP.test_outputs(renders, face, face_r, gt)
         face_composite(x, f).backward(g)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
-    torch.cuda.synchronize()
 
 
 @pytest.mark.gpu
@@ -151,14 +141,7 @@ def test_cuda_graph_replays_new_inputs(dev):
         y.backward(g)
         return o, y, x.grad, f.grad
 
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        step()
-    torch.cuda.current_stream().wait_stream(side)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        o, y, gx, gf = step()
+    graph, (o, y, gx, gf) = capture(step, 1)
     for seed in (21, 22):
         new = on(dev, *inputs(N, H, W, seed=seed))
         for r in RENDERS:

@@ -18,7 +18,8 @@ import numpy as np
 import pytest
 import torch
 
-from util import ROOT  # noqa: F401  (path setup)
+from util import no_host_sync
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.camera import get_fov, get_proj_matrix, get_view_matrix
 
@@ -206,13 +207,6 @@ def test_rasterizer_takes_tensor_tanfov_only_as_a_cuda_pair():
 # ---------------------------------------------------------------------------------------------------------------------
 # GPU
 # ---------------------------------------------------------------------------------------------------------------------
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
-
 
 def _device_cam(R, t, focal, dev):
     return {"R": torch.from_numpy(np.asarray(R, f32)).to(dev), "t": torch.from_numpy(np.asarray(t, f32)).to(dev),
@@ -407,14 +401,9 @@ def test_c4_frame_from_camera_to_backward_without_a_host_sync(dev):
 
     arm = FrameArm(rig=rig, camera=camera)
     frame(arm)  # warm-up: captures the renderer's graphs, first-use set-up
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         frame(arm)
         frame(arm)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
-    torch.cuda.synchronize()
     assert len(fr._graphs) == 1 and not fr.overflowed()
 
 

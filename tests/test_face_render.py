@@ -15,7 +15,8 @@ import numpy as np
 import pytest
 import torch
 
-from util import ROOT  # noqa: F401  (path setup)
+from util import capture, no_host_sync
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.mesh_render import FaceMeshRenderer, _bary, _ndc, _pix_ndc, face_render_reference
 from exavatar_release_b200.synthetic import make_face_mesh, make_human_mesh
@@ -338,13 +339,6 @@ def test_synthetic_face_mesh():
 # ---------------------------------------------------------------------------------------------------------------------
 
 @pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
 def face():
     m = make_face_mesh()
     m["verts"] = make_human_mesh()["verts"][m["vertex_idx"]].contiguous()
@@ -481,12 +475,8 @@ def test_two_runs_are_bit_identical_and_nothing_syncs(dev, face):
     run()
     torch.cuda.synchronize()
     a = run()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         b = run()
-    finally:
-        torch.cuda.set_sync_debug_mode("default")
-    torch.cuda.synchronize()
     for x, y in zip(a, b):
         assert torch.equal(x, y)
 
@@ -506,15 +496,7 @@ def test_forward_backward_in_one_cuda_graph_equals_eager(dev, face):
         (img * G).sum().backward()
         return img.detach(), p2f, m.grad
 
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        step()
-    torch.cuda.current_stream(dev).wait_stream(side)
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        static = step()
+    graph, static = capture(step, 1)
     from exavatar_release_b200.camera import look_at_cam_param
     new = look_at_cam_param(-10.0, shape, device=dev)
     with torch.no_grad():

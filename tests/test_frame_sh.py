@@ -17,6 +17,7 @@ import pytest
 import torch
 
 from util import settings_on, workload_settings  # noqa: F401  (also sets up the import path)
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.camera import look_at_cam_param
 from exavatar_release_b200.plan import FiveRenderPlan, merged_bucket_layout
@@ -186,13 +187,6 @@ def test_oracle_reference_equals_the_oracle_sh_render(deg):
 # ---------------------------------------------------------------------------------------------------------------------
 # GPU
 # ---------------------------------------------------------------------------------------------------------------------
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
-
 
 def _close(x, y, rel=1e-4):
     x, y = x.detach(), y.detach()

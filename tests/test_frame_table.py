@@ -4,11 +4,10 @@ the unpack bit-identical to torch's default collate of NeuMan's __getitem__ at 3
 host and device slots; slots shared with a SmplxParamTable; out-of-range slots inside guarded allocations; one graph
 replayed for every slot without a host sync; eval_neuman's ground-truth read; and a training iteration under
 IterationGraph with the table read inside the graph, bit-identical to staging the collated inputs."""
+import contextlib
 import ctypes as C
 import multiprocessing
-import os
 import re
-import sys
 
 import numpy as np
 import pytest
@@ -18,10 +17,8 @@ from torch.utils.data import default_collate
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200 import frames as FR
 from exavatar_release_b200.frames import FrameTable
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-if os.path.join(ROOT, "tools") not in sys.path:
-    sys.path.insert(0, os.path.join(ROOT, "tools"))
+from util import no_host_sync
+from util import dev  # noqa: F401
 
 
 # ---------------------------------------------------------------------------------------------------------- CPU tests
@@ -184,11 +181,6 @@ def collated(ds, i):
     return default_collate([ds[i]])
 
 
-@pytest.fixture(scope="module")
-def dev():
-    return torch.device("cuda")
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("H,W", [(37, 53), (512, 512), (1080, 1920)])
 def test_unpack_matches_collated_dataset(H, W, dev, tmp_path):
@@ -290,12 +282,9 @@ def test_one_graph_replayed_for_every_slot(dev, tmp_path):
     for rep in range(2):
         for s in (3, 0, 2, 1, 9, -1):
             n0 = lib.b2r_launch_count()
-            torch.cuda.set_sync_debug_mode("error")
-            try:
+            with no_host_sync():
                 slot_t.fill_(s)
                 g.replay()
-            finally:
-                torch.cuda.set_sync_debug_mode(0)
             assert lib.b2r_launch_count() == n0
             if 0 <= s < 4:
                 assert_batch(out, collated(ds, s), f"replay {rep} slot {s}")
@@ -387,12 +376,8 @@ def test_iteration_graph_with_the_table_matches_staged_inputs(dev, tmp_path):
         la = it_a.run(staged(batch, bgs[itr]), slot, key=warm[itr])
         replay = warm[itr] in it_b._graphs
         n0 = lib.b2r_launch_count()
-        if replay:
-            torch.cuda.set_sync_debug_mode("error")
-        try:
+        with no_host_sync() if replay else contextlib.nullcontext():
             lb = it_b.run({"bg": bgs[itr]}, table.slot_of(ds.frame_idx_list[pos]), key=warm[itr])
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
         if replay:
             assert lib.b2r_launch_count() == n0
         assert la.keys() == lb.keys()

@@ -21,7 +21,6 @@ f32 build against its f64 build on these inputs, so the reference the GPU tests 
 GPU tier: FramePlan (C ABI), the public `GaussianRasterizer` (both host routes), the stage buffers, `markVisible`, the
 merged training frame (RGB and SH scene), skinning, and one 512x512 frame, each against the oracle.
 """
-import ctypes as C
 import math
 import zlib
 
@@ -31,6 +30,7 @@ import torch
 
 from parity import compare, contributor_report, last_contributor
 from util import settings_on
+from util import dev  # noqa: F401
 from exavatar_release_b200.renderer import lbs_reference, render_settings
 from exavatar_release_b200.sh import sh_to_rgb
 from oracle import dense_autograd as DA
@@ -337,30 +337,6 @@ def test_populations_reach_their_edges():
 # GPU tier
 # ---------------------------------------------------------------------------------------------------------------------
 
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
-
-
-def _ctx_arrays(plan):
-    """(ranges (Tn,2) uint32, ids uint32, n_contrib (H,W) uint32, final_T (H,W) float32) of the plan's last forward."""
-    lib = plan.lib
-    P, W, H = plan.P, plan.W, plan.H
-    tiles = ((W + 15) // 16) * ((H + 15) // 16)
-    buf = plan.ctx_buf.cpu().numpy()
-    base = plan.ctx_buf.data_ptr()
-    off = lambda fn: fn(C.byref(plan.ws), P, W, H) - base
-    take = lambda o, n, dt: np.frombuffer(buf[o:o + n].tobytes(), dt)
-    ranges = take(off(lib.b2r_ctx_ranges), tiles * 8, np.uint32).reshape(tiles, 2)
-    ncon = take(off(lib.b2r_ctx_n_contrib), W * H * 4, np.uint32).reshape(H, W)
-    fT = take(off(lib.b2r_ctx_final_T), W * H * 4, np.float32).reshape(H, W)
-    geom = take(off(lib.b2r_ctx_geom), P * 48, np.float32).reshape(P, 12)
-    aux = take(off(lib.b2r_ctx_aux), P * 16, np.int32).reshape(P, 4)
-    return ranges, plan.ids.cpu().numpy().view(np.uint32), ncon, fT, geom, aux
-
-
 def _grad_names(mode):
     return ["means3D", "means2D", "opacities", "scales", "rotations", "shs" if mode == "sh" else "colors"]
 
@@ -386,8 +362,8 @@ def _plan_vs_oracle(dev, case, st_c, a, mode, clamp_rows=None, f64_refs=()):
     compare(case, "color", plan.color.cpu().numpy(), oc, pm[None], kind="image")
     compare(case, "depth", plan.depth.cpu().numpy(), od, pm[None], kind="image")
     compare(case, "alpha", plan.alpha.cpu().numpy(), oa, pm[None], kind="image")
-    ranges, ids, ncon, fT, _, _ = _ctx_arrays(plan)
-    contributor_report(case, last_contributor(ids, ranges, ncon, W, H), fT,
+    ctx = plan.read_ctx()
+    contributor_report(case, last_contributor(ctx["ids"], ctx["ranges"], ctx["n_contrib"], W, H), ctx["final_T"],
                        last_contributor(octx.sorted_ids(), octx.ranges(), octx.n_contrib(), W, H), octx.final_T(), pm)
     gi, gd, ga = grad_images(H, W, _seed(case, "g"))
     flat, views = grad_bucket(P, dev, M)
@@ -516,7 +492,8 @@ def test_stage_buffers_with_huge_splats(dev):
         torch.cuda.synchronize()
         status = plan.status()
         assert status["overflow"] == 0
-        ranges, ids, _, _, geom, aux = _ctx_arrays(plan)
+        lists = plan.read_ctx()
+        ranges, ids, geom, aux = lists["ranges"], lists["ids"], lists["geom"], lists["aux"]
         if flags:
             assert np.array_equal(aux[:, 2], orad)
             assert status["num_visible"] == int(vis.sum())

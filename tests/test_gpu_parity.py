@@ -12,20 +12,14 @@ import numpy as np
 import pytest
 import torch
 
-from util import kat_settings, pack, splat, workload_settings
+from util import capture, kat_settings, pack, splat, workload_settings
+from util import dev  # noqa: F401
 from exavatar_release_b200.synthetic import WORKLOADS, make_assets, make_grad_image
 from oracle import oracle as O
 
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-4
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
 
 
 def RZ():
@@ -126,17 +120,8 @@ def _stage_buffers(dev, wl_name, no_cull):
     plan = FramePlan(P, wl.width, wl.height, 4_000_000, dev)
     sc = plan.scene(0, st, assets, flags=L.B2R_FLAG_NO_TILE_CULL if no_cull else 0)
     plan.forward(sc)
-    torch.cuda.synchronize()
-    lib = plan.lib
-    buf = plan.ctx_buf.cpu().numpy()
-    base = plan.ctx_buf.data_ptr()
-    tiles = ((wl.width + 15) // 16) * ((wl.height + 15) // 16)
-    off = lambda fn: fn(C.byref(plan.ws), P, wl.width, wl.height) - base
-    geom = np.frombuffer(buf[off(lib.b2r_ctx_geom):off(lib.b2r_ctx_geom) + P * 48].tobytes(), np.float32).reshape(P, 12)
-    aux = np.frombuffer(buf[off(lib.b2r_ctx_aux):off(lib.b2r_ctx_aux) + P * 16].tobytes(), np.int32).reshape(P, 4)
-    ranges = np.frombuffer(buf[off(lib.b2r_ctx_ranges):off(lib.b2r_ctx_ranges) + tiles * 8].tobytes(), np.uint32).reshape(tiles, 2)
-    ids = plan.ids.cpu().numpy().view(np.uint32)
-    return geom, aux, ranges, ids, plan.status(), plan
+    ctx = plan.read_ctx()
+    return ctx["geom"], ctx["aux"], ctx["ranges"], ctx["ids"], plan.status(), plan
 
 
 def test_stage_geometry_matches_oracle(dev):
@@ -437,16 +422,7 @@ def test_fixed_capacity_call_is_graph_capturable(dev):
     Q = P - 7  # a shape no adaptive call has rendered yet
     try:
         rz.set_fixed_capacity(int(dups * 1.25) + 4096)
-        side = torch.cuda.Stream(dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            for _ in range(2):
-                step()
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            color = step()
+        graph, color = capture(step, 2)
         graph.replay()
         torch.cuda.synchronize(dev)
         assert torch.equal(color, ref)
@@ -669,15 +645,7 @@ def test_frame_lanes_match_serial_accumulation(dev):
         assert torch.allclose(lanes.bucket, flat, **tol), S
         assert lanes.status()["overflow"] == 0
     lanes = FrameLanes(3, P, wl.width, wl.height, 1_000_000, dev)
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        lanes.step(scenes, gis)
-    torch.cuda.current_stream(dev).wait_stream(side)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        lanes.step(scenes, gis)
+    g, _ = capture(lambda: lanes.step(scenes, gis), 1)
     lanes.bucket.zero_()
     lanes.lane_flat.zero_()
     g.replay()

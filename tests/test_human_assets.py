@@ -12,14 +12,13 @@ These tests pin
     the block size and P = 0; the warm-up clamp's gradient mask.
 """
 import ctypes as C
-import importlib.util
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import assert_close, capture, golden_generator, no_host_sync
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.human_assets import (POSE_KEYS, constant_rotation_reference, decode_smplx_pose_reference,
                                                 human_colors_reference, human_geometry_reference)
@@ -27,14 +26,6 @@ from exavatar_release_b200.human_assets import (POSE_KEYS, constant_rotation_ref
 FAKE = 0x1000  # never dereferenced: validation fails before any launch
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 P_C4 = 167618
-
-
-def _golden_module():
-    spec = importlib.util.spec_from_file_location("make_human_assets_golden",
-                                                  os.path.join(G, "make_human_assets_golden.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _fin(t):
@@ -53,7 +44,7 @@ def _geometry_inputs(inp):
 # ---------------------------------------------------------------------------------------------------------------------
 
 def test_pose_restatement_reproduces_the_reference_golden():
-    gm = _golden_module()
+    gm = golden_generator("make_human_assets_golden")
     gold = np.load(os.path.join(G, "human_assets.npz"))
     params, w = gm.pose_case()
     leaves = {k: v.clone().requires_grad_() for k, v in params.items()}
@@ -70,7 +61,7 @@ def test_pose_restatement_reproduces_the_reference_golden():
 
 @pytest.mark.parametrize("warmup", [0, 1])
 def test_geometry_restatement_reproduces_the_reference_golden(warmup):
-    gm = _golden_module()
+    gm = golden_generator("make_human_assets_golden")
     gold = np.load(os.path.join(G, "human_assets.npz"))
     inp, w = gm.geometry_case()
     mask, pose_offset = _geometry_inputs(inp)
@@ -184,7 +175,7 @@ def test_cabi_accepts_an_empty_set_without_launching():
 
 def test_host_refuses_cpu_tensors():
     from exavatar_release_b200 import decode_smplx_pose
-    params, _ = _golden_module().pose_case()
+    params, _ = golden_generator("make_human_assets_golden").pose_case()
     with pytest.raises(RuntimeError, match="CUDA tensor"):
         decode_smplx_pose({k: v.float() for k, v in params.items()})
     with pytest.raises(RuntimeError, match="CUDA"):
@@ -195,12 +186,6 @@ def test_host_refuses_cpu_tensors():
 # ---------------------------------------------------------------------------------------------------------------------
 # GPU
 # ---------------------------------------------------------------------------------------------------------------------
-
-def _close(a, b, rel, name):
-    scale = float(b.detach().abs().max())
-    err = float((a.detach().double() - b.detach().double()).abs().max())
-    assert err <= rel * max(scale, 1e-30), f"{name}: max error {err:.3e} vs {rel:.0e} x max {scale:.3e}"
-
 
 def _rowwise(a, b, rel, floor, name):
     """|a - b| <= rel * max(max |b| over the row, floor), row by row."""
@@ -215,7 +200,7 @@ def _rowwise(a, b, rel, floor, name):
 @pytest.mark.gpu
 def test_decode_against_float64_at_every_fixture_row():
     from exavatar_release_b200 import decode_smplx_pose
-    params, w = _golden_module().pose_case()
+    params, w = golden_generator("make_human_assets_golden").pose_case()
     p32 = {k: v.float().cuda().requires_grad_() for k, v in params.items()}
     p64 = {k: v.detach().cpu().double().requires_grad_() for k, v in p32.items()}
     out = decode_smplx_pose(p32)
@@ -239,7 +224,7 @@ def test_decode_against_float64_at_every_fixture_row():
 @pytest.mark.gpu
 def test_decode_rejects_rows_outside_the_55_joint_order():
     from exavatar_release_b200 import decode_smplx_pose
-    params, _ = _golden_module().pose_case()
+    params, _ = golden_generator("make_human_assets_golden").pose_case()
     p = {k: v.float().cuda() for k, v in params.items()}
     for k, bad in (("body_pose", p["body_pose"][:20]), ("root_pose", p["body_pose"][:2]),
                    ("lhand_pose", p["lhand_pose"].reshape(-1))):
@@ -309,15 +294,15 @@ def test_geometry_and_colors_at_c4_against_float64_and_bit_identical_to_fp32_tor
     r64 = human_geometry_reference(*[l64[k] for k in GEO_IN], mask, warmup)
     c64 = human_colors_reference(l64["rgb"], l64["rgb_offset"])
     for k, v in r64.items():
-        _close(res[k], v, 1e-6, k)
-    _close(rgb, c64[0], 1e-6, "rgb")
-    _close(rgb_r, c64[1], 1e-6, "rgb_refined")
+        assert_close(res[k], v, 1e-6, k)
+    assert_close(rgb, c64[0], 1e-6, "rgb")
+    assert_close(rgb_r, c64[1], 1e-6, "rgb_refined")
     w = _weights(P_C4, 9)
     _geo_loss(res, rgb, rgb_r, w).backward()
     _geo_loss(r64, *c64, [x.double() for x in w]).backward()
     assert lv["pose_offset"].grad is None
     for k in GEO_GRAD:
-        _close(lv[k].grad, l64[k].grad, 1e-5, f"d{k}")
+        assert_close(lv[k].grad, l64[k].grad, 1e-5, f"d{k}")
 
 
 @pytest.mark.gpu
@@ -424,7 +409,7 @@ def _chain_setup():
     from exavatar_release_b200 import HumanAssets
     ha = HumanAssets(model["is_rhand"], model["is_lhand"], model["is_face_expr"], device=dev)
     cam = look_at_cam_param(-6.0, (512, 512), device=dev)
-    params, _ = _golden_module().pose_case()
+    params, _ = golden_generator("make_human_assets_golden").pose_case()
     g = torch.Generator().manual_seed(21)
     P = rig.P
     leaves = {k: v.float().to(dev).requires_grad_() for k, v in params.items()}
@@ -465,26 +450,15 @@ def test_chain_runs_without_host_sync_and_a_cuda_graph_replays_it():
     torch.cuda.synchronize()
     for p in allp:
         p.grad = None
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         _chain(rig, ha, skw, self_map, cam, leaves, others, w)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     assert all(p.grad is not None and bool(torch.isfinite(p.grad).all()) for p in allp)
     # graph: capture the chain once, update every parameter in place, replay, compare with an eager run
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            for p in allp:
-                p.grad = None
-            _chain(rig, ha, skw, self_map, cam, leaves, others, w)
-    torch.cuda.current_stream().wait_stream(s)
-    for p in allp:
-        p.grad = None
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        loss_g = _chain(rig, ha, skw, self_map, cam, leaves, others, w)
+    def no_grads():
+        for p in allp:
+            p.grad = None
+
+    graph, loss_g = capture(lambda: _chain(rig, ha, skw, self_map, cam, leaves, others, w), 2, reset=no_grads)
     g = torch.Generator(device="cuda").manual_seed(5)
     with torch.no_grad():
         for p in allp:
@@ -497,5 +471,5 @@ def test_chain_runs_without_host_sync_and_a_cuda_graph_replays_it():
     want = [float(loss_e)] + [p.grad for p in list(fresh_l.values()) + list(fresh_o.values())]
     assert abs(got[0] - want[0]) <= 1e-6 * abs(want[0])
     for a, b in zip(got[1:], want[1:]):
-        _close(a, b, 1e-5, "graph vs eager gradient")
+        assert_close(a, b, 1e-5, "graph vs eager gradient")
     assert torch.equal(got[-2], want[-2]) and torch.equal(got[-1], want[-1])  # rgb, rgb_offset: the colour op alone

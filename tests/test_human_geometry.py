@@ -15,7 +15,8 @@ import numpy as np
 import pytest
 import torch
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import capture, no_host_sync
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.geometry import (VertexNormals, nearest_rows, nearest_rows_reference,
                                             vertex_normals_reference)
@@ -185,13 +186,6 @@ def test_argument_errors():
 # ---------------------------------------------------------------------------------------------------------------------
 
 @pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
 def mesh():
     return make_human_mesh()
 
@@ -309,15 +303,10 @@ def test_neither_op_syncs(dev, mesh):
     vn = VertexNormals(mesh["faces"], mesh["verts"].shape[0], flip=mesh["flip"].to(dev))
     x = mesh["verts"].to(dev)
     nearest_rows(q, t, sm), vn(x)  # loads the library and warms the allocator
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         nearest_rows(q, t, sm)
         nearest_rows(q, t, None)
         vn(x)
-    finally:
-        torch.cuda.set_sync_debug_mode("default")
-    torch.cuda.synchronize()
 
 
 @pytest.mark.gpu
@@ -334,15 +323,7 @@ def test_chain_in_one_cuda_graph_equals_eager(dev, mesh):
     t = mesh["targets"].to(dev).clone()
     sm = mesh["self_map"].to(dev)
     vn = VertexNormals(mesh["faces"], P, flip=mesh["flip"].to(dev))
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        _chain(q, qr, t, sm, table, A, tr, R, tc, vn)
-    torch.cuda.current_stream(dev).wait_stream(side)
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        static = _chain(q, qr, t, sm, table, A, tr, R, tc, vn)
+    graph, static = capture(lambda: _chain(q, qr, t, sm, table, A, tr, R, tc, vn), 1)
     g = torch.Generator().manual_seed(23)
     with torch.no_grad():
         t.mul_(1.03).add_(0.01)  # a new neutral mesh

@@ -13,7 +13,6 @@ These tests pin
 """
 import copy
 import ctypes as C
-import importlib.util
 import os
 
 import numpy as np
@@ -22,7 +21,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import capture, golden_generator, no_host_sync
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.human_nets import (TriplaneFeatures, bilinear_corners, gn_mlp, gn_mlp_reference,
                                               human_nets_reference, tri_feature_reference, triplane_grid)
@@ -30,13 +29,6 @@ from exavatar_release_b200.human_nets import (TriplaneFeatures, bilinear_corners
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 FAKE = 0x1000  # never dereferenced: validation fails before any launch
 P_C4 = 167618
-
-
-def _golden_module():
-    spec = importlib.util.spec_from_file_location("make_human_nets_golden", os.path.join(G, "make_human_nets_golden.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def gn_stack(k_in, head_dims=None, final=None):
@@ -103,7 +95,7 @@ def test_validation_without_touching_cuda():
 def test_restatement_reproduces_the_reference_golden():
     """tri_feature_reference + gn_mlp_reference (human_nets_reference) against the reference's own code in float64:
     pins the column order, the face overwrite, the pose in the middle of the concat and GroupNorm's group layout."""
-    gm = _golden_module()
+    gm = golden_generator("make_human_nets_golden")
     gold = np.load(os.path.join(G, "human_nets.npz"))
     nets = {}
     for k, (dims, relu_final) in gm.layer_dims().items():
@@ -372,34 +364,25 @@ def test_stack_bit_identical_no_sync_and_graph():
     a, b = run(), run()
     assert torch.equal(a[0], b[0]) and torch.equal(a[2], b[2])
     assert all(torch.equal(x, y) for x, y in zip(a[1], b[1]))
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         run()
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
 
     # forward + backward in one graph; replayed after an optimizer step changed the weights, equal to eager
     params = _params(trunk, heads)
     opt = torch.optim.Adam(params, lr=1e-3)
     x = ins[0].detach().clone().requires_grad_()
     static = [x] + [t.detach().clone() for t in ins[1:]]
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            for p in params:
-                p.grad = None
-            x.grad = None
-            (gn_mlp(static, trunk, heads) * gout).sum().backward()
-    torch.cuda.current_stream().wait_stream(s)
-    for p in params:
-        p.grad = None
-    x.grad = None
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        out_g = gn_mlp(static, trunk, heads)
-        (out_g * gout).sum().backward()
+
+    def step():
+        out = gn_mlp(static, trunk, heads)
+        (out * gout).sum().backward()
+        return out
+
+    def no_grads():
+        for p in (*params, x):
+            p.grad = None
+
+    graph, out_g = capture(step, 2, reset=no_grads)
     graph.replay()
     opt.step()  # new weights, same parameter storage
     graph.replay()

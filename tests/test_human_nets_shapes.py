@@ -27,7 +27,7 @@ import ctypes as C
 import pytest
 import torch
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.human_nets import (TriplaneFeatures, bilinear_corners, gn_mlp, gn_mlp_reference,
                                               tri_feature_reference, triplane_grid)
@@ -70,11 +70,6 @@ TRI_CASES = [  # (C, (H, W), P, face rows, placement)
 def _tri_id(case):
     c, (h, w), p, face, placement = case
     return f"C{c}-{h}x{w}-P{p}-{face}-{placement}"
-
-
-@pytest.fixture(scope="module")
-def dev():
-    return torch.device("cuda:0")
 
 
 # ---------------------------------------------------------------------------------------------------------------------

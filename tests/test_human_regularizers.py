@@ -10,14 +10,13 @@ These tests pin
     forward + backward replayed from one CUDA graph with a new mesh, and the f-7 human chain followed by the op.
 """
 import ctypes as C
-import importlib.util
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import capture, golden_generator, no_host_sync
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.geometry import vertex_normals_reference
 from exavatar_release_b200.regularizers import (KEYS, arm_selection_reference, human_regularizers_reference,
@@ -31,19 +30,12 @@ INPUTS = ("mean_offset", "mean_offset_offset", "scale_offset", "scale", "scale_r
           "joint_offset")
 
 
-def _golden_module():
-    spec = importlib.util.spec_from_file_location("make_regs_golden", os.path.join(G, "make_regs_golden.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
 # SMPL-X's joint names as the golden generator read them from the reference (avatar/common/utils/smpl_x.py)
 JOINTS = tuple(str(n) for n in np.load(os.path.join(G, "regs.npz"))["joints_name"])
 
 
 def _case(names=JOINTS):
-    return _golden_module().regs_inputs(list(names))
+    return golden_generator("make_regs_golden").regs_inputs(list(names))
 
 
 def _kink_row(labels):
@@ -92,7 +84,7 @@ def test_restatement_reproduces_the_reference_golden():
 
 
 def test_laplacian_table_is_the_reference_table_on_the_c4_mesh():
-    gm = _golden_module()
+    gm = golden_generator("make_regs_golden")
     gold = np.load(os.path.join(G, "regs.npz"))
     m = make_human_mesh()
     idx, w = laplacian_table(m["faces"].numpy(), P_C4)
@@ -208,7 +200,7 @@ def _c4(dev, **label_kw):
            "scale_refined": torch.exp(-5.5 + 0.3 * torch.randn(1, P_C4, 3, generator=g)),
            "rgb": torch.rand(1, P_C4, 3, generator=g), "rgb_refined": torch.rand(1, P_C4, 3, generator=g),
            "joint_offset": 1e-2 * torch.randn(55, 3, generator=g)}
-    _golden_module().pin_kinks(ins, kw, list(JOINTS))
+    golden_generator("make_regs_golden").pin_kinks(ins, kw, list(JOINTS))
     return m, regs, kw, ins
 
 
@@ -332,32 +324,25 @@ def test_bit_identical_no_sync_and_graph_replay():
     assert torch.equal(a[0], b[0]) and all(torch.equal(a[1][k], b[1][k]) for k in INPUTS)
     mesh = m["verts"].to(dev)
     leaves = {k: v.to(dev).clone().requires_grad_() for k, v in ins.items()}
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         out = regs(mesh, *[leaves[k] for k in INPUTS])
         sum(out.values()).backward()
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
 
     # forward + backward in one graph, replayed with a sheared mesh (new upper / lower split and k) and new inputs
     static_mesh = mesh.clone()
     static = {k: v.detach().clone().requires_grad_() for k, v in leaves.items()}
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            for v in static.values():
-                v.grad = None
-            sum(regs(static_mesh, *[static[k] for k in INPUTS]).values()).backward()
-    torch.cuda.current_stream().wait_stream(s)
-    for v in static.values():
-        v.grad = None
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        out_g = regs(static_mesh, *[static[k] for k in INPUTS])
-        vec_g = torch.stack([out_g[k] for k in KEYS])
-        vec_g.sum().backward()
+
+    def step():
+        out = regs(static_mesh, *[static[k] for k in INPUTS])
+        vec = torch.stack([out[k] for k in KEYS])
+        vec.sum().backward()
+        return vec
+
+    def no_grads():
+        for v in static.values():
+            v.grad = None
+
+    graph, vec_g = capture(step, 2, reset=no_grads)
     sheared = m["verts"].clone()
     sheared[:, 1] += 0.4 * sheared[:, 0]
     g = torch.Generator().manual_seed(99)

@@ -4,6 +4,7 @@ bit-identical to torch.optim.Adam over ExAvatar's per-frame groups (tests/test_a
 here) over a frame sequence with repeats; a captured `launch()` replayed 60 times with a new lr each step,
 bit-identical to eager `step()`, without a host sync; and a reduced iteration through IterationGraph, bit-identical to
 the same chain run eagerly and to the per-frame ParameterDict route, through a key change and optimizer surgery."""
+import contextlib
 import os
 
 import numpy as np
@@ -16,6 +17,7 @@ from exavatar_release_b200.human_assets import POSE_KEYS, POSE_ROWS, SmplxParamT
 from exavatar_release_b200.iteration import IterationGraph
 from exavatar_release_b200.losses import l1_ssim
 from exavatar_release_b200.optim import Adam, StaleLayoutError
+from util import no_host_sync
 
 POSITION_LR = (1.6e-4, 1.6e-6)
 FRAME_PARAMS = {"root_pose": (6,), "body_pose": (21, 6), "jaw_pose": (6,), "leye_pose": (6,), "reye_pose": (6,),
@@ -272,12 +274,9 @@ def test_captured_launch_replays_match_eager_steps():
             g.replay()
         else:
             n0 = lib.b2r_launch_count()
-            torch.cuda.set_sync_debug_mode("error")
-            try:
+            with no_host_sync():
                 graphed.stage(rows=slot)
                 g.replay()
-            finally:
-                torch.cuda.set_sync_debug_mode(0)
             assert lib.b2r_launch_count() == n0
         for pa, pb in zip(params(eager), params(graphed)):
             assert same(pa, pb), i
@@ -393,12 +392,8 @@ def test_iteration_graph_matches_eager_and_per_frame_route():
         tb = b.eager(f, x, warm[itr])
         replay = warm[itr] in it._graphs
         n0 = lib.b2r_launch_count()
-        if replay:
-            torch.cuda.set_sync_debug_mode("error")
-        try:
+        with no_host_sync() if replay else contextlib.nullcontext():
             tc = run(f, x, warm[itr])
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
         if replay:
             assert lib.b2r_launch_count() == n0  # the whole iteration replayed: no host launch
         assert ta.keys() == tb.keys() == tc.keys()
@@ -540,12 +535,8 @@ def test_iteration_graph_bit_identical_without_the_renderer():
         cur["warm"] = warm[itr]
         replay = warm[itr] in it._graphs
         n0 = lib.b2r_launch_count()
-        if replay:
-            torch.cuda.set_sync_debug_mode("error")
-        try:
+        with no_host_sync() if replay else contextlib.nullcontext():
             lc = it.run(inputs, f, key=warm[itr])
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
         if replay:
             assert lib.b2r_launch_count() == n0  # a replay: no host launch
         for k in la:

@@ -10,7 +10,6 @@ These tests pin
     `TrainingFrameRenderer` frame with ExAvatar's photometric block through the op vs. through the fp32 restatement.
 """
 import ctypes as C
-import importlib.util
 import os
 
 import numpy as np
@@ -18,7 +17,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import capture, golden_generator, no_host_sync
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.losses import C1, C2, crop_box, l1_ssim, l1_ssim_reference, ssim_window
 
@@ -27,16 +27,9 @@ FAKE = 0x1000  # never dereferenced: validation fails before any launch
 NAMES = ("b2r_l1ssim_scratch_bytes", "b2r_l1ssim_forward", "b2r_l1ssim_backward")
 
 
-def _golden_module():
-    spec = importlib.util.spec_from_file_location("make_loss_golden", os.path.join(G, "make_loss_golden.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
 def _fixture():
     """The cases of loss.npz with their inputs, rebuilt bit for bit by the generator's integer-only `loss_images`."""
-    gm = _golden_module()
+    gm = golden_generator("make_loss_golden")
     z = np.load(os.path.join(G, "loss.npz"))
     pairs = {k: gm.loss_images(*hw) for k, hw in gm.SIZES.items()}
     cases = {}
@@ -230,13 +223,6 @@ def test_l1_ssim_argument_errors():
 # GPU
 # ---------------------------------------------------------------------------------------------------------------------
 
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
-
-
 def _c4_case():
     """C4 size: 512x512, a smooth render-like pair, a box of ~60 % of the image."""
     g = torch.Generator().manual_seed(21)
@@ -330,13 +316,8 @@ def test_forward_and_backward_do_not_sync(dev):
     c = _c4_case()
     args = (c["img"].to(dev), c["target"].to(dev), c["bbox"].to(dev), c["mask"].to(dev))
     _fwd_bwd(dev, *args)  # loads the library and warms the allocator
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         _fwd_bwd(dev, *args)
-    finally:
-        torch.cuda.set_sync_debug_mode("default")
-    torch.cuda.synchronize()
 
 
 @pytest.mark.gpu
@@ -344,15 +325,7 @@ def test_cuda_graph_replay_with_new_contents_equals_eager(dev):
     c = _c4_case()
     img, target = c["img"].to(dev), c["target"].to(dev)
     bbox, mask = c["bbox"].to(dev), c["mask"].to(dev)
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        _fwd_bwd(dev, img, target, bbox, mask)
-    torch.cuda.current_stream(dev).wait_stream(side)
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        static = _fwd_bwd(dev, img, target, bbox, mask)
+    graph, static = capture(lambda: _fwd_bwd(dev, img, target, bbox, mask), 1)
     g = torch.Generator().manual_seed(5)
     with torch.no_grad():
         img.copy_(torch.rand(3, 512, 512, generator=g).to(dev))

@@ -11,7 +11,6 @@ These tests pin
     another size; and one C4 `TrainingFrameRenderer` frame with l1_ssim and the op against the fp32 restatement.
 """
 import ctypes as C
-import importlib.util
 import os
 
 import numpy as np
@@ -19,7 +18,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import capture, golden_generator, no_host_sync
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.losses import crop_box, l1_ssim
 from exavatar_release_b200.perceptual import EPS, LPIPS, lpips_reference, vgg_taps_reference
@@ -32,14 +32,7 @@ COUT = (64, 64, 128, 128, 256, 256, 256, 512, 512, 512, 512, 512, 512)
 TAPS = (64, 128, 256, 512, 512)
 
 
-def _golden_module():
-    spec = importlib.util.spec_from_file_location("make_lpips_golden", os.path.join(G, "make_lpips_golden.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-_GM = _golden_module()
+_GM = golden_generator("make_lpips_golden")
 _W = None
 
 
@@ -261,13 +254,6 @@ def test_closed_form_head_gradient_matches_f64_autograd():
 # ---------------------------------------------------------------------------------------------------------------------
 
 @pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
 def op(dev):
     feats, lins = _weights()
     return LPIPS(feats, lins, dev)
@@ -388,13 +374,8 @@ def test_forward_and_backward_do_not_sync(dev, op):
     c = _c4_case()
     args = (torch.stack((c["img"], c["target"].flip(-2))).to(dev), c["target"].to(dev), c["bbox"].to(dev))
     _fwd_bwd(op, *args)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         _fwd_bwd(op, *args)
-    finally:
-        torch.cuda.set_sync_debug_mode("default")
-    torch.cuda.synchronize()
 
 
 @pytest.mark.gpu
@@ -402,15 +383,7 @@ def test_cuda_graph_replay_with_a_box_of_another_size_equals_eager(dev, op):
     c = _c4_case()
     img = torch.stack((c["img"], c["target"].flip(-2))).to(dev)
     target, bbox = c["target"].to(dev), c["bbox"].to(dev)
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        _fwd_bwd(op, img, target, bbox)
-    torch.cuda.current_stream(dev).wait_stream(side)
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        static = _fwd_bwd(op, img, target, bbox)
+    graph, static = capture(lambda: _fwd_bwd(op, img, target, bbox), 1)
     g = torch.Generator().manual_seed(5)
     with torch.no_grad():
         img.copy_(torch.rand(2, 3, 512, 512, generator=g).to(dev))

@@ -47,7 +47,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.losses import crop_box
 from exavatar_release_b200.perceptual import EPS, LPIPS, SCALE, SHIFT, lpips_reference
@@ -428,13 +428,6 @@ class ShapeRun:
         _call(lib, op, bufs, self.img, self.target, small, self.dout, self.reuse_damage)
         self.reuse_diff = _bit_differences(after, _outputs(bufs, lay, small_crop, N, H, W))
         del after, bufs
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
 
 
 @pytest.fixture(scope="module")

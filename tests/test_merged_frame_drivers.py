@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from exavatar_release_b200.synthetic import WORKLOADS, make_grad_image, make_population_assets
+from util import dev  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -15,13 +16,6 @@ PROBE_LABELS = ["A:bin", "A:scene:fwd", "A:scene:bwd", "A:human:fwd", "A:human:b
                 "A:scene_human:bwd", "A:project_bwd",
                 "B:bin", "B:human_refined:fwd", "B:human_refined:bwd", "B:scene_human_refined:fwd",
                 "B:scene_human_refined:bwd", "B:project_bwd"]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
 
 
 def test_serial_split_and_concurrent_frames_agree(dev):

@@ -17,7 +17,8 @@ import numpy as np
 import pytest
 import torch
 
-from util import ROOT  # noqa: F401  (path setup)
+from util import capture, no_host_sync
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.geometry import vertex_normals_reference
 from exavatar_release_b200.mesh_render import (ShadedMeshRenderer, _ndc, _shade_reference, face_render_reference,
@@ -269,13 +270,6 @@ def test_argument_errors():
 # ---------------------------------------------------------------------------------------------------------------------
 
 @pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
 def body(dev):
     """The synthetic SMPL-X body posed by SmplxRig.body_mesh in camera coordinates (animate.py:81-82), and its rig."""
     from exavatar_release_b200.smplx_rig import SmplxRig
@@ -384,13 +378,8 @@ def test_two_calls_are_bit_identical_and_nothing_syncs(dev, body):
     mesh, cam, bkg = _case(body, dev, "closeup")
     r = ShadedMeshRenderer(body["faces"], mesh.shape[0], device=dev)
     a = r(mesh, cam, bkg, 0.6)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         b = r(mesh[None], cam, bkg, 0.6)
-    finally:
-        torch.cuda.set_sync_debug_mode("default")
-    torch.cuda.synchronize()
     assert torch.equal(a.view(torch.int32), b.view(torch.int32))
     assert bool((r._keys == -1).all())  # the key buffer is left clean
 
@@ -414,15 +403,7 @@ def test_captured_graph_replays_new_mesh_and_camera(dev, body):
     focal, princpt = cam["focal"].clone(), cam["princpt"].clone()
     c = {"focal": focal, "princpt": princpt}
     r(m, c, bkg, 0.75)  # allocates the key buffer
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        r(m, c, bkg, 0.75)
-    torch.cuda.current_stream(dev).wait_stream(side)
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        static = r(m, c, bkg, 0.75)
+    graph, static = capture(lambda: r(m, c, bkg, 0.75), 1)
     rig, ins = body["rig"], body["ins"]
     with torch.no_grad():
         pose = ins[2] + 0.05 * torch.randn(ins[2].shape, generator=torch.Generator().manual_seed(2)).to(dev)

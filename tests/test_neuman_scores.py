@@ -19,7 +19,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import capture, no_host_sync
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.metrics import (ALEX_CONVS, SSIM_WINDOW, NeumanScores, composite, gaussian_window,
                                            neuman_scores_reference, png_round_trip)
@@ -125,13 +126,6 @@ class CaseRun:
                              [(f"tap{k}", self.taps[k], lay.tap(sc, k)) for k in range(5)]
                              if not torch.equal(a.contiguous().view(torch.int32), b.contiguous().view(torch.int32))]
         del bufs
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
 
 
 @pytest.fixture(scope="module")
@@ -283,23 +277,12 @@ def test_repeatable_sync_free_and_graph_capturable(dev, op):
     a = op(r, t, m)
     b = op(r, t, m)
     assert torch.equal(_bits(a), _bits(b))
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         c = op(r, t, m)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     assert torch.equal(_bits(a), _bits(c))
     # a graph captured on one set of images, replayed on another
     sr, st, sm = r.clone(), t.clone(), m.clone()
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        op(sr, st, sm)
-    torch.cuda.current_stream().wait_stream(side)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        gout = op(sr, st, sm)
+    g, gout = capture(lambda: op(sr, st, sm), 1)
     r2, t2, m2 = (v.to(dev) for v in case_inputs(H, W, N, (1, True), seed=8))
     sr.copy_(r2)
     st.copy_(t2)

@@ -25,7 +25,8 @@ import numpy as np
 import pytest
 import torch
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import assert_close, golden_generator
+from util import dev  # noqa: F401
 from exavatar_release_b200.synthetic import make_human_mesh
 
 PKG = "exavatar_release_b200"
@@ -167,12 +168,6 @@ def _err(a, b):
     return float((a.double() - b.double()).abs().max()) if a.numel() else 0.0
 
 
-def _close(a, b, rel, what):
-    scale = float(b.detach().double().abs().max()) if b.numel() else 0.0
-    err = _err(a.detach(), b.detach())
-    assert err <= rel * max(scale, 1e-30), f"{what}: max error {err:.3e} vs {rel:.0e} x max {scale:.3e}"
-
-
 # ---------------------------------------------------------------------------------------------------------------------
 # CPU: the machinery itself
 # ---------------------------------------------------------------------------------------------------------------------
@@ -256,13 +251,6 @@ def test_bits_compare_nan_payloads_and_signed_zeros():
 # GPU
 # ---------------------------------------------------------------------------------------------------------------------
 
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
-
-
 @pytest.mark.gpu
 def test_poison_reaches_cuda_allocations(dev):
     """The file's premise: under poisoned(), a CUDA torch.empty is NaN / INT_MAX / 0xFF, for fresh and reused blocks."""
@@ -344,15 +332,15 @@ def test_skin_gaussians(P, J, dev):
         names = ["out.posed"] + (["out.posed_r"] if two else [])
         for x, n in zip(xs, names):
             ref = lbs_reference(x.double().cpu(), w, c["A"].double().cpu(), c["trans"].double().cpu(), R, t)
-            _close(got[n].cpu(), ref, 1e-6, (P, J, two, cam, rows, dense, n))
+            assert_close(got[n].cpu(), ref, 1e-6, (P, J, two, cam, rows, dense, n))
         gs = [c["gp"].double().cpu()] + ([c["gq"].double().cpu()] if two else [])
         dxs, dA, dtrans = _skin_backward_f64([x.double().cpu() for x in xs], w, c["A"].double().cpu(),
                                              c["trans"].double().cpu(), None if R is None else torch.inverse(R), gs)
         for n, ref in zip(("out.dxyz", "out.dxyz_r"), dxs):
-            _close(got[n].cpu(), ref, 1e-5, (P, J, n))
-        _close(got["out.dA"][:, :3, :].cpu(), dA, 1e-5, (P, J, "dA"))
+            assert_close(got[n].cpu(), ref, 1e-5, (P, J, n))
+        assert_close(got["out.dA"][:, :3, :].cpu(), dA, 1e-5, (P, J, "dA"))
         assert not bool(got["out.dA"][:, 3, :].any())
-        _close(got["out.dtrans"].cpu(), dtrans, 1e-5, (P, J, "dtrans"))
+        assert_close(got["out.dtrans"].cpu(), dtrans, 1e-5, (P, J, "dtrans"))
 
 
 # ------------------------------------------------------------------------------------------------------------- l1_ssim
@@ -420,7 +408,7 @@ def test_vertex_normals_with_vertices_in_no_face(extra, dev):
     got = check_memory(lambda: vn(x))["out"]
     ref = vertex_normals_reference(x, m["faces"], flip)
     assert bool((got[Vm:] == 0).all())
-    _close(got, ref, 1e-5, "normals")
+    assert_close(got, ref, 1e-5, "normals")
 
 
 # -------------------------------------------------------------------------------------------------------- mesh renders
@@ -735,19 +723,19 @@ def test_smplx_rig_and_body_mesh(which, dev):
     b = _leaves(ins, torch.float64)
     ref = rig.reference(*b, dtype=torch.float64, device="cuda", cache={})
     for name in ("mesh_neutral_pose", "mesh_neutral_pose_wo_upsample", "joint_mats"):
-        _close(got[f"out.rig.{name}"], getattr(ref, name), 1e-6, (which, name))
+        assert_close(got[f"out.rig.{name}"], getattr(ref, name), 1e-6, (which, name))
     for name in ("pose_offset", "expr_offset"):
-        _close(got[f"out.rig.{name}"], getattr(ref, name), 1e-5, (which, name))
+        assert_close(got[f"out.rig.{name}"], getattr(ref, name), 1e-5, (which, name))
     _loss(ref, [x.double() for x in w]).backward()
     for i, name in enumerate(names):
-        _close(got[f"out.d_rig[{i}]"], b[i].grad, 1e-5, (which, "d" + name))
+        assert_close(got[f"out.d_rig[{i}]"], b[i].grad, 1e-5, (which, "d" + name))
     c = _leaves(ins, torch.float64)
     trans = torch.tensor(RIG_TRANS, dtype=torch.float64, device="cuda")
     body = smplx_body_reference(rig.model, *c, trans)
-    _close(got["out.body"], body, 1e-6, (which, "body_mesh"))
+    assert_close(got["out.body"], body, 1e-6, (which, "body_mesh"))
     (body * _body_weights(rig).double()).sum().backward()
     for i, name in enumerate(names):
-        _close(got[f"out.d_body[{i}]"], c[i].grad, 2e-6, (which, "body d" + name))
+        assert_close(got[f"out.d_body[{i}]"], c[i].grad, 2e-6, (which, "body d" + name))
 
 
 @pytest.mark.gpu
@@ -783,8 +771,7 @@ def test_triplane_reused_with_new_planes_equals_a_fresh_object(dev):
 @pytest.mark.gpu
 def test_decode_smplx_pose(dev):
     from exavatar_release_b200 import decode_smplx_pose
-    from test_human_assets import _golden_module
-    params, w = _golden_module().pose_case()
+    params, w = golden_generator("make_human_assets_golden").pose_case()
     p32 = {k: v.float().to(dev) for k, v in params.items()}
     wd = {k: v.float().to(dev) for k, v in w.items()}
 
@@ -819,11 +806,11 @@ def test_human_assets(P, warmup, dev):
     c64 = human_colors_reference(l64["rgb"], l64["rgb_offset"])
     for k, v in r64.items():
         if f"out[0].{k}" in got:
-            _close(got[f"out[0].{k}"], v, 1e-6, k)
-    _close(got["out[1]"], c64[0], 1e-6, "rgb")
+            assert_close(got[f"out[0].{k}"], v, 1e-6, k)
+    assert_close(got["out[1]"], c64[0], 1e-6, "rgb")
     _geo_loss(r64, *c64, [x.double() for x in w]).backward()
     for k in GEO_GRAD:
-        _close(got[f"out[3].{k}"], l64[k].grad, 1e-5, f"d{k}")
+        assert_close(got[f"out[3].{k}"], l64[k].grad, 1e-5, f"d{k}")
 
 
 @pytest.mark.gpu

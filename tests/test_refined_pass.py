@@ -5,12 +5,13 @@ to scene ids with its own sorted entries on the (depth_bits, id) key (b2r_forwar
 CPU: a numpy restatement of that filter + merge against the joint sort.  GPU: the split pass against the whole pass
 (MergedFivePlan.SPLIT = False) at full C4 size -- lists, images, alpha and radii bit-equal, gradients within the tolerance of
 the backward's reordered float sums."""
-import ctypes as C
 import math
 
 import numpy as np
 import pytest
 import torch
+
+from util import dev  # noqa: F401
 
 SEG, CHUNK = 512, 2048  # the composites' segment cut and the sort's chunk length (common.cuh)
 
@@ -91,14 +92,8 @@ def _pitched_rolled(cam, pitch_deg, roll_deg):
 
 def _lists(plan):
     """Per-tile id lists of pass B (numpy), from its ranges and dup_ids."""
-    ps = plan.passes["B"]
-    lib = plan.lib
-    ptr = lib.b2r_ctx_ranges(C.byref(ps.ws), plan.P, plan.W, plan.H)
-    off = ptr - ps.ctx_buf.data_ptr()
-    tiles = ((plan.W + 15) // 16) * ((plan.H + 15) // 16)
-    ranges = ps.ctx_buf[off:off + 8 * tiles].view(torch.int32).view(tiles, 2).cpu().numpy()
-    ids = ps.ids.cpu().numpy()
-    return [ids[a:b] for a, b in ranges]
+    ctx = plan.passes["B"].read_ctx()
+    return [ctx["ids"][a:b] for a, b in ctx["ranges"]]
 
 
 def _close(x, y, what):
@@ -114,13 +109,6 @@ def _close(x, y, what):
     over = int((d > 1e-3 * y.abs() + 1e-4 * scale).sum())
     err = float(d.max())
     assert over <= 3 and err <= 5e-3 * scale, (what, over, err, scale)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
 
 
 @pytest.mark.gpu

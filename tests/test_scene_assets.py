@@ -13,7 +13,6 @@ These tests pin
     TrainingFrameRenderer (shs mode) and GaussianRenderer (rgb mode).
 """
 import ctypes as C
-import importlib.util
 import math
 import os
 
@@ -21,7 +20,7 @@ import numpy as np
 import pytest
 import torch
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import assert_close, capture, golden_generator, no_host_sync
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.scene_assets import scene_assets_reference
 from exavatar_release_b200.smplx_rig import (axis_angle_to_matrix, matrix_to_quaternion, quaternion_to_matrix,
@@ -32,20 +31,13 @@ G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 P_C4 = 130000
 
 
-def _golden_module():
-    spec = importlib.util.spec_from_file_location("make_scene_golden", os.path.join(G, "make_scene_golden.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
 # ---------------------------------------------------------------------------------------------------------------------
 # CPU
 # ---------------------------------------------------------------------------------------------------------------------
 
 @pytest.mark.parametrize("deg", [0, 1, 2, 3])
 def test_restatement_reproduces_the_reference_golden(deg):
-    gm = _golden_module()
+    gm = golden_generator("make_scene_golden")
     gold = np.load(os.path.join(G, "scene.npz"))
     params, cam, w = gm.scene_case()
     leaves = {k: v.clone().requires_grad_() for k, v in params.items()}
@@ -202,12 +194,6 @@ def _loss(out, w, rgb, q_by_matrix):
     return loss
 
 
-def _close(a, b, rel, name):
-    scale = float(b.detach().abs().max())
-    err = float((a.double() - b.double()).abs().max())
-    assert err <= rel * max(scale, 1e-30), f"{name}: max error {err:.3e} vs {rel:.0e} x max {scale:.3e}"
-
-
 def _deg(d):
     return torch.tensor([float(d)], device="cuda")
 
@@ -233,7 +219,7 @@ def test_outputs_and_gradients_against_float64(cases, case, mode):
     cam64 = None if cam is None else {k: v.double() for k, v in cam.items()}
     ref = scene_assets_reference(*[l64[k] for k in KEYS], deg.double(), cam64)
     for name in ("opacity", "scale") + (("rgb",) if rgb else ("shs",)):
-        _close(out[name], ref[name], 1e-6, name)
+        assert_close(out[name], ref[name], 1e-6, name)
     assert out["mean_3d"] is leaves["mean"]
     # quaternion: where the f64 pick wins clearly and q0 is away from 0, q itself; elsewhere R(q), and q up to sign
     m64 = rotation_6d_to_matrix(l64["rotation6d"].detach())
@@ -247,7 +233,7 @@ def test_outputs_and_gradients_against_float64(cases, case, mode):
     assert float((q32[clear] - q64[clear]).abs().max()) <= 1e-6
     near0 = q64[:, 0].abs() < 1e-6
     assert int(near0.sum()) >= 3  # the 180-degree rows
-    _close(quaternion_to_matrix(q32), quaternion_to_matrix(q64), 1e-6, "R(q)")
+    assert_close(quaternion_to_matrix(q32), quaternion_to_matrix(q64), 1e-6, "R(q)")
     sign = torch.where((q32 * q64).sum(1, keepdim=True) < 0, -1.0, 1.0).double()
     assert float((q32 * sign - q64).abs().max()) <= 1e-6
     # gradients of a seeded loss
@@ -264,7 +250,7 @@ def test_outputs_and_gradients_against_float64(cases, case, mode):
         if float(b.abs().max()) == 0:  # the coefficients above degree 0
             assert bool((a == 0).all()), k
             continue
-        _close(a, b, 1e-5, f"{case}/{mode} d{k}")
+        assert_close(a, b, 1e-5, f"{case}/{mode} d{k}")
     if rgb:
         nb = (mode + 1) ** 2
         assert bool((leaves["feature_rest"].grad[:, nb - 1:] == 0).all())  # exact zeros above the degree
@@ -392,15 +378,10 @@ def test_no_host_sync(cases):
     cam, deg = _cam(), _deg(2)
     leaves = {k: v.clone().requires_grad_() for k, v in p.items()}
     mask = torch.zeros(P_C4, dtype=torch.bool, device="cuda")
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         for c in (cam, None):
             out = scene_assets(*[leaves[k] for k in KEYS], deg if c is not None else 2, c)
             _loss(out, w, c is not None, mask).backward()
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
-    torch.cuda.synchronize()
 
 
 @pytest.mark.gpu
@@ -413,20 +394,17 @@ def test_cuda_graph_replay_across_inputs_and_degrees_equals_eager(cases):
     deg = _deg(1)
     mask = torch.zeros(P, dtype=torch.bool, device="cuda")
     leaves = {k: v.clone().requires_grad_() for k, v in p.items()}
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            for x in leaves.values():
-                x.grad = None
-            _loss(scene_assets(*[leaves[k] for k in KEYS], deg, cam), w, True, mask).backward()
-    torch.cuda.current_stream().wait_stream(s)
-    for x in leaves.values():
-        x.grad = None
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
+
+    def step():
         out = scene_assets(*[leaves[k] for k in KEYS], deg, cam)
         _loss(out, w, True, mask).backward()
+        return out
+
+    def no_grads():
+        for x in leaves.values():
+            x.grad = None
+
+    graph, out = capture(step, 2, reset=no_grads)
     for seed, d in ((11, 3.0), (12, 0.0), (13, 2.0)):
         new = _params(P, seed=seed)
         with torch.no_grad():
@@ -485,7 +463,7 @@ def test_host_argument_checks():
     # M = 1: no feature_rest rows
     out = scene_assets(*a[:5], torch.zeros(10, 0, 3, device="cuda"), _deg(0), cam)
     ref = scene_assets_reference(*a[:5], torch.zeros(10, 0, 3, device="cuda"), _deg(0), cam)
-    _close(out["rgb"], ref["rgb"], 1e-6, "M=1 rgb")
+    assert_close(out["rgb"], ref["rgb"], 1e-6, "M=1 rgb")
 
 
 @pytest.mark.gpu

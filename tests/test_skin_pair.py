@@ -14,7 +14,8 @@ import numpy as np
 import pytest
 import torch
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import capture
+from util import dev  # noqa: F401
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.camera import look_at_cam_param
 from exavatar_release_b200.renderer import lbs_reference, render_settings
@@ -144,13 +145,6 @@ def test_skin_gaussians_rejects_cpu_tensors():
 # ---------------------------------------------------------------------------------------------------------------------
 # GPU
 # ---------------------------------------------------------------------------------------------------------------------
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
-
 
 def _c4_rig(dev, world=True):
     """C4 human size: P = 167 000 Gaussians, a (V = P, 55) 4-sparse weight table read through `rows` (a random row
@@ -293,15 +287,7 @@ def test_forward_and_backward_capture_in_a_cuda_graph(dev):
         loss = (posed * gp).sum() + (posed_r * gq).sum()
         return (posed.detach(), posed_r.detach()) + torch.autograd.grad(loss, (x, xr, A, tr))
 
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        step()  # warm-up outside the capture
-    torch.cuda.current_stream(dev).wait_stream(side)
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        static_out = step()
+    graph, static_out = capture(step, 1)
     _, A2, tr2 = _rig(P, J, torch.float32, dev, seed=17)
     tr2 = tr2 + 0.05
     with torch.no_grad():

@@ -13,7 +13,6 @@ These tests pin
     gradients 5.7e-7).
 """
 import ctypes as C
-import importlib.util
 import math
 import os
 
@@ -21,20 +20,13 @@ import numpy as np
 import pytest
 import torch
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import assert_close, capture, golden_generator, no_host_sync
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.smplx_rig import batch_rodrigues, smplx_body_reference, validate_model
 from exavatar_release_b200.synthetic import make_human_mesh, make_smplx_model
 
 FAKE = 0x1000  # never dereferenced: validation fails before any launch
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
-
-def _golden_module():
-    spec = importlib.util.spec_from_file_location("make_body_golden", os.path.join(G, "make_body_golden.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _inputs(J, NB, NE, seed=0, scale=0.3, device="cpu"):
@@ -60,7 +52,7 @@ def _camera(device="cpu", dtype=torch.float32):
 
 def test_restatement_reproduces_the_reference_golden():
     """tests/golden/body.npz was written by the reference's own SMPLX layer and Model.get_smplx_outputs."""
-    gm = _golden_module()
+    gm = golden_generator("make_body_golden")
     gold = np.load(os.path.join(G, "body.npz"))
     _, model, ins, cam, w = gm.body_case()
     m = validate_model(**model)
@@ -204,16 +196,6 @@ def _weights(rig, seed=3):
     return torch.randn((rig.V, 3), generator=torch.Generator().manual_seed(seed)).cuda()
 
 
-def _err(a, b):
-    return float((a.double() - b.double()).abs().max()) / max(float(b.abs().max()), 1e-30)
-
-
-def _close(a, b, rel, name):
-    err = _err(a, b)
-    print(f"{name}: max error {err:.3e} of max")
-    assert err <= rel, f"{name}: max error {err:.3e} x max vs {rel:.0e}"
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("world", [False, True])
 def test_mesh_against_float64(c4, world):
@@ -224,7 +206,7 @@ def test_mesh_against_float64(c4, world):
     out = rig.body_mesh(*ins, *cam)
     ref = smplx_body_reference(rig.model, *[t.double() for t in ins], *[None if c is None else c.double() for c in cam])
     assert out.shape == (rig.V, 3) and out.dtype == torch.float32
-    _close(out, ref, 1e-6, "world" if world else "camera")
+    assert_close(out, ref, 1e-6, "world" if world else "camera")
 
 
 @pytest.mark.gpu
@@ -248,7 +230,7 @@ def test_gradients_against_float64_autograd(c4, case):
     for name, x, y in zip(("shape_param", "joint_offset", "full_pose", "expr", "trans"), a, b):
         assert bool(torch.isfinite(x.grad).all()), name
         assert float(y.grad.abs().max()) > 0, name
-        _close(x.grad, y.grad, 2e-6, f"{case} d{name}")
+        assert_close(x.grad, y.grad, 2e-6, f"{case} d{name}")
     if case in ("random", "near_pi"):
         # the root row moves the mesh through the root's rotation about it: with an identity root (the zero pose) a
         # root offset shifts every joint alike and the rel transforms cancel it, so its gradient is then exactly 0
@@ -279,14 +261,9 @@ def test_no_host_sync(c4):
     w = _weights(rig)
     cam = _camera("cuda")
     a = _leaves(_inputs(rig.J, rig.NB, rig.NE, seed=6))
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         (rig.body_mesh(*a, *cam) * w).sum().backward()
         (rig.body_mesh(*a) * w).sum().backward()
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
-    torch.cuda.synchronize()
 
 
 @pytest.mark.gpu
@@ -295,20 +272,17 @@ def test_cuda_graph_replay_equals_eager(c4):
     w = _weights(rig)
     cam = _camera("cuda")
     leaves = [t.cuda().requires_grad_(True) for t in _inputs(rig.J, rig.NB, rig.NE, seed=7)]
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):  # warm-up on the capture stream
-            for x in leaves:
-                x.grad = None
-            (rig.body_mesh(*leaves, *cam) * w).sum().backward()
-    torch.cuda.current_stream().wait_stream(s)
-    for x in leaves:
-        x.grad = None
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
+
+    def step():
         out = rig.body_mesh(*leaves, *cam)
         (out * w).sum().backward()
+        return out
+
+    def no_grads():
+        for x in leaves:
+            x.grad = None
+
+    graph, out = capture(step, 2, reset=no_grads)
     for seed in (8, 9):
         new = _inputs(rig.J, rig.NB, rig.NE, seed=seed, device="cuda")
         with torch.no_grad():
@@ -332,8 +306,8 @@ def test_mesh_against_the_fp32_restatement_of_exavatars_route(c4):
     out = rig.body_mesh(*ins, R, t)
     ref32 = smplx_body_reference(rig.model, *ins, R, t, dtype=torch.float32)
     ref64 = smplx_body_reference(rig.model, *[x.double() for x in ins], R.double(), t.double())
-    _close(ref32, ref64, 1e-6, "fp32 restatement vs float64")
-    _close(out, ref32, 1e-6, "op vs fp32 restatement")
+    assert_close(ref32, ref64, 1e-6, "fp32 restatement vs float64")
+    assert_close(out, ref32, 1e-6, "op vs fp32 restatement")
 
 
 @pytest.mark.gpu

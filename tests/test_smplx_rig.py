@@ -13,7 +13,6 @@ These tests pin
     the C ABI, and the rig in front of nearest_rows, skin_gaussians, TrainingFrameRenderer and l1_ssim.
 """
 import ctypes as C
-import importlib.util
 import math
 import os
 
@@ -21,7 +20,7 @@ import numpy as np
 import pytest
 import torch
 
-from util import workload_settings  # noqa: F401  (path setup)
+from util import assert_close, capture, golden_generator, no_host_sync
 from exavatar_release_b200 import _lib as L
 from exavatar_release_b200.smplx_rig import (axis_angle_to_matrix, matrix_to_axis_angle, smplx_rig_reference,
                                              subdivision_tables, upsample, validate_model)
@@ -30,13 +29,6 @@ from exavatar_release_b200.synthetic import make_human_mesh, make_smplx_model
 FAKE = 0x1000  # never dereferenced: validation fails before any launch
 P_C4 = 167618
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
-
-def _golden_module():
-    spec = importlib.util.spec_from_file_location("make_rig_golden", os.path.join(G, "make_rig_golden.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _small():
@@ -59,7 +51,7 @@ def _inputs(J, NB, NE, seed=0, scale=0.3, device="cpu"):
 
 def test_restatement_reproduces_the_reference_golden():
     """tests/golden/rig.npz was written by the reference's own SMPL-X layer, lbs and module.py lines."""
-    gm = _golden_module()
+    gm = golden_generator("make_rig_golden")
     gold = np.load(os.path.join(G, "rig.npz"))
     _, model, ins, w = gm.rig_case()
     m = validate_model(**model)
@@ -223,12 +215,6 @@ def _leaves(ins, dtype=torch.float32):
     return [t.detach().to("cuda", dtype).requires_grad_(True) for t in ins]
 
 
-def _close(a, b, rel, name):
-    scale = float(b.abs().max())
-    err = float((a.double() - b.double()).abs().max())
-    assert err <= rel * max(scale, 1e-30), f"{name}: max error {err:.3e} vs {rel:.0e} x max {scale:.3e}"
-
-
 @pytest.mark.gpu
 def test_outputs_against_float64(c4):
     rig, cache = c4
@@ -237,10 +223,10 @@ def test_outputs_against_float64(c4):
     out = rig(*ins)
     ref = _ref(rig, cache, ins)
     for name in ("mesh_neutral_pose", "mesh_neutral_pose_wo_upsample", "joint_mats"):
-        _close(getattr(out, name), getattr(ref, name), 1e-6, name)
+        assert_close(getattr(out, name), getattr(ref, name), 1e-6, name)
     # the offsets are fp32 contractions of 486 and 50 signed terms (ExAvatar's own form rounds the same way)
     for name in ("pose_offset", "expr_offset"):
-        _close(getattr(out, name), getattr(ref, name), 1e-5, name)
+        assert_close(getattr(out, name), getattr(ref, name), 1e-5, name)
     assert float((out.pose_6d.double() - ref.pose_6d).abs().max()) <= 1e-6
     outside = ~rig.mask.bool()
     assert int(outside.sum()) > 0 and bool((out.pose_offset[outside] == 0).all())
@@ -265,7 +251,7 @@ def test_gradients_against_float64_autograd(c4, case):
     _loss(_ref(rig, cache, b), [x.double() for x in w]).backward()
     for name, x, y in zip(("shape_param", "joint_offset", "full_pose", "expr"), a, b):
         assert bool(torch.isfinite(x.grad).all()), name
-        _close(x.grad, y.grad, 1e-5, f"{case} d{name}")
+        assert_close(x.grad, y.grad, 1e-5, f"{case} d{name}")
     assert bool((a[1].grad[0] == 0).all())  # get_joint_offset zeroes the root
 
 
@@ -303,13 +289,8 @@ def test_no_host_sync(c4):
     ins = _inputs(rig.J, rig.NB, rig.NE, seed=6)
     w = _loss_weights(rig)
     a = _leaves(ins)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         _loss(rig(*a), w).backward()
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
-    torch.cuda.synchronize()
 
 
 @pytest.mark.gpu
@@ -318,20 +299,17 @@ def test_cuda_graph_replay_equals_eager(c4):
     w = _loss_weights(rig)
     static = [t.cuda() for t in _inputs(rig.J, rig.NB, rig.NE, seed=7)]
     leaves = [t.clone().requires_grad_(True) for t in static]
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):  # warm-up on the capture stream
-            for x in leaves:
-                x.grad = None
-            _loss(rig(*leaves), w).backward()
-    torch.cuda.current_stream().wait_stream(s)
-    for x in leaves:
-        x.grad = None
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
+
+    def step():
         out = rig(*leaves)
         _loss(out, w).backward()
+        return out
+
+    def no_grads():
+        for x in leaves:
+            x.grad = None
+
+    graph, out = capture(step, 2, reset=no_grads)
     for seed in (8, 9):
         new = _inputs(rig.J, rig.NB, rig.NE, seed=seed, device="cuda")
         with torch.no_grad():

@@ -37,6 +37,7 @@ import torch
 from parity import compare
 from test_refined_pass import _close, _plan_classes
 from util import kat_settings, settings_on
+from util import dev  # noqa: F401
 from exavatar_release_b200.plan import RENDERS, merged_bucket_layout
 from exavatar_release_b200.sh import sh_to_rgb
 from oracle import oracle as O
@@ -196,19 +197,10 @@ def test_the_frame_reaches_every_sort_regime(size):
 
 # ------------------------------------------------------------------ GPU ------------------------------------------------
 
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    return torch.device("cuda:0")
-
-
-def _pass_lists(ps, P, W, H):
+def _pass_lists(ps):
     """(ranges (tiles, 2) int64, ids int64) of a pass's workspace."""
-    tiles = ((W + 15) // 16) * ((H + 15) // 16)
-    off = ps.lib.b2r_ctx_ranges(C.byref(ps.ws), P, W, H) - ps.ctx_buf.data_ptr()
-    ranges = ps.ctx_buf[off:off + 8 * tiles].view(torch.int32).view(tiles, 2).cpu().numpy().astype(np.int64)
-    return ranges, ps.ids.cpu().numpy().view(np.uint32).astype(np.int64)
+    ctx = ps.read_ctx()
+    return ctx["ranges"].astype(np.int64), ctx["ids"].astype(np.int64)
 
 
 def _abi_passes(dev, fr, cap_B=None):
@@ -309,10 +301,10 @@ def test_split_lists_equal_the_oracle_in_every_sort_regime(dev, size):
         st = passes[pk].status()
         assert st["overflow"] == 0, pk
         assert np.array_equal(passes[pk].radii.cpu().numpy(), fr["lists"][pk]["radii"]), pk
-    ranges, ids = _pass_lists(passes["A"], P, W, H)
+    ranges, ids = _pass_lists(passes["A"])
     for t, o in enumerate(fr["lists"]["A"]["tiles"]):
         assert np.array_equal(ids[ranges[t, 0]:ranges[t, 1]], o), f"pass A, tile {t}"
-    ranges, ids = _pass_lists(passes["B"], P, W, H)
+    ranges, ids = _pass_lists(passes["B"])
     reached = 0
     for t, o in enumerate(fr["lists"]["B"]["tiles"]):
         got = ids[ranges[t, 0]:ranges[t, 1]]
@@ -336,7 +328,7 @@ def test_split_frame_equals_the_whole_pass_and_five_oracle_renders(dev, size, mo
     lists = {}
     for cls in (Full, Split):
         plan = _run_plan(dev, cls, fr, fr["gcol"])
-        ranges, ids = _pass_lists(plan.passes["B"], P, W, H)
+        ranges, ids = _pass_lists(plan.passes["B"])
         lists[cls.SPLIT] = [ids[a:b] for a, b in ranges]
     n_lists = 0
     for t, o in enumerate(fr["lists"]["B"]["tiles"]):
@@ -406,7 +398,7 @@ def test_an_overflowed_split_pass_keeps_every_list_entry_a_valid_id(dev):
     st = passes["B"].status()
     assert st["overflow"] == 1 and st["num_dups"] == merged
     assert not passes["A"].status()["overflow"]
-    ranges, ids = _pass_lists(passes["B"], P, W, H)
+    ranges, ids = _pass_lists(passes["B"])
     assert ranges.min() >= 0 and ranges.max() <= cap and int((ranges[:, 1] - ranges[:, 0]).sum()) == cap
     for t, (a, b) in enumerate(ranges):
         got = ids[a:b]

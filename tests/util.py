@@ -1,22 +1,69 @@
 """Shared helpers for the test-suite."""
 from __future__ import annotations
 
+import contextlib
+import importlib.util
 import os
 import re
 import sys
 
 import numpy as np
+import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-if ROOT not in sys.path:
-    sys.path.insert(0, ROOT)
+for _p in (ROOT, os.path.join(ROOT, "tools")):
+    if _p not in sys.path:
+        sys.path.insert(0, _p)
 HEADER = os.path.join(ROOT, "include", "b200raster.h")
+GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
 from exavatar_release_b200.renderer import render_settings  # noqa: E402
 from exavatar_release_b200.synthetic import WORKLOADS, make_assets, make_grad_image  # noqa: E402
+from benchkit import capture  # noqa: E402,F401 -- the one warm-up-then-capture protocol, shared with the tools
 from oracle.oracle import OracleSettings  # noqa: E402
+
+
+@pytest.fixture(scope="module")
+def dev():
+    """cuda:0, or a skip without a CUDA device.  Import it (`from util import dev  # noqa: F401`): one per module."""
+    if not torch.cuda.is_available():
+        pytest.skip("needs a CUDA device")
+    return torch.device("cuda:0")
+
+
+@contextlib.contextmanager
+def no_host_sync():
+    """Any host synchronisation inside the block raises (torch's sync debug mode "error").  The device is synchronised
+    before and after, and the mode that was set before is restored."""
+    torch.cuda.synchronize()
+    prev = torch.cuda.get_sync_debug_mode()
+    torch.cuda.set_sync_debug_mode("error")
+    try:
+        yield
+    finally:
+        torch.cuda.set_sync_debug_mode(prev)
+    torch.cuda.synchronize()
+
+
+def golden_generator(name):
+    """tests/golden/<name>.py as a module: the generator of a golden file, whose functions restate the reference."""
+    spec = importlib.util.spec_from_file_location(name, os.path.join(GOLDEN, name + ".py"))
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
+
+
+def assert_close(a, b, rel, name):
+    """max|a - b| <= rel * max|b| (floored at 1e-30), in float64; an empty tensor passes.  Prints the measured error."""
+    a, b = torch.as_tensor(a).detach().double(), torch.as_tensor(b).detach().double()
+    if b.numel() == 0:
+        return
+    err = float((a - b).abs().max())
+    scale = max(float(b.abs().max()), 1e-30)
+    print(f"{name}: max|d| = {err:.3e}  rel {err / scale:.3e}  (limit {rel:.0e})")
+    assert err <= rel * scale, f"{name}: max|d| = {err:.3e} > {rel:.1e} * {scale:.3e}"
 
 
 def kat_settings(W=32, H=32, f=32.0, bg=(0.0, 0.0, 0.0), R=None, t=None, device="cpu", settings_cls=OracleSettings):

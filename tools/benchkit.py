@@ -45,8 +45,9 @@ def arg_parser(doc, iters, frames=None, rounds=5):
     return ap
 
 
-def graph_replay(fn, warmup, reset=None):
-    """`fn` run `warmup` times on a side stream, then `reset()` if given, then captured once in a CUDA graph."""
+def capture(fn, warmup, reset=None):
+    """`fn` run `warmup` times on a side stream, then `reset()` if given, then captured once in a CUDA graph:
+    (the graph, what the captured call of `fn` returned)."""
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(side):
@@ -58,8 +59,13 @@ def graph_replay(fn, warmup, reset=None):
         reset()
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph):
-        fn()
-    return graph.replay
+        out = fn()
+    return graph, out
+
+
+def graph_replay(fn, warmup, reset=None):
+    """The replay of `capture(fn, warmup, reset)`'s graph."""
+    return capture(fn, warmup, reset)[0].replay
 
 
 def alternate(arms, n, rounds, warmup):

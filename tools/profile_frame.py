@@ -47,17 +47,11 @@ def main():
     s = plan.status()
     print("status", s)
     if a.stats:
-        lib = plan.lib
-        import ctypes as C
-        tiles = ((W + 15) // 16) * ((H + 15) // 16)
-        ranges = plan.ctx_buf.cpu().numpy()
-        off = lib.b2r_ctx_ranges(C.byref(plan.ws), P, W, H) - plan.ctx_buf.data_ptr()
-        r = np.frombuffer(ranges[off:off + tiles * 8].tobytes(), dtype=np.uint32).reshape(tiles, 2)
+        ctx = plan.read_ctx()
+        r, nc = ctx["ranges"], ctx["n_contrib"]
         n = (r[:, 1] - r[:, 0]).astype(np.int64)
-        print("tiles", tiles, "D", n.sum(), "max", n.max(), "mean", n.mean(), "pct50/90/99", np.percentile(n, [50, 90, 99]))
+        print("tiles", len(r), "D", n.sum(), "max", n.max(), "mean", n.mean(), "pct50/90/99", np.percentile(n, [50, 90, 99]))
         print("tiles with n>2048:", (n > 2048).sum(), " n>1024:", (n > 1024).sum(), " n>256:", (n > 256).sum(), " n==0:", (n == 0).sum())
-        offn = lib.b2r_ctx_n_contrib(C.byref(plan.ws), P, W, H) - plan.ctx_buf.data_ptr()
-        nc = np.frombuffer(ranges[offn:offn + H * W * 4].tobytes(), dtype=np.uint32).reshape(H, W)
         tmax = nc.reshape(H // 16, 16, W // 16, 16).max(axis=(1, 3)).reshape(-1) if H % 16 == 0 and W % 16 == 0 else None
         if tmax is not None:
             print("n_contrib tile-max: sum", tmax.sum(), "max", tmax.max(), " mean pixel n_contrib", nc.mean())
