@@ -20,6 +20,8 @@ Gaussians' asset dict of SceneGaussian.forward, module.py:253-272), `decode_smpl
 module.py:673-684), `SmplxParamTable` (every frame's SMPL-X parameters in one table, the frame picked on the device),
 `IterationGraph` (a whole training iteration, forward, backward and Adam, as one CUDA graph per key for every frame),
 `FrameTable` (every training frame's image, mask, box and camera on the device, the frame picked by the same slot),
+`MotionTable` and `AvatarAnimator` (a driving motion on the device and a trained avatar animated from it, every video
+frame of animate.py / animate_view_rot.py one CUDA graph replay),
 `HumanAssets` (HumanGaussian's geometry and colour code around its networks, module.py:524-539,561-565
 and model.py:92-96), synthetic workloads and the frame-sharding helper used by bench.py.
 """
@@ -40,6 +42,7 @@ from .animation import OrbitCamera, animation_panel, orbit_points  # noqa: F401
 from .human_assets import HumanAssets, SmplxParamTable, decode_smplx_pose  # noqa: F401
 from .iteration import IterationGraph  # noqa: F401
 from .frames import FrameTable  # noqa: F401
+from .animator import AvatarAnimator, MotionTable  # noqa: F401
 
 
 def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loaded on first use
@@ -53,4 +56,5 @@ __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gau
            "render_settings", "device_render_settings", "TrainingFrameRenderer", "skin_gaussians", "l1_ssim", "nearest_rows", "VertexNormals",
            "FaceMeshRenderer", "ShadedMeshRenderer", "HumanRegularizers", "SmplxRig", "cat_full_pose", "Adam",
            "scene_assets", "LPIPS", "NeumanScores", "face_composite", "test_outputs", "OrbitCamera", "orbit_points", "animation_panel",
-           "decode_smplx_pose", "SmplxParamTable", "HumanAssets", "IterationGraph", "FrameTable"]
+           "decode_smplx_pose", "SmplxParamTable", "HumanAssets", "IterationGraph", "FrameTable",
+           "MotionTable", "AvatarAnimator"]

@@ -155,7 +155,8 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
                                int64_t W, double tanfovx, double tanfovy, const at::Tensor& bg_in, double scale_modifier,
                                const at::Tensor& view_in, const at::Tensor& proj_in, int64_t sh_degree,
                                const at::Tensor& campos_in, bool speculative, double headroom, int64_t fixed_capacity,
-                               bool debug, const c10::optional<at::Tensor>& tanfov_in) {
+                               bool debug, const c10::optional<at::Tensor>& tanfov_in,
+                               const c10::optional<at::Tensor>& status_out) {
     const bool need_grad = means3D_in.requires_grad() || means2D.requires_grad() || (present(sh_in) && sh_in->requires_grad()) ||
                            (present(colors_in) && colors_in->requires_grad()) || opac_in.requires_grad() ||
                            (present(scales_in) && scales_in->requires_grad()) ||
@@ -183,12 +184,18 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
     ctx->saved_data["m3_shape"] = means3D_in.sizes().vec();
     if (P == 0) {  // upstream returns a zero image without launching anything
       color.zero_(); depth.zero_(); alpha.zero_();
+      if (status_out.has_value() && status_out->defined()) status_out->zero_();  // no entries, no overflow
       ctx->mark_non_differentiable({radii});
       return {color, radii, depth, alpha};
     }
     const at::Tensor bg = f32c(bg_in.to(dev), "bg"), view = f32c(view_in.to(dev), "viewmatrix");
     const at::Tensor proj = f32c(proj_in.to(dev), "projmatrix"), campos = f32c(campos_in.to(dev), "campos");
     const at::Tensor tanfov = tanfov_in.has_value() && tanfov_in->defined() ? device_tanfov(*tanfov_in, dev) : at::Tensor();
+    const bool want_status = status_out.has_value() && status_out->defined();
+    if (want_status)
+      TORCH_CHECK(status_out->is_cuda() && status_out->device() == dev && status_out->scalar_type() == at::kByte &&
+                      status_out->is_contiguous() && (size_t)status_out->numel() == sizeof(B2RStatus),
+                  "b200raster: `status` must be ", sizeof(B2RStatus), " contiguous uint8 bytes on the render's device");
     const uint32_t flags = debug ? B2R_FLAG_DEBUG : 0u;
     const B2RScene sc = make_scene(P, H, W, sh_degree, flags, scale_modifier, tanfovx, tanfovy, bg, view, proj, campos,
                                    means3D, shs, colors, opac, scales, rots, cov, tanfov);
@@ -250,6 +257,10 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
       }
       st.predicted[key] = num;
     }
+    // this call's own status block, copied in stream order (a graph node when captured): no host read, no shared state
+    if (want_status)
+      TORCH_CHECK(cudaMemcpyAsync(status_out->data_ptr(), ctx_buf.data_ptr(), sizeof(B2RStatus), cudaMemcpyDeviceToDevice,
+                                  stream) == cudaSuccess, "b200raster: cannot copy the status block");
     sync_if_debug(flags, stream, "b2r_forward");
     // what must survive until backward (SURVEY.md section 8b "Ownership"); undefined tensors are saved as such
     ctx->save_for_backward({means3D, shs, colors, opac, scales, rots, cov, bg, view, proj, campos, ctx_buf, ids, ck, tanfov});
@@ -266,8 +277,8 @@ struct RasterizeFn : public torch::autograd::Function<RasterizeFn> {
   }
 
   static variable_list backward(AutogradContext* ctx, variable_list grads) {
-    // one entry per forward argument: 8 tensors, then 15 settings
-    variable_list out(23);
+    // one entry per forward argument: 8 tensors, then 15 settings and the status output
+    variable_list out(24);
     at::Tensor g_color = grads[0], g_depth = grads[2], g_alpha = grads[3];
     if (!g_color.defined() && !g_depth.defined() && !g_alpha.defined()) return out;
     const int64_t P = ctx->saved_data["P"].toInt();
@@ -345,9 +356,10 @@ std::vector<at::Tensor> rasterize(const at::Tensor& means3D, const at::Tensor& m
                                   const c10::optional<at::Tensor>& cov, int64_t H, int64_t W, double tanfovx, double tanfovy,
                                   const at::Tensor& bg, double scale_modifier, const at::Tensor& view, const at::Tensor& proj,
                                   int64_t sh_degree, const at::Tensor& campos, bool speculative, double headroom,
-                                  int64_t fixed_capacity, bool debug, const c10::optional<at::Tensor>& tanfov) {
+                                  int64_t fixed_capacity, bool debug, const c10::optional<at::Tensor>& tanfov,
+                                  const c10::optional<at::Tensor>& status) {
   return RasterizeFn::apply(means3D, means2D, sh, colors, opac, scales, rots, cov, H, W, tanfovx, tanfovy, bg, scale_modifier,
-                            view, proj, sh_degree, campos, speculative, headroom, fixed_capacity, debug, tanfov);
+                            view, proj, sh_degree, campos, speculative, headroom, fixed_capacity, debug, tanfov, status);
 }
 
 // ---- optim.Adam's step: the walk over the param groups, the state, the scalars and the segment table ----------------
@@ -563,12 +575,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return std::make_tuple(ok, row_len, row_stride);
   }, "(representable, row_len, row_stride) of a param for the Adam step");
   m.def("rasterize", &rasterize, "GaussianRasterizer forward with autograd (compiled host path over libb200raster.so); "
-        "fixed_capacity < 0: adaptive duplicate capacity; tanfov: (2) device tan(fov) in place of tanfovx / tanfovy",
+        "fixed_capacity < 0: adaptive duplicate capacity; tanfov: (2) device tan(fov) in place of tanfovx / tanfovy; "
+        "status: a B2RStatus-sized uint8 CUDA tensor that receives this call's status block, in stream order",
         py::arg("means3D"), py::arg("means2D"), py::arg("sh"), py::arg("colors"), py::arg("opac"), py::arg("scales"),
         py::arg("rots"), py::arg("cov"), py::arg("H"), py::arg("W"), py::arg("tanfovx"), py::arg("tanfovy"), py::arg("bg"),
         py::arg("scale_modifier"), py::arg("view"), py::arg("proj"), py::arg("sh_degree"), py::arg("campos"),
         py::arg("speculative"), py::arg("headroom"), py::arg("fixed_capacity"), py::arg("debug"),
-        py::arg("tanfov") = py::none());
+        py::arg("tanfov") = py::none(), py::arg("status") = py::none());
   m.def("abi_version", []() { return b2r_abi_version(); });
   m.def("recent_contexts", []() {  // ctx buffers of the recent fixed-capacity calls, oldest first
     RecentContexts& r = recent();

@@ -165,17 +165,26 @@ def last_duplicate_count(device: torch.device, P: int, W: int, H: int) -> int:
     return int(n)
 
 
-def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
+_POLICY = object()
+
+
+def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
+                        *, capacity=_POLICY, status: Optional[torch.Tensor] = None):
+    """The public call's body.  `capacity` (keyword) overrides the module's policy for this call only: an int is a
+    fixed capacity, None the adaptive policy; by default `set_fixed_capacity` decides.  `status`, a
+    (sizeof B2RStatus,) uint8 CUDA tensor, receives this call's own status block in stream order (no host read), so a
+    fixed-capacity caller can check its overflow flag later without `overflowed()`."""
     st = raster_settings
     ext = _compiled_binding()
     tanfov = device_tanfov(st)
     tx, ty = (float(st.tanfovx), float(st.tanfovy)) if tanfov is None else (0.0, 0.0)
+    cap = FIXED_CAPACITY if capacity is _POLICY else capacity
     try:
         return tuple(ext.rasterize(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                                    int(st.image_height), int(st.image_width), tx, ty, st.bg,
                                    float(st.scale_modifier), st.viewmatrix, st.projmatrix, int(st.sh_degree), st.campos,
                                    CAPACITY_MODE == "speculative", CAPACITY_HEADROOM,
-                                   -1 if FIXED_CAPACITY is None else FIXED_CAPACITY, bool(st.debug), tanfov))
+                                   -1 if cap is None else int(cap), bool(st.debug), tanfov, status))
     except Exception:
         if st.debug:  # reference behaviour with debug=True: dump the arguments, re-raise
             args = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)

@@ -6,12 +6,19 @@ regularisers as the op, one backward per frame) with the real SMPL-X rig in fron
 joint_mats leaf.  The rig's pose_6d feeds the pose-conditioned stacks, its meshes and offsets build mean_3d /
 mean_3d_refined as module.py:528-539 does, and the template is placed in the frame skin_gaussians poses in, so the
 human is in view.  Each benchmark arm replaces some of the frame's stages with a `FrameArm`.
+
+`SyntheticAvatar` is the same human as a trained avatar for the animation path: what `AvatarAnimator` takes, a motion
+folder of it (`write_motion`), and the full forward and video frame through the ops that the animator must reproduce.
 """
+import json
+import math
 import os
 import sys
 from functools import partial
 from typing import Callable, NamedTuple, Optional
 
+import cv2
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -23,6 +30,11 @@ from bench_human_nets import stack  # noqa: E402
 from bench_human_regs import INPUTS as REG_INPUTS  # noqa: E402
 from bench_human_regs import setup as regs_setup  # noqa: E402
 from exavatar_release_b200 import TrainingFrameRenderer  # noqa: E402
+from exavatar_release_b200.animation import animation_panel, orbit_points  # noqa: E402
+from exavatar_release_b200.human_assets import POSE_KEYS, POSE_ROWS, HumanAssets  # noqa: E402
+from exavatar_release_b200.mesh_render import ShadedMeshRenderer  # noqa: E402
+from exavatar_release_b200.rasterizer import GaussianRasterizer  # noqa: E402
+from exavatar_release_b200.renderer import device_render_settings  # noqa: E402
 from exavatar_release_b200.camera import look_at_cam_param  # noqa: E402
 from exavatar_release_b200.geometry import VertexNormals, nearest_rows  # noqa: E402
 from exavatar_release_b200.human_nets import TriplaneFeatures, gn_mlp  # noqa: E402
@@ -183,3 +195,113 @@ def make_frame(dev, use_graph=True):
             v.grad = None
 
     return frame, fr
+
+
+def write_motion_frame(root, idx, smplx, cam, img):
+    """One frame of a motion folder in the layout ExAvatar's animation scripts read: the SMPL-X parameters and the
+    camera as JSON, the source frame as a PNG."""
+    for sub, d in (("smplx_optimized/smplx_params_smoothed", smplx), ("cam_params", cam)):
+        os.makedirs(os.path.join(root, sub), exist_ok=True)
+        with open(os.path.join(root, sub, f"{idx}.json"), "w") as f:
+            json.dump(d, f)
+    os.makedirs(os.path.join(root, "frames"), exist_ok=True)
+    if not cv2.imwrite(os.path.join(root, "frames", f"{idx}.png"), img):
+        raise OSError(f"cannot write frame {idx}'s PNG under {root}")
+
+
+class SyntheticAvatar:
+    """A trained HumanGaussian of C4 size on the synthetic SMPL-X rig, seeded: rig, triplanes, all four GroupNorm
+    stacks (the offset heads scaled so the Gaussians stay on the body), upsampled skinning weights, masks and the mesh
+    renderer -- what AvatarAnimator takes, and the full forward it must reproduce."""
+
+    def __init__(self, dev):
+        hm = make_human_mesh()
+        model = make_smplx_model(hm)
+        self.rig, d, x, _ = setup(dev, model)
+        self.beta, self.jo, self.pose, self.expr = (t.detach() for t in x)
+        P = self.rig.P
+        self.skw = upsample(d["lbs_weights"], d["sub1"], d["sub2"]).contiguous()
+        self.self_map = hm["self_map"].to(dev)
+        verts = hm["verts"].to(dev)
+        self.tri = TriplaneFeatures(verts, verts[:, 1] > 0.6)
+        self.ha = HumanAssets(model["is_rhand"], model["is_lhand"], model["is_face_expr"], device=dev)
+        self.vn = VertexNormals(hm["faces"], P, flip=hm["flip"].to(dev))
+        self.mesh_r = ShadedMeshRenderer(hm["base_faces"], self.rig.V, device=dev)
+        torch.manual_seed(3)
+        self.nets = {"geo": stack(96, [3, 1]), "geo_offset": stack(96 + 126, [3, 1]), "rgb": stack(96, None, 3),
+                     "rgb_offset": stack(96 + 126 + 3, None, 3)}
+        with torch.no_grad():
+            for k in ("geo", "geo_offset"):
+                mo, sc = self.nets[k][1]
+                mo[0].weight.mul_(1e-3)
+                mo[0].bias.zero_()
+                sc[0].weight.mul_(1e-2)
+                sc[0].bias.fill_(math.log(0.004) if k == "geo" else 0.0)
+        g = torch.Generator().manual_seed(5)
+        self.tp = (0.3 * torch.randn((3, 32, 128, 128), generator=g)).to(dev)
+        self.tpf = (0.3 * torch.randn((3, 32, 128, 128), generator=g)).to(dev)
+
+    def animator(self, motion, **kw):
+        from exavatar_release_b200 import AvatarAnimator
+        return AvatarAnimator(motion, self.rig, self.tri, self.ha, self.mesh_r, triplane=self.tp,
+                              triplane_face=self.tpf, geo_net=self.nets["geo"], rgb_net=self.nets["rgb"],
+                              shape_param=self.beta, joint_offset=self.jo, skinning_weight=self.skw,
+                              self_map=self.self_map, **kw)
+
+    def write_motion(self, root, frame_idx, H, W, near=None):
+        """A motion folder of len(frame_idx) poses, expressions, translations, cameras near the identity and random
+        H x W frames; position `near` has its body 1.5 m closer to the camera."""
+        for i, idx in enumerate(frame_idx):
+            g = torch.Generator().manual_seed(40 + i)
+            pose = (self.pose.cpu() + 0.1 * torch.randn(self.pose.shape, generator=g)).reshape(-1)
+            smplx, r0 = {}, 0
+            for k, n in zip(POSE_KEYS, POSE_ROWS):
+                smplx[k] = pose[3 * r0:3 * (r0 + n)].tolist()
+                r0 += n
+            smplx["expr"] = (self.expr.cpu() + 0.5 * torch.randn(self.expr.shape, generator=g)).tolist()
+            trans = 0.03 * torch.randn(3, generator=g)
+            if i == near:
+                trans[2] -= 1.5
+            smplx["trans"] = trans.tolist()
+            a = 0.1 * torch.randn(2, generator=g).double()
+            Ry = torch.tensor([[math.cos(a[1]), 0.0, math.sin(a[1])], [0.0, 1.0, 0.0],
+                               [-math.sin(a[1]), 0.0, math.cos(a[1])]], dtype=torch.float64)
+            Rx = torch.tensor([[1.0, 0.0, 0.0], [0.0, math.cos(a[0]), -math.sin(a[0])],
+                               [0.0, math.sin(a[0]), math.cos(a[0])]], dtype=torch.float64)
+            cam = {"R": (Rx @ Ry).tolist(), "t": (0.05 * torch.randn(3, generator=g)).tolist(),
+                   "focal": [1.2 * H, 1.2 * H], "princpt": [W / 2, H / 2]}
+            img = np.random.default_rng(i).integers(0, 256, (H, W, 3), dtype=np.uint8)
+            write_motion_frame(root, idx, smplx, cam, img)
+
+    @torch.no_grad()
+    def full_chain(self, fr, i, image_shape, orbit=None):
+        """Video frame i (its position) as HumanGaussian.forward and the scripts compute it, through the existing ops:
+        the rig, the triplane, all four stacks, both sets posed, the refined one's normals and colours computed and
+        discarded, then the render, the body mesh (with `orbit`, an OrbitCamera: its camera and orbit_points), the mesh
+        panel and the video panel.  `fr` holds pose (55,3), expr, trans, cam and frame (H,W,3) uint8 CUDA tensors."""
+        pose, expr, trans, cam = fr["pose"], fr["expr"], fr["trans"], fr["cam"]
+        out = self.rig(self.beta, self.jo, pose, expr)
+        f = self.tri(self.tp, self.tpf)
+        net = lambda k, ins: gn_mlp(ins, *self.nets[k])  # noqa: E731
+        geo, geo_off, rgb = net("geo", [f]), net("geo_offset", [f, out.pose_6d]), net("rgb", [f])
+        ga = self.ha.geometry(out.mesh_neutral_pose, out.pose_offset, out.expr_offset, geo, geo_off)
+        rows = nearest_rows(ga["mean_3d"], out.mesh_neutral_pose_wo_upsample.contiguous(), self.self_map)
+        posed, posed_r = skin_gaussians(ga["mean_3d"], ga["mean_3d_refined"], self.skw, rows, out.joint_mats, trans,
+                                        cam["R"], cam["t"])
+        rgb_c, _ = self.ha.colors(rgb, net("rgb_offset", [f, out.pose_6d, self.vn(posed_r)]))
+        body = (self.beta, self.jo, pose, expr, trans)
+        if orbit is not None:
+            mesh, joints = self.rig.body_mesh(*body, cam["R"], cam["t"], joints=True)
+            render_cam = orbit(cam, joints[0], i)
+            mesh = orbit_points(mesh, orbit, view=True)
+            posed = orbit_points(posed, orbit)
+        else:
+            mesh = self.rig.body_mesh(*body)
+            render_cam = cam
+        dev = posed.device
+        render = GaussianRasterizer(device_render_settings(image_shape, render_cam, torch.ones(3, device=dev)))(
+            means3D=posed, means2D=torch.zeros_like(posed), opacities=self.ha.opacity, colors_precomp=rgb_c,
+            scales=ga["scale"], rotations=self.ha.rotation)[0]
+        mesh_panel = self.mesh_r(mesh, cam, torch.full((*image_shape, 3), 255.0, device=dev))
+        return {"mean_3d": posed, "scale": ga["scale"], "rgb": rgb_c, "render": render, "mesh_panel": mesh_panel,
+                "panel": animation_panel(fr["frame"], mesh_panel, render)}
