@@ -21,7 +21,8 @@ module.py:673-684), `SmplxParamTable` (every frame's SMPL-X parameters in one ta
 `IterationGraph` (a whole training iteration, forward, backward and Adam, as one CUDA graph per key for every frame),
 `FrameTable` (every training frame's image, mask, box and camera on the device, the frame picked by the same slot),
 `MotionTable` and `AvatarAnimator` (a driving motion on the device and a trained avatar animated from it, every video
-frame of animate.py / animate_view_rot.py one CUDA graph replay),
+frame of animate.py / animate_view_rot.py one CUDA graph replay), `SegmentationTable` and `AvatarTester` (eval_neuman's
+foreground masks on the device and the test pass of test.py + eval_neuman.py, every held-out frame one CUDA graph replay),
 `HumanAssets` (HumanGaussian's geometry and colour code around its networks, module.py:524-539,561-565
 and model.py:92-96), synthetic workloads and the frame-sharding helper used by bench.py.
 """
@@ -41,8 +42,9 @@ from .compose import face_composite, test_outputs  # noqa: F401
 from .animation import OrbitCamera, animation_panel, orbit_points  # noqa: F401
 from .human_assets import HumanAssets, SmplxParamTable, decode_smplx_pose  # noqa: F401
 from .iteration import IterationGraph  # noqa: F401
-from .frames import FrameTable  # noqa: F401
+from .frames import FrameTable, SegmentationTable  # noqa: F401
 from .animator import AvatarAnimator, MotionTable  # noqa: F401
+from .tester import AvatarTester  # noqa: F401
 
 
 def __getattr__(name):  # TrainingFrameRenderer pulls in the plan machinery; loaded on first use
@@ -57,4 +59,4 @@ __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gau
            "FaceMeshRenderer", "ShadedMeshRenderer", "HumanRegularizers", "SmplxRig", "cat_full_pose", "Adam",
            "scene_assets", "LPIPS", "NeumanScores", "face_composite", "test_outputs", "OrbitCamera", "orbit_points", "animation_panel",
            "decode_smplx_pose", "SmplxParamTable", "HumanAssets", "IterationGraph", "FrameTable",
-           "MotionTable", "AvatarAnimator"]
+           "MotionTable", "AvatarAnimator", "SegmentationTable", "AvatarTester"]

@@ -265,6 +265,13 @@ class B2RFrameTable(C.Structure):
                 *[(n, _fp) for n in ("pixels", "bbox", "R", "t", "focal", "princpt", "frame_idx", "slot_row", "slot")]]
 
 
+class B2RSegmentation(C.Structure):
+    """eval_neuman's segmentation bytes of every frame, in a frame table's rows (b2r_segmentation_unpack)."""
+    ID = 34
+    _fields_ = [("n_rows", C.c_int32), ("n_slots", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
+                ("host_slot", C.c_int32), ("reserved", C.c_int32), ("pixels", _fp), ("slot_row", _fp), ("slot", _fp)]
+
+
 class B2RHumanAssets(C.Structure):
     """HumanGaussian's geometry around its networks (b2r_human_geometry_forward / b2r_human_geometry_backward)."""
     ID = 21
@@ -398,6 +405,7 @@ SYMBOLS = [
     ("b2r_param_table_forward", C.c_int, [C.POINTER(B2RSmplxParamTable), _fp, _fp, _fp, _fp]),
     ("b2r_param_table_backward", C.c_int, [C.POINTER(B2RSmplxParamTable), C.POINTER(B2RSmplxParamTableGrads), _fp]),
     ("b2r_frame_unpack", C.c_int, [C.POINTER(B2RFrameTable), _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
+    ("b2r_segmentation_unpack", C.c_int, [C.POINTER(B2RSegmentation), _fp, _fp]),
     ("b2r_human_geometry_forward", C.c_int, [C.POINTER(B2RHumanAssets), _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     ("b2r_human_geometry_backward", C.c_int, [C.POINTER(B2RHumanAssets), C.POINTER(B2RHumanAssetsGrads), _fp]),
     ("b2r_human_colors_forward", C.c_int, [C.c_int32, _fp, _fp, _fp, _fp, _fp]),

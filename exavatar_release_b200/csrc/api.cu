@@ -116,6 +116,14 @@ int validate_frame_table(const B2RFrameTable* t) {
   return B2R_OK;
 }
 
+// a segmentation table's sizes and arrays, and the host slot when no device slot is given (as a frame table's)
+int validate_segmentation(const B2RSegmentation* s) {
+  if (!s || !s->pixels || !s->slot_row) return B2R_E_INVALID;
+  if (s->n_rows < 1 || s->n_slots < 1 || s->height < 1 || s->width < 1) return B2R_E_INVALID;
+  if (!s->slot && (s->host_slot < 0 || s->host_slot >= s->n_slots)) return B2R_E_INVALID;
+  return B2R_OK;
+}
+
 // sizes, row strides and every input pointer (an empty set reads nothing)
 int validate_human_assets(const B2RHumanAssets* h) {
   if (!h || h->P < 0 || (h->warmup != 0 && h->warmup != 1)) return B2R_E_INVALID;
@@ -300,6 +308,7 @@ size_t b2r_sizeof(int which) {
     case 31: return sizeof(B2RSmplxParamTable);  // 30 stays unused
     case 32: return sizeof(B2RSmplxParamTableGrads);
     case 33: return sizeof(B2RFrameTable);
+    case 34: return sizeof(B2RSegmentation);
     default: return 0;
   }
 }
@@ -840,6 +849,13 @@ int b2r_frame_unpack(const B2RFrameTable* table, float* img, float* mask, float*
   if (rc) return rc;
   if (!img || !mask || !bbox || !R || !t || !focal || !princpt || !frame_idx) return B2R_E_INVALID;
   return launch_frame_unpack(*table, img, mask, bbox, R, t, focal, princpt, frame_idx, (cudaStream_t)stream);
+}
+
+int b2r_segmentation_unpack(const B2RSegmentation* seg, float* mask, void* stream) {
+  const int rc = validate_segmentation(seg);
+  if (rc) return rc;
+  if (!mask) return B2R_E_INVALID;
+  return launch_segmentation_unpack(*seg, mask, (cudaStream_t)stream);
 }
 
 int b2r_human_geometry_forward(const B2RHumanAssets* h, float* mean_3d, float* mean_3d_refined, float* scale,

@@ -681,6 +681,7 @@ int launch_param_table_forward(const B2RSmplxParamTable& t, float* full_pose, fl
 int launch_param_table_backward(const B2RSmplxParamTable& t, const B2RSmplxParamTableGrads& g, cudaStream_t st);
 int launch_frame_unpack(const B2RFrameTable& t, float* img, float* mask, float* bbox, float* R, float* tr, float* focal,
                         float* princpt, int64_t* frame_idx, cudaStream_t st);
+int launch_segmentation_unpack(const B2RSegmentation& s, float* mask, cudaStream_t st);
 int launch_human_geometry_forward(const B2RHumanAssets& h, float* mean, float* mean_r, float* scale, float* scale_r,
                                   float* mmo, float* scale_wo, float* scale_r_wo, cudaStream_t st);
 int launch_human_geometry_backward(const B2RHumanAssets& h, const B2RHumanAssetsGrads& g, cudaStream_t st);

@@ -25,7 +25,9 @@ from __future__ import annotations
 
 import ctypes as C
 import numbers
+import os
 
+import numpy as np
 import torch
 from torch.utils.data import DataLoader, Dataset
 
@@ -285,3 +287,113 @@ class FrameTable:
               *(L.ptr(meta[name]) for name, _ in META), L.ptr(frame_idx))
         return {"img": img, "mask": mask, "bbox": meta["bbox"],
                 "cam_param": {k: meta[k] for k in ("R", "t", "focal", "princpt")}, "frame_idx": frame_idx}
+
+
+def _device_slot(fn: str, slot, table) -> tuple:
+    """(slot tensor or None, host slot) of a FrameTable-style call, checked as `FrameTable.__call__` checks it."""
+    if isinstance(slot, torch.Tensor):
+        L.cuda(fn, "slot", slot, table.device)
+        if slot.dtype != torch.int32 or slot.numel() != 1 or not slot.is_contiguous():
+            raise ValueError(f"{fn}: a tensor `slot` must be one contiguous int32 value, got {slot.dtype} "
+                             f"{tuple(slot.shape)}")
+        return slot, 0
+    if isinstance(slot, numbers.Integral) and not isinstance(slot, bool):
+        if not 0 <= int(slot) < table.n_slots:
+            raise IndexError(f"{fn}: slot {int(slot)} outside [0, {table.n_slots})")
+        if table._row[int(slot)] < 0:
+            raise IndexError(f"{fn}: slot {int(slot)} ({table.frames[int(slot)]!r}) has no frame in the table")
+        return None, int(slot)
+    raise ValueError(f"{fn}: `slot` must be an int or a (1,) int32 CUDA tensor, got {type(slot).__name__}")
+
+
+def read_segmentations(root: str, frame_ids, size) -> list:
+    """The host half of `SegmentationTable.from_folder`: `cv2.imread(root/segmentations/%05d.png)` of each frame in
+    `frame_ids`, in order, as uint8 (H, W, 3) BGR arrays, nothing uploaded.  Raises ValueError naming the frame for a
+    missing or unreadable file, and for an image whose (H, W) is not `size` (the frame table's)."""
+    import cv2
+    out = []
+    for f in frame_ids:
+        path = os.path.join(root, "segmentations", "%05d.png" % int(f))
+        img = cv2.imread(path) if os.path.isfile(path) else None
+        if img is None:
+            raise ValueError(f"SegmentationTable: frame {int(f)}: missing or unreadable {path}")
+        if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
+            raise ValueError(f"SegmentationTable: frame {int(f)}: {path} does not read as 8-bit BGR")
+        if tuple(img.shape[:2]) != tuple(size):
+            raise ValueError(f"SegmentationTable: frame {int(f)}: {path} is {img.shape[0]}x{img.shape[1]}, the "
+                             f"frames {size[0]}x{size[1]}")
+        out.append(img)
+    return out
+
+
+def _upload_segmentations(images, device) -> torch.Tensor:
+    """The (N, H, W, 4) uint8 table of BGR + pad byte, every image up through one pinned staging buffer."""
+    H, W = images[0].shape[:2]
+    if device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(device):
+        pixels = torch.empty((len(images), H, W, 4), dtype=torch.uint8, device=device)
+        staging = torch.zeros((H, W, 4), dtype=torch.uint8, pin_memory=True)
+        done = torch.cuda.Event()
+        for r, img in enumerate(images):
+            if r:
+                done.synchronize()  # the previous image's copy has read the staging buffer
+            staging[:, :, :3].copy_(torch.from_numpy(img))
+            pixels[r].copy_(staging, non_blocking=True)
+            done.record()
+        torch.cuda.current_stream(device).synchronize()
+    return pixels
+
+
+class SegmentationTable:
+    """eval_neuman's foreground mask of every frame of a `FrameTable`, on its device, in its rows: `table(slot)` is
+    `torch.FloatTensor(1 - cv2.imread(segmentations/%05d.png) / 255.).permute(2,0,1)[None]` of the slot's frame, one
+    launch (csrc/frames.cu b2r_segmentation_unpack).
+
+        masks = SegmentationTable.from_folder(subject_root, frames, "cuda")
+        mask = masks(slot_t)            # (1,3,H,W) fp32, 1 = human; channels in cv2's BGR order, as eval uses them
+
+    Storage: pixels (N, H, W, 4) uint8, the BGR bytes and a zero pad byte per pixel (8.3 MB per 1080 x 1920 frame,
+    against 24.9 MB for the fp32 mask).  The slot -> row map is the frame table's own, so one device slot reads the
+    same frame from both tables.  eval flips its images from BGR to RGB but not the mask, so the mask's B plane
+    multiplies the images' R plane; `table(slot)` keeps that."""
+
+    def __init__(self, pixels: torch.Tensor, frames: FrameTable):
+        fn = "SegmentationTable"
+        L.cuda(fn, "pixels", pixels, frames.device)
+        if pixels.dtype != torch.uint8 or not pixels.is_contiguous() or \
+                tuple(pixels.shape) != (frames.n_rows, frames.height, frames.width, 4):
+            raise ValueError(f"{fn}: `pixels` must be contiguous uint8 ({frames.n_rows}, {frames.height}, "
+                             f"{frames.width}, 4), got {pixels.dtype} {tuple(pixels.shape)}")
+        self.pixels, self.frames = pixels, frames
+        self.device = frames.device
+
+    @classmethod
+    def from_folder(cls, root: str, frames: FrameTable, device) -> "SegmentationTable":
+        """The masks of `frames`' rows, read as eval_neuman reads them (`read_segmentations`: every file is checked
+        before anything is uploaded), uploaded one frame at a time through a pinned staging buffer.  `device` must be
+        the frame table's."""
+        fn = "SegmentationTable.from_folder"
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise RuntimeError(f"{fn}: the table lives on a CUDA device, got {device}; there is no CPU fallback")
+        images = read_segmentations(root, frames.frame_idx.tolist(), (frames.height, frames.width))
+        return cls(_upload_segmentations(images, device), frames)
+
+    @property
+    def nbytes(self) -> int:
+        return self.pixels.numel()
+
+    def __call__(self, slot) -> torch.Tensor:
+        """eval's mask of the frame in `slot`, a fresh (1,3,H,W) fp32 tensor.  `slot` as `FrameTable` takes it: a host
+        int (IndexError outside [0, F) or for a slot without a frame) or a one-element int32 CUDA tensor read on the
+        device, for which a slot outside [0, F) or without a frame gives NaN.  Nothing is read back to the host."""
+        fn = "SegmentationTable"
+        ft = self.frames
+        slot_t, host_slot = _device_slot(fn, slot, ft)
+        mask = torch.empty((1, 3, ft.height, ft.width), dtype=torch.float32, device=self.device)
+        st = L.B2RSegmentation(n_rows=ft.n_rows, n_slots=ft.n_slots, height=ft.height, width=ft.width,
+                               host_slot=host_slot, pixels=L.ptr(self.pixels), slot_row=L.ptr(ft.slot_row),
+                               slot=L.ptr(slot_t))
+        L.run("b2r_segmentation_unpack", self.device, C.byref(st), L.ptr(mask))
+        return mask

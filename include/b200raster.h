@@ -212,8 +212,8 @@ int b2r_last_cuda_error(void);
  * 12 B2RRegsGrads, 13 B2RRig, 14 B2RRigGrads, 15 B2RAdamSegment, 16 B2RLpips, 17 B2RSceneAssets,
  * 18 B2RSceneAssetsGrads, 19 B2RSmplxPose, 20 B2RSmplxPoseGrads, 21 B2RHumanAssets, 22 B2RHumanAssetsGrads,
  * 23 B2RSmplxBody, 24 B2RSmplxBodyGrads, 25 B2RNeumanScores, 26 B2RFaceComposite, 27 B2RTestOutputs,
- * 28 B2ROrbitCamera, 29 B2RAnimationPanel, 31 B2RSmplxParamTable, 32 B2RSmplxParamTableGrads, 33 B2RFrameTable
- * (30 unused); 0 for anything else
+ * 28 B2ROrbitCamera, 29 B2RAnimationPanel, 31 B2RSmplxParamTable, 32 B2RSmplxParamTableGrads, 33 B2RFrameTable,
+ * 34 B2RSegmentation (30 unused); 0 for anything else
  * (7 and 9 are unused and report 0). */
 size_t b2r_sizeof(int which);
 
@@ -936,6 +936,24 @@ typedef struct B2RFrameTable {
 int b2r_frame_unpack(const B2RFrameTable* table, float* img, float* mask, float* bbox, float* R, float* t,
                      float* focal, float* princpt, int64_t* frame_idx, void* stream);
 
+/* eval_neuman's foreground mask of every frame of a split, in a frame table's rows (exavatar_release_b200/frames.py
+ * SegmentationTable): row r holds pixels (height, width, 4) uint8 -- the B, G, R bytes cv2.imread gives for the frame's
+ * segmentations/%05d.png, then one pad byte; (n_rows, ...), device, contiguous.  slot_row, slot and host_slot are the
+ * frame table's (B2RFrameTable), so one device slot reads the same frame from both tables.
+ * b2r_segmentation_unpack writes mask (3, height, width) planar: channel c of a pixel is fl32(1 - k / 255.) of its
+ * byte c, evaluated in double and rounded once (eval's `torch.FloatTensor(1 - cv2.imread(seg) / 255.)`), channels in
+ * cv2's BGR order, not reversed (eval flips its images but not the mask).  A slot outside [0, n_slots) or without a row
+ * reads no row: every output is NaN.  One launch; a thread owns 4 pixels, and with height * width a multiple of 4 and
+ * 16-byte aligned pixels and mask it loads 16 bytes and stores one float4 per plane.  No allocation, no sync. */
+typedef struct B2RSegmentation {
+  int32_t n_rows, n_slots, height, width, host_slot, reserved;
+  const uint8_t* pixels;
+  const int32_t* slot_row;
+  const int32_t* slot;
+} B2RSegmentation;
+
+int b2r_segmentation_unpack(const B2RSegmentation* seg, float* mask, void* stream);
+
 /* HumanGaussian's geometry around its networks (avatar/common/nets/module.py:524-539 with get_mean_offset_offset's
  * mask, :489-493, and model.py:92-96's warm-up clamp), per Gaussian p of P, in ExAvatar's fp32 operations and order:
  *   m = mesh + geo[0:3];  mmo = geo_offset[0:3] * (1 - mask);  mean_3d = m + expr_offset;
@@ -1005,7 +1023,7 @@ int b2r_camera_setup(const float* R, const float* t, const float* focal, int32_t
 int b2r_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, uint8_t* present, void* stream);
 
 /* Measurement hooks (host side).  Kernel ids: 0 project, 1 tile_scan, 2 scatter, 3 sort (all lists, long ones in chunks), 4 sort_merge (chunks of the long lists),
- * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_neuman_scores, b2r_face_composite_*, b2r_test_outputs, b2r_orbit_*, b2r_animation_panel, b2r_scene_assets_*, b2r_decode_pose_*, b2r_param_table_*, b2r_frame_unpack and b2r_human_* kernels).  With profiling on, every kernel launch
+ * 5 composite_fwd, 6 composite_bwd, 7 project_bwd, 8 misc (status reset, b2r_camera_setup, the b2r_skin_*, b2r_l1ssim_*, b2r_nearest_rows, b2r_vertex_normals, b2r_mesh_render_*, b2r_mesh_shade_forward, b2r_triplane_*, b2r_gn_mlp_*, b2r_regs_*, b2r_rig_*, b2r_smplx_body_*, b2r_adam_step, b2r_lpips_*, b2r_neuman_scores, b2r_face_composite_*, b2r_test_outputs, b2r_orbit_*, b2r_animation_panel, b2r_scene_assets_*, b2r_decode_pose_*, b2r_param_table_*, b2r_frame_unpack, b2r_segmentation_unpack and b2r_human_* kernels).  With profiling on, every kernel launch
  * is bracketed by CUDA events on the caller's stream; b2r_profile_read() waits for them and returns the summed
  * milliseconds and launch counts per kernel id (arrays of B2R_NUM_KERNELS).  b2r_launch_count() counts kernel
  * launches made by this library since it was loaded, profiling or not. */

@@ -9,6 +9,8 @@ human is in view.  Each benchmark arm replaces some of the frame's stages with a
 
 `SyntheticAvatar` is the same human as a trained avatar for the animation path: what `AvatarAnimator` takes, a motion
 folder of it (`write_motion`), and the full forward and video frame through the ops that the animator must reproduce.
+For the test pass it also builds a test split's tables, scene and face inputs (`test_setup`), the `AvatarTester` over
+them, and `test_chain`, Model.forward(mode='test') eagerly through the ops, which the tester must reproduce.
 """
 import json
 import math
@@ -305,3 +307,153 @@ class SyntheticAvatar:
         mesh_panel = self.mesh_r(mesh, cam, torch.full((*image_shape, 3), 255.0, device=dev))
         return {"mean_3d": posed, "scale": ga["scale"], "rgb": rgb_c, "render": render, "mesh_panel": mesh_panel,
                 "panel": animation_panel(fr["frame"], mesh_panel, render)}
+
+    def test_setup(self, root, frame_idx, H, W, capacity, n_scene=None, slots=None):
+        """A test split of len(frame_idx) frames at H x W written under `root` (segmentations/%05d.png) and read into
+        the device tables, the C4 scene, the face render's inputs and a TrainingFrameRenderer(use_graph=False) of
+        `capacity` list entries per pass.  The SMPL-X table has the slots `slots` (default the split's frames in
+        reverse order plus one frame that is not in the split), so table rows and slots differ."""
+        from exavatar_release_b200 import FaceMeshRenderer, FrameTable, SegmentationTable, SmplxParamTable
+        from exavatar_release_b200.synthetic import make_face_mesh
+        dev = self.beta.device
+        n_scene = WORKLOADS["C4"].n_scene if n_scene is None else n_scene
+        slots = [str(f) for f in reversed(frame_idx)] + ["777777"] if slots is None else slots
+        params, imgs, cams = {}, [], []
+        for key in slots:
+            g = torch.Generator().manual_seed(1000 + int(key) % 9973)
+            pose = self.pose.cpu() + 0.1 * torch.randn(self.pose.shape, generator=g)
+            six = matrix_to_rotation_6d(axis_angle_to_matrix(pose.to(torch.float64))).to(torch.float32)
+            d, r0 = {}, 0
+            for k, n in zip(POSE_KEYS, POSE_ROWS):
+                d[k] = six[r0:r0 + n].reshape(6) if n == 1 else six[r0:r0 + n].clone()
+                r0 += n
+            d["expr"] = self.expr.cpu() + 0.5 * torch.randn(self.expr.shape, generator=g)
+            d["trans"] = 0.03 * torch.randn(3, generator=g)
+            params[key] = {k: v.to(dev) for k, v in d.items()}
+        for i, idx in enumerate(frame_idx):
+            g = torch.Generator().manual_seed(40 + i)
+            a = 0.1 * torch.randn(2, generator=g).double()
+            Ry = torch.tensor([[math.cos(a[1]), 0.0, math.sin(a[1])], [0.0, 1.0, 0.0],
+                               [-math.sin(a[1]), 0.0, math.cos(a[1])]], dtype=torch.float64)
+            Rx = torch.tensor([[1.0, 0.0, 0.0], [0.0, math.cos(a[0]), -math.sin(a[0])],
+                               [0.0, math.sin(a[0]), math.cos(a[0])]], dtype=torch.float64)
+            cams.append({"R": (Rx @ Ry).float().numpy(), "t": (0.05 * torch.randn(3, generator=g)).numpy(),
+                         "focal": np.array([1.2 * H, 1.2 * H], np.float32),
+                         "princpt": np.array([W / 2, H / 2], np.float32)})
+            imgs.append(np.random.default_rng(i).integers(0, 256, (H, W, 3), dtype=np.uint8))
+            write_segmentation(root, idx, H, W, seed=100 + i)
+        table = SmplxParamTable.from_param_dict(params)
+        frames = FrameTable.from_dataset(TestSplit(frame_idx, imgs, cams), dev, slots=table.frames, workers=0)
+        masks = SegmentationTable.from_folder(root, frames, dev)
+        scene = _test_scene(dev, n_scene)
+        fm = make_face_mesh()
+        face_r = FaceMeshRenderer(fm["vertex_uv"], fm["face_uv"], fm["faces"], fm["vertex_idx"].shape[0], device=dev)
+        renderer = TrainingFrameRenderer(n_scene, self.rig.P, (H, W), dev, {"A": capacity, "B": capacity})
+        return TestSetup(frames, table, masks, scene, torch.tensor([3.0], device=dev), face_r,
+                         fm["texture"].to(dev)[None].contiguous(), fm["vertex_idx"].to(dev), renderer)
+
+    def tester(self, s, **kw):
+        """An AvatarTester of this avatar over the TestSetup `s` (keyword arguments: scorer, masks, png, ...)."""
+        from exavatar_release_b200 import AvatarTester
+        return AvatarTester(s.frames, s.params, self.rig, self.tri, self.ha, self.vn, s.face_renderer, s.renderer,
+                            triplane=self.tp, triplane_face=self.tpf, geo_net=self.nets["geo"],
+                            geo_offset_net=self.nets["geo_offset"], rgb_net=self.nets["rgb"],
+                            rgb_offset_net=self.nets["rgb_offset"], shape_param=self.beta, joint_offset=self.jo,
+                            skinning_weight=self.skw, self_map=self.self_map, scene=s.scene,
+                            active_sh_degree=s.sh_degree, face_uvmap=s.face_uvmap, face_vertex_idx=s.face_vertex_idx,
+                            **kw)
+
+    @torch.no_grad()
+    def test_chain(self, s, slot, png=True):
+        """Model.forward(mode='test') of the frame in host slot `slot` of TestSetup `s`, eagerly through the ops with
+        the tables read by host slot: the frame, its SMPL-X parameters, the rig, the triplane, all four stacks,
+        geometry without the warm-up clamp, both sets posed, normals and colours, the scene in rgb mode with the
+        frame's camera, the device camera, the five renders with bg_human = ones, the two face renders and
+        test_outputs.  Returns test_outputs' dict plus "gt" (1,3,H,W)."""
+        from exavatar_release_b200 import scene_assets, test_outputs
+        data = s.frames(slot)
+        cam = {k: v[0] for k, v in data["cam_param"].items()}
+        sp = s.params(slot)
+        out = self.rig(self.beta, self.jo, sp["full_pose"], sp["expr"])
+        f = self.tri(self.tp, self.tpf)
+        net = lambda k, ins: gn_mlp(ins, *self.nets[k])  # noqa: E731
+        geo, geo_off, rgb = net("geo", [f]), net("geo_offset", [f, out.pose_6d]), net("rgb", [f])
+        ga = self.ha.geometry(out.mesh_neutral_pose, out.pose_offset, out.expr_offset, geo, geo_off, warmup=False)
+        rows = nearest_rows(ga["mean_3d"], out.mesh_neutral_pose_wo_upsample.contiguous(), self.self_map)
+        posed, posed_r = skin_gaussians(ga["mean_3d"], ga["mean_3d_refined"], self.skw, rows, out.joint_mats,
+                                        sp["trans"], cam["R"], cam["t"])
+        rgb_c, rgb_r = self.ha.colors(rgb, net("rgb_offset", [f, out.pose_6d, self.vn(posed_r)]))
+        human = dict(mean_3d=posed, opacity=self.ha.opacity, scale=ga["scale"], rotation=self.ha.rotation, rgb=rgb_c)
+        refined = dict(mean_3d=posed_r, opacity=self.ha.opacity, scale=ga["scale_refined"], rotation=self.ha.rotation,
+                       rgb=rgb_r)
+        sc = s.scene
+        scene = scene_assets(sc["mean"], sc["opacity_logit"], sc["log_scale"], sc["rotation6d"], sc["feature_dc"],
+                             sc["feature_rest"], s.sh_degree, cam)
+        shape = (s.frames.height, s.frames.width)
+        ones = torch.ones(3, device=posed.device)
+        renders = s.renderer(scene, human, refined, cam, ones, raster_settings=device_render_settings(shape, cam, ones))
+        face = s.face_renderer(s.face_uvmap, posed[None, s.face_vertex_idx, :], cam, shape)
+        face_r = s.face_renderer(s.face_uvmap, posed_r[None, s.face_vertex_idx, :], cam, shape)
+        res = test_outputs(renders, face, face_r, gt=data["img"], png=png)
+        res["gt"] = data["img"]
+        return res
+
+
+class TestSplit:
+    """An ExAvatar-shaped test split held in memory, for `FrameTable.from_dataset`: `frame_idx_list` and dataset[i]'s
+    dict of img (3,H,W) k / 255, mask, bbox and the frame's camera."""
+
+    def __init__(self, frame_idx, imgs, cams):
+        self.frame_idx_list = list(frame_idx)
+        self.imgs, self.cams = imgs, cams
+
+    def __len__(self):
+        return len(self.frame_idx_list)
+
+    def __getitem__(self, i):
+        img = self.imgs[i]  # (H, W, 3) RGB bytes
+        H, W = img.shape[:2]
+        return {"img": torch.from_numpy(img.transpose(2, 0, 1).astype(np.float32)) / 255.,
+                "mask": torch.ones((1, H, W), dtype=torch.float32),
+                "bbox": np.array([0, 0, W, H], np.float32), "cam_param": self.cams[i],
+                "frame_idx": self.frame_idx_list[i]}
+
+
+class TestSetup(NamedTuple):
+    """What `AvatarTester` takes besides the avatar: the split's tables, the scene and the face render's inputs."""
+    frames: object  # FrameTable
+    params: object  # SmplxParamTable
+    masks: object   # SegmentationTable
+    scene: dict     # scene_assets' raw parameters (tester.SCENE_KEYS)
+    sh_degree: torch.Tensor
+    face_renderer: object
+    face_uvmap: torch.Tensor
+    face_vertex_idx: torch.Tensor
+    renderer: object
+
+
+def write_segmentation(root, idx, H, W, seed):
+    """segmentations/%05d.png in `root`: 0 on a box around the body, 255 elsewhere, and a matte-like edge noise that
+    differs between the three channels (so a channel swap changes eval's mask)."""
+    rng = np.random.default_rng(seed)
+    seg = np.full((H, W, 3), 255, np.uint8)
+    seg[H // 8:7 * H // 8, W // 4:3 * W // 4] = 0
+    noisy = rng.random((H, W)) < 0.1
+    seg[noisy] = rng.integers(0, 256, (int(noisy.sum()), 3), dtype=np.uint8)
+    os.makedirs(os.path.join(root, "segmentations"), exist_ok=True)
+    if not cv2.imwrite(os.path.join(root, "segmentations", "%05d.png" % idx), seg):
+        raise OSError(f"cannot write frame {idx}'s segmentation under {root}")
+    return seg
+
+
+def _test_scene(dev, n, seed=11, sh_degree=3):
+    """A seeded scene in front of the test cameras, as SceneGaussian stores it: scene_assets' raw parameters."""
+    c4 = WORKLOADS["C4"]
+    scene, _, _ = make_population_assets(Workload("C4 scene", c4.height, c4.width, 0, n, 0, True), seed=seed)
+    g = torch.Generator().manual_seed(seed)
+    M = (sh_degree + 1) ** 2
+    p = {"mean": scene["mean_3d"], "opacity_logit": torch.logit(scene["opacity"].clamp(1e-4, 1 - 1e-4)),
+         "log_scale": torch.log(scene["scale"]), "rotation6d": torch.randn(n, 6, generator=g),
+         "feature_dc": ((scene["rgb"] - 0.5) / 0.28209479177387814).reshape(n, 1, 3),
+         "feature_rest": 0.3 * torch.randn(n, M - 1, 3, generator=g)}
+    return {k: v.to(dev).contiguous() for k, v in p.items()}
