@@ -33,12 +33,18 @@ struct B4Stage {
   float4 b[B4_BATCH];  // C2, opacity, depth, thr2
   float4 c[B4_BATCH];  // r, g, b, id | clamp bits << 29
 };
-constexpr int B4_GROUP = 4;   // splats replayed per trip of the hit loop (their evaluations overlap: ILP 4)
-constexpr int B4_CQ = 32 + B4_GROUP;  // circular survivor queue: < B4_GROUP left over + 32 new per chunk; a multiple of B4_GROUP
+// splats replayed per trip of the hit loop (their evaluations overlap).  2 rather than 4 or 8: measured on an H100,
+// the C2 backward composite takes 82 / 100 / 170 us with groups of 2 / 4 / 8, although a group of 2 issues the most
+// instructions per splat (DESIGN.md section 3.3)
+constexpr int B4_GROUP = 2;
+// Circular survivor queue.  A replayed survivor keeps its slot until phase B has read its record from there, so the queue
+// holds < B4_QUEUE replayed-but-not-drained survivors, < B4_GROUP left over and 32 new per chunk.  A multiple of B4_GROUP.
+constexpr int B4_CQ = 32 + B4_QUEUE;
 struct B4Compact {            // warp-private circular queue of cull survivors, back to front
   float4 r[3][B4_CQ];         // [0] px,py,A2,B2  [1] C2,opacity,depth,list position (int bits)  [2] r,g,b,id bits
 };
 static_assert(B4_QUEUE % B4_GROUP == 0, "phase B runs when whole groups fill the transposition queue");
+static_assert(B4_CQ % B4_GROUP == 0, "a group never straddles the wrap of the survivor queue");
 
 __device__ __forceinline__ float rcp_approx4(float x) {
   float y;
@@ -50,8 +56,6 @@ struct B4Smem {
   B4Stage stage[2];
   B4Compact compact[2];
   float2 tb[2][B4_QUEUE][33];  // [warp][queued splat][pixel], padded rows: conflict-free both ways
-  float4 qm0[2][B4_QUEUE];     // px, py, A2, B2
-  float4 qm1[2][B4_QUEUE];     // C2, opacity, id bits, -
   float4 gpix[2][32];          // per pixel of the warp: g_r, g_g, g_b, g_depth
   int warp_max_s[2];
 };
@@ -64,8 +68,6 @@ __device__ __forceinline__ void bwd4_item(const B2RScene& sc, const Ctx& cx, con
   B4Stage (&stage)[2] = sm.stage;
   B4Compact (&compact)[2] = sm.compact;
   float2 (&tb)[2][B4_QUEUE][33] = sm.tb;
-  float4 (&qm0)[2][B4_QUEUE] = sm.qm0;
-  float4 (&qm1)[2][B4_QUEUE] = sm.qm1;
   float4 (&gpix)[2][32] = sm.gpix;
   int (&warp_max_s)[2] = sm.warp_max_s;
   B2R_TRACE_BEGIN();
@@ -141,13 +143,13 @@ __device__ __forceinline__ void bwd4_item(const B2RScene& sc, const Ctx& cx, con
     B = __fdividef(num, c.x);
   }
   float la = 0.f, olm = 1.f, lv = 0.f;
-  int qpos = 0;  // warp-uniform
+  int qpos = 0, qbase = 0;  // warp-uniform: queued splats in the transposition queue, survivor-queue slot of the first
   B4Compact& cw = compact[warp];
-  const bool lane0 = lane == 0;
   const unsigned lanes_above = 0xfffffffeu << lane;  // lanes with a higher index (= later list entries)
   const uint32_t first_grad = args.first_row;        // Gaussians below it are detached in this view: no accumulation
 
-  // phase B: 32 / B4_QUEUE lanes share a queued splat, each walks its pixel rows; combined with shuffles
+  // phase B: 32 / B4_QUEUE lanes share a queued splat, each walks its pixel rows; combined with shuffles.  The splat's
+  // record is read from its survivor-queue slot, which phase A left in place.
   auto drain = [&](const int count) {
     constexpr int SHARE = 32 / B4_QUEUE;  // lanes per queued splat
     constexpr int ROWS = 4 / SHARE;       // pixel rows (of eight) per lane
@@ -158,8 +160,10 @@ __device__ __forceinline__ void bwd4_item(const B2RScene& sc, const Ctx& cx, con
     float Sx = 0.f, Sy = 0.f, Sxx = 0.f, Sxy = 0.f, Syy = 0.f, Sq = 0.f, Sr = 0.f, Sg = 0.f, Sb = 0.f, Sd = 0.f;
     float4 m0 = make_float4(0.f, 0.f, 0.f, 0.f), m1 = make_float4(0.f, 1.f, 0.f, 0.f);
     if (live) {
-      m0 = qm0[warp][h];
-      m1 = qm1[warp][h];
+      const int slot = qbase + h < B4_CQ ? qbase + h : qbase + h - B4_CQ;
+      m0 = cw.r[0][slot];
+      const float4 r1 = cw.r[1][slot];
+      m1 = make_float4(r1.x, r1.y, cw.r[2][slot].w, 0.f);
       // ROWS pixel rows of eight per lane.  Within a row dy is constant, so only q, q dx and q dx^2 are summed per
       // pixel; the dy moments are formed once per row from the row sums.
       const float mx = m0.x - rx0, my = m0.y - ry0;
@@ -244,9 +248,9 @@ __device__ __forceinline__ void bwd4_item(const B2RScene& sc, const Ctx& cx, con
   };
 
   // One trip = B4_GROUP queued survivors.  Stage 1 (independent per splat, so the four overlap): exponent, alpha,
-  // validity, the scalar "colour" v = c . g, and the per-splat record for phase B (written by lane 0).  Stage 2: the
-  // short serial recurrences (T, B) and the two numbers per pixel that go to the transposition queue.  No branches
-  // inside a trip; a splat no pixel of the warp accepts still takes a queue slot (all-zero column).
+  // validity and the scalar "colour" v = c . g.  Stage 2: the short serial recurrences (T, B) and the two numbers per
+  // pixel that go to the transposition queue.  No branches inside a trip; a splat no pixel of the warp accepts still
+  // takes a queue slot (all-zero column).  The splats' records stay in their survivor-queue slots for phase B.
   auto replay_group = [&](const int k) {
     float araw[B4_GROUP], vv[B4_GROUP];
     bool valid[B4_GROUP];
@@ -260,11 +264,8 @@ __device__ __forceinline__ void bwd4_item(const B2RScene& sc, const Ctx& cx, con
       float v = fmaf(col.z, g_b, fmaf(col.y, g_g, col.x * g_r));
       if (HAS_DA) v += fmaf(bb.z, g_d, g_a);
       vv[u] = v;
-      if (lane0) {
-        qm0[warp][qpos + u] = a;
-        qm1[warp][qpos + u] = make_float4(bb.x, bb.y, col.w, 0.f);
-      }
     }
+    if (qpos == 0) qbase = k;
 #pragma unroll
     for (int u = 0; u < B4_GROUP; u++) {
       const float ae = valid[u] ? fminf(K_ALPHA_MAX, araw[u]) : 0.f;  // a skipped splat enters with alpha = 0 (identity)
@@ -348,10 +349,11 @@ template <bool HAS_DA>
 __global__ void __launch_bounds__(B4_THREADS, B4_MIN_BLOCKS) composite_bwd4_kernel(const B2RScene sc, const Ctx cx,
                                                                     const B2RBackwardArgs args, float* __restrict__ gacc) {
   __shared__ B4Smem sm;
-  const int n_multi = cx.ckpt ? (int)cx.classes[CLS_N_MULTI] : 0;
-  const int total_segs = cx.ckpt ? (int)cx.classes[CLS_TOTAL_SEGS] : 0;
-  const int items = 4 * (total_segs + (cx.tiles - n_multi));
-  for (int item = blockIdx.x; item < items; item += gridDim.x) {
+  // the two counters are re-read per item rather than kept live across the item loop: held in registers they spill
+  for (int item = blockIdx.x;; item += gridDim.x) {
+    const int n_multi = cx.ckpt ? (int)cx.classes[CLS_N_MULTI] : 0;
+    const int total_segs = cx.ckpt ? (int)cx.classes[CLS_TOTAL_SEGS] : 0;
+    if (item >= 4 * (total_segs + (cx.tiles - n_multi))) break;
     const int s_item = item >> 2;
     int t_pos, seg;
     if (s_item < total_segs) {
